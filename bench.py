@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Headline benchmark: Llama-2-7B training tokens/s on N GPUs of one node with TP=N (BASELINE.json).
 
-    python bench.py --gpus 1 --steps 5 --warmup 3
+    python bench.py --gpus 1 --steps 5 --warmup 3 [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -10,6 +10,11 @@ gradient accumulation), bf16 compute, fp32 master weights + fp32 gradient accumu
 ZeRO-1 optimizer (DP=1), sequence parallel on for TP>1 — the reference's tp_zero1_llama2_7B recipe
 (examples/training/llama/tp_zero1_llama_hf_pretrain/tp_zero1_llama2_7B_hf_pretrain.sh:21-41,155-172) with
 synthetic tokens and random-init weights.  Rank 0 prints ONE JSON line.
+
+Model size: fp32 master weights + fp32 gradients + AdamW moments + bf16 weights are 18 bytes per parameter, 126 GB for the
+full 7B model, which does not fit one 80 GB H100.  With fewer than 4 GPUs the default therefore keeps the Llama-2-7B layer
+geometry (hidden 4096, 32 heads of 128, MLP 11008, vocab 32000) with 12 of its 32 decoder layers per GPU (2.7B parameters on
+one GPU); ``--layers`` overrides it.
 """
 from __future__ import annotations
 
@@ -20,6 +25,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
@@ -40,7 +46,8 @@ def parse():
                          "inference latency, batch 1, seq 2048) | pp (BASELINE config 4: GPT-NeoX-20B TP x PP=2 1F1B training)")
     ap.add_argument("--seq", type=int, default=4096)
     ap.add_argument("--global-batch", type=int, default=4)
-    ap.add_argument("--layers", type=int, default=32, help="32 = Llama-2-7B (anything else is a debug run)")
+    ap.add_argument("--layers", type=int, default=0,
+                    help="decoder layers of the Llama-2-7B geometry (32 = Llama-2-7B; 0 = 32 on 4+ GPUs, else 12 per GPU)")
     ap.add_argument("--backend", default=os.environ.get("NXD_TP_BACKEND", "fused"), choices=["fused", "nccl"])
     ap.add_argument("--act-ckpt", default="none", choices=["none", "full"])
     ap.add_argument("--no-e2e", action="store_true")
@@ -51,8 +58,11 @@ def parse():
     ap.add_argument("--dp", type=int, default=1, help="data-parallel degree: ZeRO-1 shards the optimizer over it and its gradient "
                                                       "reduce-scatter kernel runs in the step (BASELINE config 3: --gpus 8 --tp 4 --dp 2)")
     ap.add_argument("--micro-batch", type=int, default=0,
-                    help="sequences per forward/backward (0 = auto: 2 up to 2 GPUs, 4 beyond — fewer fp32 wgrad read-modify-write "
-                         "passes and TP collectives off their latency floor; 4 does not fit in 180 GB at TP=1); same value in both arms")
+                    help="sequences per forward/backward (0 = auto: 1 on one GPU, 2 on two, 4 beyond — fewer fp32 wgrad "
+                         "read-modify-write passes and TP collectives off their latency floor); same value in both arms")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write what the last timed step computed (loss, gradient norm, a fixed seeded "
+                         "sample of every updated parameter) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -64,7 +74,7 @@ class ClockSampler:
          "clocks_event_reasons.sw_power_cap")
 
     def __init__(self, gpu_index: int = 0):
-        self.proc, self.path, self.gpu = None, f"/tmp/nxd_clocks_{os.getpid()}.csv", gpu_index
+        self.proc, self.path, self.gpu = None, os.path.join(tempfile.gettempdir(), f"nxd_clocks_{os.getpid()}.csv"), gpu_index
 
     def start(self):
         try:
@@ -142,11 +152,38 @@ def _tp_comm_info(tp: int, backend: str) -> dict:
 
 
 def _micro_batch(args) -> int:
-    mbs = args.micro_batch if args.micro_batch > 0 else {1: 2, 2: 2, 4: 4, 8: 4}.get(args.gpus, 1)
+    mbs = args.micro_batch if args.micro_batch > 0 else {1: 1, 2: 2, 4: 4, 8: 4}.get(args.gpus, 1)
     mbs = max(1, min(mbs, args.global_batch))
     while args.global_batch % mbs:
         mbs -= 1
     return mbs
+
+
+DUMP_BYTES = 48 << 20        # all ranks' parameter samples together (the dump is capped at 64 MB in all)
+
+
+def dump_outputs(out_dir: str, model, loss, grad_norm, rank: int, world: int) -> None:
+    """What the last timed step computed, as float32 / float64 ``.npy`` files: the loss, the gradient norm and, for every
+    parameter after the optimizer step, the same flat indices (drawn from a fixed seed per parameter shape).  The per-parameter
+    sample size divides ``DUMP_BYTES`` over all ranks' parameters."""
+    import numpy as np
+    import torch
+
+    n_params = sum(1 for _ in model.parameters())
+    sample = max(1, DUMP_BYTES // (4 * n_params * world))
+
+    os.makedirs(out_dir, exist_ok=True)
+    tag = "" if rank == 0 else f"rank{rank}."
+    np.save(os.path.join(out_dir, f"{tag}loss.npy"), np.array([float(loss.item())], dtype=np.float64))
+    if grad_norm is not None:
+        np.save(os.path.join(out_dir, f"{tag}grad_norm.npy"), np.array([float(grad_norm)], dtype=np.float64))
+    for name, p in model.named_parameters():
+        flat = p.detach().reshape(-1)
+        if flat.numel() > sample:
+            g = torch.Generator().manual_seed(flat.numel())
+            idx = torch.randperm(flat.numel(), generator=g)[:sample].sort().values.to(flat.device)
+            flat = flat[idx]
+        np.save(os.path.join(out_dir, f"{tag}param.{name}.npy"), flat.float().cpu().numpy())
 
 
 def main():
@@ -192,8 +229,8 @@ def main():
     tp = args.tp if args.tp > 0 else world // dp
     assert tp * dp == world, f"--tp {tp} x --dp {dp} != {world} GPUs"
     # dp > 1: ZeRO-1's reduce-scatter / all-gather kernels run in optimizer.step().  The bucketed variant that launches them
-    # under the backward (NXD_ZERO1_OVERLAP=1) measured SLOWER on 2 GPUs (610 vs 393 ms/step: its 16 resident CTAs keep the
-    # persistent 148-CTA GEMMs from being fully resident, so every GEMM runs a second partial wave) and stays opt-in.
+    # under the backward (NXD_ZERO1_OVERLAP=1) keeps 16 CTAs resident next to the persistent one-CTA-per-SM GEMMs, so every
+    # GEMM runs a second partial wave; it stays opt-in.
     sp = tp > 1
     cfg = nxd.neuronx_distributed_config(
         tensor_parallel_size=tp, sequence_parallel=sp,
@@ -202,7 +239,8 @@ def main():
     )
     mcfg = llama2_7b_config(sequence_parallel_enabled=sp, dtype=torch.bfloat16, device=dev,
                             max_position_embeddings=args.seq, activation_checkpointing=args.act_ckpt)
-    mcfg.num_hidden_layers = args.layers
+    layers = args.layers if args.layers > 0 else (32 if world >= 4 else 12 * world)
+    mcfg.num_hidden_layers = layers
 
     def model_fn():
         torch.manual_seed(1234)
@@ -278,6 +316,8 @@ def main():
     ms_total = float(t.item())
     clocks = sampler.stop() if sampler else None
     final_loss = float(loss.item())
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, model, loss, opt.grad_norm, rank, world)
     tokens_per_step = gbs * S
     value = tokens_per_step * args.steps / (ms_total / 1e3)
 
@@ -334,9 +374,10 @@ def main():
             "metric": "Llama-2-7B training tokens/sec (whole job, device-timed, max over ranks)",
             "value": value, "unit": "tokens/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms_total / args.steps, "higher_is_better": True, "scaling": "strong",
-            "vs_baseline": value / PUBLISHED_TOKENS_PER_S, "dtype": "bf16", "data": "synthetic",
+            # the published number is for the full 32-layer model: fewer layers are normalised by the decoder-layer count
+            "vs_baseline": value * layers / 32 / PUBLISHED_TOKENS_PER_S, "dtype": "bf16", "data": "synthetic",
             "impl": "ours",
-            "config": {"model": "llama2-7b" if args.layers == 32 else f"llama2-7b-{args.layers}L(debug)",
+            "config": {"model": "llama2-7b" if layers == 32 else f"llama2-7b-geometry-{layers}L",
                        "global_batch": gbs, "micro_batch": mbs, "seq_len": S,
                        "parallelism": f"tp{tp}" + ("+sp" if sp else "") + (f" x dp{dp}" if dp > 1 else ""),
                        "optimizer": f"AdamW fp32 master + fp32 grad-acc (ZeRO-1, dp={dp}"
@@ -344,10 +385,12 @@ def main():
                                     + (", bucketed under backward" if dp > 1 and os.environ.get("NXD_ZERO1_OVERLAP", "0") == "1" else "") + ")",
                        "tp_backend": args.backend, **_tp_comm_info(tp, args.backend),
                        "act_ckpt": args.act_ckpt, "l2": "inputs(weights+activations)>>L2, no flush needed",
-                       "baseline_note": "vs_baseline divides by the only published number: Trn1 32-core gate 6.90 seq/s @ seq 8192",
+                       "baseline_note": "vs_baseline divides by the only published number: Trn1 32-core gate 6.90 seq/s @ seq 8192 (full 32-layer "
+                                        "model; runs with fewer layers are scaled by layers / 32)",
                        "final_loss": final_loss, "loss_trace": [round(float(x), 4) for x in trace],
                        "grad_norm": float(opt.grad_norm) if opt.grad_norm is not None else None},
             "clocks": clocks, "e2e": e2e, "gpu_launches": launches, "comm": comm_report,
+            "gpu": torch.cuda.get_device_name(dev), "max_memory_allocated_gb": torch.cuda.max_memory_allocated(dev) / 2**30,
         }
         if phases:
             torch.cuda.synchronize()

@@ -1,0 +1,486 @@
+// Flash attention for sm_90a (head_dim 128, bf16): warp-level bf16 tensor-core MMAs (mma.sync m16n8k16, ldmatrix operand
+// loads from padded shared memory, cp.async double-buffered tiles), fp32 online softmax.  Role parity: reference
+// kernels/flash_attn.py:162-212 (nki_flash_attn_func → flash_fwd / flash_attn_bwd) and modules/attention call sites.
+//
+// Forward, one CTA per (64-query tile, head, batch), 4 warps, warp w owns query rows 16w..16w+15 of the tile:
+//   S = Q·K_jᵀ (fp32 fragments), running max / sum in registers, P packed to bf16 straight from the S fragments into the
+//   A operand of O += P·V_j.  Outputs: O (bf16, arbitrary b/s/h strides) and LSE (fp32 [B, H, S], natural log).
+// Backward, three launches:
+//   prep   δ = rowsum(dO ∘ O) − dLSE                                         (one warp per query row)
+//   dK/dV  one CTA per (64-key tile, kv head, batch), loops over the query tiles of every query head of the group:
+//          Sᵀ = K·Qᵀ, Pᵀ = exp(Sᵀ − LSE), dV += Pᵀ·dO, dPᵀ = V·dOᵀ, dSᵀ = Pᵀ∘(dPᵀ − δ), dK += dSᵀ·Q
+//   dQ     one CTA per (64-query tile, head, batch), loops over the key tiles: S, P, dP = dO·Vᵀ, dS, dQ += dS·K
+//   Every gradient element is owned by one thread of one CTA (no atomics), so the backward is bit-reproducible.
+#include <cuda.h>
+
+#include "common.cuh"
+#include "kernels.h"
+
+namespace nxd {
+namespace fa {
+
+constexpr int HD = 128;
+constexpr int BT = 64;                       // rows of a query or key tile
+constexpr int kThreads = 128;
+constexpr int LDS = HD + 8;                  // padded shared-memory row (elements): 272 B, ldmatrix rows hit distinct banks
+constexpr int kTile = BT * LDS;              // elements of one staged tile
+constexpr int kSmemFwd = 5 * kTile * 2;                      // Q, K×2, V×2
+constexpr int kSmemDkv = 6 * kTile * 2 + 4 * BT * 4;         // K, V, Q×2, dO×2, LSE×2, δ×2
+constexpr int kSmemDq = 6 * kTile * 2;                       // Q, dO, K×2, V×2
+constexpr float kLog2e = 1.4426950408889634f;
+
+typedef __nv_bfloat16 bf16;
+
+struct View { const bf16* p; long sb, ss, sh; };
+
+NXD_DEVICE uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// two floats → bf16x2, `lo` in the low half (the lower address)
+NXD_DEVICE uint32_t pack_bf16(float lo, float hi) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+NXD_DEVICE void cp_async16(bf16* dst, const bf16* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_addr(dst)), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+NXD_DEVICE void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+NXD_DEVICE void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// rows [s0, s0+64) of one (batch, head) slice → padded shared tile; rows ≥ S are zero-filled
+NXD_DEVICE void load_tile(bf16* sm, const bf16* base, long ss, int s0, int S) {
+  for (int i = threadIdx.x; i < BT * (HD / 8); i += kThreads) {
+    const int r = i >> 4, c = i & 15;
+    const bool ok = s0 + r < S;
+    cp_async16(sm + r * LDS + c * 8, base + (long)(ok ? s0 + r : 0) * ss + c * 8, ok);
+  }
+}
+
+NXD_DEVICE void ldsm_x4(uint32_t (&r)[4], const bf16* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_addr(p)));
+}
+NXD_DEVICE void ldsm_x4_t(uint32_t (&r)[4], const bf16* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_addr(p)));
+}
+NXD_DEVICE void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// C[16 x 64] = A[16 rows from a_row0][128] · Bᵀ where B is a 64-row tile, both with the 128-long k dimension contiguous
+// (QKᵀ, KQᵀ, VdOᵀ, dOVᵀ).  C fragment j holds columns 8j..8j+7: c0,c1 row lane/4, c2,c3 row lane/4+8, columns 2(lane%4)+{0,1}.
+NXD_DEVICE void mma_abt(float (&c)[8][4], const bf16* sa, int a_row0, const bf16* sb) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) c[j][0] = c[j][1] = c[j][2] = c[j][3] = 0.f;
+#pragma unroll
+  for (int ks = 0; ks < HD / 16; ++ks) {
+    uint32_t a[4];
+    ldsm_x4(a, sa + (a_row0 + (lane & 15)) * LDS + ks * 16 + (lane >> 4) * 8);
+#pragma unroll
+    for (int jp = 0; jp < 4; ++jp) {
+      uint32_t b[4];
+      ldsm_x4(b, sb + (jp * 16 + (lane & 7) + (lane >> 4) * 8) * LDS + ks * 16 + ((lane >> 3) & 1) * 8);
+      mma16816(c[2 * jp], a, b[0], b[1]);
+      mma16816(c[2 * jp + 1], a, b[2], b[3]);
+    }
+  }
+}
+
+// C[16 x 128] += P[16 x 64] · B where P comes as bf16 A fragments (4 k-steps) and B is a 64-row tile with the 128-wide
+// output dimension contiguous (P·V, Pᵀ·dO, dSᵀ·Q, dS·K).
+NXD_DEVICE void mma_pb(float (&c)[16][4], const uint32_t (&p)[4][4], const bf16* sb) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int ks = 0; ks < BT / 16; ++ks) {
+#pragma unroll
+    for (int dp = 0; dp < HD / 16; ++dp) {
+      uint32_t b[4];
+      ldsm_x4_t(b, sb + (ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * LDS + dp * 16 + (lane >> 4) * 8);
+      mma16816(c[2 * dp], p[ks], b[0], b[1]);
+      mma16816(c[2 * dp + 1], p[ks], b[2], b[3]);
+    }
+  }
+}
+
+// fp32 C fragments of a 16 x 64 block → bf16 A fragments of the next MMA (same thread ↔ element mapping)
+NXD_DEVICE void to_a_frags(const float (&c)[8][4], uint32_t (&p)[4][4]) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    p[ks][0] = pack_bf16(c[2 * ks][0], c[2 * ks][1]);
+    p[ks][1] = pack_bf16(c[2 * ks][2], c[2 * ks][3]);
+    p[ks][2] = pack_bf16(c[2 * ks + 1][0], c[2 * ks + 1][1]);
+    p[ks][3] = pack_bf16(c[2 * ks + 1][2], c[2 * ks + 1][3]);
+  }
+}
+
+// 16 x 128 fp32 fragments (rows row0 + lane/4 and +8) × scale → bf16 rows of a [B,S,H,128] view
+NXD_DEVICE void store_rows(const float (&c)[16][4], bf16* base, long ss, int row0, int S, float scale0, float scale1) {
+  const int lane = threadIdx.x & 31;
+  const int r0 = row0 + (lane >> 2), r1 = r0 + 8;
+#pragma unroll
+  for (int dt = 0; dt < 16; ++dt) {
+    const int d = dt * 8 + 2 * (lane & 3);
+    if (r0 < S) *(uint32_t*)(base + (long)r0 * ss + d) = pack_bf16(c[dt][0] * scale0, c[dt][1] * scale0);
+    if (r1 < S) *(uint32_t*)(base + (long)r1 * ss + d) = pack_bf16(c[dt][2] * scale1, c[dt][3] * scale1);
+  }
+}
+
+struct FwdParams {
+  View q, k, v;
+  bf16* o; long o_sb, o_ss, o_sh;
+  float* lse;
+  int B, H, Hkv, S_q, S_kv, causal;
+  float scale_log2;
+};
+
+__global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  bf16* sQ = (bf16*)smem_raw;
+  bf16* sK = sQ + kTile;        // 2 buffers
+  bf16* sV = sK + 2 * kTile;    // 2 buffers
+  // causal: the last query tiles see the most keys, so they are scheduled first
+  const int qt = gridDim.x - 1 - blockIdx.x, h = blockIdx.y, b = blockIdx.z, hk = h / (p.H / p.Hkv);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = qt * BT;
+  const bf16* qb = p.q.p + b * p.q.sb + h * p.q.sh;
+  const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
+  const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
+  const int n_kv = p.causal ? min((p.S_kv + BT - 1) / BT, qt + 1) : (p.S_kv + BT - 1) / BT;
+
+  load_tile(sQ, qb, p.q.ss, q0, p.S_q);
+  load_tile(sK, kb, p.k.ss, 0, p.S_kv);
+  load_tile(sV, vb, p.v.ss, 0, p.S_kv);
+  cp_async_commit();
+
+  float o[16][4];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  const int row[2] = {q0 + warp * 16 + (lane >> 2), q0 + warp * 16 + (lane >> 2) + 8};
+
+  for (int t = 0; t < n_kv; ++t) {
+    const int buf = t & 1;
+    if (t + 1 < n_kv) {
+      load_tile(sK + (buf ^ 1) * kTile, kb, p.k.ss, (t + 1) * BT, p.S_kv);
+      load_tile(sV + (buf ^ 1) * kTile, vb, p.v.ss, (t + 1) * BT, p.S_kv);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    float s[8][4];
+    mma_abt(s, sQ, warp * 16, sK + buf * kTile);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int key = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
+        float x = s[j][e] * p.scale_log2;
+        if (key >= p.S_kv || (p.causal && key > row[e >> 1])) x = -INFINITY;
+        s[j][e] = x;
+        mx[e >> 1] = fmaxf(mx[e >> 1], x);
+      }
+    }
+    float alpha[2], mu[2], rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float mn = fmaxf(m[r], mx[r]);
+      mu[r] = mn == -INFINITY ? 0.f : mn;         // a row with no visible key so far keeps P = 0
+      alpha[r] = exp2f(m[r] - mu[r]);
+      m[r] = mn;
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float x = exp2f(s[j][e] - mu[e >> 1]);
+        s[j][e] = x;
+        rs[e >> 1] += x;
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) l[r] = l[r] * alpha[r] + rs[r];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) { o[i][0] *= alpha[0]; o[i][1] *= alpha[0]; o[i][2] *= alpha[1]; o[i][3] *= alpha[1]; }
+    uint32_t pf[4][4];
+    to_a_frags(s, pf);
+    mma_pb(o, pf, sV + buf * kTile);
+    __syncthreads();                              // buffer `buf` is refilled at the next iteration
+  }
+  float inv[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+    inv[r] = l[r] > 0.f ? 1.f / l[r] : 0.f;
+  }
+  store_rows(o, p.o + b * p.o_sb + h * p.o_sh, p.o_ss, q0 + warp * 16, p.S_q, inv[0], inv[1]);
+  if ((lane & 3) == 0) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+      if (row[r] < p.S_q)
+        p.lse[((long)b * p.H + h) * p.S_q + row[r]] = l[r] > 0.f ? (m[r] + __log2f(l[r])) / kLog2e : -INFINITY;
+  }
+}
+
+// δ[b,h,s] = Σ_d dO·O − dLSE   (one warp per query row)
+__global__ void fa_bwd_prep_kernel(const bf16* __restrict__ o, const bf16* __restrict__ go, const float* __restrict__ dlse,
+                                   float* __restrict__ delta, int B, int S, int H, long o_sb, long o_ss, long o_sh, long g_sb,
+                                   long g_ss, long g_sh) {
+  const long w = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= (long)B * H * S) return;
+  const int s = (int)(w % S), h = (int)((w / S) % H), b = (int)(w / ((long)S * H));
+  const uint2 ov = *(const uint2*)(o + b * o_sb + s * o_ss + h * o_sh + lane * 4);
+  const uint2 gv = *(const uint2*)(go + b * g_sb + s * g_ss + h * g_sh + lane * 4);
+  const __nv_bfloat162* oh = (const __nv_bfloat162*)&ov;
+  const __nv_bfloat162* gh = (const __nv_bfloat162*)&gv;
+  float acc = 0.f;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const float2 a = __bfloat1622float2(oh[j]), c = __bfloat1622float2(gh[j]);
+    acc += a.x * c.x + a.y * c.y;
+  }
+#pragma unroll
+  for (int off = 16; off; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+  // w enumerates (b, h, s) in the [B, H, S] order of LSE / δ
+  if (lane == 0) delta[w] = acc - (dlse ? dlse[w] : 0.f);
+}
+
+struct BwdParams {
+  View q, k, v, g;
+  bf16 *dq, *dk, *dv;
+  long dq_sb, dq_ss, dq_sh, dk_sb, dk_ss, dk_sh, dv_sb, dv_ss, dv_sh;
+  const float *lse, *delta;
+  int B, H, Hkv, S_q, S_kv, causal;
+  float scale, scale_log2;
+};
+
+__global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParams p) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  bf16* sK = (bf16*)smem_raw;
+  bf16* sV = sK + kTile;
+  bf16* sQ = sV + kTile;        // 2 buffers
+  bf16* sG = sQ + 2 * kTile;    // 2 buffers
+  float* sL = (float*)(sG + 2 * kTile);   // 2 × 64 LSE (log2 units)
+  float* sD = sL + 2 * BT;                // 2 × 64 δ
+  const int kt = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
+  const int G = p.H / p.Hkv;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int k0 = kt * BT;
+  const int n_qt = (p.S_q + BT - 1) / BT;
+  const int qt0 = p.causal ? kt : 0;                 // causal: S_q == S_kv, query tiles before the key tile see none of it
+  const int per_head = n_qt > qt0 ? n_qt - qt0 : 0;
+  const int n_it = G * per_head;
+
+  load_tile(sK, p.k.p + b * p.k.sb + hk * p.k.sh, p.k.ss, k0, p.S_kv);
+  load_tile(sV, p.v.p + b * p.v.sb + hk * p.v.sh, p.v.ss, k0, p.S_kv);
+  auto issue = [&](int it, int buf) {
+    const int h = hk * G + it / per_head, q0 = (qt0 + it % per_head) * BT;
+    load_tile(sQ + buf * kTile, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
+    load_tile(sG + buf * kTile, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
+    if (threadIdx.x < BT) {
+      const int s = q0 + threadIdx.x;
+      const long i = ((long)b * p.H + h) * p.S_q + s;
+      sL[buf * BT + threadIdx.x] = s < p.S_q ? p.lse[i] * kLog2e : 0.f;
+      sD[buf * BT + threadIdx.x] = s < p.S_q ? p.delta[i] : 0.f;
+    }
+  };
+  if (n_it > 0) issue(0, 0);
+  cp_async_commit();
+
+  float dk[16][4], dv[16][4];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = 0.f;
+    dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f;
+  }
+  const int key[2] = {k0 + warp * 16 + (lane >> 2), k0 + warp * 16 + (lane >> 2) + 8};
+
+  for (int it = 0; it < n_it; ++it) {
+    const int buf = it & 1;
+    const int q0 = (qt0 + it % per_head) * BT;
+    if (it + 1 < n_it) {
+      issue(it + 1, buf ^ 1);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    const bf16* q = sQ + buf * kTile;
+    const bf16* g = sG + buf * kTile;
+    const float* L = sL + buf * BT;
+    const float* D = sD + buf * BT;
+    float pt[8][4];
+    mma_abt(pt, sK, warp * 16, q);                   // Sᵀ: rows = keys, columns = queries
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int qc = j * 8 + 2 * (lane & 3) + (e & 1);
+        const int qi = q0 + qc;
+        const bool vis = qi < p.S_q && !(p.causal && key[e >> 1] > qi);
+        pt[j][e] = vis ? exp2f(pt[j][e] * p.scale_log2 - L[qc]) : 0.f;
+      }
+    }
+    uint32_t pf[4][4];
+    to_a_frags(pt, pf);
+    mma_pb(dv, pf, g);                               // dV += Pᵀ·dO
+    float dpt[8][4];
+    mma_abt(dpt, sV, warp * 16, g);                  // dPᵀ = V·dOᵀ
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int qc = j * 8 + 2 * (lane & 3) + (e & 1);
+        dpt[j][e] = pt[j][e] * (dpt[j][e] - D[qc]);
+      }
+    }
+    to_a_frags(dpt, pf);
+    mma_pb(dk, pf, q);                               // dK += dSᵀ·Q
+    __syncthreads();
+  }
+  store_rows(dk, p.dk + b * p.dk_sb + hk * p.dk_sh, p.dk_ss, k0 + warp * 16, p.S_kv, p.scale, p.scale);
+  store_rows(dv, p.dv + b * p.dv_sb + hk * p.dv_sh, p.dv_ss, k0 + warp * 16, p.S_kv, 1.f, 1.f);
+}
+
+__global__ void __launch_bounds__(kThreads) fa_bwd_dq_kernel(const BwdParams p) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  bf16* sQ = (bf16*)smem_raw;
+  bf16* sG = sQ + kTile;
+  bf16* sK = sG + kTile;        // 2 buffers
+  bf16* sV = sK + 2 * kTile;    // 2 buffers
+  // causal: the last query tiles see the most keys, so they are scheduled first
+  const int qt = gridDim.x - 1 - blockIdx.x, h = blockIdx.y, b = blockIdx.z, hk = h / (p.H / p.Hkv);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = qt * BT;
+  const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
+  const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
+  const int n_kv = p.causal ? min((p.S_kv + BT - 1) / BT, qt + 1) : (p.S_kv + BT - 1) / BT;
+
+  load_tile(sQ, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
+  load_tile(sG, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
+  load_tile(sK, kb, p.k.ss, 0, p.S_kv);
+  load_tile(sV, vb, p.v.ss, 0, p.S_kv);
+  cp_async_commit();
+
+  const int row[2] = {q0 + warp * 16 + (lane >> 2), q0 + warp * 16 + (lane >> 2) + 8};
+  float L[2], D[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const long i = ((long)b * p.H + h) * p.S_q + row[r];
+    L[r] = row[r] < p.S_q ? p.lse[i] * kLog2e : 0.f;
+    D[r] = row[r] < p.S_q ? p.delta[i] : 0.f;
+  }
+  float dq[16][4];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
+
+  for (int t = 0; t < n_kv; ++t) {
+    const int buf = t & 1;
+    if (t + 1 < n_kv) {
+      load_tile(sK + (buf ^ 1) * kTile, kb, p.k.ss, (t + 1) * BT, p.S_kv);
+      load_tile(sV + (buf ^ 1) * kTile, vb, p.v.ss, (t + 1) * BT, p.S_kv);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    const bf16* k = sK + buf * kTile;
+    float s[8][4];
+    mma_abt(s, sQ, warp * 16, k);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int kc = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
+        const int r = row[e >> 1];
+        const bool vis = kc < p.S_kv && r < p.S_q && !(p.causal && kc > r);
+        s[j][e] = vis ? exp2f(s[j][e] * p.scale_log2 - L[e >> 1]) : 0.f;
+      }
+    }
+    float dp[8][4];
+    mma_abt(dp, sG, warp * 16, sV + buf * kTile);    // dP = dO·Vᵀ
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) dp[j][e] = s[j][e] * (dp[j][e] - D[e >> 1]);
+    }
+    uint32_t pf[4][4];
+    to_a_frags(dp, pf);
+    mma_pb(dq, pf, k);                               // dQ += dS·K
+    __syncthreads();
+  }
+  store_rows(dq, p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, q0 + warp * 16, p.S_q, p.scale, p.scale);
+}
+
+static View view(const void* ptr, const long* s) {
+  if (((uintptr_t)ptr % 16) || (s[0] % 8) || (s[1] % 8) || (s[2] % 8))
+    nxd_throw("attention: q/k/v/o rows must be 16-byte aligned", __FILE__, __LINE__);
+  return View{(const bf16*)ptr, s[0], s[1], s[2]};
+}
+
+}  // namespace fa
+
+void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
+                    int Hkv, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
+                    cudaStream_t st) {
+  using namespace fa;
+  if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
+  FwdParams p;
+  p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs);
+  p.o = (bf16*)out; p.o_sb = os[0]; p.o_ss = os[1]; p.o_sh = os[2];
+  p.lse = lse;
+  p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
+  p.scale_log2 = scale * kLog2e;
+  static bool configured = false;
+  if (!configured) {
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemFwd));
+    configured = true;
+  }
+  fa_fwd_kernel<<<dim3((S_q + BT - 1) / BT, H, B), kThreads, kSmemFwd, st>>>(p);
+  NXD_CUDA_CHECK(cudaGetLastError());
+}
+
+void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
+                    const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
+                    const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
+                    const long* dks, const long* dvs, float scale, bool causal, cudaStream_t st) {
+  using namespace fa;
+  if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
+  {
+    const long rows = (long)B * H * S_q;
+    fa_bwd_prep_kernel<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(
+        (const bf16*)o, (const bf16*)go, dlse, delta, B, S_q, H, os[0], os[1], os[2], gs[0], gs[1], gs[2]);
+  }
+  BwdParams p;
+  p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs); p.g = view(go, gs);
+  p.dq = (bf16*)dq; p.dk = (bf16*)dk; p.dv = (bf16*)dv;
+  p.dq_sb = dqs[0]; p.dq_ss = dqs[1]; p.dq_sh = dqs[2];
+  p.dk_sb = dks[0]; p.dk_ss = dks[1]; p.dk_sh = dks[2];
+  p.dv_sb = dvs[0]; p.dv_ss = dvs[1]; p.dv_sh = dvs[2];
+  p.lse = lse; p.delta = delta;
+  p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
+  p.scale = scale; p.scale_log2 = scale * kLog2e;
+  static bool configured = false;
+  if (!configured) {
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dkdv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemDkv));
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemDq));
+    configured = true;
+  }
+  fa_bwd_dkdv_kernel<<<dim3((S_kv + BT - 1) / BT, Hkv, B), kThreads, kSmemDkv, st>>>(p);
+  fa_bwd_dq_kernel<<<dim3((S_q + BT - 1) / BT, H, B), kThreads, kSmemDq, st>>>(p);
+  NXD_CUDA_CHECK(cudaGetLastError());
+}
+
+}  // namespace nxd

@@ -19,6 +19,7 @@ static int dt_code(const Tensor& t) {
   }
 }
 static cudaStream_t stream() { return at::cuda::getCurrentCUDAStream().stream(); }
+static int num_sms() { return at::cuda::getCurrentDeviceProperties()->multiProcessorCount; }
 #define CHECK_IN(t) TORCH_CHECK((t).is_cuda() && (t).is_contiguous(), #t " must be a contiguous CUDA tensor")
 
 static std::vector<Tensor> rmsnorm_fwd(const Tensor& x, const Tensor& w, double eps) {
@@ -248,7 +249,7 @@ static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v
   TORCH_CHECK(q.stride(2) % 8 == 0 && k.stride(1) % 8 == 0 && k.stride(2) % 8 == 0 && v.stride(1) % 8 == 0 && v.stride(2) % 8 == 0);
   c10::cuda::CUDAGuard guard(q.device());
   // enough CTAs for ~6 per SM (the kernel is latency-bound per CTA: 8 cache rows in flight), at least 64 rows per split
-  int splits = (6 * 148 + B * Hkv - 1) / (B * Hkv);
+  int splits = (6 * num_sms() + B * Hkv - 1) / (B * Hkv);
   splits = std::max(1, std::min(std::min(splits, 64), (L + 63) / 64));
   Tensor out = at::empty({B, 1, H, 128}, q.options());
   Tensor part_o = at::empty({B * H * splits, 128}, q.options().dtype(at::kFloat));
@@ -272,7 +273,7 @@ static std::vector<Tensor> decode_attention_partial(const Tensor& q, const Tenso
   TORCH_CHECK(H % Hkv == 0 && k.size(0) == B);
   TORCH_CHECK(q.stride(2) % 8 == 0 && k.stride(1) % 8 == 0 && k.stride(2) % 8 == 0 && v.stride(1) % 8 == 0 && v.stride(2) % 8 == 0);
   c10::cuda::CUDAGuard guard(q.device());
-  int splits = (6 * 148 + B * Hkv - 1) / (B * Hkv);
+  int splits = (6 * num_sms() + B * Hkv - 1) / (B * Hkv);
   splits = std::max(1, std::min(std::min(splits, 64), (L + 63) / 64));
   Tensor fin_o = at::empty({B, H, 128}, q.options().dtype(at::kFloat));
   Tensor fin_ml = at::empty({B, H, 2}, q.options().dtype(at::kFloat));
@@ -325,40 +326,6 @@ static std::vector<Tensor> moe_block_tkg(const Tensor& x, const c10::optional<Te
                      pre_scale, round_logits, (int)act, (float)act_alpha, (float)act_beta, (float)gate_lo, (float)gate_hi, (float)up_lo,
                      (float)up_hi, cooperative, stream());
   return {out, logits, idx, w};
-}
-// a [M,K], b [N,K]: fp8 bytes; sfa [ceil(M/128), K/128, 512], sfb [ceil(N/128), K/128, 512]: tiled E8M0 scales → [M,N] bf16
-static Tensor gemm_mxfp8(const Tensor& a, const Tensor& b, const Tensor& sfa, const Tensor& sfb, int64_t a_fmt, int64_t b_fmt) {
-  CHECK_IN(a); CHECK_IN(b); CHECK_IN(sfa); CHECK_IN(sfb);
-  TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.element_size() == 1 && b.element_size() == 1);
-  // byte tensors: K bytes per row for fp8 formats, K/2 for packed e2m1 (format 5)
-  const int M = a.size(0), N = b.size(0), K = a_fmt == 5 ? 2 * a.size(1) : a.size(1);
-  TORCH_CHECK((b_fmt == 5 ? 2 * b.size(1) : b.size(1)) == K, "gemm_mxfp8: K of a and b differ");
-  TORCH_CHECK(K % 128 == 0 && N % 8 == 0, "gemm_mxfp8: K % 128 == 0 and N % 8 == 0");
-  TORCH_CHECK(sfa.scalar_type() == at::kByte && sfb.scalar_type() == at::kByte);
-  TORCH_CHECK(sfa.numel() == (long)((M + 127) / 128) * (K / 128) * 512 && sfb.numel() == (long)((N + 127) / 128) * (K / 128) * 512,
-              "gemm_mxfp8: scale tensors must be tiled [rows/128, K/128, 512]");
-  c10::cuda::CUDAGuard guard(a.device());
-  Tensor out = at::empty({M, N}, a.options().dtype(at::kBFloat16));
-  nxd::gemm_mxfp8(a.data_ptr(), b.data_ptr(), sfa.data_ptr(), sfb.data_ptr(), out.data_ptr(), M, N, K, (int)a_fmt, (int)b_fmt, stream());
-  return out;
-}
-// a [M,K/2], b [N,K/2]: packed e2m1 bytes; sfa [ceil(M/128), K/(4·vs), 512], sfb likewise: tiled scales (E8M0 for vs 32, UE4M3 for
-// vs 16) → alpha · product, [M,N] bf16
-static Tensor gemm_f4(const Tensor& a, const Tensor& b, const Tensor& sfa, const Tensor& sfb, int64_t vec_size, double alpha) {
-  CHECK_IN(a); CHECK_IN(b); CHECK_IN(sfa); CHECK_IN(sfb);
-  TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.element_size() == 1 && b.element_size() == 1);
-  const int M = a.size(0), N = b.size(0), K = 2 * a.size(1);
-  TORCH_CHECK(2 * b.size(1) == K, "gemm_f4: K of a and b differ");
-  TORCH_CHECK(K % 256 == 0 && N % 8 == 0, "gemm_f4: K % 256 == 0 and N % 8 == 0");
-  TORCH_CHECK(vec_size == 32 || vec_size == 16, "gemm_f4: vec_size 32 (MXFP4) or 16 (NVFP4)");
-  TORCH_CHECK(sfa.scalar_type() == at::kByte && sfb.scalar_type() == at::kByte);
-  const long kc = K / (4 * vec_size);
-  TORCH_CHECK(sfa.numel() == (long)((M + 127) / 128) * kc * 512 && sfb.numel() == (long)((N + 127) / 128) * kc * 512,
-              "gemm_f4: scale tensors must be tiled [rows/128, K/(4*vec_size), 512]");
-  c10::cuda::CUDAGuard guard(a.device());
-  Tensor out = at::empty({M, N}, a.options().dtype(at::kBFloat16));
-  nxd::gemm_f4(a.data_ptr(), b.data_ptr(), sfa.data_ptr(), sfb.data_ptr(), out.data_ptr(), M, N, K, (int)vec_size, (float)alpha, stream());
-  return out;
 }
 // x [M<=8, K] bf16; w = MX byte stream of [N, K] (fp4: K/2 bytes per row, fp8: K), any integer dtype view; scale [N, K/32] uint8
 static Tensor gemv_mx(const Tensor& x, const Tensor& w, const Tensor& scale, int64_t fmt, const c10::optional<Tensor>& residual) {
@@ -469,9 +436,7 @@ static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, con
     return sbhd_out ? at::empty({s, B, h, 128}, q.options()).transpose(0, 1) : at::empty({B, s, h, 128}, q.options());
   };
   Tensor dq = mk(S, H), dk = mk(Skv, Hkv), dv = mk(Skv, Hkv);
-  const int S_pad = (S + 63) / 64 * 64;
-  Tensor stats = at::empty({2, (int64_t)B * H * S_pad + 64}, q.options().dtype(at::kFloat));
-  Tensor dq_acc = at::empty({B, H, S_pad, 128}, q.options().dtype(at::kFloat));
+  Tensor delta = at::empty({B, H, S}, q.options().dtype(at::kFloat));
   auto st3 = [](const Tensor& t, long* out) { out[0] = t.stride(0); out[1] = t.stride(1); out[2] = t.stride(2); };
   long gs[3], qs[3], ks[3], vs[3], os[3], dqs[3], dks[3], dvs[3];
   st3(go, gs); st3(q, qs); st3(k, ks); st3(v, vs); st3(o, os); st3(dq, dqs); st3(dk, dks); st3(dv, dvs);
@@ -481,8 +446,8 @@ static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, con
     dlse_p = dlse->data_ptr<float>();
   }
   nxd::flash_attn_bwd(go.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), dlse_p,
-                      dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), stats.data_ptr<float>(), dq_acc.data_ptr<float>(), B, S,
-                      Skv, H, Hkv, S_pad, gs, qs, ks, vs, os, dqs, dks, dvs, (float)scale, causal, stream());
+                      dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr<float>(), B, S, Skv, H, Hkv, gs, qs, ks,
+                      vs, os, dqs, dks, dvs, (float)scale, causal, stream());
   return {dq, dk, dv};
 }
 
@@ -497,16 +462,6 @@ static void gemm_bf16(const Tensor& a, const Tensor& b, Tensor out, bool trans_a
   nxd::GemmComm none;
   nxd::gemm_bf16(a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, trans_a, trans_b, dt_code(out), accumulate, none,
                  nullptr, stream());
-}
-
-static void gemm_bf16_2cta(const Tensor& a, const Tensor& b, Tensor out, bool trans_a, bool trans_b, bool accumulate) {
-  CHECK_IN(a); CHECK_IN(b); CHECK_IN(out);
-  TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16 && a.dim() == 2 && b.dim() == 2);
-  const int M = (int)(trans_a ? a.size(1) : a.size(0)), K = (int)(trans_a ? a.size(0) : a.size(1));
-  const int N = (int)(trans_b ? b.size(0) : b.size(1));
-  TORCH_CHECK((trans_b ? b.size(1) : b.size(0)) == K && out.size(0) == M && out.size(1) == N, "gemm shape mismatch");
-  c10::cuda::CUDAGuard g(a.device());
-  nxd::gemm_bf16_2cta(a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, trans_a, trans_b, dt_code(out), accumulate, stream());
 }
 
 // all-gather(A shards along rows) → GEMM.  `a_shard` [M/world, K]; gathered A lives in the symmetric payload at
@@ -550,33 +505,6 @@ static void gemm_rs_bf16(const Tensor& a, const Tensor& b, Tensor out, bool tran
                  stream());
 }
 
-// CTA-pair fused TP kernels.  mode 1: a = shard [M/world,K] → out [M,N];  mode 2: a = [M,K] → out [M/world,N]
-static void tp_gemm_2cta(int64_t mode, const Tensor& a, const Tensor& b, Tensor out, Tensor partial, bool trans_b,
-                         int64_t local_buf_ptr, const Tensor& peer_bufs, const Tensor& peer_flags, int64_t buf_offset,
-                         int64_t flag_offset, int64_t epoch, int64_t rank, int64_t world, int64_t comm_ctas,
-                         Tensor counters, int64_t gemm_done_target) {
-  CHECK_IN(a); CHECK_IN(b); CHECK_IN(out);
-  c10::cuda::CUDAGuard g(a.device());
-  const int K = (int)a.size(1);
-  const int N = (int)(trans_b ? b.size(0) : b.size(1));
-  auto* ctr = (uint32_t*)counters.data_ptr();           // [0] = gemm_done, [64..] = tile_done per 128-row block
-  if (mode == 1) {
-    const int M = (int)a.size(0) * (int)world;
-    TORCH_CHECK(out.size(0) == M && out.size(1) == N);
-    nxd::gemm_bf16_2cta_tp(1, (const void*)(local_buf_ptr + buf_offset), b.data_ptr(), out.data_ptr(), nullptr, a.data_ptr(),
-                           M, N, K, trans_b, (int)rank, (int)world, peer_bufs.data_ptr<int64_t>(),
-                           peer_flags.data_ptr<int64_t>(), buf_offset, (int)flag_offset, (uint32_t)epoch, (int)comm_ctas,
-                           ctr + 64, ctr, 0u, stream());
-  } else {
-    const int M = (int)a.size(0);
-    TORCH_CHECK(out.size(0) * world == M && out.size(1) == N && partial.size(0) == M && partial.size(1) == N);
-    nxd::gemm_bf16_2cta_tp(2, a.data_ptr(), b.data_ptr(), partial.data_ptr(), out.data_ptr(), nullptr, M, N, K, trans_b,
-                           (int)rank, (int)world, peer_bufs.data_ptr<int64_t>(), peer_flags.data_ptr<int64_t>(), buf_offset,
-                           (int)flag_offset, (uint32_t)epoch, (int)comm_ctas, ctr + 64, ctr, (uint32_t)gemm_done_target,
-                           stream());
-  }
-}
-
 // ---- ZeRO-1 collectives over peer memory
 static void zero1_reduce_scatter(const Tensor& peer_bufs, int64_t grad_off_bytes, const Tensor& peer_flags, int64_t flag_off,
                                  int64_t epoch, int64_t rank, int64_t world, int64_t shard_numel, double scale, Tensor out,
@@ -618,7 +546,7 @@ static Tensor symm_view(int64_t id, int64_t offset, const std::vector<int64_t>& 
   return at::from_blob(base + offset, shape, opts);
 }
 
-// ---- NVLS symmetric memory (symm_vmm.cpp) + fused TP kernels on it (tp_nvls_sm100.cu) + stand-alone collectives ----------
+// ---- NVLS symmetric memory (symm_vmm.cpp) + stand-alone collectives on it (nvls_coll.cu) ----------
 static py::tuple vmm_begin(int64_t nbytes, int64_t rank, int64_t world, bool want_multicast) {
   auto b = nxd::vmm_begin((size_t)nbytes, (int)rank, (int)world, want_multicast);
   return py::make_tuple(b.id, b.sock_name, b.multicast_supported, (int64_t)b.size);
@@ -648,6 +576,7 @@ static int64_t tp_gemm_nvls(int64_t mode, const Tensor& a, const Tensor& b, Tens
   CHECK_IN(a); CHECK_IN(b); CHECK_IN(out);
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16 && out.scalar_type() == at::kBFloat16);
   TORCH_CHECK(counters.scalar_type() == at::kInt && counters.numel() >= 64 + 8 * 256);
+  TORCH_CHECK(peer_bases.scalar_type() == at::kLong && peer_bases.is_cuda() && peer_bases.numel() >= world);
   c10::cuda::CUDAGuard g(a.device());
   const int K = (int)a.size(1);
   const int N = (int)(trans_b ? b.size(0) : b.size(1));
@@ -655,17 +584,17 @@ static int64_t tp_gemm_nvls(int64_t mode, const Tensor& a, const Tensor& b, Tens
   if (mode == 1) {
     const int M = (int)a.size(0) * (int)world;
     TORCH_CHECK(out.size(0) == M && out.size(1) == N);
-    return nxd::gemm_bf16_2cta_nvls(1, nullptr, b.data_ptr(), out.data_ptr(), nullptr, a.data_ptr(), M, N, K, trans_b, (int)rank,
-                                    (int)world, peer_bases.data_ptr<int64_t>(), mc_base, local_base, buf_offset, flag_offset,
-                                    (uint32_t)epoch, (int)comm_ctas, ctr + 64, ctr, 0u, false, true, stream());
+    return nxd::gemm_bf16_nvls(1, nullptr, b.data_ptr(), out.data_ptr(), nullptr, a.data_ptr(), M, N, K, trans_b, (int)rank,
+                               (int)world, peer_bases.data_ptr<int64_t>(), mc_base, local_base, buf_offset, flag_offset,
+                               (uint32_t)epoch, (int)comm_ctas, ctr + 64, ctr, 0u, false, true, stream());
   }
+  TORCH_CHECK(mode == 2, "tp_gemm_nvls: mode 1 or 2");
   const int M = (int)a.size(0);
   TORCH_CHECK(out.size(0) * world == M && out.size(1) == N);
-  return nxd::gemm_bf16_2cta_nvls(2, a.data_ptr(), b.data_ptr(), nullptr, out.data_ptr(), nullptr, M, N, K, trans_b, (int)rank,
-                                  (int)world, peer_bases.data_ptr<int64_t>(), mc_base, local_base, buf_offset, flag_offset,
-                                  (uint32_t)epoch, (int)comm_ctas, ctr + 64, ctr, (uint32_t)claim_base, wire_fp32, gemm_join, stream());
+  return nxd::gemm_bf16_nvls(2, a.data_ptr(), b.data_ptr(), nullptr, out.data_ptr(), nullptr, M, N, K, trans_b, (int)rank,
+                             (int)world, peer_bases.data_ptr<int64_t>(), mc_base, local_base, buf_offset, flag_offset,
+                             (uint32_t)epoch, (int)comm_ctas, ctr + 64, ctr, (uint32_t)claim_base, wire_fp32, gemm_join, stream());
 }
-
 static Tensor nvls_allreduce(const Tensor& x, const c10::optional<Tensor>& residual, const Tensor& peer_bases, int64_t mc_base,
                              int64_t local_base, int64_t flag_off, int64_t data_off, int64_t half_bytes, Tensor state,
                              int64_t rank, int64_t world) {
@@ -771,7 +700,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("multi_tensor_scale", &multi_tensor_scale);
   m.def("fused_adamw", &fused_adamw);
   m.def("gemm_bf16", &gemm_bf16);
-  m.def("gemm_bf16_2cta", &gemm_bf16_2cta);
   m.def("oneshot_allreduce", &oneshot_allreduce);
   m.def("decode_attention", &decode_attention);
   m.def("decode_attention_partial", &decode_attention_partial);
@@ -781,8 +709,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("nvls_all_to_all", &nvls_all_to_all);
   m.def("gemv_mx", &gemv_mx);
   m.def("gemv_mx_grouped", &gemv_mx_grouped);
-  m.def("gemm_mxfp8", &gemm_mxfp8);
-  m.def("gemm_f4", &gemm_f4);
   m.def("moe_block_tkg", &moe_block_tkg);
   m.def("moe_block_tkg_supported", [](int64_t T, int64_t H, int64_t E, int64_t I, int64_t K) {
     return nxd::moe_block_tkg_supported((int)T, (int)H, (int)E, (int)I, (int)K);
@@ -801,7 +727,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("causal"), py::arg("scale"), py::arg("sbhd_out"), py::arg("dlse") = py::none());
   m.def("ag_gemm_bf16", &ag_gemm_bf16);
   m.def("gemm_rs_bf16", &gemm_rs_bf16);
-  m.def("tp_gemm_2cta", &tp_gemm_2cta);
   m.def("zero1_reduce_scatter", &zero1_reduce_scatter);
   m.def("zero1_all_gather", &zero1_all_gather);
   m.def("symm_alloc", &symm_alloc);
@@ -815,7 +740,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("vmm_ptrs", &vmm_ptrs);
   m.def("vmm_free", &nxd::vmm_free);
   m.def("vmm_view", &vmm_view);
-  m.def("tp_gemm_nvls", &tp_gemm_nvls);
   m.def("nvls_allreduce", &nvls_allreduce, py::arg("x"), py::arg("residual"), py::arg("peer_bases"), py::arg("mc_base"),
         py::arg("local_base"), py::arg("flag_off"), py::arg("data_off"), py::arg("half_bytes"), py::arg("state"), py::arg("rank"),
         py::arg("world"));
@@ -823,5 +747,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("local_base"), py::arg("flag_off"), py::arg("data_off"), py::arg("half_bytes"), py::arg("state"), py::arg("rank"),
         py::arg("world"));
   m.def("nvls_all_gather", &nvls_all_gather);
+  m.def("tp_gemm_nvls", &tp_gemm_nvls);
   m.def("nvls_reduce_scatter", &nvls_reduce_scatter);
 }

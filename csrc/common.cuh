@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels of neuronx_distributed_b200.
+// Shared device helpers for the sm_90a kernels of neuronx_distributed_b200.
 // Everything here is plain CUDA C++ + inline PTX (no CUTLASS/CuTe dependency).
 #pragma once
 #include <cuda.h>

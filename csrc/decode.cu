@@ -1,4 +1,4 @@
-// Token-generation (decode) kernels for sm_100a — both are HBM-bandwidth problems, so they are plain CUDA tuned for wide
+// Token-generation (decode) kernels for sm_90a — both are HBM-bandwidth problems, so they are plain CUDA tuned for wide
 // coalesced loads rather than tensor-core kernels:
 //   decode_attention : one query token per sequence against the KV cache (flash-decoding: split over the cache length,
 //                      GQA group processed together so K/V are read once per kv head), + a combine pass over the splits.

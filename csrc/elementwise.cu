@@ -1,4 +1,4 @@
-// Hand-written sm_100a elementwise / normalisation / loss kernels.
+// Hand-written sm_90a elementwise / normalisation / loss kernels.
 //   rmsnorm fwd+bwd   (reference call site: modules/rms_norm.py:10-33)
 //   swiglu  fwd+bwd   (examples/training/llama/modeling_llama_nxd.py:208-219)
 //   rope apply        (overrides/transformer_overrides.py:20-32)

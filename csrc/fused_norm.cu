@@ -1,4 +1,4 @@
-// Residual-add fused with RMSNorm (sm_100a, HBM-bound: one pass, 16-byte accesses, fp32 math).
+// Residual-add fused with RMSNorm (sm_90a, HBM-bound: one pass, 16-byte accesses, fp32 math).
 //
 //   forward :  h = x + r                      (the updated residual stream, written once)
 //              y = h * rsqrt(mean(h^2) + eps) * w

@@ -37,7 +37,7 @@ void fused_adamw(const std::vector<TensorRef>& p, const std::vector<TensorRef>& 
                  float beta1, float beta2, float eps, float wd, float bc1, float bc2, const float* grad_scale,
                  int hf_form, cudaStream_t st);
 
-// ---- gemm_sm100.cu
+// ---- gemm_sm90.cu
 struct GemmComm {          // in-kernel NVLink communication description (all zero → plain GEMM)
   int mode = 0;            // 0 none, 1 all-gather A rows then GEMM, 2 GEMM then reduce-scatter rows
   int rank = 0, world = 1;
@@ -52,20 +52,11 @@ struct GemmComm {          // in-kernel NVLink communication description (all ze
 void gemm_bf16(const void* a, const void* b, void* out, int M, int N, int K, bool trans_a, bool trans_b, int out_dt,
                bool accumulate, const GemmComm& comm, const void* a_local_shard, cudaStream_t st);
 bool gemm_self_check_supported();
-// CTA-pair (cta_group::2) variant, plain GEMM only
-void gemm_bf16_2cta(const void* a, const void* b, void* out, int M, int N, int K, bool trans_a, bool trans_b, int out_dt,
-                    bool accumulate, cudaStream_t st);
-
-void gemm_bf16_2cta_tp(int mode, const void* a, const void* b, void* out_or_partial, void* rs_out, const void* a_local,
-                       int M, int N, int K, bool trans_b, int rank, int world, const int64_t* peer_bufs,
-                       const int64_t* peer_flags, long buf_offset, int flag_offset, uint32_t epoch, int comm_ctas,
-                       uint32_t* tile_done, uint32_t* gemm_done, uint32_t gemm_done_target, cudaStream_t st);
-
-// NVLS (multicast / in-switch reduce) variants, tp_nvls_sm100.cu
-int gemm_bf16_2cta_nvls(int mode, const void* a, const void* b, void* out, void* rs_out, const void* a_local, int M, int N, int K,
-                        bool trans_b, int rank, int world, const int64_t* peer_bases, int64_t mc_base, int64_t local_base,
-                        long buf_offset, long flag_offset, uint32_t epoch, int comm_ctas, uint32_t* tile_done, uint32_t* claim,
-                        uint32_t claim_base, bool wire_fp32, bool gemm_join, cudaStream_t st);
+// NVLS (multicast / in-switch reduce) fused TP GEMMs, gemm_sm90.cu; mode 1 = all-gather → GEMM, 2 = GEMM → reduce-scatter
+int gemm_bf16_nvls(int mode, const void* a, const void* b, void* out, void* rs_out, const void* a_local, int M, int N, int K,
+                   bool trans_b, int rank, int world, const int64_t* peer_bases, int64_t mc_base, int64_t local_base,
+                   long buf_offset, long flag_offset, uint32_t epoch, int comm_ctas, uint32_t* tile_done, uint32_t* claim,
+                   uint32_t claim_base, bool wire_fp32, bool gemm_join, cudaStream_t st);
 
 // stand-alone NVLS collectives (nvls_coll.cu); `state` = [2 + 1024] u32 device words (epoch, CTA counter, per-CTA barrier counts)
 void nvls_allreduce(const void* x, const void* residual, void* out, const int64_t* peer_bases, int64_t mc_base, int64_t local_base,
@@ -97,7 +88,7 @@ void zero1_all_gather(const float* master, const int64_t* peer_bufs, long param_
 
 void gemm_fp8(const void* a, const void* b, void* out, int M, int N, int K, const float* scale_a, const float* scale_b,
               cudaStream_t st);
-// ---- grouped (MoE blockwise) GEMMs, gemm_sm100.cu
+// ---- grouped (MoE blockwise) GEMMs, gemm_sm90.cu
 void grouped_gemm_bf16(const void* a, const void* b, void* out, int M, int N, int K, int E, bool trans_b,
                        const int* block_expert, int block_rows, int out_dt, cudaStream_t st);
 void grouped_wgrad_bf16(const void* a, const void* b, void* out, int rows_total, int Mo, int No, int E,
@@ -124,15 +115,6 @@ void moe_block_tkg(const void* x, const void* gamma, const void* router_w, const
                    int act_over_topk, int normalize, int pre_scale, int round_logits, int act, float act_alpha, float act_beta,
                    float gate_lo, float gate_hi, float up_lo, float up_hi, bool cooperative, cudaStream_t st);
 
-// ---- block-scaled MXFP8 GEMM on tcgen05 (gemm_mx_sm100.cu); a_fmt / b_fmt: 0 = e4m3, 1 = e5m2
-void gemm_mxfp8(const void* a, const void* b, const void* sfa, const void* sfb, void* out, int M, int N, int K, int a_fmt,
-                int b_fmt, cudaStream_t st);
-
-// ---- 4-bit block-scaled GEMM at the FP4 rate (gemm_mxf4_sm100.cu): packed e2m1 operands; vec_size 32 = MXFP4 (E8M0 scales),
-// 16 = NVFP4 (UE4M3 scales, alpha = product of the per-tensor factors)
-void gemm_f4(const void* a, const void* b, const void* sfa, const void* sfb, void* out, int M, int N, int K, int vec_size, float alpha,
-             cudaStream_t st);
-
 // ---- decode GEMV on MX (block-scaled fp4 / fp8) weights (gemv_mx.cu)
 void gemv_mx(const void* x, const void* w, const void* scale, const void* residual, void* y, int M, int N, int K, int fmt,
              cudaStream_t st);
@@ -150,14 +132,14 @@ void decode_rope_kv(const void* q, const void* k, const void* v, const long* pos
                     long v_sb, long v_sh, long c_sb, long c_ss, long c_sh, cudaStream_t st);
 void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, cudaStream_t st);
 
-// ---- attention (attention_sm100.cu): q [B,S_q,H,128], k/v [B,S_kv,Hkv,128] bf16 views; strides = (b, s, h) in elements
+// ---- attention (attention_sm90.cu): q [B,S_q,H,128], k/v [B,S_kv,Hkv,128] bf16 views; strides = (b, s, h) in elements
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
                     int Hkv, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
                     cudaStream_t st);
 
+// delta: fp32 scratch [B, H, S_q]; dlse may be null
 void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
-                    const float* dlse, void* dq,
-                    void* dk, void* dv, float* stats, float* dq_acc, int B, int S_q, int S_kv, int H, int Hkv, int S_pad,
+                    const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
                     const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
                     const long* dks, const long* dvs, float scale, bool causal, cudaStream_t st);
 

@@ -485,7 +485,7 @@ void nvls_embedding_gather(const void* table, const long* ids, void* out, const 
   nvls_publish_kernel<<<ctas, 512, 0, st>>>((const uint8_t*)table, r, state, bytes, -1);
   NXD_CUDA_CHECK(cudaGetLastError());
   if (ntok > 0) {
-    const int grid = (int)std::min<long>((ntok + 7) / 8, 148L * 8);
+    const int grid = (int)std::min<long>((ntok + 7) / 8, 132L * 8);     // 8 CTAs per H100 SM
     peer_row_gather_kernel<<<grid, 256, 0, st>>>(ids, (uint8_t*)out, r, state, rows_per_rank, row_bytes, ntok);
     NXD_CUDA_CHECK(cudaGetLastError());
   }

@@ -3,7 +3,7 @@
 // into this process's address space, and — when the devices sit behind an NVSwitch that supports it — an NVLS *multicast
 // object* bound to all of them: one `multimem.st` to the multicast address lands in every rank's buffer, one
 // `multimem.ld_reduce` returns the in-switch sum of every rank's copy (fp32 accumulation).  This is what the NVLS
-// variants of the fused tensor-parallel kernels (csrc/tp_nvls_sm100.cu) dereference.
+// variants of the fused tensor-parallel kernels (csrc/gemm_sm90.cu MODE 5 / 6) dereference.
 //
 // The exchange is driven from python in phases (ops/symm.py::get_vmm_workspace) because the rendezvous between the ranks
 // (names, barriers, "did multicast work for everybody") travels over the process group's host control plane:

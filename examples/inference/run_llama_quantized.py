@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Weight-quantised Llama inference (int8 / fp8 per-tensor or per-channel, optional dynamic fp8 activations → the fp8 tcgen05
+"""Weight-quantised Llama inference (int8 / fp8 per-tensor or per-channel, optional dynamic fp8 activations → the fp8 wgmma
 GEMM) — counterpart of the reference's ``examples/inference/run_llama_quantized.py``.
 
   python examples/inference/run_llama_quantized.py --quantized_dtype f8e4m3 --quantization_type per_channel_symmetric --dynamic_activations

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Llama pre-training with TP (+SP) + ZeRO-1 — the B200 counterpart of the reference's
+"""Llama pre-training with TP (+SP) + ZeRO-1 — the H100 counterpart of the reference's
 ``examples/training/llama/tp_zero1_llama_hf_pretrain/tp_zero1_llama_hf_pretrain.py`` (flags keep its names where they apply).
 
   torchrun --nproc-per-node 8 examples/training/llama/tp_zero1_llama_pretrain.py --model 7b --tensor_parallel_size 8 \

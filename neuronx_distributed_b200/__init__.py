@@ -1,14 +1,15 @@
-"""neuronx_distributed_b200 — a Blackwell-native tensor/pipeline-parallel training and inference
+"""neuronx_distributed_b200 — an H100 (sm_90a) tensor/pipeline-parallel training and inference
 library with the capabilities and public API of aws-neuron/neuronx-distributed.
 
 Top-level exports mirror reference ``src/neuronx_distributed/__init__.py:1-19``.
 """
 import os as _os
 
-# NXD_EXPERIMENTAL=1 switches on every opt-in path that has not been timed on hardware yet (docs/ROUND2.md): one flag to
-# validate them together.  Individual flags set by the user win.
-_EXPERIMENTAL_FLAGS = ("NXD_FUSED_LMHEAD_CE", "NXD_MOE_TKG_KERNEL", "NXD_EMBEDDING_RS", "NXD_NVLS_A2A", "NXD_CP_PULL", "NXD_GEMM_MX",
-                       "NXD_GEMV_MX")          # NXD_GEMM_F4 (W4A4) changes numerics and stays a separate, explicit choice
+# NXD_EXPERIMENTAL=1 switches on every opt-in path that has not been timed on hardware yet (README.md, "Opt-in paths"): one
+# flag to validate them together.  Individual flags set by the user win.  NXD_GEMM_MX / NXD_GEMM_F4 are not among them: the
+# block-scaled GEMMs do not exist on H100 and those flags raise on CUDA tensors.
+_EXPERIMENTAL_FLAGS = ("NXD_FUSED_LMHEAD_CE", "NXD_MOE_TKG_KERNEL", "NXD_EMBEDDING_RS", "NXD_NVLS_A2A", "NXD_CP_PULL",
+                       "NXD_GEMV_MX")
 if _os.environ.get("NXD_EXPERIMENTAL", "0") == "1":
     for _f in _EXPERIMENTAL_FLAGS:
         _os.environ.setdefault(_f, "1")

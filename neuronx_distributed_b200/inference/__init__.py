@@ -1,4 +1,4 @@
-"""B200-specific inference pieces: launch plans (portable artefact / program IR), KV cache, bucketing, GQA sharding strategies,
+"""H100-specific inference pieces: launch plans (portable artefact / program IR), KV cache, bucketing, GQA sharding strategies,
 HF adapter, benchmark helpers, checkpoint sharding.  The builder / functional units / runtime model are in ``trace/``."""
 from .sharding import shard_state_dict_for_rank  # noqa: F401
 

@@ -6,7 +6,7 @@ ordered list of *launches* one call performs — recorded once, replayed by a ~1
 CUDA graph at load time:
 
 * **recording** runs the bucket under a ``TorchDispatchMode``: every dispatcher op (``aten::…`` after composite ops are
-  decomposed) becomes a node; calls into the sm_100a extension are seen through a proxy of ``ops._ext.ext()`` and become
+  decomposed) becomes a node; calls into the sm_90a extension are seen through a proxy of ``ops._ext.ext()`` and become
   ``ext`` nodes (kernel name + tensor / scalar arguments); framework functions that own process-local resources —
   collectives, symmetric-memory kernels, fused GEMM+collective ops — are decorated with :func:`plan_op` and become ``py``
   nodes that re-resolve their groups / workspaces when replayed (process groups are stored by registry name);
@@ -51,10 +51,10 @@ _EXT_RESOURCE_PREFIXES = ("vmm_", "symm_", "tp_gemm", "nvls_", "gemv_allreduce",
 # writing to EVERY tensor argument: conservative — such tensors count as state, are never hoisted or dropped — but safe.
 _EXT_PURE = frozenset({"rmsnorm_fwd", "rmsnorm_bwd", "add_rmsnorm_fwd", "add_rmsnorm_bwd", "swiglu_fwd", "swiglu_bwd", "rope_apply",
                        "ce_stats", "ce_backward", "decode_attention", "decode_attention_partial", "gemv", "gemv_mx",
-                       "gemm_mxfp8", "moe_block_tkg", "moe_block_metadata", "row_argmax", "row_topk", "flash_attn_fwd",
+                       "moe_block_tkg", "moe_block_metadata", "row_argmax", "row_topk", "flash_attn_fwd",
                        "flash_attn_bwd", "moe_block_tkg_supported", "row_topk_supported", "grouped_gemm"})
 # … and the ones that write exactly these positional arguments (everything else they take is read-only)
-_EXT_WRITES = {"gemm_bf16": (2,), "gemm_bf16_2cta": (2,), "gemm_fp8": (2,), "grouped_wgrad": (2,), "decode_rope_kv": (6, 7),
+_EXT_WRITES = {"gemm_bf16": (2,), "gemm_fp8": (2,), "grouped_wgrad": (2,), "decode_rope_kv": (6, 7),
                "multi_tensor_sq_norm": (1,)}
 
 

@@ -6,7 +6,7 @@ Layout convention of ``nki_flash_attn_func`` (same as the reference):
   ``v`` as ``[B, H, S, D]`` (what ``overrides.transformer_overrides.apply_rotary_pos_emb(…, flash_attn=True)`` produces);
 * ``transpose_nki_inputs=False`` — ``q``, ``k``, ``v`` are all ``[B, H, S, D]``.
 
-The result is ``[B, H, S, D]`` in both cases.  The math runs in ``ops.attention.flash_attention`` (own tcgen05 forward /
+The result is ``[B, H, S, D]`` in both cases.  The math runs in ``ops.attention.flash_attention`` (own forward /
 backward kernels for head_dim 128 bf16, library flash attention otherwise), which wants ``[B, S, H, D]`` *views* — the
 transposes below are stride changes consumed by strided TMA descriptors, not copies."""
 from __future__ import annotations

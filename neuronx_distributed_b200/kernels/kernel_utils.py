@@ -36,7 +36,7 @@ def cast(q, k, v):
 
 
 def torch_to_nki_dtype(dtype: torch.dtype):
-    """Kernels here take torch dtypes directly; validates that the dtype is one the tcgen05 paths support."""
+    """Kernels here take torch dtypes directly; validates that the dtype is one the own kernels support."""
     if dtype not in (torch.bfloat16, torch.float16, torch.float32, torch.float8_e4m3fn, torch.float8_e5m2):
-        raise ValueError(f"Invalid dtype '{dtype}'. Not supported by the sm_100a kernels.")
+        raise ValueError(f"Invalid dtype '{dtype}'. Not supported by the sm_90a kernels.")
     return dtype

@@ -12,7 +12,7 @@ from .kernel_utils import cast
 def get_seq_tile_size(seqlen: int) -> int:
     """K/V tile length used per ring step: the local sequence is processed in tiles of at most 2048 and at least 1024
     positions (same rule as the reference, which sizes its SBUF tiles with it; here it bounds the per-step score tile the
-    block kernel keeps in TMEM/registers)."""
+    block kernel keeps in registers)."""
     return max(2048 if seqlen >= 4096 else seqlen // 2, 1024)
 
 

@@ -1,4 +1,4 @@
-"""Lightning accelerator for B200 GPUs (role of reference ``lightning/accelerator.py:17-82`` — ``NeuronXLAAccelerator``).
+"""Lightning accelerator for H100 GPUs (role of reference ``lightning/accelerator.py:17-82`` — ``NeuronXLAAccelerator``).
 
 One process drives one GPU (``torchrun`` / Lightning's subprocess launcher), so ``get_parallel_devices(n)`` is the list of
 local CUDA devices and ``auto_device_count`` is what the driver reports.  Derives from Lightning's ``CUDAAccelerator`` when

@@ -1,7 +1,7 @@
 """Llama (2/3) built from the tensor-parallel layers.
 
 Role parity with reference ``examples/training/llama/modeling_llama_nxd.py`` (attention :299-362,
-MLP :161-220, decoder :532-550, causal-LM + vocab-parallel loss :712-824).  Written for the B200
+MLP :161-220, decoder :532-550, causal-LM + vocab-parallel loss :712-824).  Written for the H100
 kernel set: activations are kept in ``[S, B, H]`` ("SBH") so sequence-parallel shards are
 contiguous row blocks that the fused AG→GEMM / GEMM→RS kernels treat as 2-D ``[tokens, H]``
 matrices; QKV is one fused GEMM; gate/up is one fused GEMM followed by the SwiGLU kernel;

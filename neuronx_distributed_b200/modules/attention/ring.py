@@ -6,9 +6,9 @@ attention of each visiting block into its output with a log-sum-exp update.  Wit
 mask, a block that originated on a *later* rank is skipped, the local block is causal, earlier blocks are dense
 (same — load-imbalanced — split as the reference: no zig-zag).
 
-B200 design: the ring transfer is an NCCL p2p exchange issued *before* the block's attention so it overlaps the
+H100 design: the ring transfer is an NCCL p2p exchange issued *before* the block's attention so it overlaps the
 compute; the exchange is itself an autograd node (its backward moves dK/dV the opposite way round the ring), so
-backward is the exact transpose of forward without a hand-written second pass.  Per-block attention is the own tcgen05
+backward is the exact transpose of forward without a hand-written second pass.  Per-block attention is the own
 flash kernel with a differentiable LSE output (``ops.attention.flash_attention_with_lse``; head_dim 128, bf16), the SDPA
 flash op for other shapes on CUDA, and an fp32 reference on CPU.
 """
@@ -29,7 +29,7 @@ def block_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: b
     if q.is_cuda:
         from ... import ops
 
-        own = ops.attention.flash_attention_with_lse(q, k, v, causal, scale)      # tcgen05 kernels, LSE differentiable
+        own = ops.attention.flash_attention_with_lse(q, k, v, causal, scale)      # own kernels, LSE differentiable
         if own is not None:
             return own
     hq, hkv = q.shape[2], k.shape[2]
@@ -109,7 +109,7 @@ def ring_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bo
 
 # ---------------------------------------------------------------------------------------------------------------------
 # Context-parallel attention WITHOUT a ring: every rank publishes its K/V slice in NVSwitch-visible symmetric memory and
-# the attention kernels read the other ranks' slices where they are (TMA loads over NVLink inside the kernel) — the
+# the attention kernels read the other ranks' slices where they are (cp.async tile loads over NVLink inside the kernel) — the
 # K/V "rotation" of the reference's ring kernels (K3/K4, kernels/ring_attention_kernel.py:118-167) happens inside the
 # attention kernel, and there are no ring steps to serialise on.  Backward re-publishes K/V, computes every block's
 # (dQ, dK, dV) from the GLOBAL softmax statistics (so no per-block LSE gradients are needed) and returns the dK/dV

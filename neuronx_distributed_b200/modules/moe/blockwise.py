@@ -8,8 +8,8 @@ of ``block_size`` and each block is multiplied by exactly one expert's weights:
     block_to_expert[b]    : expert owning block b
     token_position_to_id  : flat [num_blocks·B] token id feeding each block slot (−1 = padding)
 
-On CUDA the two projections are grouped tcgen05 GEMMs (``ops.gemm.grouped_matmul`` → MODE 3/4 of
-``csrc/gemm_sm100.cu``): the block's expert only shifts the TMA coordinate of the weight tile, the backward runs the
+On CUDA the two projections are grouped wgmma GEMMs (``ops.gemm.grouped_matmul`` → MODE 3/4 of
+``csrc/gemm_sm90.cu``): the block's expert only shifts the TMA coordinate of the weight tile, the backward runs the
 grouped dgrad and a per-expert segmented wgrad, and nothing syncs with the host.  On CPU it is a gathered einsum.
 """
 from __future__ import annotations
@@ -118,7 +118,7 @@ def blockwise_expert_mlp(hidden: torch.Tensor, expert_affinities: torch.Tensor, 
 # ---------------------------------------------------------------------------------------------------------------------
 # Reference-named surface (modules/moe/blockwise.py:136-1127).  The reference selects among a family of NKI kernels
 # (block-parallel, shard-on-hidden / -intermediate / -block, MX) by hardware generation; here there is ONE grouped
-# tcgen05 GEMM (MODE 3 forward/dgrad, MODE 4 segmented wgrad) and a PyTorch path, so the selection helpers reduce to
+# wgmma GEMM (MODE 3 forward/dgrad, MODE 4 segmented wgrad) and a PyTorch path, so the selection helpers reduce to
 # "is the CUDA extension usable for these shapes".
 # ---------------------------------------------------------------------------------------------------------------------
 DEFAULT_PADDING_VALUE = -1
@@ -152,7 +152,7 @@ def _resolve(imports) -> dict:
 
 
 def initialize_nki_components() -> dict:
-    """Inference-side building blocks by the reference's component names (``blockwise.py:43-87``): the grouped tcgen05 GEMM that
+    """Inference-side building blocks by the reference's component names (``blockwise.py:43-87``): the grouped wgmma GEMM that
     every blockwise variant runs on, the device-side block-metadata build, the fused decode block, and the enums."""
     from .nki_import import KernelImport as K
 
@@ -236,9 +236,9 @@ def check_kernel_availability(device: Optional[torch.device] = None) -> bool:
 
 
 def check_blockwise_mm_kernel_compatibility(hidden_size: int, block_size: int, intermediate_size_tp: int) -> None:
-    """The grouped UMMA tiles need 128-row blocks and 16-element (32-byte) aligned K / N (reference :683-716)."""
+    """The grouped GEMM tiles need 128-row blocks and 16-element (32-byte) aligned K / N (reference :683-716)."""
     if block_size % 128 != 0:
-        raise KernelAvailabilityError(f"block_size {block_size} must be a multiple of 128 for the grouped tcgen05 GEMM")
+        raise KernelAvailabilityError(f"block_size {block_size} must be a multiple of 128 for the grouped wgmma GEMM")
     if hidden_size % 16 != 0 or intermediate_size_tp % 16 != 0:
         raise KernelAvailabilityError(f"hidden ({hidden_size}) and intermediate/tp ({intermediate_size_tp}) must be multiples of 16")
 
@@ -302,7 +302,7 @@ def blockwise_matmul(args: BlockwiseMatmulArgs) -> torch.Tensor:
 
 class BlockwiseMatmulNKIFunc:
     """Reference entry point name (:853-1035).  ``apply`` takes the reference's positional arguments and runs the grouped
-    tcgen05 path; gradients flow through ``ops.gemm.grouped_matmul``'s autograd function."""
+    wgmma path; gradients flow through ``ops.gemm.grouped_matmul``'s autograd function."""
 
     @staticmethod
     def apply(hidden_states, expert_affinities_masked, gate_up_proj_weight, down_proj_weight, token_position_to_id,

@@ -11,7 +11,7 @@
 
 Mode selection follows the reference's ``forward`` (:1407-1500) with one deliberate difference: a ``capacity_factor`` of
 ``None`` ("full capacity") in training runs the dropless blockwise path once ``T·k`` reaches a block instead of pushing
-every token through every expert — same result, 1/E·k of the FLOPs (the grouped tcgen05 GEMM makes dropless the cheap
+every token through every expert — same result, 1/E·k of the FLOPs (the grouped wgmma GEMM makes dropless the cheap
 option here).
 """
 from __future__ import annotations

@@ -46,7 +46,7 @@ class GLUType(Enum):
 
 
 class ACTFunc(Enum):
-    """Activation id / name pairs; the ids are what the grouped-GEMM epilogue (``csrc/gemm_sm100.cu`` MODE 3) switches
+    """Activation id / name pairs; the ids are what the grouped-GEMM epilogue (``csrc/gemm_sm90.cu`` MODE 3) switches
     on when the activation is fused — same numbering as the reference's kernel enum so configs port unchanged."""
 
     def __new__(cls, ident: int, name: str):
@@ -95,7 +95,7 @@ def get_kernel_activation_func_id(act_fn: ACTFunc, glu_type: GLUType) -> int:
 DEFAULT_SELECTIVE_LOADING_THRESHOLD = 1.0     # decode: gather only the selected experts when T·k/E is below this
 DEFAULT_BLOCK_SIZE = 512
 DEFAULT_SKIP_MODE = (False, False)
-DEFAULT_LNC_SIZE = 1                          # a B200 GPU is one logical core (the two dies share L2/HBM coherently)
+DEFAULT_LNC_SIZE = 1                          # a H100 GPU is one logical core (the two dies share L2/HBM coherently)
 DEFAULT_PADDING_VALUE = -1
 DEFAULT_HIDDEN_ACT_SCALING_FACTOR = 1.702
 

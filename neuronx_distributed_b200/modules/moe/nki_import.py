@@ -2,7 +2,7 @@
 ``import_nki_beta2``: look a kernel up by name in a list of candidate modules and return ``(kernel, None)`` or
 ``(None, reason)`` instead of raising, so callers can degrade to their torch path and say why).
 
-Here the candidates are, in order: the sm_100a extension (``ops._ext.ext()``, entry points of ``csrc/*.cu``), the ``ops``
+Here the candidates are, in order: the sm_90a extension (``ops._ext.ext()``, entry points of ``csrc/*.cu``), the ``ops``
 package (Python front ends that pick the kernel or its CPU oracle), and ``modules.moe.blockwise``.  The reference's names are
 kept as aliases so code written against them imports unchanged."""
 from __future__ import annotations
@@ -48,7 +48,7 @@ def import_kernel(import_config: KernelImport) -> Tuple[Optional[Any], Optional[
     if e is not None and not import_config.module_name and hasattr(e, import_config.name):
         return getattr(e, import_config.name), None
     if import_config.is_kernel and e is None:
-        return None, f"Failed to import {import_config.name}: the sm_100a extension is not loaded ({_ext.load_error()!r})"
+        return None, f"Failed to import {import_config.name}: the sm_90a extension is not loaded ({_ext.load_error()!r})"
     for path in _candidates(import_config):
         try:
             module = importlib.import_module(path)

@@ -5,7 +5,7 @@ one module produces (q, k, v); when ``num_kv_heads < tp`` the K/V weights are re
 ``kv_size_multiplier`` times so every TP rank owns a KV head, and the K/V gradients are summed
 over the *KV-shared group* (the ranks holding replicas of the same head).
 
-B200 design: Q, K and V are computed by ONE fused column-parallel GEMM (one AG→GEMM launch
+H100 design: Q, K and V are computed by ONE fused column-parallel GEMM (one AG→GEMM launch
 under sequence parallelism) over the concatenated ``[q/tp + 2·kv·m/tp, in]`` weight.  With
 ``fuse_qkv=True`` that concatenation *is* the stored parameter (``weight_qkv``).  The KV-group
 gradient reduction is a separate identity-forward / all-reduce-backward node on the k and v

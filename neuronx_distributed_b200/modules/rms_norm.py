@@ -1,5 +1,5 @@
 """RMSNorm with fp32 statistics and a sequence-parallel-tagged weight
-(reference ``modules/rms_norm.py:10-72``).  Forward/backward run the sm_100a kernels in
+(reference ``modules/rms_norm.py:10-72``).  Forward/backward run the sm_90a kernels in
 ``csrc/elementwise.cu`` via :func:`ops.norm.rms_norm`."""
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Python front-ends of the hand-written sm_100a kernels (``csrc/``).
+"""Python front-ends of the hand-written sm_90a kernels (``csrc/``).
 
 Every op has (a) the CUDA path through the in-tree extension and (b) a plain PyTorch fp32
 reference used on CPU and as the numerics oracle in tests.  On a GPU box the CUDA path is

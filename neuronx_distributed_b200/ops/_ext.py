@@ -1,4 +1,4 @@
-"""Loader for the in-tree sm_100a extension ``nxd_b200_C``.
+"""Loader for the in-tree sm_90a (H100) extension ``nxd_b200_C``.
 
 The extension is built IN-TREE (``neuronx_distributed_b200/_build/nxd_b200_C.so``) by
 ``__graft_entry__.build()`` / ``python -m neuronx_distributed_b200.ops.build`` so that it travels
@@ -75,7 +75,7 @@ def use_cuda(*tensors: torch.Tensor) -> bool:
     if os.environ.get("NXD_ALLOW_EAGER_FALLBACK", "0") == "1":
         return False
     raise RuntimeError(
-        f"CUDA tensors given but the sm_100a extension is not loaded ({_LOAD_ERROR!r}). "
+        f"CUDA tensors given but the sm_90a extension is not loaded ({_LOAD_ERROR!r}). "
         "Build it with `python -m neuronx_distributed_b200.ops.build` or set NXD_ALLOW_EAGER_FALLBACK=1."
     )
 

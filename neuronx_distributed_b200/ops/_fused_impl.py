@@ -1,9 +1,10 @@
-"""Fused tensor-parallel linear paths on the sm_100a GEMM+collective kernels (``csrc/gemm_sm100.cu``).
+"""Fused tensor-parallel linear paths on the sm_90a GEMM+collective kernels (``csrc/gemm_sm90.cu``: peer-memory MODE 1 / 2,
+NVLS multicast MODE 5 / 6).
 
 Column + sequence-parallel  (``in_mode="gather"``):
     fwd   y      = AG(x) @ Wᵀ                  → ``ag_gemm``   (MODE 1, B K-major)
     bwd   dx     = RS(g @ W)                   → ``gemm_rs``   (MODE 2, B MN-major)
-          dW     = gᵀ @ AG(x)                  → plain tcgen05 GEMM on the gathered x saved by the forward
+          dW     = gᵀ @ AG(x)                  → plain wgmma GEMM on the gathered x saved by the forward
 Row + sequence-parallel     (``out_mode="scatter"``):
     fwd   y      = RS(x @ Wᵀ)                  → ``gemm_rs``   (MODE 2, B K-major)
     bwd   dx     = AG(g) @ W                   → ``ag_gemm``   (MODE 1, B MN-major)
@@ -11,7 +12,7 @@ Row + sequence-parallel     (``out_mode="scatter"``):
 
 Design choice vs the reference: the gathered activation is kept (one D2D copy out of the symmetric
 buffer) instead of being re-all-gathered in backward (reference layers_utils.py:82-87) — HBM is
-plentiful on B200 and NVLink is the scarce resource on these paths.  Wire dtype is bf16 with fp32
+plentiful on H100 and NVLink is the scarce resource on these paths.  Wire dtype is bf16 with fp32
 accumulation at the owner (the reference reduces fp32 on the wire, layers.py:1031-1045); see DESIGN.md.
 
 Protocol state (epochs, cumulative counters) lives in :class:`TPWorkspace`, one per process group.
@@ -31,26 +32,9 @@ BLOCK_M = 128
 MAX_ROW_BLOCKS = 64
 _FLAGS_AG = 0
 _FLAGS_RS = 2048
-_FLAGS_RS2 = 3072
 _NFLAGS = 4096
-_COMM_SMS = int(os.environ.get("NXD_AG_COMM_SMS", "16"))
-# CTAs (out of 148) that only move data inside the fused kernels; even numbers (CTA pairs).  Mutable so benchmarks can sweep.
-# Measured at TP=8 (profiles/tp_bench_tp8.json sweep): 12/16 is best for a 4096-row call, 24/24 for 16384 rows (the call is
-# NVLink-bound there and the TMA pushers need more CTAs to fill the links); 0 = pick by size.
-CONFIG = {"comm_ctas_ag": int(os.environ.get("NXD_TP_COMM_CTAS_AG", "0")),
-          "comm_ctas_rs": int(os.environ.get("NXD_TP_COMM_CTAS_RS", "0"))}
-
-
-def _comm_ctas(kind: str, rows: int) -> int:
-    v = CONFIG["comm_ctas_" + kind]
-    if v > 0:
-        return v
-    if rows >= 8192:
-        return 24
-    return 12 if kind == "ag" else 16
-_USE_2CTA_TP = os.environ.get("NXD_TP_2CTA", "1") == "1"
-TILE_M2 = 256
-# NVLS variants (csrc/tp_nvls_sm100.cu): "1" = use them when the TP group's symmetric region got a multicast mapping (default),
+_COMM_SMS = int(os.environ.get("NXD_AG_COMM_SMS", "16"))     # CTAs (of one per SM) that only push the all-gather
+# NVLS variants (MODE 5 / 6 of csrc/gemm_sm90.cu): "1" = use them when the TP group's symmetric region got a multicast mapping (default),
 # "0" = never, "force" = also without multicast (unicast fallback inside the same kernels; loopback tests of the protocol).
 _NVLS_MODE = os.environ.get("NXD_TP_NVLS", "1")
 _NVLS_FLAG_BYTES = 64 << 10          # AG flags [world][256][4] u32 at 0, RS flags [world][256] u32 at 32 KB
@@ -112,10 +96,7 @@ class TPWorkspace:
         self.ag_epoch = 0
         self.rs_calls = 0
         self.rs_counts = [0] * MAX_ROW_BLOCKS
-        self.rs2_calls = 0
-        self.gemm_done_total = 0
         self.counters: Optional[torch.Tensor] = None     # [0] gemm_done, [64:] per-128-row-block tile counters
-        self.partial: Optional[torch.Tensor] = None
         # NVLS state (separate region + protocol counters)
         self.nv: Optional[symm.VmmWorkspace] = None
         self.nv_ag_bytes = 0
@@ -126,7 +107,6 @@ class TPWorkspace:
         self.nv_counters: Optional[torch.Tensor] = None
         self.nv_checked = False
         self._ag_reader_event = None        # side-stream reader of the most recent gathered buffer (see ag_gemm_nvls)
-        self.sm_pairs = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count // 2
 
     def _ensure(self, ag_bytes: int, rs_bytes: int) -> None:
         if self.ws is not None and ag_bytes <= self.ag_bytes and rs_bytes <= self.rs_bytes:
@@ -138,7 +118,6 @@ class TPWorkspace:
         self.rs_bytes = max(self.rs_bytes, _round(rs_bytes), _round(int(os.environ.get("NXD_SYMM_MIN_MB", "32")) << 20))
         self.ws = symm.get_workspace(self.group, "tp", 2 * self.ag_bytes + 2 * self.rs_bytes, _NFLAGS)
         self.ag_epoch, self.rs_calls, self.rs_counts = 0, 0, [0] * MAX_ROW_BLOCKS
-        self.rs2_calls, self.gemm_done_total = 0, 0
         self.counters = torch.zeros(64 + 1024, dtype=torch.int32, device=torch.device("cuda", torch.cuda.current_device()))
 
     # ------------------------------------------------------------------ NVLS region
@@ -176,7 +155,7 @@ class TPWorkspace:
         # Protocol state is NEVER reset: epochs stay monotonic across re-layouts.  The VMM allocator hands back the SAME region
         # when it is already large enough (its granularity is hundreds of MB), and that region's flags still hold the epochs of
         # earlier calls — restarting the epochs at 1 made consumers see "flag >= epoch" immediately and read stale payload
-        # (found by tools/nvls_bench.py --stage numerics with NXD_SYMM_MIN_MB=1; profiles/README.md).  A brand-new region has
+        # (found with NXD_SYMM_MIN_MB=1, which forces re-layouts).  A brand-new region has
         # zero flags, which is consistent with any epoch.  Counters are at rest (zero / claim base) between kernels.
         if self.nv_counters is None:
             self.nv_counters = torch.zeros(64 + 8 * NVLS_MAX_ROW_BLOCKS, dtype=torch.int32,
@@ -232,7 +211,7 @@ class TPWorkspace:
         ms, K = a_shard.shape
         M = ms * self.world
         N = b.shape[0] if trans_b else b.shape[1]
-        if out_dtype == torch.bfloat16 and ms % TILE_M2 == 0 and ms // BLOCK_M <= NVLS_MAX_ROW_BLOCKS and self.nvls_enabled():
+        if out_dtype == torch.bfloat16 and ms % BLOCK_M == 0 and ms // BLOCK_M <= NVLS_MAX_ROW_BLOCKS and self.nvls_enabled():
             return self.ag_gemm_nvls(a_shard, b, trans_b)
         if ms // BLOCK_M > MAX_ROW_BLOCKS:
             raise RuntimeError(f"fused AG→GEMM without NVLS supports at most {MAX_ROW_BLOCKS * BLOCK_M} rows per rank (got {ms})")
@@ -241,17 +220,8 @@ class TPWorkspace:
         off = (self.ag_epoch & 1) * self.ag_bytes
         out = torch.empty(M, N, dtype=out_dtype, device=a_shard.device)
         _ext.count_launch()
-        if _USE_2CTA_TP and ms % TILE_M2 == 0 and out_dtype == torch.bfloat16 and hasattr(_ext.ext(), "tp_gemm_2cta"):
-            _ext.ext().tp_gemm_2cta(1, a_shard, b, out, out, trans_b, self.ws.local_ptr, self.ws.ptrs, self.ws.flag_ptrs,
-                                    off, _FLAGS_AG, self.ag_epoch, self.rank, self.world, _comm_ctas("ag", M), self.counters, 0)
-            # the kernel reads the own shard in place (no local copy); complete the gathered view for wgrad consumers
-            gathered = self.ws.local_tensor(off, (M, K), torch.bfloat16)
-            gathered[self.rank * ms:(self.rank + 1) * ms].copy_(a_shard)
-            self._poison((1 - (self.ag_epoch & 1)) * self.ag_bytes, self.ag_bytes)
-            return out, gathered
-        else:
-            _ext.ext().ag_gemm_bf16(a_shard, b, out, trans_b, self.ws.local_ptr, self.ws.ptrs, self.ws.flag_ptrs, off,
-                                    _FLAGS_AG, self.ag_epoch, self.rank, self.world, _COMM_SMS)
+        _ext.ext().ag_gemm_bf16(a_shard, b, out, trans_b, self.ws.local_ptr, self.ws.ptrs, self.ws.flag_ptrs, off, _FLAGS_AG,
+                                self.ag_epoch, self.rank, self.world, _COMM_SMS)
         gathered = self.ws.local_tensor(off, (M, K), torch.bfloat16)
         return out, gathered
 
@@ -273,26 +243,11 @@ class TPWorkspace:
         M, K = a.shape
         N = b.shape[0] if trans_b else b.shape[1]
         ms = M // self.world
-        if ms % TILE_M2 == 0 and ms // BLOCK_M <= NVLS_MAX_ROW_BLOCKS and self.nvls_enabled():
+        if ms % BLOCK_M == 0 and ms // BLOCK_M <= NVLS_MAX_ROW_BLOCKS and self.nvls_enabled():
             return self.gemm_rs_nvls(a, b, trans_b, gemm_join)
         if ms // BLOCK_M > MAX_ROW_BLOCKS:
             raise RuntimeError(f"fused GEMM→RS without NVLS supports at most {MAX_ROW_BLOCKS * BLOCK_M} rows per rank (got {ms})")
         self._ensure(0, M * N * 2)
-        if _USE_2CTA_TP and ms % TILE_M2 == 0 and hasattr(_ext.ext(), "tp_gemm_2cta"):
-            self.rs2_calls += 1
-            off = 2 * self.ag_bytes + (self.rs2_calls & 1) * self.rs_bytes
-            if self.partial is None or self.partial.numel() < M * N:
-                self.partial = torch.empty(M * N, dtype=torch.bfloat16, device=a.device)
-            partial = self.partial[: M * N].view(M, N)
-            comm_ctas = _comm_ctas("rs", M)
-            self.gemm_done_total = (self.gemm_done_total + 2 * self.sm_pairs - comm_ctas) & 0xFFFFFFFF
-            out = torch.empty(ms, N, dtype=torch.bfloat16, device=a.device)
-            _ext.count_launch()
-            _ext.ext().tp_gemm_2cta(2, a, b, out, partial, trans_b, self.ws.local_ptr, self.ws.ptrs, self.ws.flag_ptrs, off,
-                                    _FLAGS_RS2, self.rs2_calls, self.rank, self.world, comm_ctas, self.counters,
-                                    self.gemm_done_total)
-            self._poison(2 * self.ag_bytes + (1 - (self.rs2_calls & 1)) * self.rs_bytes, self.rs_bytes)
-            return out
         self.rs_calls += 1
         off = 2 * self.ag_bytes + (self.rs_calls & 1) * self.rs_bytes
         tiles_n = (N + 255) // 256
@@ -510,8 +465,8 @@ def select(x: torch.Tensor, weight: torch.Tensor, in_mode: str, out_mode: str, s
     rows_per_rank = rows if kind == "Column+SP" else (rows // world if rows % world == 0 else -1)
     if rows_per_rank <= 0 or rows_per_rank % BLOCK_M:
         return no(f"{rows_per_rank} rows per rank is not a multiple of {BLOCK_M}")
-    nvls_ok = rows_per_rank % TILE_M2 == 0 and rows_per_rank // BLOCK_M <= NVLS_MAX_ROW_BLOCKS and ws.nvls_enabled()
+    nvls_ok = rows_per_rank % BLOCK_M == 0 and rows_per_rank // BLOCK_M <= NVLS_MAX_ROW_BLOCKS and ws.nvls_enabled()
     if not nvls_ok and rows_per_rank // BLOCK_M > MAX_ROW_BLOCKS:
         return no(f"{rows_per_rank} rows per rank > {MAX_ROW_BLOCKS * BLOCK_M} (cudaIpc kernels); NVLS kernels take up to "
-                  f"{NVLS_MAX_ROW_BLOCKS * BLOCK_M} when rows/rank % 256 == 0 and multicast is available")
+                  f"{NVLS_MAX_ROW_BLOCKS * BLOCK_M} when multicast is available")
     return _ColumnSP(ws) if kind == "Column+SP" else _RowSP(ws)

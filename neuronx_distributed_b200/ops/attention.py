@@ -1,5 +1,5 @@
-"""Causal self-attention (flash style).  Kernel: ``csrc/attention_sm100.cu`` (tcgen05 QK^T / PV with
-TMEM accumulators, online softmax) when built; otherwise the PyTorch SDPA library call, which is
+"""Causal self-attention (flash style).  Kernel: ``csrc/attention_sm90.cu`` (tensor-core QK^T / PV with
+register accumulators, online softmax) when built; otherwise the PyTorch SDPA library call, which is
 flagged as a *library* path in DESIGN.md.  Reference call sites: ``kernels/flash_attn.py:162-212``
 (``nki_flash_attn_func``), ``modeling_llama_nxd.py:468-475``.
 
@@ -38,28 +38,17 @@ def _own_kernel_ok(q, k, v) -> bool:
 
 
 def _tma_view(t: torch.Tensor) -> torch.Tensor:
-    """The kernels read q/k/v through 2-D TMA maps built from (b, s, h) strides: head_dim must be contiguous and the batch /
-    head offsets must fold into rows or columns of that map (true for [B,S,H,D], [S,B,H,D], [B,H,S,D] memory and for slices
-    of a fused projection output); anything else is copied once."""
-    if t.stride(3) != 1 or t.data_ptr() % 16:
-        return t.contiguous()
-    ss = t.stride(1)
-    if ss % 8:
-        return t.contiguous()
-    cols = 128
-    for n, st in ((t.shape[0], t.stride(0)), (t.shape[2], t.stride(2))):
-        if n > 1 and not (st >= ss and st % ss == 0):
-            if st % 8:
-                return t.contiguous()
-            cols += (n - 1) * st
-    if cols > ss and t.shape[1] > 1:
+    """The kernels address q/k/v as ``base + b·sb + s·ss + h·sh + d`` with 16-byte row loads: head_dim must be contiguous, the
+    base 16-byte aligned and the (b, s, h) strides multiples of 8 elements (true for [B,S,H,D], [S,B,H,D], [B,H,S,D] memory
+    and for slices of a fused projection output); anything else is copied once."""
+    if t.stride(3) != 1 or t.data_ptr() % 16 or any(t.stride(i) % 8 for i in range(3)):
         return t.contiguous()
     return t
 
 
 class _FlashAttn(torch.autograd.Function):
-    """tcgen05 flash attention (``csrc/attention_sm100.cu``): forward saves (q, k, v, o, lse); backward is the transposed
-    five-GEMM kernel.  Outputs/gradients are laid out ``[S,B,H,D]`` in memory (returned as ``[B,S,H,D]`` views) so the
+    """Flash attention (``csrc/attention_sm90.cu``): forward saves (q, k, v, o, lse); backward is a dK/dV kernel and a dQ
+    kernel.  Outputs/gradients are laid out ``[S,B,H,D]`` in memory (returned as ``[B,S,H,D]`` views) so the
     model's ``[S,B,H·D]`` reshape is free."""
 
     @staticmethod
@@ -76,7 +65,7 @@ class _FlashAttn(torch.autograd.Function):
     def backward(ctx, go):
         q, k, v, o, lse = ctx.saved_tensors
         e = _ext.ext()
-        _ext.count_launch(4)   # memset + prep + main + dq convert
+        _ext.count_launch(3)   # δ prep + dK/dV + dQ
         dq, dk, dv = e.flash_attn_bwd(_tma_view(go), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale), True)
         return dq, dk, dv, None, None
 
@@ -97,7 +86,7 @@ class _FlashAttnLse(torch.autograd.Function):
     @staticmethod
     def backward(ctx, go, g_lse):
         q, k, v, o, lse = ctx.saved_tensors
-        _ext.count_launch(4)
+        _ext.count_launch(3)
         go = torch.zeros_like(o) if go is None else go
         dlse = None if g_lse is None else g_lse.float().contiguous()
         dq, dk, dv = _ext.ext().flash_attn_bwd(_tma_view(go.to(o.dtype)), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale), False, dlse)
@@ -105,7 +94,7 @@ class _FlashAttnLse(torch.autograd.Function):
 
 
 def flash_attention_with_lse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool, scale: float):
-    """``(out [B,S,H,D], lse [B,H,S] fp32)`` on the tcgen05 kernels, or ``None`` when they do not apply."""
+    """``(out [B,S,H,D], lse [B,H,S] fp32)`` on the own kernels, or ``None`` when they do not apply."""
     if _own_kernel_ok(q, k, v) and (not causal or q.shape[1] == k.shape[1]) and hasattr(_ext.ext(), "flash_attn_bwd"):
         return _FlashAttnLse.apply(q, k, v, causal, scale)
     return None

@@ -1,6 +1,6 @@
-"""Build the sm_100a extension in-tree.  ``python -m neuronx_distributed_b200.ops.build``
+"""Build the sm_90a (H100) extension in-tree.  ``python -m neuronx_distributed_b200.ops.build``
 
-Uses ``torch.utils.cpp_extension.load`` with explicit ``-gencode arch=compute_100a,code=sm_100a``
+Uses ``torch.utils.cpp_extension.load`` with explicit ``-gencode arch=compute_90a,code=sm_90a``
 (bypassing torch's arch list; nvcc cross-compiles without a GPU) and ``-lineinfo`` so ncu source
 pages map to our code."""
 from __future__ import annotations
@@ -22,10 +22,10 @@ def build(verbose: bool = False) -> Path:
     from torch.utils import cpp_extension
 
     BUILD_DIR.mkdir(parents=True, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")  # only used for a sanity print; real arch below
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")  # only used for a sanity print; real arch below
     os.environ.setdefault("MAX_JOBS", str(os.cpu_count() or 4))
     cuda_flags = [
-        "-gencode", "arch=compute_100a,code=sm_100a",
+        "-gencode", "arch=compute_90a,code=sm_90a",
         "-lineinfo", "-O3", "-std=c++17",
         "--expt-relaxed-constexpr", "--use_fast_math",
         "-Xptxas", "-v",

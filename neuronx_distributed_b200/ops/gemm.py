@@ -1,7 +1,7 @@
-"""bf16 GEMM on tcgen05 tensor cores (kernel: ``csrc/gemm_sm100.cu``).
+"""bf16 GEMM on Hopper wgmma tensor cores (kernel: ``csrc/gemm_sm90.cu``).
 
 ``matmul(a, b, trans_a, trans_b)`` computes ``op(a) @ op(b)`` for row-major 2-D bf16 tensors with
-fp32 accumulation in TMEM.  The three layouts training needs map to UMMA operand majors without
+fp32 accumulation in registers.  The three layouts training needs map to wgmma operand majors without
 any transposition copies:
 
     fwd   : x[M,K] @ W[N,K]^T     → A K-major,  B K-major     ("nt")
@@ -17,7 +17,6 @@ import torch
 from . import _ext
 
 _MIN_DIM = 64
-_USE_2CTA = os.environ.get("NXD_GEMM_2CTA", "1") == "1"   # CTA-pair kernel (cta_group::2)
 
 
 def fused_wgrad_enabled() -> bool:
@@ -55,10 +54,7 @@ def matmul(a: torch.Tensor, b: torch.Tensor, trans_a: bool = False, trans_b: boo
             out = torch.empty(M, N, dtype=out_dtype, device=a.device)
             accumulate = False
         _ext.count_launch()
-        if _USE_2CTA and M >= 256 and hasattr(_ext.ext(), "gemm_bf16_2cta"):
-            _ext.ext().gemm_bf16_2cta(a, b, out, bool(trans_a), bool(trans_b), bool(accumulate))
-        else:
-            _ext.ext().gemm_bf16(a, b, out, bool(trans_a), bool(trans_b), bool(accumulate))
+        _ext.ext().gemm_bf16(a, b, out, bool(trans_a), bool(trans_b), bool(accumulate))
         return out
     if a.is_cuda and a.dtype == torch.bfloat16 and not os.environ.get("NXD_DISABLE_TCGEN05_GEMM") \
             and (not a.is_contiguous() or not b.is_contiguous()):
@@ -84,7 +80,7 @@ def linear_nt(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
 
 # ---------------------------------------------------------------------------------------------------------------------
 # Grouped (MoE blockwise) GEMM: rows of ``x`` come in ``block_size``-row blocks, block i is multiplied by the weights of
-# expert ``block_to_expert[i]``.  CUDA: MODE 3/4 of ``csrc/gemm_sm100.cu`` (the per-block expert only shifts the TMA
+# expert ``block_to_expert[i]``.  CUDA: MODE 3/4 of ``csrc/gemm_sm90.cu`` (the per-block expert only shifts the TMA
 # coordinate of the weight tile — no per-block weight copies, no host sync); CPU / odd shapes: plain loop.
 # Role of the reference's blockwise NKI kernels (modules/moe/blockwise.py:180-468, 1037-1127).
 def _grouped_ok(x: torch.Tensor, w: torch.Tensor, block_size: int) -> bool:

@@ -1,7 +1,7 @@
 """fp8 × fp8 linear with outer-product scales: ``y = (xq @ wqᵀ) · xs[:, None] · ws[None, :]``.
 
-CUDA: the fp8 instantiation of the tcgen05 GEMM (``csrc/gemm_sm100.cu``: ``kind::f8f6f4`` UMMA, e4m3 operands staged by
-TMA as 128-byte swizzle rows of 128 elements, fp32 accumulation in TMEM, scales applied in the epilogue).
+CUDA: the fp8 instantiation of the wgmma GEMM (``csrc/gemm_sm90.cu``: ``wgmma m64n256k32.e4m3``, e4m3 operands staged by
+TMA as 128-byte swizzle rows of 128 elements, fp32 accumulation in registers, scales applied in the epilogue).
 CPU: fp32 reference.  Reference: quantization/quantization_layers.py (scaled matmul of the quantised parallel layers)."""
 from __future__ import annotations
 

@@ -6,14 +6,11 @@ byte (low nibble first; ``uint16`` x4 words are a view of the same bytes), MXFP8
 
 * ``rows <= 8`` on CUDA (token generation): ``csrc/gemv_mx.cu`` — the codes are decoded in registers, nothing is expanded in
   memory, so a decode step reads 4.25 / 8.25 bits per weight instead of 16;
-* MXFP8 or MXFP4 weights, more rows, opt-in ``NXD_GEMM_MX=1``: activations are quantised to MXFP8 online and both operands go through
-  the block-scaled tensor-core GEMM (``csrc/gemm_mx_sm100.cu``, ``tcgen05.mma.kind::mxf8f6f4.block_scale``: the E8M0 scales
-  are applied inside the tensor core, nothing is de-quantised) — W8A8-MX numerics, oracle :func:`matmul_mxfp8_reference`;
-* MXFP4 weights, opt-in ``NXD_GEMM_F4=1``: activations quantised to MXFP4 as well and both operands read packed at the FP4 rate
-  (``csrc/gemm_mxf4_sm100.cu``, ``kind::mxf4`` with E8M0 scales; the same kernel runs NVFP4 — UE4M3 scales per 16 elements —
-  through :func:`matmul_f4`) — W4A4 numerics, oracle :func:`matmul_f4_reference`;
-* otherwise: de-quantise to the activation dtype and run the dense GEMM (tcgen05 bf16 kernel on CUDA) — numerically the
-  oracle ``experimental…mx_torch.mx_matmul``."""
+* otherwise: de-quantise to the activation dtype and run the dense GEMM (wgmma bf16 kernel on CUDA) — numerically the
+  oracle ``experimental…mx_torch.mx_matmul``.
+
+Block-scaled and 4-bit tensor-core MMAs do not exist on H100, so the opt-in block-scaled GEMM paths (``NXD_GEMM_MX=1``,
+``NXD_GEMM_F4=1``) raise on CUDA tensors; :func:`matmul_mxfp8_reference` and :func:`matmul_f4_reference` keep their numerics."""
 from __future__ import annotations
 
 import os
@@ -50,8 +47,8 @@ def dequantize(weight: torch.Tensor, scale: torch.Tensor, kind: str, dtype: torc
 def tile_scales(scale: torch.Tensor, pad: int = 127) -> torch.Tensor:
     """E8M0 scales ``[R, K/32]`` → the chunked layout the block-scaled GEMM streams: ``[ceil(R/128), K/128, 512]`` where the
     512-byte chunk of (row tile, 128-wide K block) holds scale (r, j) at byte ``(r % 32) * 16 + (r // 32) * 4 + j`` — what
-    ``tcgen05.cp.32x128b.warpx4`` spreads over 4 TMEM columns.  Rows are padded with ``pad`` (E8M0 127 = 2^0).  The same chunking
-    serves the 4-bit kinds (:func:`matmul_f4`): a chunk is always 128 rows × 4 consecutive scales, whatever they span."""
+    a Blackwell ``tcgen05.cp.32x128b.warpx4`` spreads over 4 tensor-memory columns (kept as the layout the CPU test replays).  Rows are padded with ``pad`` (E8M0 127 = 2^0).  The same chunking
+    serves the 4-bit kinds: a chunk is always 128 rows × 4 consecutive scales, whatever they span."""
     R, KB = scale.shape
     assert KB % 4 == 0, "the number of scale columns must be a multiple of 4"
     T = (R + 127) // 128
@@ -67,25 +64,17 @@ def matmul_mxfp8_reference(a_q: torch.Tensor, a_scale: torch.Tensor, b_q: torch.
     return dequantize(a_q, a_scale, a_kind) @ dequantize(b_q, b_scale, b_kind).t()
 
 
-def gemm_mx_eligible(x2d: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor, kind: str) -> bool:
-    if os.environ.get("NXD_GEMM_MX", "0") != "1":                 # opt-in until the kernel has run on hardware
+def _no_block_scaled_mma(flag: str, *tensors: torch.Tensor) -> bool:
+    if os.environ.get(flag, "0") != "1" or not all(t.is_cuda for t in tensors):
         return False
-    return (x2d.is_cuda and kind in _MMA_FMT and x2d.shape[1] % 128 == 0 and scale.shape[0] % 8 == 0
-            and weight.is_contiguous() and _ext.use_cuda(x2d, weight, scale) and hasattr(_ext.ext(), "gemm_mxfp8"))
+    raise RuntimeError(f"{flag}=1: block-scaled / FP4 tensor-core GEMMs need Blackwell tensor cores; H100 has neither")
 
 
-def matmul_mxfp8(a_q: torch.Tensor, a_scale: torch.Tensor, b_q: torch.Tensor, b_scale: torch.Tensor, a_kind: str = "mxfp8",
-                 b_kind: str = "mxfp8", b_scale_tiled: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``[M, K] · [N, K]ᵀ`` on MX operands (byte streams or x4 words; MXFP8 or MXFP4 — the TMA engine unpacks e2m1 pairs into the
-    8-bit containers the tensor core reads) with E8M0 block scales → bf16 ``[M, N]``."""
-    a8 = a_q.contiguous().view(torch.uint8).reshape(a_scale.shape[0], -1)
-    b8 = b_q.contiguous().view(torch.uint8).reshape(b_scale.shape[0], -1)
-    _ext.count_launch()
-    return _ext.ext().gemm_mxfp8(a8, b8, tile_scales(a_scale), b_scale_tiled if b_scale_tiled is not None else tile_scales(b_scale),
-                                 _MMA_FMT[a_kind], _MMA_FMT[b_kind])
+def gemm_mx_eligible(x2d: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor, kind: str) -> bool:
+    return _no_block_scaled_mma("NXD_GEMM_MX", x2d, weight, scale)
 
 
-# ---- 4-bit × 4-bit at the FP4 rate (csrc/gemm_mxf4_sm100.cu) ------------------------------------------------------------
+# ---- 4-bit quantisers and the W4A4 oracle ------------------------------------------------------------
 _E2M1 = (0.0, 0.5, 1.0, 1.5, 2.0, 3.0, 4.0, 6.0)
 
 
@@ -141,23 +130,7 @@ def matmul_f4_reference(a_q, a_scale, b_q, b_scale, vec_size: int = 32, a_global
 
 
 def gemm_f4_eligible(M: int, N: int, K: int, *tensors: torch.Tensor) -> bool:
-    if os.environ.get("NXD_GEMM_F4", "0") != "1":                 # opt-in: W4A4 numerics, and the kernel has not run on hardware yet
-        return False
-    return (K % 256 == 0 and N % 8 == 0 and all(t.is_cuda for t in tensors) and _ext.use_cuda(*tensors)
-            and hasattr(_ext.ext(), "gemm_f4"))
-
-
-def matmul_f4(a_q: torch.Tensor, a_scale: torch.Tensor, b_q: torch.Tensor, b_scale: torch.Tensor, vec_size: int = 32,
-              a_global=1.0, b_global=1.0, b_scale_tiled: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``[M, K] · [N, K]ᵀ`` with BOTH operands e2m1 (packed bytes or x4 words) → bf16 ``[M, N]`` on
-    ``tcgen05.mma.kind::mxf4`` (``vec_size`` 32, E8M0 scales) or ``kind::mxf4nvf4`` (``vec_size`` 16, UE4M3 scales, the product of
-    the per-tensor factors applied in the epilogue): twice the tensor-core rate and half the operand bytes of the 8-bit kinds."""
-    a8 = a_q.contiguous().view(torch.uint8).reshape(a_scale.shape[0], -1)
-    b8 = b_q.contiguous().view(torch.uint8).reshape(b_scale.shape[0], -1)
-    pad = 127 if vec_size == 32 else 0x38                          # 2^0 / 1.0: padded rows never reach the output anyway
-    _ext.count_launch()
-    return _ext.ext().gemm_f4(a8, b8, tile_scales(a_scale, pad), b_scale_tiled if b_scale_tiled is not None else tile_scales(b_scale, pad),
-                              int(vec_size), float(a_global) * float(b_global))
+    return _no_block_scaled_mma("NXD_GEMM_F4", *tensors)
 
 
 def gemv_eligible(x2d: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor) -> bool:
@@ -194,20 +167,10 @@ def linear_mx(x: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor, kind: 
         r2 = None if residual is None else residual.reshape(-1, residual.shape[-1]).contiguous()
         y = _ext.ext().gemv_mx(x2.contiguous(), weight, scale, _FMT[kind], r2)
         return y.view(*x.shape[:-1], y.shape[-1])
-    if kind == "mxfp4" and gemm_f4_eligible(x2.shape[0], scale.shape[0], x2.shape[1], x2, weight, scale):
-        xq, xs = quantize_mxfp4(x2)                                  # W4A4: activations to MXFP4 online, both operands at the FP4 rate
-        y = matmul_f4(xq, xs, weight, scale, 32)
-        if residual is not None:
-            y = y + residual.reshape(-1, residual.shape[-1]).to(y.dtype)
-        return y.view(*x.shape[:-1], y.shape[-1]).to(x.dtype)
-    if gemm_mx_eligible(x2, weight, scale, kind):
-        from ..quantization.microscaling.mx_torch import quantize_mxfp8
-
-        xq, xs = quantize_mxfp8(x2.contiguous())
-        y = matmul_mxfp8(xq, xs, weight, scale, "mxfp8", kind)
-        if residual is not None:
-            y = y + residual.reshape(-1, residual.shape[-1]).to(y.dtype)
-        return y.view(*x.shape[:-1], y.shape[-1]).to(x.dtype)
+    # the opt-in block-scaled GEMMs do not exist on H100: raise rather than silently de-quantise
+    _no_block_scaled_mma("NXD_GEMM_MX", x2, weight, scale)
+    if kind == "mxfp4":
+        _no_block_scaled_mma("NXD_GEMM_F4", x2, weight, scale)
     w = dequantize(weight, scale, kind, x.dtype if x.dtype in (torch.bfloat16, torch.float16) else torch.float32)
     y = torch.nn.functional.linear(x.to(w.dtype), w)
     if residual is not None:

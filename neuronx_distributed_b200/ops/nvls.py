@@ -5,7 +5,7 @@ the loopback tests, fabrics without NVLS) the same kernels run over unicast peer
 
 Used by ``parallel_layers.comm.all_reduce`` for latency-bound tensors (decode-time RowParallelLinear /
 ParallelEmbedding outputs without sequence parallel — reference layers.py:1040-1043, mappings.py:196-211) and by
-``tools/nvls_probe.py`` for the link-bandwidth numbers in ``profiles/``.
+``tools/nvls_probe.py`` to measure the link bandwidth.
 """
 from __future__ import annotations
 

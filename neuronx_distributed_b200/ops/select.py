@@ -1,4 +1,4 @@
-"""Row-wise arg-max / top-k on the sm_100a selection kernels (``csrc/select.cu``) with plain PyTorch as the CPU path and the
+"""Row-wise arg-max / top-k on the sm_90a selection kernels (``csrc/select.cu``) with plain PyTorch as the CPU path and the
 numerics oracle.  ``index_offset`` shifts the returned indices (global id of a vocab shard's first column)."""
 from __future__ import annotations
 

@@ -2,7 +2,7 @@
 
 Native part: ``csrc/symm.cpp`` — ``cudaMalloc`` + CUDA-IPC handle exchange; every rank ends up
 with a table of device pointers to all peers' buffers plus a flags region, which the fused
-GEMM+collective kernels (``csrc/gemm_sm100.cu``) and the ZeRO-1 reduce-scatter kernel dereference
+GEMM+collective kernels (``csrc/gemm_sm90.cu``) and the ZeRO-1 reduce-scatter kernel dereference
 directly (P2P ld/st over NVSwitch).  Handles travel over the gloo control group.
 
 A :class:`SymmWorkspace` is created lazily per (process group, purpose) and reused; kernels use

@@ -1,7 +1,7 @@
 """Dispatch of TP linear layers onto the fused GEMM+collective kernels.
 
 ``dispatch(x, weight, in_mode, out_mode, seq_dim, group)`` returns an object with
-``forward``/``backward`` when the sm_100a fused path applies, else ``None`` (the caller then
+``forward``/``backward`` when the sm_90a fused path applies, else ``None`` (the caller then
 runs collectives + matmul through the library path).  Filled in by ``_fused_impl`` once the
 extension exposes the kernels; selection can be forced off with ``NXD_TP_BACKEND=nccl``.
 """

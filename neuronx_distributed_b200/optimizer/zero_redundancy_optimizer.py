@@ -2,7 +2,7 @@
 
 Role parity with reference ``optimizer/zero_redundancy_optimizer.py`` (``NeuronZero1Optimizer``
 :30, ``NeuronEPZero1Optimizer`` :163) whose base class lives in torch_xla (external, K13 in
-SURVEY §2.9) — this is a from-scratch implementation designed for B200:
+SURVEY §2.9) — this is a from-scratch implementation designed for H100:
 
 * **Flat contiguous buffers.**  Per (param-group, dtype) the model parameters are re-pointed
   into one flat ``param_flat`` buffer and gradients accumulate into one flat fp32 (or bf16)

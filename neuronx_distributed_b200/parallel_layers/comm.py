@@ -6,7 +6,7 @@ calls issued through ``torch.distributed``; in CPU mode they run on gloo, which 
 reduce-scatter, so that one is emulated (all-reduce + local slice — simpler and deterministic
 compared with the reference's reduce-to-root + scatter :82-121).
 
-The hot tensor-parallel paths do NOT go through this file on B200: they use the fused
+The hot tensor-parallel paths do NOT go through this file on H100: they use the fused
 GEMM+collective kernels in ``ops/tp_fused.py``.
 """
 from __future__ import annotations

@@ -5,7 +5,7 @@ Capability parity with reference ``parallel_layers/grads.py`` (``get_grad_norm``
 :259-327, ``allreduce_sequence_parallel_gradients`` :330-346,
 ``allreduce_context_parallel_gradients`` :348-366).
 
-B200 design: squared norms are produced by ONE multi-tensor kernel launch
+H100 design: squared norms are produced by ONE multi-tensor kernel launch
 (``ops.optim.multi_tensor_sq_norm`` → a single fp32 scalar on device) instead of a python loop of
 ``torch.norm`` calls, the scalar all-reduces stay on device (no host sync; the clip coefficient is
 applied with a device-side ``clamp`` exactly as the reference's ``torch.where(coeff<1)`` trick),

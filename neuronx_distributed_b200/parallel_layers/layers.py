@@ -4,7 +4,7 @@ Capability parity with reference ``parallel_layers/layers.py`` (``ParallelEmbedd
 ``LinearWithAsyncCommunication`` :434, ``ColumnParallelLinear`` :561, ``RowParallelLinear``
 :815, conv layers :1309/:1432, ``SPMDRank`` :1543) and ``layers_utils.py:16-140``.
 
-B200 design notes
+H100 design notes
 -----------------
 * A TP linear is ONE autograd node (:class:`_TPLinear`) covering gather → GEMM → reduce in
   both directions, so the forward and backward each map to a single fused GEMM+collective
@@ -471,7 +471,7 @@ class _TPLinear(torch.autograd.Function):
                 if bias is not None:
                     y = y + bias
                 return y
-            y = ops.gemm.linear_nt(total, weight)          # tcgen05 kernel on CUDA bf16, torch.matmul otherwise
+            y = ops.gemm.linear_nt(total, weight)          # wgmma kernel on CUDA bf16, torch.matmul otherwise
             if n > 1 and out_mode in ("scatter", "reduce"):
                 od = y.dtype
                 yr = y.to(reduce_dtype) if reduce_dtype is not None else y

@@ -4,7 +4,7 @@ Capability parity with reference ``parallel_layers/loss_functions.py`` (``parall
 :217, ``_ParallelCrossEntropy`` :10-129, ``DistributedLogprob`` / ``from_parallel_logits_to_logprobs``
 :131-215).
 
-B200 design: one pass over the local ``[T, V/tp]`` logits produces three per-row statistics
+H100 design: one pass over the local ``[T, V/tp]`` logits produces three per-row statistics
 (local max, local sum-exp relative to that max, target logit if owned); the three reference
 all-reduces (MAX, SUM, SUM) collapse into ONE all-gather of a ``[T, 3]`` fp32 tensor followed by
 a log-sum-exp merge, and the softmax is *recomputed* in backward from the saved logits and the

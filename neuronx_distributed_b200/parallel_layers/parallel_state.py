@@ -4,7 +4,7 @@ Capability parity with reference ``src/neuronx_distributed/parallel_layers/paral
 (``initialize_model_parallel`` :391-747, getters :833-1223, kv/token-shuffle/draft groups
 :1285-1564, ``get_zero1_sharding_groups`` :1684-1706, ``rmsg`` :1648).
 
-Design (B200-first, not a port):
+Design (H100-first, not a port):
 
 * The rank grid is the same ``[PP, DP, CP, TP]`` / ``[PP, DP_exp, EP, TP]`` row-major layout
   (TP fastest varying) because checkpoint file names and ZeRO-1 shard ownership are defined
@@ -144,7 +144,7 @@ def ascending_ring_PG_group(lnc_size: int = 1, cluster_ranks_nonexp=None, cluste
 
     Behind an NVSwitch every GPU is one hop from every other, so this is the ONLY placement policy here: it keeps a TP
     group inside one NVLink domain (8 GPUs) and puts DP / PP across nodes.  The reference's second policy
-    (:177-325, interleaved rings for the Trn2 torus) has no B200 counterpart and maps to this one.
+    (:177-325, interleaved rings for the Trn2 torus) has no H100 counterpart and maps to this one.
     """
     return RankMesh(tp * dp * pp * cp, tp, pp, cp, ep_model_degree)
 
@@ -170,7 +170,7 @@ class PG_Group_Logic(enum.Enum):  # noqa: N801  (reference spelling, :326-335)
 
 
 def get_logic_chosen(lnc_size: int = 1, hardware_type: Any = None, tp: int = 1):
-    """Reference parallel_state.py:341-357 picks a placement by hardware generation; B200 has one."""
+    """Reference parallel_state.py:341-357 picks a placement by hardware generation; H100 has one."""
     return PG_Group_Logic.LOGIC1
 
 

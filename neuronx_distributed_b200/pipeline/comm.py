@@ -2,7 +2,7 @@
 
 Role parity with reference ``pipeline/comm.py`` (tensor send/recv :41-106, python-object metadata
 exchange :114-211).  XLA has no point-to-point primitive, so the reference emulates send/recv with
-2-rank all-gathers; on B200 these are real NCCL ``isend``/``irecv`` issued as ONE batched group per
+2-rank all-gathers; on H100 these are real NCCL ``isend``/``irecv`` issued as ONE batched group per
 schedule step (``batch_isend_irecv``) on NCCL's own stream, so activation traffic overlaps compute.
 Shape/dtype metadata travels once per (direction, chunk) over the gloo PP group and is cached.
 """

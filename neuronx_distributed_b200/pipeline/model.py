@@ -5,7 +5,7 @@ manual) partition into stages, 1F1B / interleaved / inference schedules, micro-b
 stage IO, tied-weight handling, loss extraction, ``local_*`` accessors with original parameter
 names, ``_debug_mode`` for partition-only tests.
 
-B200 design (differs from the XLA engine):
+H100 design (differs from the XLA engine):
 * eager CUDA — no graph breaks / mark_step; every task is ordinary stream-ordered work;
 * stage IO goes over NCCL ``batch_isend_irecv`` (one group per schedule step) on NCCL's stream and is
   awaited just-in-time, so activation/gradient transfers overlap the neighbouring compute;

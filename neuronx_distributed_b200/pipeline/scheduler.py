@@ -15,7 +15,7 @@ Construction here is two-phase instead of the reference's step-id arithmetic:
    forward it just ran.
 
 The engine executes sends asynchronously on an NCCL side stream, so the rule is conservative on
-B200 but is kept so CPU/gloo (blocking p2p) runs the same schedules.
+H100 but is kept so CPU/gloo (blocking p2p) runs the same schedules.
 """
 from __future__ import annotations
 

@@ -142,7 +142,7 @@ def matmul_mx_single_tile(a_x4: torch.Tensor, b_x4: torch.Tensor, a_scale: torch
 def matmul_mx(a_x4: torch.Tensor, b_x4: torch.Tensor, a_scale: torch.Tensor, b_scale: torch.Tensor,
               accumulation_dtype: torch.dtype = torch.float32, output_dtype: torch.dtype = torch.bfloat16,
               tile_k: int = 128) -> torch.Tensor:
-    """Tiled MX GEMM oracle: accumulates K in ``tile_k``-element steps in ``accumulation_dtype`` (TMEM accumulates in
+    """Tiled MX GEMM oracle: accumulates K in ``tile_k``-element steps in ``accumulation_dtype`` (a tensor core accumulates in
     fp32; pass bf16 to study a lower-precision accumulator)."""
     per_word_a = 4
     k_elems = a_x4.shape[1] * per_word_a

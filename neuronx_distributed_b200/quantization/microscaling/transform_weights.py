@@ -160,7 +160,7 @@ def reshape_pad_proj(W, scale, bias, pad_multiple: int = 512):
     ``pad_multiple`` elements (scales padded with the E8M0 bias, i.e. 2⁰; weights / bias with zero).
 
     The reference hard-codes the gpt-oss-120b geometry (128 experts, 2880 → 3072); here the target is derived from the
-    tensor so that any expert geometry can be aligned for the 128-row UMMA tiles.
+    tensor so that any expert geometry can be aligned for the 128-row GEMM tiles.
     """
     w = W      # reference parameter names in the signature
     E, R = w.shape[0], w.shape[1]

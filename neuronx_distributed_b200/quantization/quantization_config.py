@@ -1,9 +1,9 @@
 """Quantization configuration (reference ``quantization/quantization_config.py:10-256``).
 
 Same enums / config dictionaries as the reference so that model code written against it ports unchanged; the dtype table
-is the Blackwell one: e4m3 saturates at 448 (``float8_e4m3fn``, the tcgen05 ``kind::f8f6f4`` operand format — the
+is the OCP / NVIDIA one: e4m3 saturates at 448 (``float8_e4m3fn``, the e4m3 wgmma operand format — the
 reference clamps to the Trainium e4m3 range of 240), microscaling blocks are 32 elements along K with UE8M0 scales
-(what ``tcgen05.mma.kind::mxf8f6f4.block_scale`` consumes).
+(the OCP MX block-scale format).
 """
 from __future__ import annotations
 

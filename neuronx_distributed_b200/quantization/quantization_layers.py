@@ -6,13 +6,13 @@ optionally ``input_scale`` (static activation quantisation) and ``bias``; all of
 attributes the checkpoint sharder needs, plus ``get_tensor_from_state_dict`` hooks so that torch ``qint8`` packed
 checkpoints load directly (``QuantizedParallelLinearLayerStateDictAdaptor``).
 
-Execution on B200:
+Execution on H100:
 
 * weight-only, per-tensor / per-channel — the quantised values are exact in bf16, so the GEMM runs on the upcast weight
   and the scale is a per-output-feature multiply in the epilogue (no de-quantised copy of the weight is scaled);
 * blockwise / MX — block scales are expanded once per call into a bf16 weight, then the bf16 GEMM;
-* fp8 weights with dynamic or static fp8 activations — ``ops.gemm_fp8``: tcgen05 ``kind::f8f6f4`` GEMM with the
-  (per-token × per-channel) scale product applied in the TMEM epilogue.
+* fp8 weights with dynamic or static fp8 activations — ``ops.gemm_fp8``: e4m3 wgmma GEMM with the
+  (per-token × per-channel) scale product applied in the epilogue.
 
 Layers can be built empty (``QuantizedColumnParallel(in, out, …)`` → load a quantised checkpoint) or from a float layer
 (``from_float``), which — a superset of the reference — also quantises the float layer's weights when they are

@@ -17,7 +17,7 @@ reference (HLO)                          here (launch plan)
 ``prepare_parameter_usage_map`` …        ``LaunchPlan.weight_usage`` / ``kernel_weight_names`` (views are looked through)
 =======================================  ================================================================================
 
-What gets hoisted on B200 is not a compiler-chosen tiling (the tcgen05 GEMMs read K-major weights through TMA in every
+What gets hoisted on H100 is not a compiler-chosen tiling (the wgmma GEMMs read K-major weights through TMA in every
 bucket) but everything a bucket recomputes from frozen weights on each call: dtype casts, transposes that end in a copy,
 de-quantisation of int8 / fp8 / MX weights, input-independent masks and rotary tables."""
 from __future__ import annotations

@@ -2,7 +2,7 @@
 
 Reference (``trace/model_builder.py:441-1369``, ``model_builder_v2.py:33-319``): XLA-trace each bucket (context
 encoding / token generation / speculation) to HLO → neuronx-cc → NEFF, optimise weight layout across buckets, build
-a state (KV cache) initialiser, write per-rank sharded safetensors.  On B200 "compile" means: run every bucket's step
+a state (KV cache) initialiser, write per-rank sharded safetensors.  On H100 "compile" means: run every bucket's step
 once to warm up allocators/NCCL, then capture it into a CUDA graph with persistent input/output/state buffers;
 weights are shared by all buckets by construction (same parameter tensors), so no layout pass is needed.
 ``shard_checkpoint`` keeps the reference's output format: ``tp{rank}_sharded_checkpoint.safetensors``."""

@@ -106,7 +106,7 @@ class CompilationArtifacts:
     plan: Any = None                                       # LaunchPlan the program interprets (None: the module itself runs)
 
     def get_neff_bytes(self) -> bytes:
-        """The reference returns the NEFF file; the nearest B200 artefact is a description of the captured program."""
+        """The reference returns the NEFF file; the nearest H100 artefact is a description of the captured program."""
         return repr({"key": self.key, "captured_cuda_graph": self.captured, "args": self.compiler_args}).encode()
 
 

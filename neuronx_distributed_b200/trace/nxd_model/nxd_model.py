@@ -139,7 +139,7 @@ class NxDModel(BaseNxDModel):
         return self.units[key]
 
     def get_hlo(self, key: str):
-        """The reference returns the HLO proto of a bucket; the B200 analogue is the bucket's call description."""
+        """The reference returns the HLO proto of a bucket; the H100 analogue is the bucket's call description."""
         return self._unit(key)[0].hlo
 
     def get_metaneff(self, key: str):

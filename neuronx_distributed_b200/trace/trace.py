@@ -1,6 +1,6 @@
 """v0 inference API + checkpoint-sharding helpers (reference ``trace/trace.py:62-825``).
 
-``parallel_model_trace(func, example_inputs, tp_degree=…)`` returns a :class:`ParallelModel`; on B200 each rank is its own
+``parallel_model_trace(func, example_inputs, tp_degree=…)`` returns a :class:`ParallelModel`; on H100 each rank is its own
 ``torchrun`` process, so the returned wrapper holds THIS rank's captured program (the reference's wrapper holds one traced
 model per rank inside a single process)."""
 from __future__ import annotations

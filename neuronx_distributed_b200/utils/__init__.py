@@ -2,7 +2,7 @@
 
 The reference has one global switch, ``NXD_CPU_MODE`` (reference
 ``src/neuronx_distributed/utils/__init__.py:6-26``), that swaps XLA collectives for gloo.
-Here the split is *device kind*: CUDA (NCCL process groups + sm_100a kernels) or CPU
+Here the split is *device kind*: CUDA (NCCL process groups + sm_90a kernels) or CPU
 (gloo process groups + plain PyTorch math).  CPU mode is chosen automatically when no GPU
 is visible, or forced with ``NXD_CPU_MODE=1`` so the whole library is testable with
 ``torchrun --nproc-per-node N`` on a laptop.

@@ -301,8 +301,8 @@ import enum as _enum  # noqa: E402
 
 
 class LogicalNCConfig(_enum.IntEnum):
-    """Logical cores per device.  A B200 is ONE logical device (its two dies share L2/HBM coherently and are scheduled
-    as one 148-SM grid), so only ``LNC_1`` is ever returned; ``LNC_2`` exists for configs ported from Trn2."""
+    """Logical cores per device.  A H100 is ONE logical device (its two dies share L2/HBM coherently and are scheduled
+    as one grid over all its SMs), so only ``LNC_1`` is ever returned; ``LNC_2`` exists for configs ported from Trn2."""
 
     LNC_1 = 1
     LNC_2 = 2

@@ -8,7 +8,7 @@ from typing import Any, Dict, Union
 
 
 class hardware(Enum):  # noqa: N801  (reference spelling)
-    """Target platform.  This framework targets exactly one (``B200``); the Trainium names of the reference resolve to it
+    """Target platform.  This framework targets exactly one GPU (H100; the member keeps its name ``B200``); the Trainium names of the reference resolve to it
     so that scripts passing ``hardware_type="trn2"`` keep working."""
 
     B200 = "b200"

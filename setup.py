@@ -1,8 +1,8 @@
 """Packaging of neuronx_distributed_b200.
 
     pip install -e .            development install: the CUDA extension is compiled in-tree on first use (or by `build_ext`)
-    python setup.py build_ext   compile the sm_100a extension now (nvcc cross-compiles without a GPU)
-    pip wheel .                 wheel with the prebuilt extension inside the package (platform wheel, sm_100a only)
+    python setup.py build_ext   compile the sm_90a extension now (nvcc cross-compiles without a GPU)
+    pip wheel .                 wheel with the prebuilt extension inside the package (platform wheel, sm_90a only)
 
 Console scripts mirror the reference's (`nxd_convert_zero_checkpoints`, reference setup.py:62-64) and add the sharded-checkpoint
 converter that the reference ships as a plain script (`scripts/checkpoint_converter.py`)."""
@@ -24,7 +24,7 @@ class BinaryDistribution(Distribution):
 
 class build_ext(Command):
     """Compile csrc/*.cu + csrc/*.cpp into neuronx_distributed_b200/_build/ (same entry point as `__graft_entry__.build()`)."""
-    description = "compile the sm_100a CUDA extension in-tree"
+    description = "compile the sm_90a CUDA extension in-tree"
     user_options = []
 
     def initialize_options(self):
@@ -52,8 +52,8 @@ class build_py_with_extension(build_py):
 setup(
     name="neuronx-distributed-b200",
     version=version["__version__"],
-    description="Tensor / pipeline / sequence / context / expert parallel training and inference for NVIDIA B200 (sm_100a): "
-                "PyTorch + hand-written tcgen05 / TMA kernels + NCCL / NVSwitch",
+    description="Tensor / pipeline / sequence / context / expert parallel training and inference for NVIDIA H100 (sm_90a): "
+                "PyTorch + hand-written wgmma / TMA kernels + NCCL / NVSwitch",
     packages=find_packages(include=["neuronx_distributed_b200", "neuronx_distributed_b200.*"]),
     package_data={"neuronx_distributed_b200": ["_build/*.so"]},
     python_requires=">=3.10",

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on B200 via gpurun)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "multigpu: test needs >= 2 CUDA devices")
 
 

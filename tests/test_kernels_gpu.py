@@ -1,4 +1,4 @@
-"""Numerics of every hand-written CUDA kernel vs a plain PyTorch fp32 reference (B200 only)."""
+"""Numerics of every hand-written CUDA kernel vs a plain PyTorch fp32 reference (H100, sm_90a)."""
 import os
 import sys
 
@@ -81,7 +81,7 @@ def test_tiny_llama_trains_on_cuda_kernels():
 @pytest.mark.parametrize("layout", ["bshd", "sbhd", "fused"])
 @pytest.mark.parametrize("causal", [True, False])
 def test_flash_attention_fwd_bwd_vs_fp32_reference(layout, causal):
-    """tcgen05 flash attention (fwd + 5-GEMM bwd) through the autograd front-end vs plain fp32 softmax(QKᵀ)V."""
+    """Flash attention (fwd + dK/dV and dQ bwd kernels) through the autograd front-end vs plain fp32 softmax(QKᵀ)V."""
     import math
 
     from neuronx_distributed_b200.ops import _ext, attention
@@ -110,6 +110,38 @@ def test_flash_attention_fwd_bwd_vs_fp32_reference(layout, causal):
     s = torch.einsum("bqhd,bkhd->bhqk", qf, kk) / math.sqrt(D)
     if causal:
         s = s.masked_fill(~torch.ones(S, S, device=dev, dtype=torch.bool).tril(), float("-inf"))
+    ro = torch.einsum("bhqk,bkhd->bqhd", s.softmax(-1), vv)
+    ro.backward(go.float())
+
+    def rel(a, b):
+        return ((a.float() - b).abs().max() / b.abs().max()).item()
+
+    assert rel(o, ro) < 2e-2
+    assert rel(q.grad, qf.grad) < 3e-2 and rel(k.grad, kf.grad) < 3e-2 and rel(v.grad, vf.grad) < 3e-2
+
+
+@pytest.mark.parametrize("causal,S_q,S_kv", [(True, 200, 200), (False, 200, 328), (False, 130, 70)])
+def test_flash_attention_ragged_lengths_vs_fp32_reference(causal, S_q, S_kv):
+    """Lengths that are not multiples of the 64-row tiles (zero-filled tails, masked keys, unwritten rows), and non-causal
+    attention with S_q != S_kv."""
+    import math
+
+    from neuronx_distributed_b200.ops import _ext, attention
+
+    torch.manual_seed(2)
+    B, H, Hkv, D = 2, 4, 2, 128
+    q = torch.randn(B, S_q, H, D, device="cuda").bfloat16().requires_grad_(True)
+    k, v = (torch.randn(B, S_kv, Hkv, D, device="cuda").bfloat16().requires_grad_(True) for _ in range(2))
+    n0 = _ext.launches()
+    o = attention.flash_attention(q, k, v, causal=causal)
+    go = torch.randn(B, S_q, H, D, device="cuda").bfloat16()
+    o.backward(go)
+    assert _ext.launches() > n0, "own attention kernels did not run"
+    qf, kf, vf = (t.detach().float().requires_grad_(True) for t in (q, k, v))
+    kk, vv = kf.repeat_interleave(H // Hkv, 2), vf.repeat_interleave(H // Hkv, 2)
+    s = torch.einsum("bqhd,bkhd->bhqk", qf, kk) / math.sqrt(D)
+    if causal:
+        s = s.masked_fill(~torch.ones(S_q, S_kv, device="cuda", dtype=torch.bool).tril(), float("-inf"))
     ro = torch.einsum("bhqk,bkhd->bqhd", s.softmax(-1), vv)
     ro.backward(go.float())
 

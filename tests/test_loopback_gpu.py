@@ -65,17 +65,21 @@ def _fused_tp(rank, world):
     assert ws.nvls_enabled() and not ws.nv.has_multicast
     for wire in ("bf16", "fp32"):
         os.environ["NXD_TP_WIRE"] = wire
-        for it, (ms, N, K) in enumerate([(256, 512, 256), (512, 1000, 512), (256, 512, 256)]):
+        # (rows per rank, N, K, trans_b): trans_b=False is the [K, N] MN-major weight operand of the backward (dgrad)
+        cases = [(256, 512, 256, True), (512, 1000, 512, True), (256, 512, 256, True), (128, 384, 256, True),
+                 (128, 256, 384, False), (256, 512, 256, False)]
+        for it, (ms, N, K, tb) in enumerate(cases):
             xs = [_inputs(r, (ms, K), 40 + it) for r in range(world)]
-            w = _inputs(0, (N, K), 50 + it, 0.05)
-            out, gathered = ws.ag_gemm(xs[rank], w, True)
+            w = _inputs(0, (N, K) if tb else (K, N), 50 + it, 0.05)
+            wt = w.float().t() if tb else w.float()
+            out, gathered = ws.ag_gemm(xs[rank], w, tb)
             full = torch.cat(xs)
             assert torch.equal(gathered, full)
-            assert _relerr(out, full.float() @ w.float().t()) < 2e-2
+            assert _relerr(out, full.float() @ wt) < 2e-2, (wire, it)
             # GEMM → reduce-scatter: every rank has its own [world*ms, K] operand
             a = [_inputs(r, (world * ms, K), 60 + it) for r in range(world)]
-            o = ws.gemm_rs(a[rank], w, True)
-            ref = sum(x.float() @ w.float().t() for x in a)[rank * ms:(rank + 1) * ms]
+            o = ws.gemm_rs(a[rank], w, tb)
+            ref = sum(x.float() @ wt for x in a)[rank * ms:(rank + 1) * ms]
             assert _relerr(o, ref) < 2e-2, (wire, it)
     os.environ["NXD_TP_WIRE"] = "bf16"
     # a larger shape mid-stream re-lays the region out (barrier, epochs keep counting) and must keep working, first call included

@@ -1,4 +1,7 @@
 """MoE correctness vs a dense per-token reference (role of reference test_impl_correctness.py)."""
+import os
+import tempfile
+
 import torch
 
 from dist_utils import run_distributed
@@ -58,7 +61,12 @@ def _moe_worker(rank, world):
     loss = y.pow(2).mean() + 0.01 * load_balancing_loss_func(rl, E, k)
     loss.backward()
     assert layer.expert_mlps.mlp_op.down_proj.weight.grad is not None
-    torch.save(y.detach(), f"/tmp/moe_y_w{world}_r{rank}.pt")
+    torch.save(y.detach(), _out_path(world, rank))
+
+
+def _out_path(world, rank):
+    # per user: the worker processes of one test run hand their outputs over through the temp directory
+    return os.path.join(tempfile.gettempdir(), f"moe_y_u{os.getuid()}_w{world}_r{rank}.pt")
 
 
 def test_moe_modes_match_reference():
@@ -68,6 +76,6 @@ def test_moe_modes_match_reference():
 def test_moe_tensor_parallel_matches_single():
     run_distributed(_moe_worker, 1, timeout=90)
     run_distributed(_moe_worker, 2, timeout=90)
-    full = torch.load("/tmp/moe_y_w1_r0.pt")
-    got = torch.cat([torch.load(f"/tmp/moe_y_w2_r{r}.pt") for r in range(2)], 0)
+    full = torch.load(_out_path(1, 0))
+    got = torch.cat([torch.load(_out_path(2, r)) for r in range(2)], 0)
     torch.testing.assert_close(got, full, rtol=1e-4, atol=1e-5)

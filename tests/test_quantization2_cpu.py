@@ -412,7 +412,7 @@ def test_mx_scale_tiling_layout():
 
 
 def test_fp4_gemm_quantisers_oracle_and_scale_addressing():
-    """4-bit × 4-bit GEMM (``csrc/gemm_mxf4_sm100.cu``): the MXFP4 / NVFP4 quantisers (round-to-nearest-even on the e2m1 grid),
+    """4-bit formats: the MXFP4 / NVFP4 quantisers (round-to-nearest-even on the e2m1 grid),
     the oracle, and a replay of the kernel's scale addressing — which chunk column and which scale bytes each K=64 MMA reads —
     against the un-tiled scale matrix."""
     import torch

@@ -1,4 +1,4 @@
-"""Numerics + timing of the tcgen05 flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
+"""Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
 usage: python tools/fa_check.py [--perf] [--bwd]"""
 import argparse
 import json

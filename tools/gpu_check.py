@@ -161,52 +161,6 @@ def check_gemm(perf=False):
     report("gemm_f32_accumulate", relerr(out, ref) < 1e-3, err=relerr(out, ref))
 
 
-def check_gemm_2cta():
-    torch.manual_seed(0)
-    e = ops._ext.ext()
-    for (M, N, K) in [(256, 256, 64), (512, 512, 256), (4096, 1536, 4096), (1000, 264, 72), (384, 768, 192)]:
-        for ta, tb in ((False, True), (False, False), (True, False)):
-            a = torch.randn((K, M) if ta else (M, K), device=dev, dtype=torch.bfloat16)
-            b = torch.randn((N, K) if tb else (K, N), device=dev, dtype=torch.bfloat16)
-            ref = (a.float().t() if ta else a.float()) @ (b.float().t() if tb else b.float())
-            out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-            e.gemm_bf16_2cta(a, b, out, ta, tb, False)
-            torch.cuda.synchronize()
-            err = relerr(out, ref)
-            report(f"gemm2cta_{M}x{N}x{K}_ta{int(ta)}_tb{int(tb)}", err < 1e-2, err=err)
-    M, N, K = 512, 512, 128
-    a = torch.randn(M, K, device=dev, dtype=torch.bfloat16); b = torch.randn(N, K, device=dev, dtype=torch.bfloat16)
-    out = torch.ones(M, N, device=dev, dtype=torch.float32)
-    e.gemm_bf16_2cta(a, b, out, False, True, True)
-    report("gemm2cta_f32_accumulate", relerr(out, a.float() @ b.float().t() + 1) < 1e-3)
-    # weight-gradient layout (A, B MN-major), fp32 output, few tiles and a long K → split-K with atomic fp32 partials
-    for (M, N, K) in [(512, 4096, 16384), (4096, 512, 16384), (1536, 4096, 8192), (2752, 4096, 16384)]:
-        a = torch.randn(K, M, device=dev, dtype=torch.bfloat16); b = torch.randn(K, N, device=dev, dtype=torch.bfloat16)
-        ref = a.float().t() @ b.float()
-        out = torch.empty(M, N, device=dev, dtype=torch.float32)
-        e.gemm_bf16_2cta(a, b, out, True, False, False)
-        e1 = relerr(out, ref)
-        e.gemm_bf16_2cta(a, b, out, True, False, True)             # accumulate on top: 2x
-        e2 = relerr(out, 2 * ref)
-        report(f"gemm2cta_splitk_wgrad_{M}x{N}x{K}", e1 < 2e-3 and e2 < 2e-3, err=e1, err_acc=e2)
-        import os as _os
-        t_on = timeit(lambda: e.gemm_bf16_2cta(a, b, out, True, False, True))
-        _os.environ["NXD_GEMM_SPLITK"] = "0"
-        t_off = timeit(lambda: e.gemm_bf16_2cta(a, b, out, True, False, True))
-        _os.environ["NXD_GEMM_SPLITK"] = "1"
-        report(f"gemm2cta_splitk_perf_{M}x{N}x{K}", True, splitk_tflops=2.0 * M * N * K / t_on / 1e9, no_split_tflops=2.0 * M * N * K / t_off / 1e9)
-    for (M, N, K) in [(4096, 1536, 4096), (4096, 4096, 1376), (4096, 12288, 4096), (4096, 22016, 4096), (4096, 4096, 11008),
-                      (8192, 8192, 8192), (4096, 4096, 512), (16384, 4096, 512), (16384, 4096, 1376), (16384, 4096, 1536),
-                      (4096, 4096, 2048), (16384, 1536, 4096), (16384, 2752, 4096)]:
-        a = torch.randn(M, K, device=dev, dtype=torch.bfloat16); b = torch.randn(N, K, device=dev, dtype=torch.bfloat16)
-        out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-        t2 = timeit(lambda: e.gemm_bf16_2cta(a, b, out, False, True, False))
-        t1 = timeit(lambda: e.gemm_bf16(a, b, out, False, True, False))
-        tl = timeit(lambda: torch.matmul(a, b.t()))
-        fl = 2.0 * M * N * K
-        report(f"gemm2cta_perf_{M}x{N}x{K}", True, cta2_tflops=fl / t2 / 1e9, cta1_tflops=fl / t1 / 1e9, cublas_tflops=fl / tl / 1e9)
-
-
 def check_gemm_perf():
     peaks = {}
     for (M, N, K) in [(4096, 1536, 4096), (4096, 2752, 4096), (4096, 4096, 512), (4096, 4096, 1376), (4096, 4000, 4096),
@@ -256,7 +210,7 @@ def check_decode(perf=False):
 
 
 def check_fp8(perf=False):
-    """fp8 (e4m3) tcgen05 GEMM with row/column scales vs the fp32 product of the same quantised operands."""
+    """fp8 (e4m3) wgmma GEMM with row/column scales vs the fp32 product of the same quantised operands."""
     from neuronx_distributed_b200.ops import gemm_fp8
 
     torch.manual_seed(0)
@@ -325,8 +279,6 @@ if __name__ == "__main__":
         check_fp8(perf=what == "fp8")
     if what in ("grouped", "all"):
         check_grouped(perf=what == "grouped")
-    if what in ("gemm2",):
-        check_gemm_2cta()
     if what in ("gemm_perf", "all"):
         check_gemm_perf()
     bad = [r["name"] for r in RESULTS if not r["ok"]]

@@ -1,4 +1,4 @@
-"""Interleaving-level model of the flag / epoch protocol of the fused TP kernels (csrc/tp_nvls_sm100.cu, ops/_fused_impl.py).
+"""Interleaving-level model of the flag / epoch protocol of the fused TP kernels (csrc/gemm_sm90.cu MODE 5 / 6, ops/_fused_impl.py).
 
 Every rank is a coroutine that performs one atomic action per step (a payload write, a flag release, a flag poll, a payload
 read); a seeded scheduler picks which rank moves next, so slow / fast rank skews of any size occur.  Checked invariants:

@@ -1,4 +1,4 @@
-"""Event-level model of tma_push_stream (csrc/gemm2cta_sm100.cu): random load/store latencies and item-ready times; asserts that a
+"""Event-level model of tma_push_stream (the all-gather pusher protocol of the fused TP GEMMs): random load/store latencies and item-ready times; asserts that a
 smem stage is never reloaded before its previous store has been read out, that no chunk is stored before it is loaded or before
 its item is ready, and that an item's flag is published only after all of its stores have completed, in order."""
 import random

@@ -1,7 +1,7 @@
 """Micro-benchmark of the fused TP kernels vs the NCCL + GEMM baseline on the Llama-2-7B shapes.
 
 torchrun --nproc-per-node N tools/tp_bench.py        → gpurun_out/tp_bench_tpN.json
-Reports per op: fused µs, baseline µs (NCCL collective + own tcgen05 GEMM, and + cuBLAS), and the roofline
+Reports per op: fused µs, baseline µs (NCCL collective + own GEMM, and + cuBLAS), and the roofline
 max(FLOPs / measured-GEMM-peak, NVLink-bytes / 770 GB/s) with the achieved fraction."""
 import json
 import os
