@@ -171,6 +171,39 @@ static void gemm_fp8(const Tensor& a, const Tensor& b, Tensor out, const Tensor&
                 stream());
 }
 
+// a e4m3 [M, K], b e4m3 [N, K]; scale_a fp32 [K/group, M] with unit column stride (row stride >= M, a multiple of 4);
+// scale_b fp32 [K/group, N] contiguous → bf16 [M, N]
+static Tensor gemm_fp8_block(const Tensor& a, const Tensor& b, const Tensor& scale_a, const Tensor& scale_b, int64_t group) {
+  CHECK_IN(a); CHECK_IN(b); CHECK_IN(scale_b);
+  TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn && a.dim() == 2 && b.dim() == 2 &&
+              a.size(1) == b.size(1), "gemm_fp8_block: a [M, K] and b [N, K] must be e4m3");
+  const int M = a.size(0), K = a.size(1), N = b.size(0);
+  TORCH_CHECK(group > 0 && K % group == 0, "gemm_fp8_block: K must be a multiple of the group size");
+  TORCH_CHECK(scale_a.is_cuda() && scale_a.scalar_type() == at::kFloat && scale_a.dim() == 2 && scale_a.size(0) == K / group &&
+              scale_a.size(1) == M && scale_a.stride(1) == 1 && reinterpret_cast<uintptr_t>(scale_a.data_ptr()) % 16 == 0,
+              "gemm_fp8_block: scale_a must be fp32 [K/group, M] with unit column stride and a 16-byte aligned start");
+  TORCH_CHECK(scale_b.scalar_type() == at::kFloat && scale_b.dim() == 2 && scale_b.size(0) == K / group && scale_b.size(1) == N,
+              "gemm_fp8_block: scale_b must be fp32 [K/group, N]");
+  c10::cuda::CUDAGuard guard(a.device());
+  Tensor out = at::empty({M, N}, a.options().dtype(at::kBFloat16));
+  nxd::gemm_fp8_block(a.data_ptr(), b.data_ptr(), out.data_ptr(), scale_a.data_ptr<float>(), scale_a.stride(0),
+                      scale_b.data_ptr<float>(), M, N, K, (int)group, stream());
+  return out;
+}
+
+// x bf16 [M, K] → (e4m3 [M, K], fp32 scales [K/group, round_up(M, 4)]: group-major, the layout gemm_fp8_block reads)
+static std::vector<Tensor> quantize_fp8_groups(const Tensor& x, int64_t group, bool mx, double clamp_bound) {
+  CHECK_IN(x);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.size(1) % group == 0, "quantize_fp8_groups: bf16 [M, K], K % group == 0");
+  const int M = x.size(0), K = x.size(1);
+  const long ld = ((long)M + 3) / 4 * 4;
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor q = at::empty({M, K}, x.options().dtype(at::kFloat8_e4m3fn));
+  Tensor s = at::empty({K / group, ld}, x.options().dtype(at::kFloat));
+  nxd::quantize_fp8_groups(x.data_ptr(), q.data_ptr(), s.data_ptr<float>(), M, K, ld, (int)group, mx, (float)clamp_bound, stream());
+  return {q, s};
+}
+
 static Tensor oneshot_allreduce(const Tensor& x, const Tensor& peer_bufs, const Tensor& peer_flags, int64_t slot_bytes,
                                 Tensor state, int64_t rank, int64_t world) {
   TORCH_CHECK(x.is_cuda() && x.is_contiguous() && (x.scalar_type() == at::kBFloat16 || x.scalar_type() == at::kFloat));
@@ -720,6 +753,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("row_topk_supported", &row_topk_supported);
   m.def("gemv", &gemv, py::arg("x"), py::arg("w"), py::arg("residual") = py::none());
   m.def("gemm_fp8", &gemm_fp8);
+  m.def("gemm_fp8_block", &gemm_fp8_block);
+  m.def("quantize_fp8_groups", &quantize_fp8_groups);
   m.def("grouped_gemm", &grouped_gemm);
   m.def("grouped_wgrad", &grouped_wgrad);
   m.def("flash_attn_fwd", &flash_attn_fwd);

@@ -641,6 +641,22 @@ static int sm_count() {
   return n;
 }
 
+CUtensorMap make_tmap_2d(const void* ptr, CUtensorMapDataType dt, uint64_t rows, uint64_t cols, uint64_t row_bytes,
+                         uint32_t box_cols, uint32_t box_rows, CUtensorMapSwizzle swizzle) {
+  ensure_driver_context();
+  CUtensorMap m;
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {row_bytes};
+  cuuint32_t box[2] = {box_cols, box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = get_encode()(&m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) nxd_throw("cuTensorMapEncodeTiled failed: " + std::to_string((int)r), __FILE__, __LINE__);
+  return m;
+}
+
+int device_sm_count() { return sm_count(); }
+
 template <bool AK, bool BK, int MODE, typename OutT>
 static void launch(const CUtensorMap& ta, const CUtensorMap& tb, void* out, int M, int N, int K, bool accumulate,
                    const CommDev& c, int grid, cudaStream_t st, const CUtensorMap* ta_local = nullptr) {

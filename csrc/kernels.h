@@ -88,6 +88,13 @@ void zero1_all_gather(const float* master, const int64_t* peer_bufs, long param_
 
 void gemm_fp8(const void* a, const void* b, void* out, int M, int N, int K, const float* scale_a, const float* scale_b,
               cudaStream_t st);
+// ---- block-scaled fp8 GEMM and its activation quantiser (gemm_fp8_block_sm90.cu); group = 32, 64 or 128 elements of K
+// out[M,N] (bf16) = Σ_g (a[:, g] · b[:, g]ᵀ) ∘ scale_a[g, :M] ⊗ scale_b[g, :N];  scale_a [K/group, scale_a_ld], scale_b [K/group, N]
+void gemm_fp8_block(const void* a, const void* b, void* out, const float* scale_a, long scale_a_ld, const float* scale_b,
+                    int M, int N, int K, int group, cudaStream_t st);
+// x bf16 [M, K] → q e4m3 [M, K] and fp32 scale [K/group, scale_ld] (group-major); mx: OCP MX power-of-two scales, else absmax / 448
+void quantize_fp8_groups(const void* x, void* q, float* scale, int M, int K, long scale_ld, int group, bool mx, float clamp_bound,
+                         cudaStream_t st);
 // ---- grouped (MoE blockwise) GEMMs, gemm_sm90.cu
 void grouped_gemm_bf16(const void* a, const void* b, void* out, int M, int N, int K, int E, bool trans_b,
                        const int* block_expert, int block_rows, int out_dt, cudaStream_t st);

@@ -6,8 +6,8 @@ Top-level exports mirror reference ``src/neuronx_distributed/__init__.py:1-19``.
 import os as _os
 
 # NXD_EXPERIMENTAL=1 switches on every opt-in path that has not been timed on hardware yet (README.md, "Opt-in paths"): one
-# flag to validate them together.  Individual flags set by the user win.  NXD_GEMM_MX / NXD_GEMM_F4 are not among them: the
-# block-scaled GEMMs do not exist on H100 and those flags raise on CUDA tensors.
+# flag to validate them together.  Individual flags set by the user win.  NXD_GEMM_MX / NXD_GEMM_F4 are not among them:
+# NXD_GEMM_MX also quantises the activations (W8A8-MX numerics), a choice of the user's, and H100 has no FP4 tensor-core MMA.
 _EXPERIMENTAL_FLAGS = ("NXD_FUSED_LMHEAD_CE", "NXD_MOE_TKG_KERNEL", "NXD_EMBEDDING_RS", "NXD_NVLS_A2A", "NXD_CP_PULL",
                        "NXD_GEMV_MX")
 if _os.environ.get("NXD_EXPERIMENTAL", "0") == "1":

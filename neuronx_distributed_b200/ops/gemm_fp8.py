@@ -1,13 +1,28 @@
-"""fp8 × fp8 linear with outer-product scales: ``y = (xq @ wqᵀ) · xs[:, None] · ws[None, :]``.
+"""FP8 (e4m3) linear layers on the Hopper FP8 tensor cores.
 
-CUDA: the fp8 instantiation of the wgmma GEMM (``csrc/gemm_sm90.cu``: ``wgmma m64n256k32.e4m3``, e4m3 operands staged by
-TMA as 128-byte swizzle rows of 128 elements, fp32 accumulation in registers, scales applied in the epilogue).
-CPU: fp32 reference.  Reference: quantization/quantization_layers.py (scaled matmul of the quantised parallel layers)."""
+* :func:`scaled_linear` — per-token × per-channel scales: ``y = (xq @ wqᵀ) · xs[:, None] · ws[None, :]``.  CUDA: the fp8
+  instantiation of the wgmma GEMM (``csrc/gemm_sm90.cu``: ``wgmma m64n256k32.e4m3``, e4m3 operands staged by TMA as 128-byte
+  swizzle rows of 128 elements, fp32 accumulation in registers, scales applied in the epilogue).
+* :func:`blockscaled_linear` — one scale per group of G ∈ {32, 64, 128} consecutive input features on both operands (block-wise
+  FP8 checkpoints, MXFP8): ``y = Σ_g (xq[:, g] @ wq[:, g]ᵀ) · xs[:, g] ⊗ ws[:, g]``.  CUDA: ``csrc/gemm_fp8_block_sm90.cu``,
+  one ``wgmma m64n128k32.e4m3`` chain per group into a temporary accumulator that is promoted into the fp32 main accumulator
+  with the group's scales, in registers.  Weight scales may be per (row, group) ``[N, K/G]`` or per 2-D block ``[N/bn, K/G]``,
+  fp32 or E8M0.
+* :func:`quantize_groups` — the matching per-token activation quantiser (``absmax`` or OCP ``mx`` scale rule); CUDA: one
+  bandwidth-bound kernel that writes the codes and the scales in the layout the GEMM reads.
+
+CPU, and shapes or dtypes the kernels do not take: the fp32 oracle of the same quantised operands.  Reference:
+quantization/quantization_layers.py (scaled matmul of the quantised parallel layers)."""
 from __future__ import annotations
+
+from typing import Optional, Tuple
 
 import torch
 
 from . import _ext
+
+_E4M3_MAX = 448.0
+GROUP_SIZES = (32, 64, 128)
 
 
 def scaled_linear(xq: torch.Tensor, xs: torch.Tensor, wq: torch.Tensor, ws: torch.Tensor,
@@ -25,3 +40,93 @@ def scaled_linear(xq: torch.Tensor, xs: torch.Tensor, wq: torch.Tensor, ws: torc
         return out.view(*shape[:-1], wq.shape[0])
     y = (x2.float() @ wq.float().t()) * s2 * ws.float().reshape(1, -1)
     return y.to(out_dtype).view(*shape[:-1], wq.shape[0])
+
+
+# ---- block-scaled ----------------------------------------------------------------------------------------------------
+def _quantize_groups_reference(x2: torch.Tensor, group_size: int, rule: str, clamp_bound: Optional[float]
+                               ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Torch oracle of the group quantiser: ``[M, K]`` → (e4m3 ``[M, K]``, fp32 ``[M, K/G]``)."""
+    M, K = x2.shape
+    xf = x2.float()
+    if clamp_bound is not None:
+        xf = xf.clamp(-clamp_bound, clamp_bound)
+    xb = xf.reshape(M, K // group_size, group_size)
+    amax = xb.abs().amax(-1)
+    if rule == "mx":
+        scale = torch.pow(2.0, torch.floor(torch.log2(amax.clamp(min=2.0 ** -100))) - 8)
+    else:
+        scale = (amax / _E4M3_MAX).clamp(min=1e-12)
+    q = (xb / scale.unsqueeze(-1)).clamp(-_E4M3_MAX, _E4M3_MAX).to(torch.float8_e4m3fn).reshape(M, K)
+    return q, scale
+
+
+def quantize_groups(x: torch.Tensor, group_size: int, rule: str = "absmax", clamp_bound: Optional[float] = None
+                    ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Per-token group quantisation to e4m3: ``x [..., K]`` → (codes ``[..., K]``, fp32 scales ``[..., K/G]``), ``x ≈ codes · scale``
+    per group of ``group_size`` consecutive elements.
+
+    ``rule="absmax"``: ``scale = max(amax / 448, 1e-12)`` (per-row ``quantize_activation_dynamic`` when G = K);
+    ``rule="mx"``: OCP MX ``scale = 2^(⌊log2 amax⌋ − 8)`` (``mx_torch.quantize_mx``).  Codes are ``clamp(x / scale, ±448)`` rounded
+    to nearest-even; ``clamp_bound`` clips ``x`` first.  On CUDA (bf16 input) the scales are a transposed view of the group-major
+    buffer :func:`blockscaled_linear` streams, and codes and scales are bit-identical to the torch oracle on the same CUDA tensor
+    (torch computes ``amax / 448`` as a product with the rounded reciprocal on CUDA and as a true division on CPU, so an absmax
+    scale can differ in the last bit between devices)."""
+    assert rule in ("absmax", "mx"), rule
+    K = x.shape[-1]
+    assert K % group_size == 0, f"K={K} is not a multiple of the group size {group_size}"
+    lead = x.shape[:-1]
+    x2 = x.reshape(-1, K)
+    if (group_size in GROUP_SIZES and x2.dtype == torch.bfloat16 and K % 8 == 0 and _ext.use_cuda(x2)
+            and hasattr(_ext.ext(), "quantize_fp8_groups")):
+        _ext.count_launch()
+        q, sbuf = _ext.ext().quantize_fp8_groups(x2.contiguous(), group_size, rule == "mx",
+                                                 float("inf") if clamp_bound is None else float(clamp_bound))
+        xs = sbuf[:, : x2.shape[0]].t()
+    else:
+        q, xs = _quantize_groups_reference(x2, group_size, rule, clamp_bound)
+    return q.view(*lead, K), xs.reshape(*lead, K // group_size)
+
+
+def weight_scales_kn(ws: torch.Tensor, n: int, k: int, group_size: int) -> torch.Tensor:
+    """Weight scales ``[N, K/G]`` or ``[N/bn, K/G]`` (2-D blocks), fp32 or E8M0 ``uint8`` → the fp32 ``[K/G, N]`` layout of the
+    block-scaled GEMM.  Depends on the weight only, so compiled inference hoists it out of the per-call plan."""
+    s = torch.pow(2.0, ws.float() - 127.0) if ws.dtype == torch.uint8 else ws.float()
+    s = s.reshape(-1, k // group_size)
+    if s.shape[0] != n:
+        assert n % s.shape[0] == 0, f"{s.shape[0]} scale rows do not tile {n} weight rows"
+        s = s.repeat_interleave(n // s.shape[0], dim=0)
+    return s.t().contiguous()
+
+
+def _dequant_groups(q: torch.Tensor, s: torch.Tensor, group_size: int) -> torch.Tensor:
+    R, K = q.shape
+    return (q.float().reshape(R, K // group_size, group_size) * s.float().unsqueeze(-1)).reshape(R, K)
+
+
+def blockscaled_linear(xq: torch.Tensor, xs: torch.Tensor, wq: torch.Tensor, ws: torch.Tensor, group_size: int,
+                       out_dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """``dequant(xq, xs) @ dequant(wq, ws)ᵀ`` for e4m3 codes with one scale per ``group_size`` input features.
+
+    ``xq [..., K]`` / ``xs [..., K/G]`` as :func:`quantize_groups` returns them; ``wq [N, K]``; ``ws`` fp32 or E8M0 ``[N, K/G]`` or
+    ``[N/bn, K/G]``.  CUDA with e4m3 operands, G ∈ {32, 64, 128}, ``K % 128 == 0``, ``N % 8 == 0`` and bf16 output: the
+    block-scaled wgmma GEMM; otherwise the fp32 oracle."""
+    K = xq.shape[-1]
+    lead = xq.shape[:-1]
+    x2 = xq.reshape(-1, K)
+    M, N = x2.shape[0], wq.shape[0]
+    xs2 = xs.reshape(M, K // group_size)
+    sb = weight_scales_kn(ws, N, K, group_size)
+    if (group_size in GROUP_SIZES and K % 128 == 0 and N % 8 == 0 and out_dtype == torch.bfloat16
+            and xq.dtype == torch.float8_e4m3fn and wq.dtype == torch.float8_e4m3fn and _ext.use_cuda(x2, wq, xs2, sb)
+            and hasattr(_ext.ext(), "gemm_fp8_block")):
+        sa = xs2.t()                                # [K/G, M]: a view of the quantiser's group-major buffer needs no copy
+        if not (sa.dtype == torch.float32 and sa.stride(1) == 1 and sa.stride(0) >= M and sa.stride(0) % 4 == 0
+                and sa.data_ptr() % 16 == 0):
+            buf = torch.zeros(K // group_size, (M + 3) // 4 * 4, dtype=torch.float32, device=x2.device)
+            buf[:, :M] = xs2.t()
+            sa = buf[:, :M]
+        _ext.count_launch()
+        y = _ext.ext().gemm_fp8_block(x2.contiguous(), wq.contiguous(), sa, sb, group_size)
+        return y.view(*lead, N)
+    y = _dequant_groups(x2, xs2, group_size) @ _dequant_groups(wq.reshape(N, K), sb.t(), group_size).t()
+    return y.to(out_dtype).view(*lead, N)

@@ -6,11 +6,14 @@ byte (low nibble first; ``uint16`` x4 words are a view of the same bytes), MXFP8
 
 * ``rows <= 8`` on CUDA (token generation): ``csrc/gemv_mx.cu`` — the codes are decoded in registers, nothing is expanded in
   memory, so a decode step reads 4.25 / 8.25 bits per weight instead of 16;
+* ``NXD_GEMM_MX=1`` with MXFP8 e4m3 weights on CUDA (prefill): the activations are quantised to MXFP8 as well (OCP ``mx``
+  scale rule, 32-element groups) and the block-scaled FP8 GEMM of ``ops.gemm_fp8`` runs on the codes — W8A8-MX numerics, the
+  oracle :func:`matmul_mxfp8_reference` of the quantised activations;
 * otherwise: de-quantise to the activation dtype and run the dense GEMM (wgmma bf16 kernel on CUDA) — numerically the
   oracle ``experimental…mx_torch.mx_matmul``.
 
-Block-scaled and 4-bit tensor-core MMAs do not exist on H100, so the opt-in block-scaled GEMM paths (``NXD_GEMM_MX=1``,
-``NXD_GEMM_F4=1``) raise on CUDA tensors; :func:`matmul_mxfp8_reference` and :func:`matmul_f4_reference` keep their numerics."""
+H100 has no 4-bit tensor-core MMA and the block-scaled GEMM takes e4m3 operands only, so ``NXD_GEMM_F4=1`` and
+``NXD_GEMM_MX=1`` with MXFP4 or e5m2 MX weights raise on CUDA tensors; :func:`matmul_f4_reference` keeps the 4-bit numerics."""
 from __future__ import annotations
 
 import os
@@ -67,11 +70,26 @@ def matmul_mxfp8_reference(a_q: torch.Tensor, a_scale: torch.Tensor, b_q: torch.
 def _no_block_scaled_mma(flag: str, *tensors: torch.Tensor) -> bool:
     if os.environ.get(flag, "0") != "1" or not all(t.is_cuda for t in tensors):
         return False
-    raise RuntimeError(f"{flag}=1: block-scaled / FP4 tensor-core GEMMs need Blackwell tensor cores; H100 has neither")
+    raise RuntimeError(f"{flag}=1: H100 has no FP4 tensor-core MMA; the block-scaled FP8 GEMM takes MXFP8 e4m3 weights only")
 
 
 def gemm_mx_eligible(x2d: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor, kind: str) -> bool:
-    return _no_block_scaled_mma("NXD_GEMM_MX", x2d, weight, scale)
+    """True when ``NXD_GEMM_MX=1`` routes this CUDA call to the block-scaled FP8 GEMM; raises for MX kinds it cannot take."""
+    if os.environ.get("NXD_GEMM_MX", "0") != "1" or not all(t.is_cuda for t in (x2d, weight, scale)):
+        return False
+    if kind not in ("mxfp8", "mxfp8_e4m3"):
+        raise RuntimeError(f"NXD_GEMM_MX=1: the block-scaled FP8 GEMM takes MXFP8 e4m3 weights only, not {kind}")
+    return True
+
+
+def _linear_mx_blockscaled(x2: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor) -> torch.Tensor:
+    """W8A8-MX: activations quantised with the OCP MX rule in 32-element groups, then the block-scaled FP8 GEMM."""
+    from . import gemm_fp8
+
+    N = scale.shape[0]
+    wq = weight.contiguous().view(torch.uint8).reshape(N, -1).view(torch.float8_e4m3fn)
+    xq, xs = gemm_fp8.quantize_groups(x2, 32, "mx")
+    return gemm_fp8.blockscaled_linear(xq, xs, wq, scale, 32)
 
 
 # ---- 4-bit quantisers and the W4A4 oracle ------------------------------------------------------------
@@ -167,10 +185,13 @@ def linear_mx(x: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor, kind: 
         r2 = None if residual is None else residual.reshape(-1, residual.shape[-1]).contiguous()
         y = _ext.ext().gemv_mx(x2.contiguous(), weight, scale, _FMT[kind], r2)
         return y.view(*x.shape[:-1], y.shape[-1])
-    # the opt-in block-scaled GEMMs do not exist on H100: raise rather than silently de-quantise
-    _no_block_scaled_mma("NXD_GEMM_MX", x2, weight, scale)
     if kind == "mxfp4":
-        _no_block_scaled_mma("NXD_GEMM_F4", x2, weight, scale)
+        _no_block_scaled_mma("NXD_GEMM_F4", x2, weight, scale)       # no FP4 tensor-core MMA on H100: raise, never de-quantise
+    if gemm_mx_eligible(x2, weight, scale, kind):
+        y = _linear_mx_blockscaled(x2, weight, scale).view(*x.shape[:-1], scale.shape[0])
+        if residual is not None:
+            y = y + residual.to(y.dtype)
+        return y.to(x.dtype)
     w = dequantize(weight, scale, kind, x.dtype if x.dtype in (torch.bfloat16, torch.float16) else torch.float32)
     y = torch.nn.functional.linear(x.to(w.dtype), w)
     if residual is not None:

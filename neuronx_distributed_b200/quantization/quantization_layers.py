@@ -12,7 +12,13 @@ Execution on H100:
   and the scale is a per-output-feature multiply in the epilogue (no de-quantised copy of the weight is scaled);
 * blockwise / MX — block scales are expanded once per call into a bf16 weight, then the bf16 GEMM;
 * fp8 weights with dynamic or static fp8 activations — ``ops.gemm_fp8``: e4m3 wgmma GEMM with the
-  (per-token × per-channel) scale product applied in the epilogue.
+  (per-token × per-channel) scale product applied in the epilogue;
+* blockwise e4m3 weights with K-blocks of 32, 64 or 128 and dynamic activations — W8A8 with the activations quantised per
+  token and per K-block (``ops.gemm_fp8.quantize_groups``) and the block-scaled FP8 GEMM (``ops.gemm_fp8.blockscaled_linear``):
+  per-group wgmma partial sums promoted into fp32 with both scales, no de-quantised copy of the weight.  1-D (per output row)
+  and 2-D (e.g. 128 × 128) blocks, fp32 and E8M0 block scales; the same numerics on CPU (fp32 oracle);
+* MXFP8 weights with ``NXD_GEMM_MX=1`` on CUDA (more than 8 rows) — ``ops.gemm_mx.linear_mx``: MXFP8 activations and the
+  block-scaled FP8 GEMM.
 
 Layers can be built empty (``QuantizedColumnParallel(in, out, …)`` → load a quantised checkpoint) or from a float layer
 (``from_float``), which — a superset of the reference — also quantises the float layer's weights when they are
@@ -338,6 +344,19 @@ class BaseQuantizeParallelLinear(ProcessGroupSafeDeepcopy, nn.Module, metaclass=
             return True
         return self.per_channel_axis == out_axis % len(self.weight_shape)
 
+    def _blockscaled_group(self) -> int:
+        """Size G of the K-blocks when the layer runs W8A8 on the block-scaled FP8 GEMM (block-wise e4m3 weight, dynamic
+        activations, G ∈ {32, 64, 128} dividing this rank's K so row-parallel shards keep whole blocks), else 0."""
+        if (self.quantization_type != QuantizationType.BLOCKWISE_SYMMETRIC
+                or self.activation_quantization_type != ActivationQuantizationType.DYNAMIC
+                or self.weight.dtype != torch.float8_e4m3fn or self.weight.dim() != 2 or self.mx_swizzle
+                or 1 not in self.block_axis):
+            return 0
+        G, K = self.block_size[self.block_axis.index(1)], self.weight.shape[1]
+        if G not in (32, 64, 128) or K % G or self.scale.dim() != 2 or self.scale.shape[1] != K // G:
+            return 0
+        return G
+
     def _linear_2d(self, x: torch.Tensor) -> torch.Tensor:
         """``x [..., K] @ weight[N, K]ᵀ`` with the layer's quantisation scheme; returns ``[..., N]`` in x's dtype class."""
         out_dtype = x.dtype if x.dtype in (torch.bfloat16, torch.float16, torch.float32) else self.dequantized_dtype
@@ -360,6 +379,12 @@ class BaseQuantizeParallelLinear(ProcessGroupSafeDeepcopy, nn.Module, metaclass=
                 return gemm_fp8.scaled_linear(xq, xs, self.weight, ws, out_dtype=out_dtype)
             y = torch.matmul(xq.float(), self.weight.float().t()) * xs.float() * ws.reshape(1, -1)
             return y.to(out_dtype)
+        G = self._blockscaled_group()
+        if G:
+            from ..ops import gemm_fp8
+
+            xq, xs = gemm_fp8.quantize_groups(x, G, "absmax", None if self.clamp_bound == float("inf") else self.clamp_bound)
+            return gemm_fp8.blockscaled_linear(xq, xs, self.weight, self.scale, G, out_dtype=out_dtype)
         if self._scale_is_output_only(0):
             y = torch.nn.functional.linear(x.to(out_dtype), direct_cast_dequantize(self.weight, out_dtype))
             return scale_dequantize(y, w_scale.reshape(1, -1) if w_scale.numel() > 1 else w_scale, out_dtype)
@@ -369,6 +394,9 @@ class BaseQuantizeParallelLinear(ProcessGroupSafeDeepcopy, nn.Module, metaclass=
             x2 = x.reshape(-1, x.shape[-1])
             if gemm_mx.gemv_eligible(x2.contiguous(), self.weight, self.scale):
                 # token generation on MX weights: decode the codes in registers, read 4.25 / 8.25 bits per weight
+                return gemm_mx.linear_mx(x, self.weight, self.scale).to(out_dtype)
+            if gemm_mx.gemm_mx_eligible(x2, self.weight, self.scale, gemm_mx.kind_of(self.weight)):
+                # prefill on MXFP8 weights (opt-in): MXFP8 activations and the block-scaled FP8 GEMM
                 return gemm_mx.linear_mx(x, self.weight, self.scale).to(out_dtype)
         return torch.nn.functional.linear(x.to(out_dtype), self._dequantized_weight(self.weight, self.scale, out_dtype))
 
