@@ -65,8 +65,10 @@ __global__ void __launch_bounds__(256) rmsnorm_fwd_kernel(const T* __restrict__ 
 // RMSNorm backward. Persistent CTAs stride over rows; each thread owns fixed columns so the
 // dW partial lives in registers across rows.  partial_dw: [gridDim.x, H] fp32.
 //   dx = rstd * (g*w - xhat * mean_H(g*w*xhat)),  dw = sum_rows g*xhat
+// Packets beyond the register cache (very wide rows) are re-read in the second pass and accumulate dW in place in the
+// CTA's own partial row, which no other CTA touches.
 // =====================================================================================
-template <typename T, int MAXV>
+template <typename T, int MAXV, bool WIDE>
 __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const T* __restrict__ g, const T* __restrict__ x,
                                                           const T* __restrict__ w, const float* __restrict__ rstd,
                                                           T* __restrict__ dx, float* __restrict__ partial_dw, int rows,
@@ -75,6 +77,7 @@ __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const T* __restrict__ 
   constexpr int N = P::N;
   __shared__ float red[32];
   const int nvec = H / N;
+  float* pdw = partial_dw + (size_t)blockIdx.x * H;
   float dw[MAXV][N];
   P pw[MAXV];
 #pragma unroll
@@ -84,6 +87,9 @@ __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const T* __restrict__ 
     for (int j = 0; j < N; ++j) dw[i][j] = 0.f;
     if (v < nvec) pw[i].load_nc(w + v * N);
   }
+  for (int v = threadIdx.x + MAXV * blockDim.x; WIDE && v < nvec; v += blockDim.x)
+#pragma unroll
+    for (int j = 0; j < N; ++j) pdw[v * N + j] = 0.f;
   for (int row = blockIdx.x; row < rows; row += gridDim.x) {
     const T* xr = x + (size_t)row * H;
     const T* gr = g + (size_t)row * H;
@@ -105,6 +111,11 @@ __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const T* __restrict__ 
         }
       }
     }
+    for (int v = threadIdx.x + MAXV * blockDim.x; WIDE && v < nvec; v += blockDim.x) {
+      P qx, qg, qw; qx.load(xr + v * N); qg.load(gr + v * N); qw.load_nc(w + v * N);
+#pragma unroll
+      for (int j = 0; j < N; ++j) { const float xh = qx.f(j) * rs; dot += qg.f(j) * qw.f(j) * xh; }
+    }
     dot = block_sum(dot, red) / (float)H;
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) {
@@ -119,14 +130,23 @@ __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const T* __restrict__ 
         po.store(dxr + v * N);
       }
     }
+    for (int v = threadIdx.x + MAXV * blockDim.x; WIDE && v < nvec; v += blockDim.x) {
+      P qx, qg, qw, po; qx.load(xr + v * N); qg.load(gr + v * N); qw.load_nc(w + v * N);
+#pragma unroll
+      for (int j = 0; j < N; ++j) {
+        const float xh = qx.f(j) * rs, gg = qg.f(j);
+        po.set(j, rs * (gg * qw.f(j) - xh * dot));
+        pdw[v * N + j] += gg * xh;
+      }
+      po.store(dxr + v * N);
+    }
   }
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
     const int v = threadIdx.x + i * blockDim.x;
     if (v < nvec) {
-      float* o = partial_dw + (size_t)blockIdx.x * H + v * N;
 #pragma unroll
-      for (int j = 0; j < N; ++j) o[j] = dw[i][j];
+      for (int j = 0; j < N; ++j) pdw[v * N + j] = dw[i][j];
     }
   }
 }
@@ -231,8 +251,10 @@ __global__ void __launch_bounds__(256) rope_kernel(const T* __restrict__ x, T* _
 // =====================================================================================
 // Cross-entropy statistics: per row (max, sum exp(x-max), target logit if owned, sum x).
 // One CTA per row; online softmax per thread then block merge.
+// VEC: rows are read as 16-byte packets, which needs a 16-byte aligned base and V % (16 / sizeof(T)) == 0 (every row
+// start aligned).  Otherwise the whole row goes through the element loop.
 // =====================================================================================
-template <typename T>
+template <typename T, bool VEC>
 __global__ void __launch_bounds__(256) ce_stats_kernel(const T* __restrict__ logits, const int64_t* __restrict__ target,
                                                        float* __restrict__ stats, int V, int vocab_start) {
   using P = Pack16<T>;
@@ -241,7 +263,7 @@ __global__ void __launch_bounds__(256) ce_stats_kernel(const T* __restrict__ log
   const int row = blockIdx.x;
   const T* xr = logits + (size_t)row * V;
   float m = -INFINITY, s = 0.f, sx = 0.f;
-  const int nvec = V / N;
+  const int nvec = VEC ? V / N : 0;
   for (int v = threadIdx.x; v < nvec; v += blockDim.x) {
     P p; p.load(xr + v * N);
     float lm = p.f(0);
@@ -254,7 +276,7 @@ __global__ void __launch_bounds__(256) ce_stats_kernel(const T* __restrict__ log
     s = s * __expf(m - nm) + acc;
     m = nm;
   }
-  for (int c = nvec * N + threadIdx.x; c < V; c += blockDim.x) {  // ragged tail
+  for (int c = nvec * N + threadIdx.x; c < V; c += blockDim.x) {  // ragged tail, or the whole row without VEC
     const float f = to_f32<T>(xr[c]);
     const float nm = fmaxf(m, f);
     s = s * __expf(m - nm) + __expf(f - nm);
@@ -272,7 +294,7 @@ __global__ void __launch_bounds__(256) ce_stats_kernel(const T* __restrict__ log
   }
 }
 
-template <typename T>
+template <typename T, bool VEC>
 __global__ void __launch_bounds__(256) ce_bwd_kernel(const T* __restrict__ logits, const int64_t* __restrict__ target,
                                                      const float* __restrict__ lse, const float* __restrict__ gout,
                                                      T* __restrict__ grad, int V, int vocab_start, float smoothing,
@@ -285,7 +307,7 @@ __global__ void __launch_bounds__(256) ce_bwd_kernel(const T* __restrict__ logit
   const float l = lse[row], g = gout[row];
   const long local = (long)target[row] - vocab_start;
   const float sm_term = smoothing * inv_vocab;
-  const int nvec = V / N;
+  const int nvec = VEC ? V / N : 0;
   for (int v = threadIdx.x; v < nvec; v += blockDim.x) {
     P p, o; p.load(xr + v * N);
 #pragma unroll
@@ -340,10 +362,13 @@ void rmsnorm_bwd(const void* g, const void* x, const void* w, const float* rstd,
                  int rows, int H, int dt, cudaStream_t st) {
   const int grid = rmsnorm_bwd_num_partials(rows);
   DISPATCH_DTYPE(dt, {
-    const int nvec = H / Pack16<T>::N;
-    if (H % Pack16<T>::N || nvec > 256 * 4) nxd_throw("rmsnorm_bwd: unsupported H", __FILE__, __LINE__);
+    if (H % Pack16<T>::N) nxd_throw("rmsnorm_bwd: H must be a multiple of the 16-byte vector width", __FILE__, __LINE__);
     const int th = pick_threads<T>(H);
-    rmsnorm_bwd_kernel<T, 4><<<grid, th, 0, st>>>((const T*)g, (const T*)x, (const T*)w, rstd, (T*)dx, partial, rows, H);
+    // the wide-row loops cost registers (one CTA per SM fewer), so rows that fit the register cache do not carry them
+    if (H / Pack16<T>::N > 4 * th)
+      rmsnorm_bwd_kernel<T, 4, true><<<grid, th, 0, st>>>((const T*)g, (const T*)x, (const T*)w, rstd, (T*)dx, partial, rows, H);
+    else
+      rmsnorm_bwd_kernel<T, 4, false><<<grid, th, 0, st>>>((const T*)g, (const T*)x, (const T*)w, rstd, (T*)dx, partial, rows, H);
   });
   reduce_partials_kernel<<<(H + 255) / 256, 256, 0, st>>>(partial, dw, grid, H);
   NXD_CUDA_CHECK(cudaGetLastError());
@@ -407,15 +432,19 @@ void rope_apply(const void* x, void* out, const float* cos_t, const float* sin_t
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 
+// Vocab shards need not be a multiple of the vector width (Llama-2-13B's 32016 over TP=4 is 8004 columns per rank;
+// BERT's 30522 and GPT-2's 50257 at any TP), and logits may be a view at any element offset.
+template <typename T> static bool ce_vec_ok(const void* p, int V) {
+  return (uintptr_t)p % 16 == 0 && V % Pack16<T>::N == 0;
+}
+
 void ce_stats(const void* logits, const int64_t* target, float* stats, int rows, int V, int vocab_start, int dt,
               cudaStream_t st) {
   DISPATCH_DTYPE(dt, {
-    if (((uintptr_t)logits % 16) || (V % Pack16<T>::N)) {
-      // rows would be misaligned for 16-byte loads → scalar path through the tail loop
-      ce_stats_kernel<T><<<rows, 256, 0, st>>>((const T*)logits, target, stats, V, vocab_start);
-    } else {
-      ce_stats_kernel<T><<<rows, 256, 0, st>>>((const T*)logits, target, stats, V, vocab_start);
-    }
+    if (ce_vec_ok<T>(logits, V))
+      ce_stats_kernel<T, true><<<rows, 256, 0, st>>>((const T*)logits, target, stats, V, vocab_start);
+    else
+      ce_stats_kernel<T, false><<<rows, 256, 0, st>>>((const T*)logits, target, stats, V, vocab_start);
   });
   NXD_CUDA_CHECK(cudaGetLastError());
 }
@@ -423,8 +452,12 @@ void ce_stats(const void* logits, const int64_t* target, float* stats, int rows,
 void ce_backward(const void* logits, const int64_t* target, const float* lse, const float* gout, void* grad, int rows,
                  int V, int vocab_start, float smoothing, int vocab, int dt, cudaStream_t st) {
   DISPATCH_DTYPE(dt, {
-    ce_bwd_kernel<T><<<rows, 256, 0, st>>>((const T*)logits, target, lse, gout, (T*)grad, V, vocab_start, smoothing,
-                                           1.f / (float)vocab);
+    if (ce_vec_ok<T>(logits, V) && ce_vec_ok<T>(grad, V))
+      ce_bwd_kernel<T, true><<<rows, 256, 0, st>>>((const T*)logits, target, lse, gout, (T*)grad, V, vocab_start,
+                                                   smoothing, 1.f / (float)vocab);
+    else
+      ce_bwd_kernel<T, false><<<rows, 256, 0, st>>>((const T*)logits, target, lse, gout, (T*)grad, V, vocab_start,
+                                                    smoothing, 1.f / (float)vocab);
   });
   NXD_CUDA_CHECK(cudaGetLastError());
 }

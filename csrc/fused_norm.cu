@@ -14,7 +14,7 @@
 
 namespace nxd {
 
-template <typename T, int MAXV>
+template <typename T, int MAXV, bool WIDE>
 __global__ void __launch_bounds__(256) add_rmsnorm_fwd_kernel(const T* __restrict__ x, const T* __restrict__ r,
                                                               const T* __restrict__ w, T* __restrict__ h,
                                                               T* __restrict__ y, float* __restrict__ rstd_out, int H,
@@ -43,6 +43,19 @@ __global__ void __launch_bounds__(256) add_rmsnorm_fwd_kernel(const T* __restric
       cache[i].store(h + base + v * N);
     }
   }
+  // tail beyond the register cache (very wide rows): h is re-read in the second pass, as rmsnorm_fwd_kernel re-reads x
+  for (int v = threadIdx.x + MAXV * blockDim.x; WIDE && v < nvec; v += blockDim.x) {
+    P px, pr, ph;
+    px.load(x + base + v * N);
+    pr.load(r + base + v * N);
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+      ph.set(j, px.f(j) + pr.f(j));
+      const float f = ph.f(j);
+      ss += f * f;
+    }
+    ph.store(h + base + v * N);
+  }
   ss = block_sum(ss, red);
   const float rstd = rsqrtf(ss / (float)H + eps);
   if (threadIdx.x == 0) rstd_out[row] = rstd;
@@ -57,10 +70,19 @@ __global__ void __launch_bounds__(256) add_rmsnorm_fwd_kernel(const T* __restric
       po.store(y + base + v * N);
     }
   }
+  for (int v = threadIdx.x + MAXV * blockDim.x; WIDE && v < nvec; v += blockDim.x) {
+    P ph, pw, po;
+    ph.load(h + base + v * N);
+    pw.load_nc(w + v * N);
+#pragma unroll
+    for (int j = 0; j < N; ++j) po.set(j, ph.f(j) * rstd * pw.f(j));
+    po.store(y + base + v * N);
+  }
 }
 
 // Persistent CTAs stride over rows; each thread owns fixed columns so the dW partial lives in registers across rows.
-template <typename T, int MAXV>
+// Packets beyond the register cache are re-read and accumulate dW in place in the CTA's own partial row.
+template <typename T, int MAXV, bool WIDE>
 __global__ void __launch_bounds__(256) add_rmsnorm_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ gh,
                                                               const T* __restrict__ h, const T* __restrict__ w,
                                                               const float* __restrict__ rstd, T* __restrict__ dh,
@@ -69,6 +91,7 @@ __global__ void __launch_bounds__(256) add_rmsnorm_bwd_kernel(const T* __restric
   constexpr int N = P::N;
   __shared__ float red[32];
   const int nvec = H / N;
+  float* pdw = partial_dw + (size_t)blockIdx.x * H;
   float dw[MAXV][N];
   P pw[MAXV];
 #pragma unroll
@@ -78,6 +101,9 @@ __global__ void __launch_bounds__(256) add_rmsnorm_bwd_kernel(const T* __restric
     for (int j = 0; j < N; ++j) dw[i][j] = 0.f;
     if (v < nvec) pw[i].load_nc(w + v * N);
   }
+  for (int v = threadIdx.x + MAXV * blockDim.x; WIDE && v < nvec; v += blockDim.x)
+#pragma unroll
+    for (int j = 0; j < N; ++j) pdw[v * N + j] = 0.f;
   for (int row = blockIdx.x; row < rows; row += gridDim.x) {
     const size_t base = (size_t)row * H;
     const float rs = rstd[row];
@@ -97,6 +123,11 @@ __global__ void __launch_bounds__(256) add_rmsnorm_bwd_kernel(const T* __restric
         }
       }
     }
+    for (int v = threadIdx.x + MAXV * blockDim.x; WIDE && v < nvec; v += blockDim.x) {
+      P qh, qg, qw; qh.load(h + base + v * N); qg.load(gy + base + v * N); qw.load_nc(w + v * N);
+#pragma unroll
+      for (int j = 0; j < N; ++j) { const float hh = qh.f(j) * rs; dot += qg.f(j) * qw.f(j) * hh; }
+    }
     dot = block_sum(dot, red) / (float)H;
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) {
@@ -112,14 +143,24 @@ __global__ void __launch_bounds__(256) add_rmsnorm_bwd_kernel(const T* __restric
         po.store(dh + base + v * N);
       }
     }
+    for (int v = threadIdx.x + MAXV * blockDim.x; WIDE && v < nvec; v += blockDim.x) {
+      P qh, qg, qw, pr, po;
+      qh.load(h + base + v * N); qg.load(gy + base + v * N); qw.load_nc(w + v * N); pr.load(gh + base + v * N);
+#pragma unroll
+      for (int j = 0; j < N; ++j) {
+        const float hh = qh.f(j) * rs, gg = qg.f(j);
+        po.set(j, pr.f(j) + rs * (gg * qw.f(j) - hh * dot));
+        pdw[v * N + j] += gg * hh;
+      }
+      po.store(dh + base + v * N);
+    }
   }
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
     const int v = threadIdx.x + i * blockDim.x;
     if (v < nvec) {
-      float* o = partial_dw + (size_t)blockIdx.x * H + v * N;
 #pragma unroll
-      for (int j = 0; j < N; ++j) o[j] = dw[i][j];
+      for (int j = 0; j < N; ++j) pdw[v * N + j] = dw[i][j];
     }
   }
 }
@@ -151,10 +192,13 @@ template <typename T> static int fn_pick_threads(int H) {
 void add_rmsnorm_fwd(const void* x, const void* r, const void* w, void* h, void* y, float* rstd, int rows, int H,
                      float eps, int dt, cudaStream_t st) {
   FN_DISPATCH_DTYPE(dt, {
-    const int nvec = H / Pack16<T>::N;
-    if (H % Pack16<T>::N || nvec > 256 * 4) nxd_throw("add_rmsnorm: unsupported H", __FILE__, __LINE__);
+    if (H % Pack16<T>::N) nxd_throw("add_rmsnorm: H must be a multiple of the 16-byte vector width", __FILE__, __LINE__);
     const int th = fn_pick_threads<T>(H);
-    add_rmsnorm_fwd_kernel<T, 4><<<rows, th, 0, st>>>((const T*)x, (const T*)r, (const T*)w, (T*)h, (T*)y, rstd, H, eps);
+    // the wide-row loops cost registers (one CTA per SM fewer), so rows that fit the register cache do not carry them
+    if (H / Pack16<T>::N > 4 * th)
+      add_rmsnorm_fwd_kernel<T, 4, true><<<rows, th, 0, st>>>((const T*)x, (const T*)r, (const T*)w, (T*)h, (T*)y, rstd, H, eps);
+    else
+      add_rmsnorm_fwd_kernel<T, 4, false><<<rows, th, 0, st>>>((const T*)x, (const T*)r, (const T*)w, (T*)h, (T*)y, rstd, H, eps);
   });
   NXD_CUDA_CHECK(cudaGetLastError());
 }
@@ -163,11 +207,15 @@ void add_rmsnorm_bwd(const void* gy, const void* gh, const void* h, const void* 
                      float* partial, float* dw, int rows, int H, int dt, cudaStream_t st) {
   const int grid = rmsnorm_bwd_num_partials(rows);
   FN_DISPATCH_DTYPE(dt, {
-    const int nvec = H / Pack16<T>::N;
-    if (H % Pack16<T>::N || nvec > 256 * 4) nxd_throw("add_rmsnorm_bwd: unsupported H", __FILE__, __LINE__);
+    if (H % Pack16<T>::N) nxd_throw("add_rmsnorm_bwd: H must be a multiple of the 16-byte vector width", __FILE__, __LINE__);
     const int th = fn_pick_threads<T>(H);
-    add_rmsnorm_bwd_kernel<T, 4><<<grid, th, 0, st>>>((const T*)gy, (const T*)gh, (const T*)h, (const T*)w, rstd, (T*)dh,
-                                                     partial, rows, H);
+    // the wide-row loops cost registers (one CTA per SM fewer), so rows that fit the register cache do not carry them
+    if (H / Pack16<T>::N > 4 * th)
+      add_rmsnorm_bwd_kernel<T, 4, true><<<grid, th, 0, st>>>((const T*)gy, (const T*)gh, (const T*)h, (const T*)w, rstd,
+                                                              (T*)dh, partial, rows, H);
+    else
+      add_rmsnorm_bwd_kernel<T, 4, false><<<grid, th, 0, st>>>((const T*)gy, (const T*)gh, (const T*)h, (const T*)w, rstd,
+                                                               (T*)dh, partial, rows, H);
   });
   fused_norm_reduce_partials_kernel<<<(H + 255) / 256, 256, 0, st>>>(partial, dw, grid, H);
   NXD_CUDA_CHECK(cudaGetLastError());
