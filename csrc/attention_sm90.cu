@@ -1,4 +1,4 @@
-// Flash attention for sm_90a (head_dim 128, bf16): warp-level bf16 tensor-core MMAs (mma.sync m16n8k16, ldmatrix operand
+// Flash attention for sm_90a (head_dim 64, 80, 96 or 128, bf16): warp-level bf16 tensor-core MMAs (mma.sync m16n8k16, ldmatrix operand
 // loads from padded shared memory, cp.async double-buffered tiles), fp32 online softmax.  Role parity: reference
 // kernels/flash_attn.py:162-212 (nki_flash_attn_func → flash_fwd / flash_attn_bwd) and modules/attention call sites.
 //
@@ -11,7 +11,14 @@
 //          Sᵀ = K·Qᵀ, Pᵀ = exp(Sᵀ − LSE), dV += Pᵀ·dO, dPᵀ = V·dOᵀ, dSᵀ = Pᵀ∘(dPᵀ − δ), dK += dSᵀ·Q
 //   dQ     one CTA per (64-query tile, head, batch), loops over the key tiles: S, P, dP = dO·Vᵀ, dS, dQ += dS·K
 //   Every gradient element is owned by one thread of one CTA (no atomics), so the backward is bit-reproducible.
+// Every kernel is a template on the head dimension HD; the tile shapes (64 query / key rows) are the same for all of them.
+// Optional key-padding mask (template flag MASK, uint8 [B, S_kv], key j of batch b visible iff mask[b, j] != 0): a masked
+// key is treated like a key past S_kv, so it contributes nothing and its dK / dV are exactly 0.  The forward and dQ kernels
+// stage each key tile's 64 flags in shared memory next to K / V; a dK/dV thread owns two fixed key rows and reads their
+// flags once.  A query row that sees no key gets O = 0, LSE = −inf and dQ = 0.
 #include <cuda.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -19,14 +26,16 @@
 namespace nxd {
 namespace fa {
 
-constexpr int HD = 128;
 constexpr int BT = 64;                       // rows of a query or key tile
 constexpr int kThreads = 128;
-constexpr int LDS = HD + 8;                  // padded shared-memory row (elements): 272 B, ldmatrix rows hit distinct banks
-constexpr int kTile = BT * LDS;              // elements of one staged tile
-constexpr int kSmemFwd = 5 * kTile * 2;                      // Q, K×2, V×2
-constexpr int kSmemDkv = 6 * kTile * 2 + 4 * BT * 4;         // K, V, Q×2, dO×2, LSE×2, δ×2
-constexpr int kSmemDq = 6 * kTile * 2;                       // Q, dO, K×2, V×2
+// padded shared-memory row (elements): 144 / 176 / 208 / 272 B for HD = 64 / 80 / 96 / 128.  Each stride is 16 B more than
+// a multiple of 32 B, so the 8 row addresses of one ldmatrix 8x8 matrix start in distinct 4-bank groups (conflict-free).
+template <int HD> constexpr int LDS = HD + 8;
+template <int HD> constexpr int kTile = BT * LDS<HD>;              // elements of one staged tile
+template <int HD> constexpr int kSmemFwd = 5 * kTile<HD> * 2;                      // Q, K×2, V×2
+template <int HD> constexpr int kSmemDkv = 6 * kTile<HD> * 2 + 4 * BT * 4;         // K, V, Q×2, dO×2, LSE×2, δ×2
+template <int HD> constexpr int kSmemDq = 6 * kTile<HD> * 2;                       // Q, dO, K×2, V×2
+constexpr int kSmemFlags = 2 * BT;                                                 // key-mask flags ×2 (MASK kernels)
 constexpr float kLog2e = 1.4426950408889634f;
 
 typedef __nv_bfloat16 bf16;
@@ -48,11 +57,23 @@ template <int N>
 NXD_DEVICE void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // rows [s0, s0+64) of one (batch, head) slice → padded shared tile; rows ≥ S are zero-filled
+template <int HD>
 NXD_DEVICE void load_tile(bf16* sm, const bf16* base, long ss, int s0, int S) {
-  for (int i = threadIdx.x; i < BT * (HD / 8); i += kThreads) {
-    const int r = i >> 4, c = i & 15;
+  constexpr int kChunks = HD / 8;                                   // 16-byte chunks per row
+  constexpr bool kPow2 = (kChunks & (kChunks - 1)) == 0;
+  for (int i = threadIdx.x; i < BT * kChunks; i += kThreads) {
+    const int r = kPow2 ? i >> (kChunks == 16 ? 4 : 3) : i / kChunks, c = kPow2 ? i & (kChunks - 1) : i % kChunks;
     const bool ok = s0 + r < S;
-    cp_async16(sm + r * LDS + c * 8, base + (long)(ok ? s0 + r : 0) * ss + c * 8, ok);
+    cp_async16(sm + r * LDS<HD> + c * 8, base + (long)(ok ? s0 + r : 0) * ss + c * 8, ok);
+  }
+}
+
+// visibility flags of keys [s0, s0+64) (1 = visible; keys ≥ S are 0) → shared memory.  Plain loads: the mask row has no
+// alignment guarantee.  Read after the next __syncthreads.
+NXD_DEVICE void load_flags(uint8_t* sm, const uint8_t* mask, int s0, int S) {
+  if (threadIdx.x < BT) {
+    const int s = s0 + threadIdx.x;
+    sm[threadIdx.x] = s < S && mask[s] != 0;
   }
 }
 
@@ -70,8 +91,9 @@ NXD_DEVICE void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uin
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// C[16 x 64] = A[16 rows from a_row0][128] · Bᵀ where B is a 64-row tile, both with the 128-long k dimension contiguous
+// C[16 x 64] = A[16 rows from a_row0][HD] · Bᵀ where B is a 64-row tile, both with the HD-long k dimension contiguous
 // (QKᵀ, KQᵀ, VdOᵀ, dOVᵀ).  C fragment j holds columns 8j..8j+7: c0,c1 row lane/4, c2,c3 row lane/4+8, columns 2(lane%4)+{0,1}.
+template <int HD>
 NXD_DEVICE void mma_abt(float (&c)[8][4], const bf16* sa, int a_row0, const bf16* sb) {
   const int lane = threadIdx.x & 31;
 #pragma unroll
@@ -79,27 +101,28 @@ NXD_DEVICE void mma_abt(float (&c)[8][4], const bf16* sa, int a_row0, const bf16
 #pragma unroll
   for (int ks = 0; ks < HD / 16; ++ks) {
     uint32_t a[4];
-    ldsm_x4(a, sa + (a_row0 + (lane & 15)) * LDS + ks * 16 + (lane >> 4) * 8);
+    ldsm_x4(a, sa + (a_row0 + (lane & 15)) * LDS<HD> + ks * 16 + (lane >> 4) * 8);
 #pragma unroll
     for (int jp = 0; jp < 4; ++jp) {
       uint32_t b[4];
-      ldsm_x4(b, sb + (jp * 16 + (lane & 7) + (lane >> 4) * 8) * LDS + ks * 16 + ((lane >> 3) & 1) * 8);
+      ldsm_x4(b, sb + (jp * 16 + (lane & 7) + (lane >> 4) * 8) * LDS<HD> + ks * 16 + ((lane >> 3) & 1) * 8);
       mma16816(c[2 * jp], a, b[0], b[1]);
       mma16816(c[2 * jp + 1], a, b[2], b[3]);
     }
   }
 }
 
-// C[16 x 128] += P[16 x 64] · B where P comes as bf16 A fragments (4 k-steps) and B is a 64-row tile with the 128-wide
+// C[16 x HD] += P[16 x 64] · B where P comes as bf16 A fragments (4 k-steps) and B is a 64-row tile with the HD-wide
 // output dimension contiguous (P·V, Pᵀ·dO, dSᵀ·Q, dS·K).
-NXD_DEVICE void mma_pb(float (&c)[16][4], const uint32_t (&p)[4][4], const bf16* sb) {
+template <int HD>
+NXD_DEVICE void mma_pb(float (&c)[HD / 8][4], const uint32_t (&p)[4][4], const bf16* sb) {
   const int lane = threadIdx.x & 31;
 #pragma unroll
   for (int ks = 0; ks < BT / 16; ++ks) {
 #pragma unroll
     for (int dp = 0; dp < HD / 16; ++dp) {
       uint32_t b[4];
-      ldsm_x4_t(b, sb + (ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * LDS + dp * 16 + (lane >> 4) * 8);
+      ldsm_x4_t(b, sb + (ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * LDS<HD> + dp * 16 + (lane >> 4) * 8);
       mma16816(c[2 * dp], p[ks], b[0], b[1]);
       mma16816(c[2 * dp + 1], p[ks], b[2], b[3]);
     }
@@ -117,12 +140,13 @@ NXD_DEVICE void to_a_frags(const float (&c)[8][4], uint32_t (&p)[4][4]) {
   }
 }
 
-// 16 x 128 fp32 fragments (rows row0 + lane/4 and +8) × scale → bf16 rows of a [B,S,H,128] view
-NXD_DEVICE void store_rows(const float (&c)[16][4], bf16* base, long ss, int row0, int S, float scale0, float scale1) {
+// 16 x HD fp32 fragments (rows row0 + lane/4 and +8) × scale → bf16 rows of a [B,S,H,HD] view
+template <int HD>
+NXD_DEVICE void store_rows(const float (&c)[HD / 8][4], bf16* base, long ss, int row0, int S, float scale0, float scale1) {
   const int lane = threadIdx.x & 31;
   const int r0 = row0 + (lane >> 2), r1 = r0 + 8;
 #pragma unroll
-  for (int dt = 0; dt < 16; ++dt) {
+  for (int dt = 0; dt < HD / 8; ++dt) {
     const int d = dt * 8 + 2 * (lane & 3);
     if (r0 < S) *(uint32_t*)(base + (long)r0 * ss + d) = pack_bf16(c[dt][0] * scale0, c[dt][1] * scale0);
     if (r1 < S) *(uint32_t*)(base + (long)r1 * ss + d) = pack_bf16(c[dt][2] * scale1, c[dt][3] * scale1);
@@ -135,13 +159,17 @@ struct FwdParams {
   float* lse;
   int B, H, Hkv, S_q, S_kv, causal;
   float scale_log2;
+  const uint8_t* mask; long mask_sb;            // key-padding mask [B, S_kv] (MASK kernels only)
 };
 
+template <int HD, bool MASK>
 __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
+  constexpr int kTl = kTile<HD>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   bf16* sQ = (bf16*)smem_raw;
-  bf16* sK = sQ + kTile;        // 2 buffers
-  bf16* sV = sK + 2 * kTile;    // 2 buffers
+  bf16* sK = sQ + kTl;          // 2 buffers
+  bf16* sV = sK + 2 * kTl;      // 2 buffers
+  uint8_t* sM = (uint8_t*)(sV + 2 * kTl);       // 2 × 64 key flags (MASK)
   // causal: the last query tiles see the most keys, so they are scheduled first
   const int qt = gridDim.x - 1 - blockIdx.x, h = blockIdx.y, b = blockIdx.z, hk = h / (p.H / p.Hkv);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -149,32 +177,36 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
   const bf16* qb = p.q.p + b * p.q.sb + h * p.q.sh;
   const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
+  const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
   const int n_kv = p.causal ? min((p.S_kv + BT - 1) / BT, qt + 1) : (p.S_kv + BT - 1) / BT;
 
-  load_tile(sQ, qb, p.q.ss, q0, p.S_q);
-  load_tile(sK, kb, p.k.ss, 0, p.S_kv);
-  load_tile(sV, vb, p.v.ss, 0, p.S_kv);
+  load_tile<HD>(sQ, qb, p.q.ss, q0, p.S_q);
+  load_tile<HD>(sK, kb, p.k.ss, 0, p.S_kv);
+  load_tile<HD>(sV, vb, p.v.ss, 0, p.S_kv);
   cp_async_commit();
+  if (MASK) load_flags(sM, mb, 0, p.S_kv);
 
-  float o[16][4];
+  float o[HD / 8][4];
 #pragma unroll
-  for (int i = 0; i < 16; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  for (int i = 0; i < HD / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const int row[2] = {q0 + warp * 16 + (lane >> 2), q0 + warp * 16 + (lane >> 2) + 8};
 
   for (int t = 0; t < n_kv; ++t) {
     const int buf = t & 1;
     if (t + 1 < n_kv) {
-      load_tile(sK + (buf ^ 1) * kTile, kb, p.k.ss, (t + 1) * BT, p.S_kv);
-      load_tile(sV + (buf ^ 1) * kTile, vb, p.v.ss, (t + 1) * BT, p.S_kv);
+      load_tile<HD>(sK + (buf ^ 1) * kTl, kb, p.k.ss, (t + 1) * BT, p.S_kv);
+      load_tile<HD>(sV + (buf ^ 1) * kTl, vb, p.v.ss, (t + 1) * BT, p.S_kv);
       cp_async_commit();
+      if (MASK) load_flags(sM + (buf ^ 1) * BT, mb, (t + 1) * BT, p.S_kv);
       cp_async_wait<1>();
     } else {
       cp_async_wait<0>();
     }
     __syncthreads();
+    const uint8_t* fl = sM + buf * BT;
     float s[8][4];
-    mma_abt(s, sQ, warp * 16, sK + buf * kTile);
+    mma_abt<HD>(s, sQ, warp * 16, sK + buf * kTl);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -182,7 +214,7 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
       for (int e = 0; e < 4; ++e) {
         const int key = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
         float x = s[j][e] * p.scale_log2;
-        if (key >= p.S_kv || (p.causal && key > row[e >> 1])) x = -INFINITY;
+        if (key >= p.S_kv || (p.causal && key > row[e >> 1]) || (MASK && !fl[j * 8 + 2 * (lane & 3) + (e & 1)])) x = -INFINITY;
         s[j][e] = x;
         mx[e >> 1] = fmaxf(mx[e >> 1], x);
       }
@@ -209,10 +241,10 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
 #pragma unroll
     for (int r = 0; r < 2; ++r) l[r] = l[r] * alpha[r] + rs[r];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) { o[i][0] *= alpha[0]; o[i][1] *= alpha[0]; o[i][2] *= alpha[1]; o[i][3] *= alpha[1]; }
+    for (int i = 0; i < HD / 8; ++i) { o[i][0] *= alpha[0]; o[i][1] *= alpha[0]; o[i][2] *= alpha[1]; o[i][3] *= alpha[1]; }
     uint32_t pf[4][4];
     to_a_frags(s, pf);
-    mma_pb(o, pf, sV + buf * kTile);
+    mma_pb<HD>(o, pf, sV + buf * kTl);
     __syncthreads();                              // buffer `buf` is refilled at the next iteration
   }
   float inv[2];
@@ -222,7 +254,7 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
     l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
     inv[r] = l[r] > 0.f ? 1.f / l[r] : 0.f;
   }
-  store_rows(o, p.o + b * p.o_sb + h * p.o_sh, p.o_ss, q0 + warp * 16, p.S_q, inv[0], inv[1]);
+  store_rows<HD>(o, p.o + b * p.o_sb + h * p.o_sh, p.o_ss, q0 + warp * 16, p.S_q, inv[0], inv[1]);
   if ((lane & 3) == 0) {
 #pragma unroll
     for (int r = 0; r < 2; ++r)
@@ -231,7 +263,8 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
   }
 }
 
-// δ[b,h,s] = Σ_d dO·O − dLSE   (one warp per query row)
+// δ[b,h,s] = Σ_d dO·O − dLSE   (one warp per query row; lane i reads elements 4i..4i+3, lanes past HD/4 read nothing)
+template <int HD>
 __global__ void fa_bwd_prep_kernel(const bf16* __restrict__ o, const bf16* __restrict__ go, const float* __restrict__ dlse,
                                    float* __restrict__ delta, int B, int S, int H, long o_sb, long o_ss, long o_sh, long g_sb,
                                    long g_ss, long g_sh) {
@@ -239,15 +272,17 @@ __global__ void fa_bwd_prep_kernel(const bf16* __restrict__ o, const bf16* __res
   const int lane = threadIdx.x & 31;
   if (w >= (long)B * H * S) return;
   const int s = (int)(w % S), h = (int)((w / S) % H), b = (int)(w / ((long)S * H));
-  const uint2 ov = *(const uint2*)(o + b * o_sb + s * o_ss + h * o_sh + lane * 4);
-  const uint2 gv = *(const uint2*)(go + b * g_sb + s * g_ss + h * g_sh + lane * 4);
-  const __nv_bfloat162* oh = (const __nv_bfloat162*)&ov;
-  const __nv_bfloat162* gh = (const __nv_bfloat162*)&gv;
   float acc = 0.f;
+  if (HD == 128 || lane < HD / 4) {
+    const uint2 ov = *(const uint2*)(o + b * o_sb + s * o_ss + h * o_sh + lane * 4);
+    const uint2 gv = *(const uint2*)(go + b * g_sb + s * g_ss + h * g_sh + lane * 4);
+    const __nv_bfloat162* oh = (const __nv_bfloat162*)&ov;
+    const __nv_bfloat162* gh = (const __nv_bfloat162*)&gv;
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const float2 a = __bfloat1622float2(oh[j]), c = __bfloat1622float2(gh[j]);
-    acc += a.x * c.x + a.y * c.y;
+    for (int j = 0; j < 2; ++j) {
+      const float2 a = __bfloat1622float2(oh[j]), c = __bfloat1622float2(gh[j]);
+      acc += a.x * c.x + a.y * c.y;
+    }
   }
 #pragma unroll
   for (int off = 16; off; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
@@ -262,15 +297,18 @@ struct BwdParams {
   const float *lse, *delta;
   int B, H, Hkv, S_q, S_kv, causal;
   float scale, scale_log2;
+  const uint8_t* mask; long mask_sb;            // key-padding mask [B, S_kv] (MASK kernels only)
 };
 
+template <int HD, bool MASK>
 __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParams p) {
+  constexpr int kTl = kTile<HD>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   bf16* sK = (bf16*)smem_raw;
-  bf16* sV = sK + kTile;
-  bf16* sQ = sV + kTile;        // 2 buffers
-  bf16* sG = sQ + 2 * kTile;    // 2 buffers
-  float* sL = (float*)(sG + 2 * kTile);   // 2 × 64 LSE (log2 units)
+  bf16* sV = sK + kTl;
+  bf16* sQ = sV + kTl;          // 2 buffers
+  bf16* sG = sQ + 2 * kTl;      // 2 buffers
+  float* sL = (float*)(sG + 2 * kTl);     // 2 × 64 LSE (log2 units)
   float* sD = sL + 2 * BT;                // 2 × 64 δ
   const int kt = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
   const int G = p.H / p.Hkv;
@@ -281,12 +319,12 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
   const int per_head = n_qt > qt0 ? n_qt - qt0 : 0;
   const int n_it = G * per_head;
 
-  load_tile(sK, p.k.p + b * p.k.sb + hk * p.k.sh, p.k.ss, k0, p.S_kv);
-  load_tile(sV, p.v.p + b * p.v.sb + hk * p.v.sh, p.v.ss, k0, p.S_kv);
+  load_tile<HD>(sK, p.k.p + b * p.k.sb + hk * p.k.sh, p.k.ss, k0, p.S_kv);
+  load_tile<HD>(sV, p.v.p + b * p.v.sb + hk * p.v.sh, p.v.ss, k0, p.S_kv);
   auto issue = [&](int it, int buf) {
     const int h = hk * G + it / per_head, q0 = (qt0 + it % per_head) * BT;
-    load_tile(sQ + buf * kTile, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
-    load_tile(sG + buf * kTile, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
+    load_tile<HD>(sQ + buf * kTl, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
+    load_tile<HD>(sG + buf * kTl, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
     if (threadIdx.x < BT) {
       const int s = q0 + threadIdx.x;
       const long i = ((long)b * p.H + h) * p.S_q + s;
@@ -297,13 +335,18 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
   if (n_it > 0) issue(0, 0);
   cp_async_commit();
 
-  float dk[16][4], dv[16][4];
+  float dk[HD / 8][4], dv[HD / 8][4];
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < HD / 8; ++i) {
     dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = 0.f;
     dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f;
   }
   const int key[2] = {k0 + warp * 16 + (lane >> 2), k0 + warp * 16 + (lane >> 2) + 8};
+  bool kvis[2] = {true, true};                       // this thread's two key rows are not masked
+  if (MASK) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) kvis[r] = key[r] < p.S_kv && p.mask[b * p.mask_sb + key[r]] != 0;
+  }
 
   for (int it = 0; it < n_it; ++it) {
     const int buf = it & 1;
@@ -316,27 +359,27 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
       cp_async_wait<0>();
     }
     __syncthreads();
-    const bf16* q = sQ + buf * kTile;
-    const bf16* g = sG + buf * kTile;
+    const bf16* q = sQ + buf * kTl;
+    const bf16* g = sG + buf * kTl;
     const float* L = sL + buf * BT;
     const float* D = sD + buf * BT;
     float pt[8][4];
-    mma_abt(pt, sK, warp * 16, q);                   // Sᵀ: rows = keys, columns = queries
+    mma_abt<HD>(pt, sK, warp * 16, q);               // Sᵀ: rows = keys, columns = queries
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int qc = j * 8 + 2 * (lane & 3) + (e & 1);
         const int qi = q0 + qc;
-        const bool vis = qi < p.S_q && !(p.causal && key[e >> 1] > qi);
+        const bool vis = qi < p.S_q && !(p.causal && key[e >> 1] > qi) && (!MASK || kvis[e >> 1]);
         pt[j][e] = vis ? exp2f(pt[j][e] * p.scale_log2 - L[qc]) : 0.f;
       }
     }
     uint32_t pf[4][4];
     to_a_frags(pt, pf);
-    mma_pb(dv, pf, g);                               // dV += Pᵀ·dO
+    mma_pb<HD>(dv, pf, g);                           // dV += Pᵀ·dO
     float dpt[8][4];
-    mma_abt(dpt, sV, warp * 16, g);                  // dPᵀ = V·dOᵀ
+    mma_abt<HD>(dpt, sV, warp * 16, g);              // dPᵀ = V·dOᵀ
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
@@ -346,32 +389,41 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
       }
     }
     to_a_frags(dpt, pf);
-    mma_pb(dk, pf, q);                               // dK += dSᵀ·Q
+    mma_pb<HD>(dk, pf, q);                           // dK += dSᵀ·Q
     __syncthreads();
   }
-  store_rows(dk, p.dk + b * p.dk_sb + hk * p.dk_sh, p.dk_ss, k0 + warp * 16, p.S_kv, p.scale, p.scale);
-  store_rows(dv, p.dv + b * p.dv_sb + hk * p.dv_sh, p.dv_ss, k0 + warp * 16, p.S_kv, 1.f, 1.f);
+  store_rows<HD>(dk, p.dk + b * p.dk_sb + hk * p.dk_sh, p.dk_ss, k0 + warp * 16, p.S_kv, p.scale, p.scale);
+  store_rows<HD>(dv, p.dv + b * p.dv_sb + hk * p.dv_sh, p.dv_ss, k0 + warp * 16, p.S_kv, 1.f, 1.f);
 }
 
-__global__ void __launch_bounds__(kThreads) fa_bwd_dq_kernel(const BwdParams p) {
+// CTAs per SM the dQ kernel is compiled for (0: no bound).  Left to itself ptxas spills at HD = 80 / 96, and at 64 with the
+// mask, to reach an occupancy the shared memory does not allow (Q, dO, K×2, V×2 tiles: 54 / 66 / 78 / 102 KB).
+template <int HD, bool MASK> constexpr int kDqMinBlocks = HD == 64 ? (MASK ? 3 : 4) : HD == 128 ? 0 : 2;
+
+template <int HD, bool MASK>
+__global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK>)) fa_bwd_dq_kernel(const BwdParams p) {
+  constexpr int kTl = kTile<HD>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   bf16* sQ = (bf16*)smem_raw;
-  bf16* sG = sQ + kTile;
-  bf16* sK = sG + kTile;        // 2 buffers
-  bf16* sV = sK + 2 * kTile;    // 2 buffers
+  bf16* sG = sQ + kTl;
+  bf16* sK = sG + kTl;          // 2 buffers
+  bf16* sV = sK + 2 * kTl;      // 2 buffers
+  uint8_t* sM = (uint8_t*)(sV + 2 * kTl);       // 2 × 64 key flags (MASK)
   // causal: the last query tiles see the most keys, so they are scheduled first
   const int qt = gridDim.x - 1 - blockIdx.x, h = blockIdx.y, b = blockIdx.z, hk = h / (p.H / p.Hkv);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = qt * BT;
   const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
+  const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
   const int n_kv = p.causal ? min((p.S_kv + BT - 1) / BT, qt + 1) : (p.S_kv + BT - 1) / BT;
 
-  load_tile(sQ, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
-  load_tile(sG, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
-  load_tile(sK, kb, p.k.ss, 0, p.S_kv);
-  load_tile(sV, vb, p.v.ss, 0, p.S_kv);
+  load_tile<HD>(sQ, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
+  load_tile<HD>(sG, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
+  load_tile<HD>(sK, kb, p.k.ss, 0, p.S_kv);
+  load_tile<HD>(sV, vb, p.v.ss, 0, p.S_kv);
   cp_async_commit();
+  if (MASK) load_flags(sM, mb, 0, p.S_kv);
 
   const int row[2] = {q0 + warp * 16 + (lane >> 2), q0 + warp * 16 + (lane >> 2) + 8};
   float L[2], D[2];
@@ -381,36 +433,38 @@ __global__ void __launch_bounds__(kThreads) fa_bwd_dq_kernel(const BwdParams p) 
     L[r] = row[r] < p.S_q ? p.lse[i] * kLog2e : 0.f;
     D[r] = row[r] < p.S_q ? p.delta[i] : 0.f;
   }
-  float dq[16][4];
+  float dq[HD / 8][4];
 #pragma unroll
-  for (int i = 0; i < 16; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
+  for (int i = 0; i < HD / 8; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
 
   for (int t = 0; t < n_kv; ++t) {
     const int buf = t & 1;
     if (t + 1 < n_kv) {
-      load_tile(sK + (buf ^ 1) * kTile, kb, p.k.ss, (t + 1) * BT, p.S_kv);
-      load_tile(sV + (buf ^ 1) * kTile, vb, p.v.ss, (t + 1) * BT, p.S_kv);
+      load_tile<HD>(sK + (buf ^ 1) * kTl, kb, p.k.ss, (t + 1) * BT, p.S_kv);
+      load_tile<HD>(sV + (buf ^ 1) * kTl, vb, p.v.ss, (t + 1) * BT, p.S_kv);
       cp_async_commit();
+      if (MASK) load_flags(sM + (buf ^ 1) * BT, mb, (t + 1) * BT, p.S_kv);
       cp_async_wait<1>();
     } else {
       cp_async_wait<0>();
     }
     __syncthreads();
-    const bf16* k = sK + buf * kTile;
+    const bf16* k = sK + buf * kTl;
+    const uint8_t* fl = sM + buf * BT;
     float s[8][4];
-    mma_abt(s, sQ, warp * 16, k);
+    mma_abt<HD>(s, sQ, warp * 16, k);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int kc = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
         const int r = row[e >> 1];
-        const bool vis = kc < p.S_kv && r < p.S_q && !(p.causal && kc > r);
+        const bool vis = kc < p.S_kv && r < p.S_q && !(p.causal && kc > r) && (!MASK || fl[j * 8 + 2 * (lane & 3) + (e & 1)]);
         s[j][e] = vis ? exp2f(s[j][e] * p.scale_log2 - L[e >> 1]) : 0.f;
       }
     }
     float dp[8][4];
-    mma_abt(dp, sG, warp * 16, sV + buf * kTile);    // dP = dO·Vᵀ
+    mma_abt<HD>(dp, sG, warp * 16, sV + buf * kTl);  // dP = dO·Vᵀ
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
@@ -418,10 +472,10 @@ __global__ void __launch_bounds__(kThreads) fa_bwd_dq_kernel(const BwdParams p) 
     }
     uint32_t pf[4][4];
     to_a_frags(dp, pf);
-    mma_pb(dq, pf, k);                               // dQ += dS·K
+    mma_pb<HD>(dq, pf, k);                           // dQ += dS·K
     __syncthreads();
   }
-  store_rows(dq, p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, q0 + warp * 16, p.S_q, p.scale, p.scale);
+  store_rows<HD>(dq, p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, q0 + warp * 16, p.S_q, p.scale, p.scale);
 }
 
 static View view(const void* ptr, const long* s) {
@@ -430,11 +484,51 @@ static View view(const void* ptr, const long* s) {
   return View{(const bf16*)ptr, s[0], s[1], s[2]};
 }
 
+// f(std::integral_constant<int, HD>, std::integral_constant<bool, MASK>) for the runtime head dimension and mask flag
+template <class F>
+static void dispatch(int D, bool mask, F&& f) {
+  auto with_mask = [&](auto hd) {
+    if (mask) f(hd, std::true_type{});
+    else f(hd, std::false_type{});
+  };
+  switch (D) {
+    case 64: with_mask(std::integral_constant<int, 64>{}); break;
+    case 80: with_mask(std::integral_constant<int, 80>{}); break;
+    case 96: with_mask(std::integral_constant<int, 96>{}); break;
+    case 128: with_mask(std::integral_constant<int, 128>{}); break;
+    default: nxd_throw("attention: head_dim must be 64, 80, 96 or 128", __FILE__, __LINE__);
+  }
+}
+
+template <int HD, bool MASK>
+static void launch_fwd(const FwdParams& p, cudaStream_t st) {
+  constexpr int smem = kSmemFwd<HD> + (MASK ? kSmemFlags : 0);
+  static bool configured = false;
+  if (!configured) {
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_fwd_kernel<HD, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = true;
+  }
+  fa_fwd_kernel<HD, MASK><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem, st>>>(p);
+}
+
+template <int HD, bool MASK>
+static void launch_bwd(const BwdParams& p, cudaStream_t st) {
+  constexpr int smem_dkv = kSmemDkv<HD>, smem_dq = kSmemDq<HD> + (MASK ? kSmemFlags : 0);
+  static bool configured = false;
+  if (!configured) {
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dkdv_kernel<HD, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dkv));
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dq_kernel<HD, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dq));
+    configured = true;
+  }
+  fa_bwd_dkdv_kernel<HD, MASK><<<dim3((p.S_kv + BT - 1) / BT, p.Hkv, p.B), kThreads, smem_dkv, st>>>(p);
+  fa_bwd_dq_kernel<HD, MASK><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem_dq, st>>>(p);
+}
+
 }  // namespace fa
 
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
-                    int Hkv, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    cudaStream_t st) {
+                    int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
+                    const void* kpm, long kpm_sb, cudaStream_t st) {
   using namespace fa;
   if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
   FwdParams p;
@@ -443,26 +537,18 @@ void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, floa
   p.lse = lse;
   p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
   p.scale_log2 = scale * kLog2e;
-  static bool configured = false;
-  if (!configured) {
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemFwd));
-    configured = true;
-  }
-  fa_fwd_kernel<<<dim3((S_q + BT - 1) / BT, H, B), kThreads, kSmemFwd, st>>>(p);
+  p.mask = (const uint8_t*)kpm; p.mask_sb = kpm_sb;
+  dispatch(D, kpm != nullptr, [&](auto hd, auto mk) { launch_fwd<decltype(hd)::value, decltype(mk)::value>(p, st); });
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 
 void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
-                    const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
-                    const long* dks, const long* dvs, float scale, bool causal, cudaStream_t st) {
+                    int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
+                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb,
+                    cudaStream_t st) {
   using namespace fa;
   if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
-  {
-    const long rows = (long)B * H * S_q;
-    fa_bwd_prep_kernel<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(
-        (const bf16*)o, (const bf16*)go, dlse, delta, B, S_q, H, os[0], os[1], os[2], gs[0], gs[1], gs[2]);
-  }
   BwdParams p;
   p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs); p.g = view(go, gs);
   p.dq = (bf16*)dq; p.dk = (bf16*)dk; p.dv = (bf16*)dv;
@@ -472,14 +558,14 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
   p.lse = lse; p.delta = delta;
   p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
   p.scale = scale; p.scale_log2 = scale * kLog2e;
-  static bool configured = false;
-  if (!configured) {
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dkdv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemDkv));
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemDq));
-    configured = true;
-  }
-  fa_bwd_dkdv_kernel<<<dim3((S_kv + BT - 1) / BT, Hkv, B), kThreads, kSmemDkv, st>>>(p);
-  fa_bwd_dq_kernel<<<dim3((S_q + BT - 1) / BT, H, B), kThreads, kSmemDq, st>>>(p);
+  p.mask = (const uint8_t*)kpm; p.mask_sb = kpm_sb;
+  dispatch(D, kpm != nullptr, [&](auto hd, auto mk) {
+    constexpr int HD = decltype(hd)::value;
+    const long rows = (long)B * H * S_q;
+    fa_bwd_prep_kernel<HD><<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(
+        (const bf16*)o, (const bf16*)go, dlse, delta, B, S_q, H, os[0], os[1], os[2], gs[0], gs[1], gs[2]);
+    launch_bwd<HD, decltype(mk)::value>(p, st);
+  });
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 

@@ -439,34 +439,55 @@ static void grouped_wgrad(const Tensor& x, const Tensor& dy, Tensor out, const T
 
 // ---- attention ----------------------------------------------------------------------------------
 static void check_qkv(const Tensor& t, const char* name) {
-  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kBFloat16 && t.dim() == 4 && t.size(3) == 128 && t.stride(3) == 1,
-              name, ": expected a bf16 CUDA [B,S,H,128] view with contiguous head_dim");
+  const int64_t d = t.dim() == 4 ? t.size(3) : 0;
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kBFloat16 && t.dim() == 4 && (d == 64 || d == 80 || d == 96 || d == 128) &&
+                  t.stride(3) == 1,
+              name, ": expected a bf16 CUDA [B,S,H,D] view with D in {64, 80, 96, 128} and contiguous head_dim");
+}
+// optional key-padding mask [B, S_kv] (bool / uint8, key visible iff nonzero) → (data, batch stride), or null
+static const void* check_kpm(const c10::optional<Tensor>& m, const Tensor& q, int64_t B, int64_t Skv, long* sb) {
+  *sb = 0;
+  if (!m.has_value()) return nullptr;
+  TORCH_CHECK(m->scalar_type() == at::kBool || m->scalar_type() == at::kByte, "key_padding_mask: expected bool or uint8");
+  TORCH_CHECK(m->dim() == 2 && m->size(0) == B && m->size(1) == Skv, "key_padding_mask: expected shape [B, S_kv] = [", B, ", ",
+              Skv, "], got ", m->sizes());
+  TORCH_CHECK(m->size(1) <= 1 || m->stride(1) == 1, "key_padding_mask: the key dimension must be contiguous");
+  TORCH_CHECK(m->device() == q.device(), "key_padding_mask: expected it on ", q.device(), ", got ", m->device());
+  *sb = m->stride(0);
+  return m->data_ptr();
 }
 // returns (out [B,S,H,D] view — memory laid out [S,B,H,D] when sbhd_out —, lse [B,H,S] fp32)
 static std::vector<Tensor> flash_attn_fwd(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
-                                          bool sbhd_out) {
+                                          bool sbhd_out, const c10::optional<Tensor>& key_padding_mask) {
   check_qkv(q, "q"); check_qkv(k, "k"); check_qkv(v, "v");
-  const int B = q.size(0), S = q.size(1), H = q.size(2), Skv = k.size(1), Hkv = k.size(2);
+  const int B = q.size(0), S = q.size(1), H = q.size(2), D = q.size(3), Skv = k.size(1), Hkv = k.size(2);
   TORCH_CHECK(k.size(0) == B && v.size(0) == B && v.size(1) == Skv && v.size(2) == Hkv && H % Hkv == 0);
+  TORCH_CHECK(k.size(3) == D && v.size(3) == D, "q, k and v must have the same head_dim");
+  long kpm_sb;
+  const void* kpm = check_kpm(key_padding_mask, q, B, Skv, &kpm_sb);
   c10::cuda::CUDAGuard guard(q.device());
-  Tensor out = sbhd_out ? at::empty({S, B, H, 128}, q.options()).transpose(0, 1) : at::empty({B, S, H, 128}, q.options());
+  Tensor out = sbhd_out ? at::empty({S, B, H, D}, q.options()).transpose(0, 1) : at::empty({B, S, H, D}, q.options());
   Tensor lse = at::empty({B, H, S}, q.options().dtype(at::kFloat));
   const long qs[3] = {q.stride(0), q.stride(1), q.stride(2)}, ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   const long vs[3] = {v.stride(0), v.stride(1), v.stride(2)}, os[3] = {out.stride(0), out.stride(1), out.stride(2)};
-  nxd::flash_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, Skv, H, Hkv,
-                      qs, ks, vs, os, (float)scale, causal, stream());
+  nxd::flash_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, Skv, H, Hkv, D,
+                      qs, ks, vs, os, (float)scale, causal, kpm, kpm_sb, stream());
   return {out, lse};
 }
 
 static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& o,
                                           const Tensor& lse, bool causal, double scale, bool sbhd_out,
-                                          const c10::optional<Tensor>& dlse) {
+                                          const c10::optional<Tensor>& dlse, const c10::optional<Tensor>& key_padding_mask) {
   check_qkv(q, "q"); check_qkv(k, "k"); check_qkv(v, "v"); check_qkv(go, "grad_out"); check_qkv(o, "out");
-  const int B = q.size(0), S = q.size(1), H = q.size(2), Skv = k.size(1), Hkv = k.size(2);
+  const int B = q.size(0), S = q.size(1), H = q.size(2), D = q.size(3), Skv = k.size(1), Hkv = k.size(2);
+  TORCH_CHECK(k.size(3) == D && v.size(3) == D && go.size(3) == D && o.size(3) == D,
+              "q, k, v, out and grad_out must have the same head_dim");
   TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * H * S);
+  long kpm_sb;
+  const void* kpm = check_kpm(key_padding_mask, q, B, Skv, &kpm_sb);
   c10::cuda::CUDAGuard guard(q.device());
   auto mk = [&](int s, int h) {
-    return sbhd_out ? at::empty({s, B, h, 128}, q.options()).transpose(0, 1) : at::empty({B, s, h, 128}, q.options());
+    return sbhd_out ? at::empty({s, B, h, D}, q.options()).transpose(0, 1) : at::empty({B, s, h, D}, q.options());
   };
   Tensor dq = mk(S, H), dk = mk(Skv, Hkv), dv = mk(Skv, Hkv);
   Tensor delta = at::empty({B, H, S}, q.options().dtype(at::kFloat));
@@ -479,8 +500,8 @@ static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, con
     dlse_p = dlse->data_ptr<float>();
   }
   nxd::flash_attn_bwd(go.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), dlse_p,
-                      dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr<float>(), B, S, Skv, H, Hkv, gs, qs, ks,
-                      vs, os, dqs, dks, dvs, (float)scale, causal, stream());
+                      dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr<float>(), B, S, Skv, H, Hkv, D, gs, qs, ks,
+                      vs, os, dqs, dks, dvs, (float)scale, causal, kpm, kpm_sb, stream());
   return {dq, dk, dv};
 }
 
@@ -757,9 +778,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("quantize_fp8_groups", &quantize_fp8_groups);
   m.def("grouped_gemm", &grouped_gemm);
   m.def("grouped_wgrad", &grouped_wgrad);
-  m.def("flash_attn_fwd", &flash_attn_fwd);
+  m.def("flash_attn_fwd", &flash_attn_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("causal"), py::arg("scale"),
+        py::arg("sbhd_out"), py::arg("key_padding_mask") = py::none());
   m.def("flash_attn_bwd", &flash_attn_bwd, py::arg("go"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"), py::arg("lse"),
-        py::arg("causal"), py::arg("scale"), py::arg("sbhd_out"), py::arg("dlse") = py::none());
+        py::arg("causal"), py::arg("scale"), py::arg("sbhd_out"), py::arg("dlse") = py::none(),
+        py::arg("key_padding_mask") = py::none());
   m.def("ag_gemm_bf16", &ag_gemm_bf16);
   m.def("gemm_rs_bf16", &gemm_rs_bf16);
   m.def("zero1_reduce_scatter", &zero1_reduce_scatter);

@@ -139,15 +139,17 @@ void decode_rope_kv(const void* q, const void* k, const void* v, const long* pos
                     long v_sb, long v_sh, long c_sb, long c_ss, long c_sh, cudaStream_t st);
 void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, cudaStream_t st);
 
-// ---- attention (attention_sm90.cu): q [B,S_q,H,128], k/v [B,S_kv,Hkv,128] bf16 views; strides = (b, s, h) in elements
+// ---- attention (attention_sm90.cu): q [B,S_q,H,D], k/v [B,S_kv,Hkv,D] bf16 views, D ∈ {64, 80, 96, 128}; strides = (b, s, h)
+// in elements.  kpm: optional key-padding mask, uint8 [B, S_kv] with row stride kpm_sb (key visible iff nonzero), or null.
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
-                    int Hkv, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    cudaStream_t st);
+                    int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
+                    const void* kpm, long kpm_sb, cudaStream_t st);
 
 // delta: fp32 scratch [B, H, S_q]; dlse may be null
 void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
-                    const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
-                    const long* dks, const long* dvs, float scale, bool causal, cudaStream_t st);
+                    int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
+                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb,
+                    cudaStream_t st);
 
 }  // namespace nxd

@@ -7,8 +7,8 @@ Layout convention of ``nki_flash_attn_func`` (same as the reference):
 * ``transpose_nki_inputs=False`` — ``q``, ``k``, ``v`` are all ``[B, H, S, D]``.
 
 The result is ``[B, H, S, D]`` in both cases.  The math runs in ``ops.attention.flash_attention`` (own forward /
-backward kernels for head_dim 128 bf16, library flash attention otherwise), which wants ``[B, S, H, D]`` *views* — the
-transposes below are stride changes consumed by strided TMA descriptors, not copies."""
+backward kernels for bf16 with head_dim 64, 80, 96 or 128, library flash attention otherwise), which wants ``[B, S, H, D]``
+*views* — the transposes below are stride changes consumed by strided TMA descriptors, not copies."""
 from __future__ import annotations
 
 from typing import Optional

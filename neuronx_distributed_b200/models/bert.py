@@ -11,6 +11,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+from .. import ops
 from ..parallel_layers import parallel_state as ps
 from ..parallel_layers.layer_norm import LayerNorm
 from ..parallel_layers.layers import ColumnParallelLinear, ParallelEmbedding, RowParallelLinear
@@ -72,11 +73,11 @@ class BertSelfAttention(nn.Module):
         self.dense = RowParallelLinear(cfg.hidden_size, cfg.hidden_size, bias=True, input_is_parallel=True,
                                        init_method=_init(cfg.initializer_range), dtype=cfg.dtype, device=cfg.device)
 
-    def forward(self, x, attn_bias):
+    def forward(self, x, key_padding_mask):
         B, S, _ = x.shape
-        q, k, v = (lin(x).view(B, S, self.heads_local, self.head_dim).transpose(1, 2) for lin in (self.query, self.key, self.value))
-        o = F.scaled_dot_product_attention(q, k, v, attn_mask=attn_bias)        # bidirectional + padding mask
-        return self.dense(o.transpose(1, 2).reshape(B, S, self.heads_local * self.head_dim))
+        q, k, v = (lin(x).view(B, S, self.heads_local, self.head_dim) for lin in (self.query, self.key, self.value))
+        o = ops.attention.flash_attention(q, k, v, causal=False, key_padding_mask=key_padding_mask)   # bidirectional
+        return self.dense(o.reshape(B, S, self.heads_local * self.head_dim))
 
 
 class BertLayer(nn.Module):
@@ -91,8 +92,8 @@ class BertLayer(nn.Module):
         self.output_norm = LayerNorm(cfg.hidden_size, cfg.layer_norm_eps, dtype=cfg.dtype, device=cfg.device)
         self.dropout = nn.Dropout(cfg.hidden_dropout_prob)
 
-    def forward(self, x, attn_bias):
-        x = self.attention_norm(x + self.dropout(self.attention(x, attn_bias)))          # post-LN, as in BERT
+    def forward(self, x, key_padding_mask):
+        x = self.attention_norm(x + self.dropout(self.attention(x, key_padding_mask)))   # post-LN, as in BERT
         return self.output_norm(x + self.dropout(self.output(F.gelu(self.intermediate(x)))))
 
 
@@ -106,12 +107,9 @@ class BertModel(nn.Module):
 
     def forward(self, input_ids, token_type_ids=None, attention_mask=None):
         x = self.embeddings(input_ids, token_type_ids)
-        bias = None
-        if attention_mask is not None:
-            bias = torch.zeros(attention_mask.shape, dtype=x.dtype, device=x.device).masked_fill(attention_mask == 0, float("-inf"))
-            bias = bias[:, None, None, :]
+        key_padding_mask = attention_mask != 0 if attention_mask is not None else None     # [B, S], True = real token
         for layer in self.layers:
-            x = layer(x, bias)
+            x = layer(x, key_padding_mask)
         return x, torch.tanh(self.pooler(x[:, 0]))
 
 

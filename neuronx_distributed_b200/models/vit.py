@@ -10,6 +10,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+from .. import ops
 from ..parallel_layers import parallel_state as ps
 from ..parallel_layers.layer_norm import LayerNorm
 from ..parallel_layers.layers import ColumnParallelLinear, OutputChannelParallelConv2d, RowParallelLinear
@@ -67,8 +68,8 @@ class ViTLayer(nn.Module):
     def forward(self, x):
         B, N, _ = x.shape
         q, k, v = self.qkv(self.layernorm_before(x)).chunk(3, dim=-1)
-        q, k, v = (t.reshape(B, N, self.heads_local, self.head_dim).transpose(1, 2) for t in (q, k, v))
-        a = F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(B, N, self.heads_local * self.head_dim)
+        q, k, v = (t.reshape(B, N, self.heads_local, self.head_dim) for t in (q, k, v))
+        a = ops.attention.flash_attention(q, k, v, causal=False).reshape(B, N, self.heads_local * self.head_dim)
         x = x + self.out(a)
         return x + self.fc2(F.gelu(self.fc1(self.layernorm_after(x))))
 

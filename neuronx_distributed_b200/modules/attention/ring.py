@@ -9,7 +9,7 @@ mask, a block that originated on a *later* rank is skipped, the local block is c
 H100 design: the ring transfer is an NCCL p2p exchange issued *before* the block's attention so it overlaps the
 compute; the exchange is itself an autograd node (its backward moves dK/dV the opposite way round the ring), so
 backward is the exact transpose of forward without a hand-written second pass.  Per-block attention is the own
-flash kernel with a differentiable LSE output (``ops.attention.flash_attention_with_lse``; head_dim 128, bf16), the SDPA
+flash kernel with a differentiable LSE output (``ops.attention.flash_attention_with_lse``; head_dim 64/80/96/128, bf16), the SDPA
 flash op for other shapes on CUDA, and an fp32 reference on CPU.
 """
 from __future__ import annotations
@@ -121,9 +121,8 @@ def _block_backward(q, k, v, out, lse, dout, causal: bool, scale: float):
     if q.is_cuda:
         from ... import ops
 
-        e = ops._ext.ext()
-        if (e is not None and hasattr(e, "flash_attn_bwd") and q.dtype == torch.bfloat16 and q.shape[-1] == 128
-                and (not causal or q.shape[1] == k.shape[1])):
+        if ops.attention.flash_kernels_apply(q, k, v) and (not causal or q.shape[1] == k.shape[1]):
+            e = ops._ext.ext()
             ops._ext.count_launch(4)
             tv = ops.attention._tma_view
             dq, dk, dv = e.flash_attn_bwd(tv(dout.to(out.dtype)), tv(q), tv(k), tv(v), tv(out), lse.contiguous(), bool(causal),

@@ -1,7 +1,7 @@
-"""Causal self-attention (flash style).  Kernel: ``csrc/attention_sm90.cu`` (tensor-core QK^T / PV with
-register accumulators, online softmax) when built; otherwise the PyTorch SDPA library call, which is
-flagged as a *library* path in DESIGN.md.  Reference call sites: ``kernels/flash_attn.py:162-212``
-(``nki_flash_attn_func``), ``modeling_llama_nxd.py:468-475``.
+"""Self-attention (flash style), causal or not, with an optional key-padding mask.  Kernel: ``csrc/attention_sm90.cu``
+(tensor-core QK^T / PV with register accumulators, online softmax) for bf16 CUDA tensors with head_dim 64, 80, 96 or 128;
+otherwise the PyTorch SDPA library call, which is flagged as a *library* path in DESIGN.md.  Reference call sites:
+``kernels/flash_attn.py:162-212`` (``nki_flash_attn_func``), ``modeling_llama_nxd.py:468-475``.
 
 Layout: q ``[B, S, Hq, D]``, k/v ``[B, S, Hkv, D]`` → out ``[B, S, Hq, D]``.
 """
@@ -17,24 +17,50 @@ import torch.nn.functional as F
 from . import _ext
 
 
-def _sdpa(q, k, v, causal: bool, scale: Optional[float]):
+#: head sizes the flash kernels are compiled for
+FLASH_HEAD_DIMS = (64, 80, 96, 128)
+
+
+def _sdpa(q, k, v, causal: bool, scale: Optional[float], key_padding_mask: Optional[torch.Tensor] = None):
     hq, hkv = q.shape[2], k.shape[2]
     qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
     if hq != hkv:
         kt = kt.repeat_interleave(hq // hkv, dim=1)
         vt = vt.repeat_interleave(hq // hkv, dim=1)
-    o = F.scaled_dot_product_attention(qt, kt, vt, is_causal=causal, scale=scale)
+    if key_padding_mask is None:
+        o = F.scaled_dot_product_attention(qt, kt, vt, is_causal=causal, scale=scale)
+    else:
+        # additive bias [B, 1, 1 or S_q, S_kv]: 0 where visible, −inf where masked (or above the diagonal when causal)
+        visible = key_padding_mask.bool()[:, None, None, :]
+        if causal:
+            sq, sk = q.shape[1], k.shape[1]
+            visible = visible & torch.ones(sq, sk, dtype=torch.bool, device=q.device).tril()
+        bias = torch.zeros(visible.shape, dtype=q.dtype, device=q.device).masked_fill(~visible, float("-inf"))
+        o = F.scaled_dot_product_attention(qt, kt, vt, attn_mask=bias, scale=scale)
     return o.transpose(1, 2)
 
 
-def _own_kernel_ok(q, k, v) -> bool:
+def flash_kernels_apply(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor) -> bool:
+    """True when the own flash kernels handle these tensors: bf16 CUDA, 4-D ``[B, S, H, D]`` with D in
+    :data:`FLASH_HEAD_DIMS` (the same for q, k and v), and the extension loaded.  ``NXD_DISABLE_OWN_ATTENTION=1`` turns
+    them off (the SDPA path is then used, e.g. as a comparison baseline)."""
     if os.environ.get("NXD_DISABLE_OWN_ATTENTION", "0") == "1":
         return False
     if not (q.is_cuda and q.dtype == torch.bfloat16 and k.dtype == torch.bfloat16 and v.dtype == torch.bfloat16
-            and q.shape[-1] == 128 and q.dim() == 4):
+            and q.dim() == 4 and k.dim() == 4 and v.dim() == 4 and q.shape[-1] in FLASH_HEAD_DIMS
+            and k.shape[-1] == q.shape[-1] and v.shape[-1] == q.shape[-1]):
         return False
     e = _ext.ext()
-    return e is not None and hasattr(e, "flash_attn_fwd")
+    return e is not None and hasattr(e, "flash_attn_fwd") and hasattr(e, "flash_attn_bwd")
+
+
+def _kernel_mask(m: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """Key-padding mask as the kernels read it: bool / uint8 ``[B, S_kv]`` with a contiguous key dimension."""
+    if m is None:
+        return None
+    if m.dtype not in (torch.bool, torch.uint8):
+        m = m != 0
+    return m if m.stride(-1) == 1 else m.contiguous()
 
 
 def _tma_view(t: torch.Tensor) -> torch.Tensor:
@@ -52,22 +78,22 @@ class _FlashAttn(torch.autograd.Function):
     model's ``[S,B,H·D]`` reshape is free."""
 
     @staticmethod
-    def forward(ctx, q, k, v, causal, scale):
+    def forward(ctx, q, k, v, causal, scale, mask=None):
         e = _ext.ext()
         q, k, v = _tma_view(q), _tma_view(k), _tma_view(v)
         _ext.count_launch()
-        o, lse = e.flash_attn_fwd(q, k, v, bool(causal), float(scale), True)
-        ctx.save_for_backward(q, k, v, o, lse)
+        o, lse = e.flash_attn_fwd(q, k, v, bool(causal), float(scale), True, mask)
+        ctx.save_for_backward(q, k, v, o, lse, mask)
         ctx.causal, ctx.scale = causal, scale
         return o
 
     @staticmethod
     def backward(ctx, go):
-        q, k, v, o, lse = ctx.saved_tensors
+        q, k, v, o, lse, mask = ctx.saved_tensors
         e = _ext.ext()
         _ext.count_launch(3)   # δ prep + dK/dV + dQ
-        dq, dk, dv = e.flash_attn_bwd(_tma_view(go), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale), True)
-        return dq, dk, dv, None, None
+        dq, dk, dv = e.flash_attn_bwd(_tma_view(go), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale), True, None, mask)
+        return dq, dk, dv, None, None, None
 
 
 class _FlashAttnLse(torch.autograd.Function):
@@ -95,17 +121,26 @@ class _FlashAttnLse(torch.autograd.Function):
 
 def flash_attention_with_lse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool, scale: float):
     """``(out [B,S,H,D], lse [B,H,S] fp32)`` on the own kernels, or ``None`` when they do not apply."""
-    if _own_kernel_ok(q, k, v) and (not causal or q.shape[1] == k.shape[1]) and hasattr(_ext.ext(), "flash_attn_bwd"):
+    if flash_kernels_apply(q, k, v) and (not causal or q.shape[1] == k.shape[1]):
         return _FlashAttnLse.apply(q, k, v, causal, scale)
     return None
 
 
 def flash_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True,
-                    scale: Optional[float] = None) -> torch.Tensor:
+                    scale: Optional[float] = None, key_padding_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """softmax(q·kᵀ·scale)·v for q ``[B, S_q, H, D]``, k/v ``[B, S_kv, Hkv, D]`` (H a multiple of Hkv) → ``[B, S_q, H, D]``.
+
+    ``causal``: query i sees keys ≤ i (needs S_q == S_kv on the own kernels).  ``key_padding_mask``: ``[B, S_kv]`` bool
+    (or integer, nonzero = visible); key j of batch b is visible iff ``key_padding_mask[b, j]``.  It combines with
+    ``causal`` and GQA and is never read on the host, so the call stays capturable in CUDA graphs and launch plans.
+
+    On the own kernels a masked key contributes nothing and gets dK = dV = 0, and a query row that sees no key at all gets
+    O = 0 and dQ = 0.  The SDPA fallback (CPU, other dtypes or head sizes) follows SDPA's rule for such a row, which is NaN
+    on some SDPA backends and versions."""
     scale = scale if scale is not None else 1.0 / math.sqrt(q.shape[-1])
-    if _own_kernel_ok(q, k, v) and (not causal or q.shape[1] == k.shape[1]):
-        return _FlashAttn.apply(q, k, v, causal, scale)
-    return _sdpa(q, k, v, causal, scale)
+    if flash_kernels_apply(q, k, v) and (not causal or q.shape[1] == k.shape[1]):
+        return _FlashAttn.apply(q, k, v, causal, scale, _kernel_mask(key_padding_mask))
+    return _sdpa(q, k, v, causal, scale, key_padding_mask)
 
 
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, positions: torch.Tensor,

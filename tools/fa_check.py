@@ -1,9 +1,15 @@
 """Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
-usage: python tools/fa_check.py [--perf] [--bwd]"""
+usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd]
+
+--perf times forward and forward+backward of the own kernels and of SDPA in the same process, alternating, at the shapes
+the models run (BERT-large with right padding, ViT-B/16, GPT-NeoX-20B per rank at TP=8, Pythia-2.8B, Llama-2-7B).  FLOPs
+come from the shapes: 4·D per visible (query, key) pair forward, 2.5× that backward; causal counts only the lower
+triangle and a key-padding mask only the visible keys."""
 import argparse
 import json
 import math
 import os
+import subprocess
 import sys
 
 import torch
@@ -12,8 +18,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from neuronx_distributed_b200.ops import _ext, attention  # noqa: E402
 
 
-def ref_attn(q, k, v, causal, scale):
-    # q [B,S,H,D] fp32 math
+def ref_attn(q, k, v, causal, scale, mask=None):
+    # q [B,S,H,D] fp32 math; mask: optional key-padding mask [B, S_kv] (True = visible, no fully masked row)
     B, S, H, D = q.shape
     Hkv = k.shape[2]
     qf, kf, vf = q.float().transpose(1, 2), k.float().transpose(1, 2), v.float().transpose(1, 2)
@@ -24,8 +30,89 @@ def ref_attn(q, k, v, causal, scale):
     if causal:
         m = torch.ones(S, k.shape[1], device=q.device, dtype=torch.bool).tril()
         s = s.masked_fill(~m, float("-inf"))
+    if mask is not None:
+        s = s.masked_fill(~mask[:, None, None, :], float("-inf"))
     p = s.softmax(-1)
     return (p @ vf).transpose(1, 2), torch.logsumexp(s, -1)
+
+
+def gpu_info():
+    """Name, power limit and max SM clock of the GPU the numbers are measured on (read in the same run)."""
+    info = {"gpu": torch.cuda.get_device_name()}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader",
+                              "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
+        info["power_limit"], info["max_sm_clock"] = (x.strip() for x in out.strip().split(","))
+    except Exception as ex:  # noqa: BLE001 - the record still has the device name
+        info["power_limit"] = f"unavailable ({type(ex).__name__})"
+    return info
+
+
+# name, B, S, H, D, causal, padded fraction of the keys (right padding, per-sequence lengths drawn around it)
+PERF_SHAPES = [
+    ("bert_large", 32, 512, 16, 64, False, 0.15),
+    ("vit_b16", 64, 197, 12, 64, False, 0.0),
+    ("neox20b_tp8", 1, 2048, 8, 96, True, 0.0),
+    ("pythia2.8b", 4, 2048, 32, 80, True, 0.0),
+    ("llama2_7b", 4, 4096, 32, 128, True, 0.0),
+]
+
+
+def perf(e, bwd: bool):
+    dev = torch.device("cuda")
+    print(json.dumps(gpu_info()), flush=True)
+    g = torch.Generator(device=dev).manual_seed(0)
+    for (name, B, S, H, D, causal, pad) in PERF_SHAPES:
+        q, k, v, go = (torch.randn(B, S, H, D, device=dev, generator=g).bfloat16() for _ in range(4))
+        scale = 1.0 / math.sqrt(D)
+        mask = None
+        if pad > 0:
+            lens = (S * (1.0 - 2 * pad * torch.rand(B, device=dev, generator=g))).long().clamp(1, S)
+            mask = torch.arange(S, device=dev)[None, :] < lens[:, None]
+        vis_keys = mask.sum(1).double() if mask is not None else torch.full((B,), float(S), device=dev, dtype=torch.float64)
+        pairs = float((vis_keys * ((S + 1) / 2 if causal else S)).sum()) * H      # visible (query, key) pairs
+        fl = 4 * D * pairs
+        qt, kt, vt, gt = (t.transpose(1, 2) for t in (q, k, v, go))
+        bias = None
+        if mask is not None:                        # the additive bias the models pass to SDPA
+            bias = torch.zeros(B, 1, 1, S, device=dev, dtype=q.dtype).masked_fill(~mask[:, None, None, :], float("-inf"))
+
+        def own_f():
+            return e.flash_attn_fwd(q, k, v, causal, scale, True, mask)
+
+        def sdpa_f(qq=qt, kk=kt, vv=vt):
+            if bias is None:
+                return torch.nn.functional.scaled_dot_product_attention(qq, kk, vv, is_causal=causal)
+            return torch.nn.functional.scaled_dot_product_attention(qq, kk, vv, attn_mask=bias)
+
+        qr, kr, vr = (t.detach().requires_grad_(True) for t in (qt, kt, vt))
+
+        def own_fb():
+            o, lse = own_f()
+            e.flash_attn_bwd(go, q, k, v, o, lse, causal, scale, True, None, mask)
+
+        def sdpa_fb():
+            torch.autograd.grad(sdpa_f(qr, kr, vr), (qr, kr, vr), gt)
+
+        # alternate own / SDPA three times and keep each one's best, so drift of the shared clock hits both alike
+        t = {"own_fwd": [], "sdpa_fwd": [], "own_fwd_bwd": [], "sdpa_fwd_bwd": []}
+        for _ in range(3):
+            t["own_fwd"].append(time_fn(own_f))
+            t["sdpa_fwd"].append(time_fn(sdpa_f))
+            if bwd:
+                t["own_fwd_bwd"].append(time_fn(own_fb))
+                t["sdpa_fwd_bwd"].append(time_fn(sdpa_fb))
+        rec = {"bench": name, "B": B, "S": S, "H": H, "D": D, "causal": causal, "visible_key_frac": round(float(vis_keys.sum()) / (B * S), 3)}
+        for key, vals in t.items():
+            if not vals:
+                continue
+            ms = min(vals)
+            tf = (3.5 if "bwd" in key else 1.0) * fl / ms / 1e9
+            rec[key + "_ms"], rec[key + "_tflops"] = round(ms, 4), round(tf, 1)
+        rec["own_vs_sdpa_fwd"] = round(rec["sdpa_fwd_ms"] / rec["own_fwd_ms"], 2)
+        if bwd:
+            rec["own_vs_sdpa_fwd_bwd"] = round(rec["sdpa_fwd_bwd_ms"] / rec["own_fwd_bwd_ms"], 2)
+        print(json.dumps(rec), flush=True)
 
 
 def time_fn(fn, iters=20):
@@ -45,17 +132,19 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--perf", action="store_true")
     ap.add_argument("--bwd", action="store_true")
+    ap.add_argument("--head-dim", type=int, default=128, choices=attention.FLASH_HEAD_DIMS)
     a = ap.parse_args()
     dev = torch.device("cuda")
     e = _ext.ext()
     ok_all = True
     torch.manual_seed(0)
-    cases = [  # B, S, H, Hkv, causal, layout
-        (1, 128, 1, 1, False, "bshd"), (1, 256, 2, 2, True, "bshd"), (2, 512, 4, 2, True, "sbhd"),
-        (2, 384, 4, 4, False, "bhsd"), (1, 1024, 8, 8, True, "fused"), (2, 200, 2, 1, True, "bshd"),
+    cases = [  # B, S, H, Hkv, causal, layout, masked (right padding)
+        (1, 128, 1, 1, False, "bshd", False), (1, 256, 2, 2, True, "bshd", False), (2, 512, 4, 2, True, "sbhd", False),
+        (2, 384, 4, 4, False, "bhsd", False), (1, 1024, 8, 8, True, "fused", False), (2, 200, 2, 1, True, "bshd", False),
+        (3, 300, 4, 2, False, "bshd", True), (3, 300, 4, 2, True, "sbhd", True),
     ]
-    for (B, S, H, Hkv, causal, layout) in cases:
-        D = 128
+    for (B, S, H, Hkv, causal, layout, masked) in cases:
+        D = a.head_dim
         if layout == "bshd":
             q = torch.randn(B, S, H, D, device=dev).bfloat16(); k = torch.randn(B, S, Hkv, D, device=dev).bfloat16()
             v = torch.randn(B, S, Hkv, D, device=dev).bfloat16()
@@ -74,48 +163,33 @@ def main():
             v = f[..., (H + Hkv) * D:].view(S, B, Hkv, D).transpose(0, 1)
         q = q * 2.0      # larger logits → exercises the lazy rescale
         scale = 1.0 / math.sqrt(D)
-        o, lse = e.flash_attn_fwd(q, k, v, causal, scale, True)
-        ro, rl = ref_attn(q, k, v, causal, scale)
+        mask = None
+        if masked:   # right padding; each row keeps at least its first key, so causal rows are never empty
+            lens = torch.tensor([S, S - 77, 1][:B], device=dev)
+            mask = torch.arange(S, device=dev)[None, :] < lens[:, None]
+        o, lse = e.flash_attn_fwd(q, k, v, causal, scale, True, mask)
+        ro, rl = ref_attn(q, k, v, causal, scale, mask)
         err = (o.float() - ro).abs().max().item() / ro.abs().max().item()
         lerr = (lse - rl).abs().max().item()
         ok = err < 2e-2 and lerr < 2e-2 and bool(torch.isfinite(o.float()).all())
         ok_all &= ok
-        print(json.dumps({"check": f"fa_fwd_B{B}_S{S}_H{H}_{Hkv}_{'c' if causal else 'f'}_{layout}", "ok": ok,
+        tag = f"D{D}_B{B}_S{S}_H{H}_{Hkv}_{'c' if causal else 'f'}_{layout}{'_masked' if masked else ''}"
+        print(json.dumps({"check": f"fa_fwd_{tag}", "ok": ok,
                           "err": round(err, 5), "lse_err": round(lerr, 5)}), flush=True)
         if a.bwd and hasattr(e, "flash_attn_bwd"):
             go = torch.randn_like(o)
             qq, kk, vv = (t.detach().float().requires_grad_(True) for t in (q, k, v))
-            r2, _ = ref_attn(qq, kk, vv, causal, scale)
+            r2, _ = ref_attn(qq, kk, vv, causal, scale, mask)
             r2.backward(go.float())
-            dq, dk, dv = e.flash_attn_bwd(go, q, k, v, o, lse, causal, scale, True)
+            dq, dk, dv = e.flash_attn_bwd(go, q, k, v, o, lse, causal, scale, True, None, mask)
             res = {}
             for n, g, r in (("dq", dq, qq.grad), ("dk", dk, kk.grad), ("dv", dv, vv.grad)):
                 res[n] = round((g.float() - r).abs().max().item() / r.abs().max().item(), 5)
             ok = all(x < 3e-2 for x in res.values())
             ok_all &= ok
-            print(json.dumps({"check": f"fa_bwd_B{B}_S{S}_H{H}_{Hkv}_{'c' if causal else 'f'}_{layout}", "ok": ok, **res}), flush=True)
+            print(json.dumps({"check": f"fa_bwd_{tag}", "ok": ok, **res}), flush=True)
     if a.perf:
-        for (B, S, H) in ((4, 4096, 32), (1, 8192, 32), (8, 2048, 32)):
-            D = 128
-            q, k, v = (torch.randn(B, S, H, D, device=dev).bfloat16() for _ in range(3))
-            scale = 1.0 / math.sqrt(D)
-            fl = 4 * B * H * S * S * D / 2
-            t_own = time_fn(lambda: e.flash_attn_fwd(q, k, v, True, scale, True))
-            qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
-            t_lib = time_fn(lambda: torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, is_causal=True))
-            rec = {"bench": f"fa_fwd_B{B}_S{S}_H{H}", "own_ms": round(t_own, 4), "own_tflops": round(fl / t_own / 1e9, 1),
-                   "sdpa_ms": round(t_lib, 4), "sdpa_tflops": round(fl / t_lib / 1e9, 1)}
-            if a.bwd and hasattr(e, "flash_attn_bwd"):
-                o, lse = e.flash_attn_fwd(q, k, v, True, scale, True)
-                go = torch.randn_like(o)
-                t_b = time_fn(lambda: e.flash_attn_bwd(go, q, k, v, o, lse, True, scale, True))
-                qr, kr, vr = (t.detach().requires_grad_(True) for t in (qt, kt, vt))
-                oo = torch.nn.functional.scaled_dot_product_attention(qr, kr, vr, is_causal=True)
-                got = go.transpose(1, 2)
-                t_lb = time_fn(lambda: torch.autograd.grad(oo, (qr, kr, vr), got, retain_graph=True))
-                rec.update({"own_bwd_ms": round(t_b, 4), "own_bwd_tflops": round(2.5 * fl / t_b / 1e9, 1),
-                            "sdpa_bwd_ms": round(t_lb, 4), "sdpa_bwd_tflops": round(2.5 * fl / t_lb / 1e9, 1)})
-            print(json.dumps(rec), flush=True)
+        perf(e, a.bwd)
     print(json.dumps({"all_ok": ok_all}))
     sys.exit(0 if ok_all else 1)
 
