@@ -16,6 +16,10 @@
 // key is treated like a key past S_kv, so it contributes nothing and its dK / dV are exactly 0.  The forward and dQ kernels
 // stage each key tile's 64 flags in shared memory next to K / V; a dK/dV thread owns two fixed key rows and reads their
 // flags once.  A query row that sees no key gets O = 0, LSE = −inf and dQ = 0.
+// Optional sliding window (template flag WINDOW, causal only): query i sees key j iff i − W < j ≤ i.  The forward and dQ
+// kernels start their key-tile loop at the first tile that holds a key inside the window of the tile's first query row; the
+// dK/dV kernel stops its query-tile loop at the last tile whose rows can still see the key tile.  The per-element predicate
+// removes the rest.  W ≥ S computes exactly what the causal kernels compute.
 #include <cuda.h>
 
 #include <type_traits>
@@ -160,9 +164,10 @@ struct FwdParams {
   int B, H, Hkv, S_q, S_kv, causal;
   float scale_log2;
   const uint8_t* mask; long mask_sb;            // key-padding mask [B, S_kv] (MASK kernels only)
+  int window;                                   // sliding window W, 1 ≤ W ≤ S_kv (WINDOW kernels only)
 };
 
-template <int HD, bool MASK>
+template <int HD, bool MASK, bool WINDOW>
 __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
   constexpr int kTl = kTile<HD>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -179,12 +184,15 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
   const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
   const int n_kv = p.causal ? min((p.S_kv + BT - 1) / BT, qt + 1) : (p.S_kv + BT - 1) / BT;
+  // window: keys ≤ q0 − W are outside the window of every row of the tile, so whole tiles of them are skipped
+  const int t_lo = WINDOW ? max(0, q0 - p.window + 1) / BT : 0;
+  const int b_lo = t_lo & 1;
 
   load_tile<HD>(sQ, qb, p.q.ss, q0, p.S_q);
-  load_tile<HD>(sK, kb, p.k.ss, 0, p.S_kv);
-  load_tile<HD>(sV, vb, p.v.ss, 0, p.S_kv);
+  load_tile<HD>(sK + b_lo * kTl, kb, p.k.ss, t_lo * BT, p.S_kv);
+  load_tile<HD>(sV + b_lo * kTl, vb, p.v.ss, t_lo * BT, p.S_kv);
   cp_async_commit();
-  if (MASK) load_flags(sM, mb, 0, p.S_kv);
+  if (MASK) load_flags(sM + b_lo * BT, mb, t_lo * BT, p.S_kv);
 
   float o[HD / 8][4];
 #pragma unroll
@@ -192,7 +200,7 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const int row[2] = {q0 + warp * 16 + (lane >> 2), q0 + warp * 16 + (lane >> 2) + 8};
 
-  for (int t = 0; t < n_kv; ++t) {
+  for (int t = t_lo; t < n_kv; ++t) {
     const int buf = t & 1;
     if (t + 1 < n_kv) {
       load_tile<HD>(sK + (buf ^ 1) * kTl, kb, p.k.ss, (t + 1) * BT, p.S_kv);
@@ -214,7 +222,9 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
       for (int e = 0; e < 4; ++e) {
         const int key = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
         float x = s[j][e] * p.scale_log2;
-        if (key >= p.S_kv || (p.causal && key > row[e >> 1]) || (MASK && !fl[j * 8 + 2 * (lane & 3) + (e & 1)])) x = -INFINITY;
+        if (key >= p.S_kv || (p.causal && key > row[e >> 1]) || (MASK && !fl[j * 8 + 2 * (lane & 3) + (e & 1)]) ||
+            (WINDOW && key <= row[e >> 1] - p.window))
+          x = -INFINITY;
         s[j][e] = x;
         mx[e >> 1] = fmaxf(mx[e >> 1], x);
       }
@@ -298,9 +308,10 @@ struct BwdParams {
   int B, H, Hkv, S_q, S_kv, causal;
   float scale, scale_log2;
   const uint8_t* mask; long mask_sb;            // key-padding mask [B, S_kv] (MASK kernels only)
+  int window;                                   // sliding window W, 1 ≤ W ≤ S_kv (WINDOW kernels only)
 };
 
-template <int HD, bool MASK>
+template <int HD, bool MASK, bool WINDOW>
 __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParams p) {
   constexpr int kTl = kTile<HD>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -316,7 +327,9 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
   const int k0 = kt * BT;
   const int n_qt = (p.S_q + BT - 1) / BT;
   const int qt0 = p.causal ? kt : 0;                 // causal: S_q == S_kv, query tiles before the key tile see none of it
-  const int per_head = n_qt > qt0 ? n_qt - qt0 : 0;
+  // window: the last query row that sees key k0 + 63 is k0 + 63 + W − 1
+  const int qt_end = WINDOW ? min(n_qt, (k0 + BT - 1 + p.window - 1) / BT + 1) : n_qt;
+  const int per_head = qt_end > qt0 ? qt_end - qt0 : 0;
   const int n_it = G * per_head;
 
   load_tile<HD>(sK, p.k.p + b * p.k.sb + hk * p.k.sh, p.k.ss, k0, p.S_kv);
@@ -371,7 +384,8 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
       for (int e = 0; e < 4; ++e) {
         const int qc = j * 8 + 2 * (lane & 3) + (e & 1);
         const int qi = q0 + qc;
-        const bool vis = qi < p.S_q && !(p.causal && key[e >> 1] > qi) && (!MASK || kvis[e >> 1]);
+        const bool vis = qi < p.S_q && !(p.causal && key[e >> 1] > qi) && (!MASK || kvis[e >> 1]) &&
+                         !(WINDOW && qi >= key[e >> 1] + p.window);
         pt[j][e] = vis ? exp2f(pt[j][e] * p.scale_log2 - L[qc]) : 0.f;
       }
     }
@@ -397,11 +411,12 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
 }
 
 // CTAs per SM the dQ kernel is compiled for (0: no bound).  Left to itself ptxas spills at HD = 80 / 96, and at 64 with the
-// mask, to reach an occupancy the shared memory does not allow (Q, dO, K×2, V×2 tiles: 54 / 66 / 78 / 102 KB).
-template <int HD, bool MASK> constexpr int kDqMinBlocks = HD == 64 ? (MASK ? 3 : 4) : HD == 128 ? 0 : 2;
+// mask or the window, to reach an occupancy the shared memory does not allow (Q, dO, K×2, V×2 tiles: 54 / 66 / 78 / 102 KB).
+// EXTRA: the kernel has the mask or window predicate (a few more live registers).
+template <int HD, bool EXTRA> constexpr int kDqMinBlocks = HD == 64 ? (EXTRA ? 3 : 4) : HD == 128 ? 0 : 2;
 
-template <int HD, bool MASK>
-__global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK>)) fa_bwd_dq_kernel(const BwdParams p) {
+template <int HD, bool MASK, bool WINDOW>
+__global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) fa_bwd_dq_kernel(const BwdParams p) {
   constexpr int kTl = kTile<HD>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   bf16* sQ = (bf16*)smem_raw;
@@ -417,13 +432,15 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK>)) fa_bwd_dq_
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
   const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
   const int n_kv = p.causal ? min((p.S_kv + BT - 1) / BT, qt + 1) : (p.S_kv + BT - 1) / BT;
+  const int t_lo = WINDOW ? max(0, q0 - p.window + 1) / BT : 0;     // as in the forward
+  const int b_lo = t_lo & 1;
 
   load_tile<HD>(sQ, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
   load_tile<HD>(sG, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
-  load_tile<HD>(sK, kb, p.k.ss, 0, p.S_kv);
-  load_tile<HD>(sV, vb, p.v.ss, 0, p.S_kv);
+  load_tile<HD>(sK + b_lo * kTl, kb, p.k.ss, t_lo * BT, p.S_kv);
+  load_tile<HD>(sV + b_lo * kTl, vb, p.v.ss, t_lo * BT, p.S_kv);
   cp_async_commit();
-  if (MASK) load_flags(sM, mb, 0, p.S_kv);
+  if (MASK) load_flags(sM + b_lo * BT, mb, t_lo * BT, p.S_kv);
 
   const int row[2] = {q0 + warp * 16 + (lane >> 2), q0 + warp * 16 + (lane >> 2) + 8};
   float L[2], D[2];
@@ -437,7 +454,7 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK>)) fa_bwd_dq_
 #pragma unroll
   for (int i = 0; i < HD / 8; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
 
-  for (int t = 0; t < n_kv; ++t) {
+  for (int t = t_lo; t < n_kv; ++t) {
     const int buf = t & 1;
     if (t + 1 < n_kv) {
       load_tile<HD>(sK + (buf ^ 1) * kTl, kb, p.k.ss, (t + 1) * BT, p.S_kv);
@@ -459,7 +476,8 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK>)) fa_bwd_dq_
       for (int e = 0; e < 4; ++e) {
         const int kc = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
         const int r = row[e >> 1];
-        const bool vis = kc < p.S_kv && r < p.S_q && !(p.causal && kc > r) && (!MASK || fl[j * 8 + 2 * (lane & 3) + (e & 1)]);
+        const bool vis = kc < p.S_kv && r < p.S_q && !(p.causal && kc > r) && (!MASK || fl[j * 8 + 2 * (lane & 3) + (e & 1)]) &&
+                         !(WINDOW && kc <= r - p.window);
         s[j][e] = vis ? exp2f(s[j][e] * p.scale_log2 - L[e >> 1]) : 0.f;
       }
     }
@@ -484,12 +502,17 @@ static View view(const void* ptr, const long* s) {
   return View{(const bf16*)ptr, s[0], s[1], s[2]};
 }
 
-// f(std::integral_constant<int, HD>, std::integral_constant<bool, MASK>) for the runtime head dimension and mask flag
+// f(std::integral_constant<int, HD>, std::integral_constant<bool, MASK>, std::integral_constant<bool, WINDOW>) for the runtime
+// head dimension, mask flag and window flag
 template <class F>
-static void dispatch(int D, bool mask, F&& f) {
+static void dispatch(int D, bool mask, bool window, F&& f) {
+  auto with_window = [&](auto hd, auto mk) {
+    if (window) f(hd, mk, std::true_type{});
+    else f(hd, mk, std::false_type{});
+  };
   auto with_mask = [&](auto hd) {
-    if (mask) f(hd, std::true_type{});
-    else f(hd, std::false_type{});
+    if (mask) with_window(hd, std::true_type{});
+    else with_window(hd, std::false_type{});
   };
   switch (D) {
     case 64: with_mask(std::integral_constant<int, 64>{}); break;
@@ -500,37 +523,39 @@ static void dispatch(int D, bool mask, F&& f) {
   }
 }
 
-template <int HD, bool MASK>
+template <int HD, bool MASK, bool WINDOW>
 static void launch_fwd(const FwdParams& p, cudaStream_t st) {
   constexpr int smem = kSmemFwd<HD> + (MASK ? kSmemFlags : 0);
   static bool configured = false;
   if (!configured) {
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_fwd_kernel<HD, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_fwd_kernel<HD, MASK, WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
-  fa_fwd_kernel<HD, MASK><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem, st>>>(p);
+  fa_fwd_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem, st>>>(p);
 }
 
-template <int HD, bool MASK>
+template <int HD, bool MASK, bool WINDOW>
 static void launch_bwd(const BwdParams& p, cudaStream_t st) {
   constexpr int smem_dkv = kSmemDkv<HD>, smem_dq = kSmemDq<HD> + (MASK ? kSmemFlags : 0);
   static bool configured = false;
   if (!configured) {
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dkdv_kernel<HD, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dkv));
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dq_kernel<HD, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dq));
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dkdv_kernel<HD, MASK, WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dkv));
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dq_kernel<HD, MASK, WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dq));
     configured = true;
   }
-  fa_bwd_dkdv_kernel<HD, MASK><<<dim3((p.S_kv + BT - 1) / BT, p.Hkv, p.B), kThreads, smem_dkv, st>>>(p);
-  fa_bwd_dq_kernel<HD, MASK><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem_dq, st>>>(p);
+  fa_bwd_dkdv_kernel<HD, MASK, WINDOW><<<dim3((p.S_kv + BT - 1) / BT, p.Hkv, p.B), kThreads, smem_dkv, st>>>(p);
+  fa_bwd_dq_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem_dq, st>>>(p);
 }
 
 }  // namespace fa
 
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
                     int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    const void* kpm, long kpm_sb, cudaStream_t st) {
+                    const void* kpm, long kpm_sb, int window, cudaStream_t st) {
   using namespace fa;
   if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
+  if (window < 0) nxd_throw("attention: window must be >= 0 (0 = none)", __FILE__, __LINE__);
+  if (window > 0 && !causal) nxd_throw("attention: a sliding window needs causal attention", __FILE__, __LINE__);
   FwdParams p;
   p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs);
   p.o = (bf16*)out; p.o_sb = os[0]; p.o_ss = os[1]; p.o_sh = os[2];
@@ -538,17 +563,22 @@ void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, floa
   p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
   p.scale_log2 = scale * kLog2e;
   p.mask = (const uint8_t*)kpm; p.mask_sb = kpm_sb;
-  dispatch(D, kpm != nullptr, [&](auto hd, auto mk) { launch_fwd<decltype(hd)::value, decltype(mk)::value>(p, st); });
+  p.window = window < S_kv ? window : S_kv;       // W ≥ S_kv sees every causal key; the clamp keeps tile bounds in range
+  dispatch(D, kpm != nullptr, window > 0, [&](auto hd, auto mk, auto wd) {
+    launch_fwd<decltype(hd)::value, decltype(mk)::value, decltype(wd)::value>(p, st);
+  });
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 
 void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
                     int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
-                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb,
+                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, int window,
                     cudaStream_t st) {
   using namespace fa;
   if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
+  if (window < 0) nxd_throw("attention: window must be >= 0 (0 = none)", __FILE__, __LINE__);
+  if (window > 0 && !causal) nxd_throw("attention: a sliding window needs causal attention", __FILE__, __LINE__);
   BwdParams p;
   p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs); p.g = view(go, gs);
   p.dq = (bf16*)dq; p.dk = (bf16*)dk; p.dv = (bf16*)dv;
@@ -559,12 +589,13 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
   p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
   p.scale = scale; p.scale_log2 = scale * kLog2e;
   p.mask = (const uint8_t*)kpm; p.mask_sb = kpm_sb;
-  dispatch(D, kpm != nullptr, [&](auto hd, auto mk) {
+  p.window = window < S_kv ? window : S_kv;
+  dispatch(D, kpm != nullptr, window > 0, [&](auto hd, auto mk, auto wd) {
     constexpr int HD = decltype(hd)::value;
     const long rows = (long)B * H * S_q;
     fa_bwd_prep_kernel<HD><<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(
         (const bf16*)o, (const bf16*)go, dlse, delta, B, S_q, H, os[0], os[1], os[2], gs[0], gs[1], gs[2]);
-    launch_bwd<HD, decltype(mk)::value>(p, st);
+    launch_bwd<HD, decltype(mk)::value, decltype(wd)::value>(p, st);
   });
   NXD_CUDA_CHECK(cudaGetLastError());
 }

@@ -271,8 +271,17 @@ static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, 
 }
 
 // ---- decode ---------------------------------------------------------------------------------------
-// q [B,1,H,128]; k/v cache [B,L,Hkv,128] (any b/s/h strides, head_dim contiguous); positions [B] int64 (attend to ≤ pos)
-static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions, double scale) {
+// q [B,1,H,128]; k/v cache [B,L,Hkv,128] (any b/s/h strides, head_dim contiguous); positions [B] int64 (attend to ≤ pos);
+// window > 0: only the last `window` positions up to pos are visible
+static int decode_splits(int B, int Hkv, int L, int64_t window) {
+  TORCH_CHECK(window >= 0, "decode_attention: window must be >= 0 (0 = none)");
+  const int rows = window > 0 && window < L ? (int)window : L;      // cache rows one sequence reads at most
+  // enough CTAs for ~6 per SM (the kernel is latency-bound per CTA: 8 cache rows in flight), at least 64 rows per split
+  int splits = (6 * num_sms() + B * Hkv - 1) / (B * Hkv);
+  return std::max(1, std::min(std::min(splits, 64), (rows + 63) / 64));
+}
+static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions, double scale,
+                               int64_t window) {
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) == 1 && q.size(3) == 128 && q.stride(3) == 1);
   TORCH_CHECK(k.scalar_type() == at::kBFloat16 && k.dim() == 4 && k.size(3) == 128 && k.stride(3) == 1 && v.stride(3) == 1 &&
               v.sizes() == k.sizes());
@@ -281,23 +290,21 @@ static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v
   TORCH_CHECK(H % Hkv == 0 && k.size(0) == B);
   TORCH_CHECK(q.stride(2) % 8 == 0 && k.stride(1) % 8 == 0 && k.stride(2) % 8 == 0 && v.stride(1) % 8 == 0 && v.stride(2) % 8 == 0);
   c10::cuda::CUDAGuard guard(q.device());
-  // enough CTAs for ~6 per SM (the kernel is latency-bound per CTA: 8 cache rows in flight), at least 64 rows per split
-  int splits = (6 * num_sms() + B * Hkv - 1) / (B * Hkv);
-  splits = std::max(1, std::min(std::min(splits, 64), (L + 63) / 64));
+  const int splits = decode_splits(B, Hkv, L, window);
   Tensor out = at::empty({B, 1, H, 128}, q.options());
   Tensor part_o = at::empty({B * H * splits, 128}, q.options().dtype(at::kFloat));
   Tensor part_ml = at::empty({B * H * splits, 2}, q.options().dtype(at::kFloat));
   const long ks[3] = {k.stride(0), k.stride(1), k.stride(2)}, vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   nxd::decode_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), out.data_ptr(),
                         part_o.data_ptr<float>(), part_ml.data_ptr<float>(), B, H, Hkv, L, ks, vs, q.stride(0), q.stride(2),
-                        out.stride(0), out.stride(2), (float)scale, splits, stream());
+                        out.stride(0), out.stride(2), (float)scale, splits, (int)std::min<int64_t>(window, INT32_MAX), stream());
   return out;
 }
 // This rank's contribution to distributed flash-decoding: un-normalised output (relative to the row maximum) [B,H,128] fp32 and
 // (row maximum in natural-log units, row sum) [B,H,2] fp32 over the local cache shard; ``positions`` are LOCAL (may be < 0 or
 // >= L: nothing / everything of this shard is visible).
 static std::vector<Tensor> decode_attention_partial(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions,
-                                                    double scale) {
+                                                    double scale, int64_t window) {
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) == 1 && q.size(3) == 128 && q.stride(3) == 1);
   TORCH_CHECK(k.scalar_type() == at::kBFloat16 && k.dim() == 4 && k.size(3) == 128 && k.stride(3) == 1 && v.stride(3) == 1 &&
               v.sizes() == k.sizes());
@@ -306,8 +313,7 @@ static std::vector<Tensor> decode_attention_partial(const Tensor& q, const Tenso
   TORCH_CHECK(H % Hkv == 0 && k.size(0) == B);
   TORCH_CHECK(q.stride(2) % 8 == 0 && k.stride(1) % 8 == 0 && k.stride(2) % 8 == 0 && v.stride(1) % 8 == 0 && v.stride(2) % 8 == 0);
   c10::cuda::CUDAGuard guard(q.device());
-  int splits = (6 * num_sms() + B * Hkv - 1) / (B * Hkv);
-  splits = std::max(1, std::min(std::min(splits, 64), (L + 63) / 64));
+  const int splits = decode_splits(B, Hkv, L, window);
   Tensor fin_o = at::empty({B, H, 128}, q.options().dtype(at::kFloat));
   Tensor fin_ml = at::empty({B, H, 2}, q.options().dtype(at::kFloat));
   Tensor part_o = at::empty({B * H * splits, 128}, q.options().dtype(at::kFloat));
@@ -315,7 +321,7 @@ static std::vector<Tensor> decode_attention_partial(const Tensor& q, const Tenso
   const long ks[3] = {k.stride(0), k.stride(1), k.stride(2)}, vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   nxd::decode_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), nullptr, part_o.data_ptr<float>(),
                         part_ml.data_ptr<float>(), B, H, Hkv, L, ks, vs, q.stride(0), q.stride(2), 0, 0, (float)scale, splits,
-                        stream(), fin_o.data_ptr<float>(), fin_ml.data_ptr<float>());
+                        (int)std::min<int64_t>(window, INT32_MAX), stream(), fin_o.data_ptr<float>(), fin_ml.data_ptr<float>());
   return {fin_o, fin_ml};
 }
 // x [T,H] bf16; gamma [H] bf16 or none; router_w [E,H] bf16; router_bias [E] fp32 or none; w_gu [El,H,2I]; w_dn [El,I,H]
@@ -456,13 +462,19 @@ static const void* check_kpm(const c10::optional<Tensor>& m, const Tensor& q, in
   *sb = m->stride(0);
   return m->data_ptr();
 }
+// sliding window W (query i sees keys i − W < j ≤ i), 0 = none; causal attention only
+static void check_window(int64_t window, bool causal) {
+  TORCH_CHECK(window >= 0, "window must be >= 0 (0 = none)");
+  TORCH_CHECK(window == 0 || causal, "a sliding window needs causal attention");
+}
 // returns (out [B,S,H,D] view — memory laid out [S,B,H,D] when sbhd_out —, lse [B,H,S] fp32)
 static std::vector<Tensor> flash_attn_fwd(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
-                                          bool sbhd_out, const c10::optional<Tensor>& key_padding_mask) {
+                                          bool sbhd_out, const c10::optional<Tensor>& key_padding_mask, int64_t window) {
   check_qkv(q, "q"); check_qkv(k, "k"); check_qkv(v, "v");
   const int B = q.size(0), S = q.size(1), H = q.size(2), D = q.size(3), Skv = k.size(1), Hkv = k.size(2);
   TORCH_CHECK(k.size(0) == B && v.size(0) == B && v.size(1) == Skv && v.size(2) == Hkv && H % Hkv == 0);
   TORCH_CHECK(k.size(3) == D && v.size(3) == D, "q, k and v must have the same head_dim");
+  check_window(window, causal);
   long kpm_sb;
   const void* kpm = check_kpm(key_padding_mask, q, B, Skv, &kpm_sb);
   c10::cuda::CUDAGuard guard(q.device());
@@ -471,18 +483,20 @@ static std::vector<Tensor> flash_attn_fwd(const Tensor& q, const Tensor& k, cons
   const long qs[3] = {q.stride(0), q.stride(1), q.stride(2)}, ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   const long vs[3] = {v.stride(0), v.stride(1), v.stride(2)}, os[3] = {out.stride(0), out.stride(1), out.stride(2)};
   nxd::flash_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, Skv, H, Hkv, D,
-                      qs, ks, vs, os, (float)scale, causal, kpm, kpm_sb, stream());
+                      qs, ks, vs, os, (float)scale, causal, kpm, kpm_sb, (int)std::min<int64_t>(window, Skv), stream());
   return {out, lse};
 }
 
 static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& o,
                                           const Tensor& lse, bool causal, double scale, bool sbhd_out,
-                                          const c10::optional<Tensor>& dlse, const c10::optional<Tensor>& key_padding_mask) {
+                                          const c10::optional<Tensor>& dlse, const c10::optional<Tensor>& key_padding_mask,
+                                          int64_t window) {
   check_qkv(q, "q"); check_qkv(k, "k"); check_qkv(v, "v"); check_qkv(go, "grad_out"); check_qkv(o, "out");
   const int B = q.size(0), S = q.size(1), H = q.size(2), D = q.size(3), Skv = k.size(1), Hkv = k.size(2);
   TORCH_CHECK(k.size(3) == D && v.size(3) == D && go.size(3) == D && o.size(3) == D,
               "q, k, v, out and grad_out must have the same head_dim");
   TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * H * S);
+  check_window(window, causal);
   long kpm_sb;
   const void* kpm = check_kpm(key_padding_mask, q, B, Skv, &kpm_sb);
   c10::cuda::CUDAGuard guard(q.device());
@@ -501,7 +515,7 @@ static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, con
   }
   nxd::flash_attn_bwd(go.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), dlse_p,
                       dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr<float>(), B, S, Skv, H, Hkv, D, gs, qs, ks,
-                      vs, os, dqs, dks, dvs, (float)scale, causal, kpm, kpm_sb, stream());
+                      vs, os, dqs, dks, dvs, (float)scale, causal, kpm, kpm_sb, (int)std::min<int64_t>(window, Skv), stream());
   return {dq, dk, dv};
 }
 
@@ -755,8 +769,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fused_adamw", &fused_adamw);
   m.def("gemm_bf16", &gemm_bf16);
   m.def("oneshot_allreduce", &oneshot_allreduce);
-  m.def("decode_attention", &decode_attention);
-  m.def("decode_attention_partial", &decode_attention_partial);
+  m.def("decode_attention", &decode_attention, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"), py::arg("scale"),
+        py::arg("window") = 0);
+  m.def("decode_attention_partial", &decode_attention_partial, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"),
+        py::arg("scale"), py::arg("window") = 0);
   m.def("nvls_embedding_gather", &nvls_embedding_gather);
   m.def("nvls_publish", &nvls_publish);
   m.def("ptr_view", &ptr_view);
@@ -779,10 +795,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("grouped_gemm", &grouped_gemm);
   m.def("grouped_wgrad", &grouped_wgrad);
   m.def("flash_attn_fwd", &flash_attn_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("causal"), py::arg("scale"),
-        py::arg("sbhd_out"), py::arg("key_padding_mask") = py::none());
+        py::arg("sbhd_out"), py::arg("key_padding_mask") = py::none(), py::arg("window") = 0);
   m.def("flash_attn_bwd", &flash_attn_bwd, py::arg("go"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"), py::arg("lse"),
         py::arg("causal"), py::arg("scale"), py::arg("sbhd_out"), py::arg("dlse") = py::none(),
-        py::arg("key_padding_mask") = py::none());
+        py::arg("key_padding_mask") = py::none(), py::arg("window") = 0);
   m.def("ag_gemm_bf16", &ag_gemm_bf16);
   m.def("gemm_rs_bf16", &gemm_rs_bf16);
   m.def("zero1_reduce_scatter", &zero1_reduce_scatter);

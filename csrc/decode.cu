@@ -3,6 +3,7 @@
 //   decode_attention : one query token per sequence against the KV cache (flash-decoding: split over the cache length,
 //                      GQA group processed together so K/V are read once per kv head), + a combine pass over the splits.
 //                      Role of the reference's token-generation attention (modules/attention, models' TKG path).
+//                      Optional sliding window W: only cache rows positions[b] − W < j ≤ positions[b] are read.
 //   gemv_bf16        : y[M≤8, N] = x[M, K] · W[N, K]ᵀ (+ optional residual) for batch-1..8 decode; every weight byte is read once
 //                      with 16-byte loads, fp32 accumulation.
 #include <cuda.h>
@@ -22,13 +23,19 @@ template <int G>
 __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
     const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc, const __nv_bfloat16* __restrict__ vc,
     const long* __restrict__ positions, float* __restrict__ part_o, float* __restrict__ part_ml, int B, int H, int Hkv, int L,
-    long k_sb, long k_ss, long k_sh, long v_sb, long v_ss, long v_sh, long q_sb, long q_sh, float scale_log2, int splits) {
+    long k_sb, long k_ss, long k_sh, long v_sb, long v_ss, long v_sh, long q_sb, long q_sh, float scale_log2, int splits,
+    int window) {
   const int kvh = blockIdx.x, b = blockIdx.y, split = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sub = lane >> 4, l16 = lane & 15;               // position slot within the warp step, 8-dim slice
-  const int n_valid = min((int)positions[b] + 1, L);
+  // visible rows [lo, hi): the splits divide this range.  Positions may lie outside [0, L) (the local positions of a sequence
+  // shard); then the range is clipped to the cache, and it is empty when the window ends before row 0 or starts past L.
+  const long pos = positions[b];
+  const int hi = (int)min(pos + 1, (long)L);
+  const int lo = window > 0 ? (int)min(max(pos - window + 1, 0L), (long)L) : 0;
+  const int n_valid = max(hi - lo, 0);
   const int per = (n_valid + splits - 1) / splits;
-  const int s0 = split * per, s1 = min(n_valid, s0 + per);
+  const int s0 = lo + split * per, s1 = min(hi, s0 + per);
 
   auto load8 = [](const __nv_bfloat16* p, float (&f)[8], float mul) {
     const uint4 a = *reinterpret_cast<const uint4*>(p);
@@ -249,14 +256,14 @@ void decode_rope_kv(const void* q, const void* k, const void* v, const long* pos
 
 void decode_attention(const void* q, const void* k, const void* v, const long* positions, void* out, float* part_o,
                       float* part_ml, int B, int H, int Hkv, int L, const long* ks, const long* vs, long q_sb, long q_sh,
-                      long o_sb, long o_sh, float scale, int splits, cudaStream_t st, float* fin_o, float* fin_ml) {
+                      long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o, float* fin_ml) {
   const int G = H / Hkv;
   dim3 grid(Hkv, B, splits);
   const float sl2 = scale * 1.4426950408889634f;
 #define NXD_DEC(Gv)                                                                                                  \
   decode_attn_kernel<Gv><<<grid, kDecThreads, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k,             \
       (const __nv_bfloat16*)v, positions, part_o, part_ml, B, H, Hkv, L, ks[0], ks[1], ks[2], vs[0], vs[1], vs[2], q_sb, \
-      q_sh, sl2, splits)
+      q_sh, sl2, splits, window)
   switch (G) {
     case 1: NXD_DEC(1); break;
     case 2: NXD_DEC(2); break;

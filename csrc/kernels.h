@@ -132,8 +132,9 @@ void gemv_mx_grouped(const void* x, const void* w, const void* scale, const long
 // ---- decode (decode.cu)
 void decode_attention(const void* q, const void* k, const void* v, const long* positions, void* out, float* part_o,
                       float* part_ml, int B, int H, int Hkv, int L, const long* ks, const long* vs, long q_sb, long q_sh,
-                      long o_sb, long o_sh, float scale, int splits, cudaStream_t st, float* fin_o = nullptr,
+                      long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o = nullptr,
                       float* fin_ml = nullptr);   // fin_o/fin_ml: un-normalised [B*H,128] + (max, sum) [B*H,2] instead of ``out``
+                                                  // window: keys positions[b] − window < j ≤ positions[b] visible (0: no window)
 void decode_rope_kv(const void* q, const void* k, const void* v, const long* positions, const float* cos_t, const float* sin_t,
                     void* q_out, void* kc, void* vc, int B, int H, int Hkv, int D, int L, long q_sb, long q_sh, long k_sb, long k_sh,
                     long v_sb, long v_sh, long c_sb, long c_ss, long c_sh, cudaStream_t st);
@@ -141,15 +142,16 @@ void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int 
 
 // ---- attention (attention_sm90.cu): q [B,S_q,H,D], k/v [B,S_kv,Hkv,D] bf16 views, D ∈ {64, 80, 96, 128}; strides = (b, s, h)
 // in elements.  kpm: optional key-padding mask, uint8 [B, S_kv] with row stride kpm_sb (key visible iff nonzero), or null.
+// window: sliding window W (causal only; query i sees keys i − W < j ≤ i), or 0 for none.
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
                     int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    const void* kpm, long kpm_sb, cudaStream_t st);
+                    const void* kpm, long kpm_sb, int window, cudaStream_t st);
 
 // delta: fp32 scratch [B, H, S_q]; dlse may be null
 void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
                     int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
-                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb,
+                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, int window,
                     cudaStream_t st);
 
 }  // namespace nxd

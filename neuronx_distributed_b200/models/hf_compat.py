@@ -89,6 +89,10 @@ def config_from_hf(hf_config: Any, **overrides):
         if scaling.get("type", scaling.get("rope_type")) == "linear":
             kw["rope_scaling_factor"] = float(scaling["factor"])
         cls = LlamaConfig
+        if str(d.get("model_type", "")).lower() in ("mistral", "mixtral"):
+            # Mistral / Mixtral attend within a sliding window (None: full attention).  Qwen2 carries the field too but
+            # gates it with ``use_sliding_window`` and per-layer limits, so it is read for these two families only.
+            kw["sliding_window"] = d.get("sliding_window")
         if fam == "mixtral":
             kw.update(num_local_experts=d["num_local_experts"], num_experts_per_tok=d["num_experts_per_tok"],
                       router_aux_loss_coef=d.get("router_aux_loss_coef", 0.02))

@@ -52,6 +52,8 @@ class LlamaConfig:
     context_parallel: bool = False
     cp_layout: str = "contiguous"           # "zigzag": rank r holds sequence chunks (r, 2·cp−1−r); needs the pull attention path
     device: Optional[torch.device] = None       # construct parameters directly here (e.g. cuda)
+    # sliding-window attention (Mistral / Mixtral): query i sees keys i − W < j ≤ i; None = full causal attention
+    sliding_window: Optional[int] = None
 
     def __post_init__(self):
         if self.num_key_value_heads is None:
@@ -145,12 +147,14 @@ class LlamaAttention(nn.Module):
         if self.cfg.context_parallel and ps.get_context_model_parallel_size() > 1:
             from ..modules.attention.ring import pull_attention, ring_attention
 
+            if self.cfg.sliding_window is not None:
+                raise NotImplementedError("sliding_window is not supported with context parallelism")
             if self.cfg.cp_layout != "contiguous":
                 o = pull_attention(q, k, v, causal=True, layout=self.cfg.cp_layout)      # the ring keeps the contiguous split
             else:
                 o = (pull_attention if _CP_PULL else ring_attention)(q, k, v, causal=True)
         else:
-            o = ops.attention.flash_attention(q, k, v, causal=True)
+            o = ops.attention.flash_attention(q, k, v, causal=True, sliding_window=self.cfg.sliding_window)
         o = o.transpose(0, 1).reshape(S, B, self.num_heads_local * self.head_dim)
         return self.o_proj(o)
 

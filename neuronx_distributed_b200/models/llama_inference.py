@@ -61,6 +61,7 @@ class LlamaForInference(nn.Module):
     def _attn_block(self, layer_idx: int, layer, x: torch.Tensor, positions: Optional[torch.Tensor], prefill: bool,
                     kv_len: Optional[int], tree=None) -> torch.Tensor:
         att = layer.self_attn
+        sw = self.cfg.sliding_window                       # Mistral / Mixtral window (None: full causal attention)
         h = layer.input_layernorm(x)
         q, k, v = att.qkv_proj(h)                          # [S, B, h*D]
         S, B = q.shape[0], q.shape[1]
@@ -76,7 +77,7 @@ class LlamaForInference(nn.Module):
             sin = self.rope_sin[positions].unsqueeze(1)
             q, k = _rope_per_batch(q, cos, sin), _rope_per_batch(k, cos, sin)
             write_decode_sharded(self.kv.k[layer_idx], self.kv.v[layer_idx], k, v, positions, self.kv_rank)   # owner-only write
-            o = flash_decode_attention(q, self.kv.k[layer_idx], self.kv.v[layer_idx], positions, self.kv_group)
+            o = flash_decode_attention(q, self.kv.k[layer_idx], self.kv.v[layer_idx], positions, self.kv_group, sliding_window=sw)
         elif not prefill and S > 1:
             # speculation window: W new tokens per sequence at positions p..p+W-1, causal among themselves, full cache before
             W = S
@@ -88,7 +89,7 @@ class LlamaForInference(nn.Module):
             q, k = _rope_window(q, cos, sin), _rope_window(k, cos, sin)
             self.kv.write_window(layer_idx, k, v, positions)
             kc, vc = self.kv.get(layer_idx, kv_len)
-            o = _window_attention(q, kc, vc, positions, None if tree is None else tree[0])
+            o = _window_attention(q, kc, vc, positions, None if tree is None else tree[0], sw, depth)
         elif prefill:
             cos, sin = self.rope_cos[:S], self.rope_sin[:S]
             q, k = ops.rope.apply_rotary(q, cos, sin), ops.rope.apply_rotary(k, cos, sin)
@@ -96,7 +97,7 @@ class LlamaForInference(nn.Module):
                 self.kv.write_prefill_sharded(layer_idx, k, v, self.kv_rank)
             else:
                 self.kv.write_prefill(layer_idx, k, v)
-            o = ops.attention.flash_attention(q, k, v, causal=True)
+            o = ops.attention.flash_attention(q, k, v, causal=True, sliding_window=sw)
         elif (q.is_cuda and q.dtype == torch.bfloat16 and self.kv.kv_quant is None and self.kv.seq_shards == 1
               and ops._ext.ext() is not None and hasattr(ops._ext.ext(), "decode_rope_kv")):
             # one launch: RoPE of q and k at each sequence's position + append of k / v to the cache (csrc/decode.cu)
@@ -104,7 +105,7 @@ class LlamaForInference(nn.Module):
             q = ops._ext.ext().decode_rope_kv(q, k, v, positions.to(torch.long).contiguous(), self.rope_cos, self.rope_sin,
                                               self.kv.k[layer_idx], self.kv.v[layer_idx])
             kc, vc = self.kv.get(layer_idx, kv_len)
-            o = _decode_attention(q, kc, vc, positions)
+            o = _decode_attention(q, kc, vc, positions, sw)
         else:
             # one new token per sequence at its own position
             cos = self.rope_cos[positions].unsqueeze(1)     # [B, 1, D/2] → per-batch tables
@@ -112,7 +113,7 @@ class LlamaForInference(nn.Module):
             q, k = _rope_per_batch(q, cos, sin), _rope_per_batch(k, cos, sin)
             self.kv.write_decode(layer_idx, k, v, positions)
             kc, vc = self.kv.get(layer_idx, kv_len)
-            o = _decode_attention(q, kc, vc, positions)
+            o = _decode_attention(q, kc, vc, positions, sw)
         o = o.transpose(0, 1).reshape(S, B, att.num_heads_local * D)
         return _row_linear_plus_residual(att.o_proj, o, x)
 
@@ -239,9 +240,12 @@ def _rope_window(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch
 
 
 def _window_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor,
-                      tree_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+                      tree_mask: Optional[torch.Tensor] = None, sliding_window: Optional[int] = None,
+                      depth: Optional[torch.Tensor] = None) -> torch.Tensor:
     """q [B,W,H,D] in cache slots p..p+W-1 vs cache k/v [B,L,Hkv,D].  Chain: token w sees slots ≤ p+w.  Tree (``tree_mask``
-    [W,W]): node w sees every slot < p (the committed sequence) and the window slots of its ancestors."""
+    [W,W]): node w sees every slot < p (the committed sequence) and the window slots of its ancestors.
+    ``sliding_window`` SW: a token at sequence position p + ``depth[w]`` (chain: depth w) also only sees keys whose sequence
+    position is > p + depth[w] − SW; a committed slot c sits at position c, window slot p + u at p + depth[u]."""
     B, W, H, D = q.shape
     Hkv, L = k.shape[2], k.shape[1]
     qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
@@ -256,11 +260,21 @@ def _window_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positio
         inside = (rel >= 0) & (rel < W)
         tm = tree_mask.to(q.device)[:, rel.clamp(0, W - 1)].permute(1, 0, 2)                   # [B, W, L]
         mask = ((rel < 0)[:, None, :] | (inside[:, None, :] & tm))[:, None]
+    if sliding_window is not None:
+        depth = torch.arange(W, device=q.device) if depth is None else depth.to(q.device)
+        rel = cols[None, :] - positions[:, None]                                               # [B, L]
+        kpos = torch.where(rel < W, positions[:, None] + depth[rel.clamp(0, W - 1)], cols[None, :])
+        kpos = torch.where(rel < 0, cols[None, :], kpos)                                       # sequence position of each slot
+        qpos = positions[:, None] + depth[None, :]                                             # [B, W]
+        mask = mask & (kpos[:, None, :] > qpos[:, :, None] - sliding_window)[:, None]
     return torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask).transpose(1, 2)
 
 
-def _decode_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor) -> torch.Tensor:
-    """q [B,1,H,D] vs cache k/v [B,L,Hkv,D]; keys beyond each sequence's position are masked."""
+def _decode_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor,
+                      sliding_window: Optional[int] = None) -> torch.Tensor:
+    """q [B,1,H,D] vs cache k/v [B,L,Hkv,D]; keys beyond each sequence's position (and, with ``sliding_window`` SW, keys at or
+    before position − SW) are masked."""
+    window = ops.attention.check_window(sliding_window)
     B, _, H, D = q.shape
     Hkv, L = k.shape[2], k.shape[1]
     e = ops._ext.ext() if q.is_cuda else None
@@ -268,11 +282,11 @@ def _decode_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positio
             and H // Hkv in (1, 2, 4, 8) and k.stride(3) == 1 and v.stride(3) == 1):
         # flash-decoding kernel (csrc/decode.cu): split over the cache length, GQA group shares each K/V read
         ops._ext.count_launch(2)
-        return e.decode_attention(q.contiguous(), k, v, positions.to(torch.long).contiguous(), 1.0 / math.sqrt(D))
+        return e.decode_attention(q.contiguous(), k, v, positions.to(torch.long).contiguous(), 1.0 / math.sqrt(D), window)
     qt = q.transpose(1, 2)                                   # [B,H,1,D]
     kt, vt = k.transpose(1, 2), v.transpose(1, 2)
     if H != Hkv:
         kt, vt = kt.repeat_interleave(H // Hkv, 1), vt.repeat_interleave(H // Hkv, 1)
-    mask = (torch.arange(L, device=q.device)[None, :] <= positions[:, None])[:, None, None, :]
+    mask = ops.attention.decode_visibility(positions, L, window)[:, None, None, :]
     o = torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask)
     return o.transpose(1, 2)

@@ -36,28 +36,32 @@ def write_decode_sharded(k_cache: torch.Tensor, v_cache: torch.Tensor, k_new: to
     v_cache[b, off] = keep * v_new[:, 0] + (1 - keep) * v_cache[b, off]
 
 
-def _local_partial(q_all: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, local_pos: torch.Tensor, scale: float):
+def _local_partial(q_all: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, local_pos: torch.Tensor, scale: float,
+                   sliding_window: Optional[int] = None):
     """Partial attention of ``q_all [B, 1, H, D]`` over this rank's cache shard, cache index ≤ ``local_pos[b]`` visible
-    (``local_pos`` may be negative: nothing visible yet).  Returns un-normalised ``o [B, H, D]`` relative to the row maximum
+    (``local_pos`` may be negative: nothing visible yet), and with ``sliding_window`` W only indices > ``local_pos[b]`` − W
+    (both ends shift by the shard offset, so local positions need no other change).  Returns un-normalised ``o [B, H, D]`` relative to the row maximum
     ``m [B, H]`` (natural-log units, −inf when nothing is visible) and the row sum ``l [B, H]``, all fp32.
 
     CUDA / bf16 / head_dim 128: the split-KV decode kernel (``csrc/decode.cu`` ``decode_attn_kernel`` + the partial combine):
     K/V are read once per KV head for the whole GQA group.  Otherwise fp32 torch math."""
     from ...ops import _ext
+    from ...ops.attention import check_window, decode_visibility
 
+    window = check_window(sliding_window)
     B, _, H, D = q_all.shape
     l_local, Hkv = k_cache.shape[1], k_cache.shape[2]
     if (_ext.use_cuda(q_all, k_cache, v_cache) and q_all.dtype == torch.bfloat16 and k_cache.dtype == torch.bfloat16 and D == 128
             and H % Hkv == 0 and (H // Hkv) in (1, 2, 4, 8) and hasattr(_ext.ext(), "decode_attention_partial")):
         _ext.count_launch(2)
         o, ml = _ext.ext().decode_attention_partial(q_all.contiguous(), k_cache, v_cache, local_pos.to(torch.long).contiguous(),
-                                                    float(scale))
+                                                    float(scale), window)
         return o, ml[..., 0], ml[..., 1]
     g = H // Hkv
     kf = k_cache.float().repeat_interleave(g, dim=2)                    # [B, L_local, H, D]
     vf = v_cache.float().repeat_interleave(g, dim=2)
     s = torch.einsum("bhd,blhd->bhl", q_all[:, 0].float(), kf) * scale  # [B, H, L_local]
-    valid = torch.arange(l_local, device=q_all.device)[None, :] <= local_pos[:, None]          # [B, L_local]
+    valid = decode_visibility(local_pos, l_local, window)                                        # [B, L_local]
     s = s.masked_fill(~valid[:, None, :], float("-inf"))
     m = s.max(dim=-1).values                                            # [B, H]  (−inf if this shard has nothing yet)
     p = torch.exp(s - torch.where(torch.isinf(m), torch.zeros_like(m), m).unsqueeze(-1))
@@ -66,9 +70,10 @@ def _local_partial(q_all: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Te
 
 
 def flash_decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, positions: torch.Tensor,
-                           group, scale: Optional[float] = None) -> torch.Tensor:
+                           group, scale: Optional[float] = None, sliding_window: Optional[int] = None) -> torch.Tensor:
     """q ``[B, 1, H_local, D]`` (this rank's query heads), caches ``[B, L_local, Hkv, D]`` (this rank's sequence shard of the
-    shared KV heads), ``positions`` ``[B]`` = index of the newest token (attend to ≤ position).  Returns ``[B, 1, H_local, D]``.
+    shared KV heads), ``positions`` ``[B]`` = index of the newest token (attend to ≤ position; with ``sliding_window`` W only
+    to the last W positions).  Returns ``[B, 1, H_local, D]``.
     Collectives go through ``parallel_layers.comm`` (NCCL / gloo; recordable in launch plans)."""
     from ...parallel_layers import comm
 
@@ -85,7 +90,7 @@ def flash_decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torc
     else:
         q_all = q
     # 2. partial attention over the local shard: global position p is local index p − r·L_local
-    o, m, l = _local_partial(q_all, k_cache, v_cache, positions - r * l_local, scale)
+    o, m, l = _local_partial(q_all, k_cache, v_cache, positions - r * l_local, scale, sliding_window)
     # 3. combine across the group
     if n > 1:
         m_glob = comm.all_reduce(m.clone(), op="max", group=group)

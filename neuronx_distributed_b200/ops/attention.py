@@ -1,4 +1,4 @@
-"""Self-attention (flash style), causal or not, with an optional key-padding mask.  Kernel: ``csrc/attention_sm90.cu``
+"""Self-attention (flash style), causal or not, with an optional key-padding mask and, when causal, an optional sliding window.  Kernel: ``csrc/attention_sm90.cu``
 (tensor-core QK^T / PV with register accumulators, online softmax) for bf16 CUDA tensors with head_dim 64, 80, 96 or 128;
 otherwise the PyTorch SDPA library call, which is flagged as a *library* path in DESIGN.md.  Reference call sites:
 ``kernels/flash_attn.py:162-212`` (``nki_flash_attn_func``), ``modeling_llama_nxd.py:468-475``.
@@ -21,20 +21,33 @@ from . import _ext
 FLASH_HEAD_DIMS = (64, 80, 96, 128)
 
 
-def _sdpa(q, k, v, causal: bool, scale: Optional[float], key_padding_mask: Optional[torch.Tensor] = None):
+def window_visibility(s_q: int, s_kv: int, window: Optional[int], device=None) -> torch.Tensor:
+    """``[S_q, S_kv]`` bool: causal visibility, limited to the last ``window`` keys (query i sees i − W < j ≤ i) when
+    ``window`` is set."""
+    i = torch.arange(s_q, device=device)[:, None]
+    j = torch.arange(s_kv, device=device)[None, :]
+    vis = j <= i
+    return vis if window is None else vis & (j > i - window)
+
+
+def _sdpa(q, k, v, causal: bool, scale: Optional[float], key_padding_mask: Optional[torch.Tensor] = None,
+          window: Optional[int] = None):
     hq, hkv = q.shape[2], k.shape[2]
     qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
     if hq != hkv:
         kt = kt.repeat_interleave(hq // hkv, dim=1)
         vt = vt.repeat_interleave(hq // hkv, dim=1)
-    if key_padding_mask is None:
+    if key_padding_mask is None and window is None:
         o = F.scaled_dot_product_attention(qt, kt, vt, is_causal=causal, scale=scale)
     else:
-        # additive bias [B, 1, 1 or S_q, S_kv]: 0 where visible, −inf where masked (or above the diagonal when causal)
-        visible = key_padding_mask.bool()[:, None, None, :]
+        # additive bias [B or 1, 1, 1 or S_q, S_kv]: 0 where visible, −inf where masked (or above the diagonal when causal, or
+        # outside the window)
+        sq, sk = q.shape[1], k.shape[1]
+        visible = torch.ones(1, 1, 1, sk, dtype=torch.bool, device=q.device)
+        if key_padding_mask is not None:
+            visible = key_padding_mask.bool()[:, None, None, :]
         if causal:
-            sq, sk = q.shape[1], k.shape[1]
-            visible = visible & torch.ones(sq, sk, dtype=torch.bool, device=q.device).tril()
+            visible = visible & window_visibility(sq, sk, window, q.device)
         bias = torch.zeros(visible.shape, dtype=q.dtype, device=q.device).masked_fill(~visible, float("-inf"))
         o = F.scaled_dot_product_attention(qt, kt, vt, attn_mask=bias, scale=scale)
     return o.transpose(1, 2)
@@ -78,13 +91,13 @@ class _FlashAttn(torch.autograd.Function):
     model's ``[S,B,H·D]`` reshape is free."""
 
     @staticmethod
-    def forward(ctx, q, k, v, causal, scale, mask=None):
+    def forward(ctx, q, k, v, causal, scale, mask=None, window=0):
         e = _ext.ext()
         q, k, v = _tma_view(q), _tma_view(k), _tma_view(v)
         _ext.count_launch()
-        o, lse = e.flash_attn_fwd(q, k, v, bool(causal), float(scale), True, mask)
+        o, lse = e.flash_attn_fwd(q, k, v, bool(causal), float(scale), True, mask, int(window))
         ctx.save_for_backward(q, k, v, o, lse, mask)
-        ctx.causal, ctx.scale = causal, scale
+        ctx.causal, ctx.scale, ctx.window = causal, scale, window
         return o
 
     @staticmethod
@@ -92,8 +105,9 @@ class _FlashAttn(torch.autograd.Function):
         q, k, v, o, lse, mask = ctx.saved_tensors
         e = _ext.ext()
         _ext.count_launch(3)   # δ prep + dK/dV + dQ
-        dq, dk, dv = e.flash_attn_bwd(_tma_view(go), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale), True, None, mask)
-        return dq, dk, dv, None, None, None
+        dq, dk, dv = e.flash_attn_bwd(_tma_view(go), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale), True, None, mask,
+                                      int(ctx.window))
+        return dq, dk, dv, None, None, None, None
 
 
 class _FlashAttnLse(torch.autograd.Function):
@@ -127,37 +141,64 @@ def flash_attention_with_lse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, 
 
 
 def flash_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True,
-                    scale: Optional[float] = None, key_padding_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+                    scale: Optional[float] = None, key_padding_mask: Optional[torch.Tensor] = None,
+                    sliding_window: Optional[int] = None) -> torch.Tensor:
     """softmax(q·kᵀ·scale)·v for q ``[B, S_q, H, D]``, k/v ``[B, S_kv, Hkv, D]`` (H a multiple of Hkv) → ``[B, S_q, H, D]``.
 
     ``causal``: query i sees keys ≤ i (needs S_q == S_kv on the own kernels).  ``key_padding_mask``: ``[B, S_kv]`` bool
     (or integer, nonzero = visible); key j of batch b is visible iff ``key_padding_mask[b, j]``.  It combines with
     ``causal`` and GQA and is never read on the host, so the call stays capturable in CUDA graphs and launch plans.
+    ``sliding_window``: W ≥ 1 (causal only) limits query i to keys i − W < j ≤ i, the last W keys including its own (the rule
+    of Mistral / Mixtral); ``None`` means no window, and W ≥ S_kv is plain causal attention.  On the own kernels key tiles
+    wholly outside the window are skipped, so the work grows as S·W instead of S²/2.
 
     On the own kernels a masked key contributes nothing and gets dK = dV = 0, and a query row that sees no key at all gets
     O = 0 and dQ = 0.  The SDPA fallback (CPU, other dtypes or head sizes) follows SDPA's rule for such a row, which is NaN
     on some SDPA backends and versions."""
+    if sliding_window is not None and not causal:
+        raise ValueError("flash_attention: sliding_window needs causal=True")
+    window = check_window(sliding_window)
     scale = scale if scale is not None else 1.0 / math.sqrt(q.shape[-1])
     if flash_kernels_apply(q, k, v) and (not causal or q.shape[1] == k.shape[1]):
-        return _FlashAttn.apply(q, k, v, causal, scale, _kernel_mask(key_padding_mask))
-    return _sdpa(q, k, v, causal, scale, key_padding_mask)
+        return _FlashAttn.apply(q, k, v, causal, scale, _kernel_mask(key_padding_mask), window)
+    return _sdpa(q, k, v, causal, scale, key_padding_mask, window or None)
+
+
+def check_window(sliding_window: Optional[int]) -> int:
+    """``sliding_window`` (``None`` or ≥ 1) → the kernels' integer form (0 = no window); raises ``ValueError`` otherwise."""
+    if sliding_window is None:
+        return 0
+    if int(sliding_window) < 1:
+        raise ValueError(f"sliding_window must be >= 1 or None, got {sliding_window}")
+    return int(sliding_window)
 
 
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, positions: torch.Tensor,
-                     scale: Optional[float] = None) -> torch.Tensor:
+                     scale: Optional[float] = None, sliding_window: Optional[int] = None) -> torch.Tensor:
     """One new token per sequence against a KV cache: ``q [B,1,H,D]``, caches ``[B,L,Hkv,D]`` (any batch / sequence / head
-    strides), ``positions [B]`` = cache index of the newest token (keys ≤ position are visible).  CUDA bf16 with head_dim 128:
-    the split-KV flash-decoding kernel (``csrc/decode.cu``); otherwise SDPA with a length mask."""
+    strides), ``positions [B]`` = cache index of the newest token (keys ≤ position are visible; with ``sliding_window`` W only
+    keys position − W < j ≤ position, and the kernel reads only those rows).  CUDA bf16 with head_dim 128: the split-KV
+    flash-decoding kernel (``csrc/decode.cu``); otherwise SDPA with a length mask."""
     B, _, H, D = q.shape
     Hkv, L = k_cache.shape[2], k_cache.shape[1]
+    window = check_window(sliding_window)
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     e = _ext.ext() if q.is_cuda else None
     if (e is not None and hasattr(e, "decode_attention") and D == 128 and q.dtype == torch.bfloat16 and k_cache.dtype == torch.bfloat16
             and H // Hkv in (1, 2, 4, 8) and k_cache.stride(3) == 1 and v_cache.stride(3) == 1):
         _ext.count_launch(2)
-        return e.decode_attention(q.contiguous(), k_cache, v_cache, positions.to(torch.long).contiguous(), float(scale))
+        return e.decode_attention(q.contiguous(), k_cache, v_cache, positions.to(torch.long).contiguous(), float(scale), window)
     qt, kt, vt = q.transpose(1, 2), k_cache.transpose(1, 2), v_cache.transpose(1, 2)
     if H != Hkv:
         kt, vt = kt.repeat_interleave(H // Hkv, 1), vt.repeat_interleave(H // Hkv, 1)
-    mask = (torch.arange(L, device=q.device)[None, :] <= positions[:, None])[:, None, None, :]
+    mask = decode_visibility(positions, L, window)[:, None, None, :]
     return torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask, scale=scale).transpose(1, 2)
+
+
+def decode_visibility(positions: torch.Tensor, length: int, window: int = 0) -> torch.Tensor:
+    """``[B, length]`` bool: cache index j is visible to the token at ``positions[b]`` iff j ≤ position and, with a window
+    W > 0, j > position − W."""
+    j = torch.arange(length, device=positions.device)[None, :]
+    p = positions[:, None]
+    vis = j <= p
+    return vis if window <= 0 else vis & (j > p - window)

@@ -1,10 +1,15 @@
 """Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
-usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd]
+usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window]
 
 --perf times forward and forward+backward of the own kernels and of SDPA in the same process, alternating, at the shapes
 the models run (BERT-large with right padding, ViT-B/16, GPT-NeoX-20B per rank at TP=8, Pythia-2.8B, Llama-2-7B).  FLOPs
 come from the shapes: 4·D per visible (query, key) pair forward, 2.5× that backward; causal counts only the lower
-triangle and a key-padding mask only the visible keys."""
+triangle and a key-padding mask only the visible keys.
+
+--window (with --perf) times sliding-window attention instead, at the Mistral-7B per-GPU shape (B = 1, H = 32, Hkv = 8,
+D = 128, W = 4096) for S = 4k … 32k: the windowed kernels, the same kernels causal without a window, and SDPA with the windowed
+mask, all counted over the pairs the window leaves visible; then the decode kernel on a 32k cache with and without the
+window."""
 import argparse
 import json
 import math
@@ -115,6 +120,96 @@ def perf(e, bwd: bool):
         print(json.dumps(rec), flush=True)
 
 
+def visible_pairs(S: int, W: int) -> int:
+    """(query, key) pairs with i − W < j ≤ i: Σ_i min(i + 1, W)."""
+    w = min(W, S)
+    return w * (w + 1) // 2 + (S - w) * w
+
+
+def window_perf(e, bwd: bool, W: int = 4096):
+    dev = torch.device("cuda")
+    print(json.dumps(gpu_info()), flush=True)
+    B, H, Hkv, D = 1, 32, 8, 128
+    scale = 1.0 / math.sqrt(D)
+    g = torch.Generator(device=dev).manual_seed(0)
+    for S in (4096, 8192, 16384, 32768):
+        q, go = (torch.randn(B, S, H, D, device=dev, generator=g).bfloat16() for _ in range(2))
+        k, v = (torch.randn(B, S, Hkv, D, device=dev, generator=g).bfloat16() for _ in range(2))
+        fl = 4 * D * H * B * visible_pairs(S, W)                  # forward FLOPs over the pairs the window keeps
+
+        def own(window):
+            def f():
+                return e.flash_attn_fwd(q, k, v, True, scale, True, None, window)
+
+            def fb():
+                o, lse = f()
+                e.flash_attn_bwd(go, q, k, v, o, lse, True, scale, True, None, None, window)
+            return f, fb
+
+        qt, gt = q.transpose(1, 2), go.transpose(1, 2)
+        kt, vt = (t.transpose(1, 2).repeat_interleave(H // Hkv, 1) for t in (k, v))
+        bias = torch.zeros(S, S, device=dev, dtype=q.dtype).masked_fill(
+            ~attention.window_visibility(S, S, W, dev), float("-inf"))[None, None]
+        qr, kr, vr = (t.detach().requires_grad_(True) for t in (qt, kt, vt))
+
+        def sdpa_f():
+            return torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, attn_mask=bias)
+
+        def sdpa_fb():
+            o = torch.nn.functional.scaled_dot_product_attention(qr, kr, vr, attn_mask=bias)
+            torch.autograd.grad(o, (qr, kr, vr), gt)
+
+        fns = {"window": own(W), "causal": own(0), "sdpa_mask": (sdpa_f, sdpa_fb)}
+        # the windowed result against the masked SDPA one, at the shape that is timed
+        ow, _ = fns["window"][0]()
+        err = ((ow.float() - sdpa_f().transpose(1, 2).float()).abs().max() / ow.float().abs().max()).item()
+        t = {}
+        iters = max(3, 20 * 4096 // S)
+        for _ in range(2):                                        # alternate, keep each one's best
+            for name, (f, fb) in fns.items():
+                for key, fn in ((name + "_fwd", f), (name + "_fwd_bwd", fb if bwd else None)):
+                    if fn is None:
+                        continue
+                    try:
+                        t.setdefault(key, []).append(time_fn(fn, iters))
+                    except torch.OutOfMemoryError:
+                        t.setdefault(key, []).append(float("nan"))
+                        torch.cuda.empty_cache()
+        rec = {"bench": "mistral7b_window", "B": B, "S": S, "H": H, "Hkv": Hkv, "D": D, "W": W,
+               "visible_pairs_frac_of_causal": round(visible_pairs(S, W) / visible_pairs(S, S), 4),
+               "window_vs_sdpa_mask_rel_err": round(err, 5)}
+        for key, vals in t.items():
+            ms = min(vals)
+            rec[key + "_ms"] = round(ms, 4) if ms == ms else None
+            # TFLOP/s over the window's visible pairs for every column, so the causal column shows the cost of ignoring W
+            rec[key + "_tflops"] = round((3.5 if "bwd" in key else 1.0) * fl / ms / 1e9, 1) if ms == ms else None
+        for key in ("fwd", "fwd_bwd"):
+            if rec.get(f"window_{key}_ms") and rec.get(f"causal_{key}_ms"):
+                rec[f"causal_over_window_{key}"] = round(rec[f"causal_{key}_ms"] / rec[f"window_{key}_ms"], 2)
+            if rec.get(f"window_{key}_ms") and rec.get(f"sdpa_mask_{key}_ms"):
+                rec[f"sdpa_mask_over_window_{key}"] = round(rec[f"sdpa_mask_{key}_ms"] / rec[f"window_{key}_ms"], 2)
+        print(json.dumps(rec), flush=True)
+        del bias, q, k, v, go, qt, kt, vt, qr, kr, vr, fns, ow
+        torch.cuda.empty_cache()
+    # decode: one token per sequence against a 32k cache, newest position at the end of the cache
+    L = 32768
+    for Bd in (1, 8):
+        qd = torch.randn(Bd, 1, H, D, device=dev, generator=g).bfloat16()
+        kc, vc = (torch.randn(Bd, L, Hkv, D, device=dev, generator=g).bfloat16() for _ in range(2))
+        pos = torch.full((Bd,), L - 1, device=dev, dtype=torch.long)
+        t = {"full": [], "window": []}
+        for _ in range(3):
+            t["full"].append(time_fn(lambda: e.decode_attention(qd, kc, vc, pos, scale, 0)))
+            t["window"].append(time_fn(lambda: e.decode_attention(qd, kc, vc, pos, scale, W)))
+        rec = {"bench": "mistral7b_decode", "B": Bd, "L": L, "H": H, "Hkv": Hkv, "D": D, "W": W}
+        for name, rows in (("full", L), ("window", W)):
+            ms = min(t[name])
+            rec[name + "_us"] = round(ms * 1e3, 2)
+            rec[name + "_kv_GBps"] = round(2 * Bd * rows * Hkv * D * 2 / ms / 1e6, 1)   # K and V rows read, bf16
+        rec["full_over_window"] = round(rec["full_us"] / rec["window_us"], 2)
+        print(json.dumps(rec), flush=True)
+
+
 def time_fn(fn, iters=20):
     for _ in range(3):
         fn()
@@ -132,6 +227,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--perf", action="store_true")
     ap.add_argument("--bwd", action="store_true")
+    ap.add_argument("--window", action="store_true", help="with --perf: the sliding-window table instead of the model shapes")
     ap.add_argument("--head-dim", type=int, default=128, choices=attention.FLASH_HEAD_DIMS)
     a = ap.parse_args()
     dev = torch.device("cuda")
@@ -189,7 +285,7 @@ def main():
             ok_all &= ok
             print(json.dumps({"check": f"fa_bwd_{tag}", "ok": ok, **res}), flush=True)
     if a.perf:
-        perf(e, a.bwd)
+        (window_perf if a.window else perf)(e, a.bwd)
     print(json.dumps({"all_ok": ok_all}))
     sys.exit(0 if ok_all else 1)
 
