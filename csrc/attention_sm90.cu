@@ -20,8 +20,14 @@
 // kernels start their key-tile loop at the first tile that holds a key inside the window of the tile's first query row; the
 // dK/dV kernel stops its query-tile loop at the last tile whose rows can still see the key tile.  The per-element predicate
 // removes the rest.  W ≥ S computes exactly what the causal kernels compute.
+// Query offset (WINDOW kernels only): `q_offset` = off ≥ 0 is the global position of query row 0 minus that of key row 0, so
+// query i sees key j iff i + off − W < j ≤ i + off.  This is one off-diagonal block of context-parallel attention, whose
+// queries sit `off` positions after its keys.  Whole query rows (and tiles) of such a block can see no key: they get O = 0,
+// LSE = −inf and dQ = 0, and keys no row sees get dK = dV = 0.  off = 0 is the diagonal rule above.
 #include <cuda.h>
 
+#include <algorithm>
+#include <cstdint>
 #include <type_traits>
 
 #include "common.cuh"
@@ -164,7 +170,8 @@ struct FwdParams {
   int B, H, Hkv, S_q, S_kv, causal;
   float scale_log2;
   const uint8_t* mask; long mask_sb;            // key-padding mask [B, S_kv] (MASK kernels only)
-  int window;                                   // sliding window W, 1 ≤ W ≤ S_kv (WINDOW kernels only)
+  int window;                                   // sliding window W, 1 ≤ W ≤ S_kv + q_offset (WINDOW kernels only)
+  int q_offset;                                 // query row 0 minus key row 0 in global positions (WINDOW kernels only)
 };
 
 template <int HD, bool MASK, bool WINDOW>
@@ -183,9 +190,12 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
   const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
   const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
-  const int n_kv = p.causal ? min((p.S_kv + BT - 1) / BT, qt + 1) : (p.S_kv + BT - 1) / BT;
-  // window: keys ≤ q0 − W are outside the window of every row of the tile, so whole tiles of them are skipped
-  const int t_lo = WINDOW ? max(0, q0 - p.window + 1) / BT : 0;
+  const int off = WINDOW ? p.q_offset : 0;
+  // causal: the tile's last row sees keys up to q0 + 63 + off
+  const int n_kv =
+      p.causal ? min((p.S_kv + BT - 1) / BT, WINDOW ? (q0 + BT - 1 + off) / BT + 1 : qt + 1) : (p.S_kv + BT - 1) / BT;
+  // window: keys ≤ q0 + off − W are outside the window of every row of the tile, so whole tiles of them are skipped
+  const int t_lo = WINDOW ? max(0, q0 + off - p.window + 1) / BT : 0;
   const int b_lo = t_lo & 1;
 
   load_tile<HD>(sQ, qb, p.q.ss, q0, p.S_q);
@@ -222,8 +232,8 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
       for (int e = 0; e < 4; ++e) {
         const int key = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
         float x = s[j][e] * p.scale_log2;
-        if (key >= p.S_kv || (p.causal && key > row[e >> 1]) || (MASK && !fl[j * 8 + 2 * (lane & 3) + (e & 1)]) ||
-            (WINDOW && key <= row[e >> 1] - p.window))
+        if (key >= p.S_kv || (p.causal && key > row[e >> 1] + off) || (MASK && !fl[j * 8 + 2 * (lane & 3) + (e & 1)]) ||
+            (WINDOW && key <= row[e >> 1] + off - p.window))
           x = -INFINITY;
         s[j][e] = x;
         mx[e >> 1] = fmaxf(mx[e >> 1], x);
@@ -257,6 +267,7 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
     mma_pb<HD>(o, pf, sV + buf * kTl);
     __syncthreads();                              // buffer `buf` is refilled at the next iteration
   }
+  if (WINDOW) cp_async_wait<0>();                 // an offset tile that sees no key skips the loop with its first loads in flight
   float inv[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -308,7 +319,8 @@ struct BwdParams {
   int B, H, Hkv, S_q, S_kv, causal;
   float scale, scale_log2;
   const uint8_t* mask; long mask_sb;            // key-padding mask [B, S_kv] (MASK kernels only)
-  int window;                                   // sliding window W, 1 ≤ W ≤ S_kv (WINDOW kernels only)
+  int window;                                   // sliding window W, 1 ≤ W ≤ S_kv + q_offset (WINDOW kernels only)
+  int q_offset;                                 // query row 0 minus key row 0 in global positions (WINDOW kernels only)
 };
 
 template <int HD, bool MASK, bool WINDOW>
@@ -326,9 +338,11 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k0 = kt * BT;
   const int n_qt = (p.S_q + BT - 1) / BT;
-  const int qt0 = p.causal ? kt : 0;                 // causal: S_q == S_kv, query tiles before the key tile see none of it
-  // window: the last query row that sees key k0 + 63 is k0 + 63 + W − 1
-  const int qt_end = WINDOW ? min(n_qt, (k0 + BT - 1 + p.window - 1) / BT + 1) : n_qt;
+  const int off = WINDOW ? p.q_offset : 0;
+  // causal: S_q == S_kv, query rows before k0 − off see none of the key tile
+  const int qt0 = p.causal ? (WINDOW ? max(0, k0 - off) / BT : kt) : 0;
+  // window: the last query row that sees key k0 + 63 is k0 + 63 + W − 1 − off (a negative bound leaves the range empty)
+  const int qt_end = WINDOW ? min(n_qt, (k0 + 2 * BT - 2 + p.window - off) / BT) : n_qt;
   const int per_head = qt_end > qt0 ? qt_end - qt0 : 0;
   const int n_it = G * per_head;
 
@@ -384,8 +398,8 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
       for (int e = 0; e < 4; ++e) {
         const int qc = j * 8 + 2 * (lane & 3) + (e & 1);
         const int qi = q0 + qc;
-        const bool vis = qi < p.S_q && !(p.causal && key[e >> 1] > qi) && (!MASK || kvis[e >> 1]) &&
-                         !(WINDOW && qi >= key[e >> 1] + p.window);
+        const bool vis = qi < p.S_q && !(p.causal && key[e >> 1] > qi + off) && (!MASK || kvis[e >> 1]) &&
+                         !(WINDOW && qi + off >= key[e >> 1] + p.window);
         pt[j][e] = vis ? exp2f(pt[j][e] * p.scale_log2 - L[qc]) : 0.f;
       }
     }
@@ -406,6 +420,7 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
     mma_pb<HD>(dk, pf, q);                           // dK += dSᵀ·Q
     __syncthreads();
   }
+  if (WINDOW) cp_async_wait<0>();                    // a key tile no offset query sees skips the loop with K / V in flight
   store_rows<HD>(dk, p.dk + b * p.dk_sb + hk * p.dk_sh, p.dk_ss, k0 + warp * 16, p.S_kv, p.scale, p.scale);
   store_rows<HD>(dv, p.dv + b * p.dv_sb + hk * p.dv_sh, p.dv_ss, k0 + warp * 16, p.S_kv, 1.f, 1.f);
 }
@@ -431,8 +446,10 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) 
   const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
   const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
-  const int n_kv = p.causal ? min((p.S_kv + BT - 1) / BT, qt + 1) : (p.S_kv + BT - 1) / BT;
-  const int t_lo = WINDOW ? max(0, q0 - p.window + 1) / BT : 0;     // as in the forward
+  const int off = WINDOW ? p.q_offset : 0;
+  const int n_kv =
+      p.causal ? min((p.S_kv + BT - 1) / BT, WINDOW ? (q0 + BT - 1 + off) / BT + 1 : qt + 1) : (p.S_kv + BT - 1) / BT;
+  const int t_lo = WINDOW ? max(0, q0 + off - p.window + 1) / BT : 0;     // as in the forward
   const int b_lo = t_lo & 1;
 
   load_tile<HD>(sQ, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
@@ -476,8 +493,8 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) 
       for (int e = 0; e < 4; ++e) {
         const int kc = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
         const int r = row[e >> 1];
-        const bool vis = kc < p.S_kv && r < p.S_q && !(p.causal && kc > r) && (!MASK || fl[j * 8 + 2 * (lane & 3) + (e & 1)]) &&
-                         !(WINDOW && kc <= r - p.window);
+        const bool vis = kc < p.S_kv && r < p.S_q && !(p.causal && kc > r + off) && (!MASK || fl[j * 8 + 2 * (lane & 3) + (e & 1)]) &&
+                         !(WINDOW && kc <= r + off - p.window);
         s[j][e] = vis ? exp2f(s[j][e] * p.scale_log2 - L[e >> 1]) : 0.f;
       }
     }
@@ -493,6 +510,7 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) 
     mma_pb<HD>(dq, pf, k);                           // dQ += dS·K
     __syncthreads();
   }
+  if (WINDOW) cp_async_wait<0>();                    // as in the forward
   store_rows<HD>(dq, p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, q0 + warp * 16, p.S_q, p.scale, p.scale);
 }
 
@@ -547,15 +565,28 @@ static void launch_bwd(const BwdParams& p, cudaStream_t st) {
   fa_bwd_dq_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem_dq, st>>>(p);
 }
 
+static void check_args(int S_q, int S_kv, bool causal, int window, int q_offset) {
+  if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
+  if (window < 0) nxd_throw("attention: window must be >= 0 (0 = none)", __FILE__, __LINE__);
+  if (window > 0 && !causal) nxd_throw("attention: a sliding window needs causal attention", __FILE__, __LINE__);
+  if (q_offset < 0) nxd_throw("attention: q_offset must be >= 0", __FILE__, __LINE__);
+  if (q_offset > 0 && window == 0) nxd_throw("attention: q_offset needs a sliding window", __FILE__, __LINE__);
+  // tile bounds reach 2·S + q_offset + 2·64 in 32-bit arithmetic
+  if (2L * S_kv + q_offset + 2 * BT > INT32_MAX) nxd_throw("attention: q_offset too large", __FILE__, __LINE__);
+}
+
+// W ≥ S_kv + q_offset sees every causal key; the clamp keeps tile bounds in range
+static int clamp_window(int window, int S_kv, int q_offset) {
+  return (int)std::min<long>(window, (long)S_kv + q_offset);
+}
+
 }  // namespace fa
 
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
                     int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    const void* kpm, long kpm_sb, int window, cudaStream_t st) {
+                    const void* kpm, long kpm_sb, int window, int q_offset, cudaStream_t st) {
   using namespace fa;
-  if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
-  if (window < 0) nxd_throw("attention: window must be >= 0 (0 = none)", __FILE__, __LINE__);
-  if (window > 0 && !causal) nxd_throw("attention: a sliding window needs causal attention", __FILE__, __LINE__);
+  check_args(S_q, S_kv, causal, window, q_offset);
   FwdParams p;
   p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs);
   p.o = (bf16*)out; p.o_sb = os[0]; p.o_ss = os[1]; p.o_sh = os[2];
@@ -563,7 +594,8 @@ void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, floa
   p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
   p.scale_log2 = scale * kLog2e;
   p.mask = (const uint8_t*)kpm; p.mask_sb = kpm_sb;
-  p.window = window < S_kv ? window : S_kv;       // W ≥ S_kv sees every causal key; the clamp keeps tile bounds in range
+  p.window = clamp_window(window, S_kv, q_offset);
+  p.q_offset = q_offset;
   dispatch(D, kpm != nullptr, window > 0, [&](auto hd, auto mk, auto wd) {
     launch_fwd<decltype(hd)::value, decltype(mk)::value, decltype(wd)::value>(p, st);
   });
@@ -574,11 +606,9 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
                     int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
                     const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, int window,
-                    cudaStream_t st) {
+                    int q_offset, cudaStream_t st) {
   using namespace fa;
-  if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
-  if (window < 0) nxd_throw("attention: window must be >= 0 (0 = none)", __FILE__, __LINE__);
-  if (window > 0 && !causal) nxd_throw("attention: a sliding window needs causal attention", __FILE__, __LINE__);
+  check_args(S_q, S_kv, causal, window, q_offset);
   BwdParams p;
   p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs); p.g = view(go, gs);
   p.dq = (bf16*)dq; p.dk = (bf16*)dk; p.dv = (bf16*)dv;
@@ -589,7 +619,8 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
   p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
   p.scale = scale; p.scale_log2 = scale * kLog2e;
   p.mask = (const uint8_t*)kpm; p.mask_sb = kpm_sb;
-  p.window = window < S_kv ? window : S_kv;
+  p.window = clamp_window(window, S_kv, q_offset);
+  p.q_offset = q_offset;
   dispatch(D, kpm != nullptr, window > 0, [&](auto hd, auto mk, auto wd) {
     constexpr int HD = decltype(hd)::value;
     const long rows = (long)B * H * S_q;

@@ -142,16 +142,17 @@ void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int 
 
 // ---- attention (attention_sm90.cu): q [B,S_q,H,D], k/v [B,S_kv,Hkv,D] bf16 views, D ∈ {64, 80, 96, 128}; strides = (b, s, h)
 // in elements.  kpm: optional key-padding mask, uint8 [B, S_kv] with row stride kpm_sb (key visible iff nonzero), or null.
-// window: sliding window W (causal only; query i sees keys i − W < j ≤ i), or 0 for none.
+// window: sliding window W (causal only; query i sees keys i − W < j ≤ i), or 0 for none.  q_offset ≥ 0 (window only): global
+// position of query row 0 minus that of key row 0, so query i sees keys i + q_offset − W < j ≤ i + q_offset.
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
                     int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    const void* kpm, long kpm_sb, int window, cudaStream_t st);
+                    const void* kpm, long kpm_sb, int window, int q_offset, cudaStream_t st);
 
 // delta: fp32 scratch [B, H, S_q]; dlse may be null
 void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
                     int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
                     const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, int window,
-                    cudaStream_t st);
+                    int q_offset, cudaStream_t st);
 
 }  // namespace nxd

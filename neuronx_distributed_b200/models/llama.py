@@ -147,12 +147,15 @@ class LlamaAttention(nn.Module):
         if self.cfg.context_parallel and ps.get_context_model_parallel_size() > 1:
             from ..modules.attention.ring import pull_attention, ring_attention
 
-            if self.cfg.sliding_window is not None:
-                raise NotImplementedError("sliding_window is not supported with context parallelism")
+            w = self.cfg.sliding_window
+            if w is not None and not _CP_WINDOW:
+                raise NotImplementedError("sliding_window with context parallelism is opt-in until the windowed ring has run on "
+                                          "several GPUs: set NXD_CP_WINDOW=1")
             if self.cfg.cp_layout != "contiguous":
-                o = pull_attention(q, k, v, causal=True, layout=self.cfg.cp_layout)      # the ring keeps the contiguous split
+                # the ring keeps the contiguous split
+                o = pull_attention(q, k, v, causal=True, layout=self.cfg.cp_layout, sliding_window=w)
             else:
-                o = (pull_attention if _CP_PULL else ring_attention)(q, k, v, causal=True)
+                o = (pull_attention if _CP_PULL else ring_attention)(q, k, v, causal=True, sliding_window=w)
         else:
             o = ops.attention.flash_attention(q, k, v, causal=True, sliding_window=self.cfg.sliding_window)
         o = o.transpose(0, 1).reshape(S, B, self.num_heads_local * self.head_dim)
@@ -170,6 +173,10 @@ _LMHEAD_CE_CHUNK = int(os.environ.get("NXD_LMHEAD_CE_CHUNK", "2048"))
 # context parallelism without a ring: K/V published in symmetric memory, peers' slices read inside the attention kernel
 # (modules/attention/ring.py ``pull_attention``).  Opt-in: CPU-verified against the ring and dense attention only.
 _CP_PULL = os.environ.get("NXD_CP_PULL", "0") == "1"
+# sliding window under context parallelism (ring / pull attention with the windowed block plan).  Opt-in: CPU-verified
+# multi-process and emulated in one process on an H100 (tests/test_cp_sliding_window_*.py); the NCCL ring with a window has
+# not yet run on more than one GPU.  Without it a windowed model raises NotImplementedError at CP > 1, as before.
+_CP_WINDOW = os.environ.get("NXD_CP_WINDOW", "0") == "1"
 
 
 class LlamaDecoderLayer(nn.Module):

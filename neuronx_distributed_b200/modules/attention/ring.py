@@ -11,6 +11,11 @@ compute; the exchange is itself an autograd node (its backward moves dK/dV the o
 backward is the exact transpose of forward without a hand-written second pass.  Per-block attention is the own
 flash kernel with a differentiable LSE output (``ops.attention.flash_attention_with_lse``; head_dim 64/80/96/128, bf16), the SDPA
 flash op for other shapes on CUDA, and an fp32 reference on CPU.
+
+Sliding window W (Mistral / Mixtral): a block whose queries sit ``off`` positions after its keys is computed by the windowed
+kernels with that query offset, and is empty once off ≥ W + c − 1 (c = chunk length).  So with the contiguous split a rank
+needs K/V only from the previous ceil((W − 1)/c) ranks, and the ring stops after that many hops.  ``_visible_pairs`` is the one
+block plan both the ring and the pull implementation iterate.
 """
 from __future__ import annotations
 
@@ -23,31 +28,74 @@ import torch.distributed as dist
 from ...parallel_layers import parallel_state as ps
 
 
-def block_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool, scale: float
-                    ) -> Tuple[torch.Tensor, torch.Tensor]:
-    """q [B,Sq,H,D], k/v [B,Sk,Hkv,D] → (out [B,Sq,H,D], lse [B,H,Sq] fp32)."""
+def _block_visibility(sq: int, sk: int, window: Optional[int], q_offset: int, device) -> torch.Tensor:
+    """``[sq, sk]`` visibility of a causal block.  CP blocks have equal lengths; a shorter query block aligns its last row with
+    the last key, as SDPA's flash op does."""
+    from ... import ops
+
+    return ops.attention.window_visibility(sq, sk, window, device, q_offset + sk - sq)
+
+
+def block_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool, scale: float,
+                    window: Optional[int] = None, q_offset: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+    """q [B,Sq,H,D], k/v [B,Sk,Hkv,D] → (out [B,Sq,H,D], lse [B,H,Sq] fp32).
+
+    A causal block sees keys j ≤ i + q_offset, and with a sliding ``window`` W only j > i + q_offset − W (``q_offset``: global
+    position of query row 0 minus that of key row 0).  A dense block (``causal=False``) sees every key, so ``window`` and
+    ``q_offset`` apply to causal blocks only.  A row that sees no key gets O = 0 and LSE = −inf."""
+    if not causal:
+        window, q_offset = None, 0
     if q.is_cuda:
         from ... import ops
 
-        own = ops.attention.flash_attention_with_lse(q, k, v, causal, scale)      # own kernels, LSE differentiable
+        own = ops.attention.flash_attention_with_lse(q, k, v, causal, scale, window, q_offset)   # own kernels, LSE differentiable
         if own is not None:
             return own
     hq, hkv = q.shape[2], k.shape[2]
     qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
     if hq != hkv:
         kt, vt = kt.repeat_interleave(hq // hkv, 1), vt.repeat_interleave(hq // hkv, 1)
-    if q.is_cuda and q.dtype in (torch.bfloat16, torch.float16):
+    # the SDPA flash op takes no mask, so a windowed block it would get goes to the masked fp32 path below
+    if q.is_cuda and q.dtype in (torch.bfloat16, torch.float16) and window is None and q_offset == 0:
         out, lse = torch.ops.aten._scaled_dot_product_flash_attention(qt, kt, vt, 0.0, causal, False, scale=scale)[:2]
         return out.transpose(1, 2), lse.float()
     s = torch.matmul(qt.float(), kt.float().transpose(-1, -2)) * scale
     if causal:
-        sq, sk = s.shape[-2], s.shape[-1]
-        mask = torch.ones(sq, sk, dtype=torch.bool, device=s.device).tril(diagonal=sk - sq)
-        s = s.masked_fill(~mask, float("-inf"))
-    lse = torch.logsumexp(s, dim=-1)
-    p = torch.exp(s - lse.unsqueeze(-1))
+        vis = _block_visibility(s.shape[-2], s.shape[-1], window, q_offset, s.device)
+        s = s.masked_fill(~vis, float("-inf"))
+        # a row with no visible key (possible with an offset window): logsumexp over zeros keeps its gradient finite, its
+        # P is exp(−inf) = 0, and its LSE is set to −inf afterwards
+        empty = ~vis.any(-1)
+        lse = torch.logsumexp(s.masked_fill(empty[:, None], 0.0), dim=-1)
+        p = torch.exp(s - lse.unsqueeze(-1))
+        lse = lse.masked_fill(empty, float("-inf"))
+    else:
+        lse = torch.logsumexp(s, dim=-1)
+        p = torch.exp(s - lse.unsqueeze(-1))
     out = torch.matmul(p, vt.float()).to(q.dtype)
     return out.transpose(1, 2), lse
+
+
+def _merge_block(out: Optional[torch.Tensor], lse: Optional[torch.Tensor], o_b: torch.Tensor, lse_b: torch.Tensor):
+    """Fold one block's ``(o_b [B,S,H,D], lse_b [B,H,S])`` into the running ``(out fp32, lse)`` by log-sum-exp weights;
+    ``out is None`` starts the merge.  A row for which both LSEs are −inf (no key seen yet, e.g. an offset window) keeps O = 0
+    and LSE = −inf, with no NaN in the forward or the backward, whatever the block order."""
+    if out is None:
+        return o_b.float(), lse_b.float()
+    empty = torch.isneginf(lse) & torch.isneginf(lse_b)
+    lse, lse_b = lse.masked_fill(empty, 0.0), lse_b.masked_fill(empty, 0.0)      # both O are 0 there: any finite weights do
+    new = torch.logaddexp(lse, lse_b)
+    w_old = torch.exp(lse - new).transpose(1, 2).unsqueeze(-1)     # [B,S,H,1]
+    w_new = torch.exp(lse_b - new).transpose(1, 2).unsqueeze(-1)
+    return out * w_old + o_b.float() * w_new, new.masked_fill(empty, float("-inf"))
+
+
+def _window_arg(sliding_window: Optional[int], causal: bool) -> Optional[int]:
+    from ... import ops
+
+    if sliding_window is not None and not causal:
+        raise ValueError("sliding_window needs causal=True")
+    return ops.attention.check_window(sliding_window) or None
 
 
 class _RingShift(torch.autograd.Function):
@@ -71,33 +119,39 @@ def _exchange(x: torch.Tensor, group, send_to: int, recv_from: int) -> torch.Ten
     return buf
 
 
+def ring_hops(cp: int, chunk: int, window: Optional[int]) -> int:
+    """Ring shifts per pass: cp − 1, or with a sliding window only as far back as a block can still be visible,
+    min(cp − 1, ceil((W − 1) / chunk)).  It depends on shapes only, so every rank derives the same count."""
+    return cp - 1 if window is None else min(cp - 1, -(-(window - 1) // chunk))
+
+
 def ring_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True,
-                   scale: Optional[float] = None, group=None) -> torch.Tensor:
-    """q/k/v: this rank's ``[B, S/cp, H, D]`` slices → attention output for the local queries."""
+                   scale: Optional[float] = None, group=None, sliding_window: Optional[int] = None) -> torch.Tensor:
+    """q/k/v: this rank's ``[B, S/cp, H, D]`` slices (contiguous split) → attention output for the local queries.
+
+    ``sliding_window`` W (causal only): query i sees keys i − W < j ≤ i in global positions; the ring then stops after
+    :func:`ring_hops` shifts, so a rank receives K/V only from the ranks its window reaches."""
     group = group if group is not None else ps.get_context_model_parallel_group()
     cp = dist.get_world_size(group)
     scale = scale if scale is not None else 1.0 / math.sqrt(q.shape[-1])
+    window = _window_arg(sliding_window, causal)
     if cp == 1:
-        return block_attention(q, k, v, causal, scale)[0]
+        return block_attention(q, k, v, causal, scale, window)[0]
     r = dist.get_rank(group)
     ranks = dist.get_process_group_ranks(group)
     nxt, prv = ranks[(r + 1) % cp], ranks[(r - 1) % cp]
+    hops = ring_hops(cp, q.shape[1], window)
+    plan = _visible_pairs(r, cp, "contiguous", causal, window, q.shape[1])
+    blocks = {src: (blk_causal, off) for _, src, _, blk_causal, off in plan}           # one block per source rank
     out: Optional[torch.Tensor] = None
     lse: Optional[torch.Tensor] = None
     kv = torch.stack([k, v])  # travel together: one message per hop
-    for step in range(cp):
+    for step in range(hops + 1):
         src = (r - step) % cp                       # origin rank of the block currently held
-        nxt_kv = _RingShift.apply(kv, group, nxt, prv) if step < cp - 1 else None   # start next hop early
-        if not causal or src <= r:
-            o_b, lse_b = block_attention(q, kv[0], kv[1], causal and src == r, scale)
-            if out is None:
-                out, lse = o_b.float(), lse_b
-            else:
-                new_lse = torch.logaddexp(lse, lse_b)
-                w_old = torch.exp(lse - new_lse).transpose(1, 2).unsqueeze(-1)     # [B,S,H,1]
-                w_new = torch.exp(lse_b - new_lse).transpose(1, 2).unsqueeze(-1)
-                out = out * w_old + o_b.float() * w_new
-                lse = new_lse
+        nxt_kv = _RingShift.apply(kv, group, nxt, prv) if step < hops else None   # start next hop early
+        if src in blocks:
+            o_b, lse_b = block_attention(q, kv[0], kv[1], blocks[src][0], scale, window, blocks[src][1])
+            out, lse = _merge_block(out, lse, o_b, lse_b)
         if nxt_kv is None:
             last_kv = kv
         kv = nxt_kv
@@ -115,9 +169,12 @@ def ring_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bo
 # (dQ, dK, dV) from the GLOBAL softmax statistics (so no per-block LSE gradients are needed) and returns the dK/dV
 # contributions to their owners with ONE reduce-scatter (in-switch sum on NVLS).
 # ---------------------------------------------------------------------------------------------------------------------
-def _block_backward(q, k, v, out, lse, dout, causal: bool, scale: float):
+def _block_backward(q, k, v, out, lse, dout, causal: bool, scale: float, window: Optional[int] = None, q_offset: int = 0):
     """Gradients of one K/V block given the GLOBAL output ``out`` / log-normaliser ``lse`` of the rows:
-    P = exp(S − lse), dV = Pᵀ dO, dS = P ∘ (dO Vᵀ − rowsum(dO ∘ out)), dQ = dS K · scale, dK = dSᵀ Q · scale."""
+    P = exp(S − lse), dV = Pᵀ dO, dS = P ∘ (dO Vᵀ − rowsum(dO ∘ out)), dQ = dS K · scale, dK = dSᵀ Q · scale.
+    ``window`` / ``q_offset``: the visibility of a causal block, as in :func:`block_attention`."""
+    if not causal:
+        window, q_offset = None, 0
     if q.is_cuda:
         from ... import ops
 
@@ -126,7 +183,7 @@ def _block_backward(q, k, v, out, lse, dout, causal: bool, scale: float):
             ops._ext.count_launch(4)
             tv = ops.attention._tma_view
             dq, dk, dv = e.flash_attn_bwd(tv(dout.to(out.dtype)), tv(q), tv(k), tv(v), tv(out), lse.contiguous(), bool(causal),
-                                          float(scale), False, None)
+                                          float(scale), False, None, None, ops.attention.check_window(window), int(q_offset))
             return dq, dk, dv
     hq, hkv = q.shape[2], k.shape[2]
     g = hq // hkv
@@ -134,8 +191,7 @@ def _block_backward(q, k, v, out, lse, dout, causal: bool, scale: float):
     kt, vt = k.transpose(1, 2).float().repeat_interleave(g, 1), v.transpose(1, 2).float().repeat_interleave(g, 1)
     s = torch.matmul(qt, kt.transpose(-1, -2)) * scale
     if causal:
-        sq, sk = s.shape[-2], s.shape[-1]
-        s = s.masked_fill(~torch.ones(sq, sk, dtype=torch.bool, device=s.device).tril(diagonal=sk - sq), float("-inf"))
+        s = s.masked_fill(~_block_visibility(s.shape[-2], s.shape[-1], window, q_offset, s.device), float("-inf"))
     p = torch.exp(s - lse.unsqueeze(-1))
     dv = torch.matmul(p.transpose(-1, -2), dot)
     ds = p * (torch.matmul(dot, vt.transpose(-1, -2)) - (dot * ot).sum(-1, keepdim=True))
@@ -157,8 +213,15 @@ def _chunk_ids(rank: int, cp: int, layout: str):
     raise ValueError(f"unknown context-parallel layout {layout!r}")
 
 
-def _visible_pairs(rank: int, cp: int, layout: str, causal: bool):
-    """(local query chunk index, source rank, source chunk index, is_diagonal) for every block this rank computes; own rank first."""
+def _visible_pairs(rank: int, cp: int, layout: str, causal: bool, window: Optional[int] = None, chunk: int = 1):
+    """The block plan of one rank: ``(local query chunk, source rank, source chunk, causal, q_offset)`` for every non-empty
+    block it computes, own rank first, then the ranks before it round the ring.
+
+    ``chunk``: positions per sequence chunk; ``q_offset`` is the global position of the block's query row 0 minus that of its
+    key row 0, (gq − gk)·chunk.  ``causal`` says whether the block needs the causal rule (with ``window`` W, the windowed rule
+    at that offset); a block with ``causal=False`` sees every key.  Without a window only the diagonal is causal.  With one,
+    a block is empty, and left out, iff q_offset ≥ W + chunk − 1, and fully visible iff q_offset > 0 and
+    W ≥ q_offset + chunk."""
     mine = _chunk_ids(rank, cp, layout)
     pairs = []
     for step in range(cp):
@@ -166,14 +229,20 @@ def _visible_pairs(rank: int, cp: int, layout: str, causal: bool):
         theirs = _chunk_ids(src, cp, layout)
         for qi, gq in enumerate(mine):
             for kj, gk in enumerate(theirs):
-                if not causal or gk <= gq:
-                    pairs.append((qi, src, kj, causal and gk == gq))
+                off = (gq - gk) * chunk
+                if not causal:
+                    pairs.append((qi, src, kj, False, off))
+                elif gk <= gq:
+                    if window is None:
+                        pairs.append((qi, src, kj, gk == gq, off))
+                    elif off < window + chunk - 1:
+                        pairs.append((qi, src, kj, gk == gq or window < off + chunk, off))
     return pairs
 
 
 class _PullAttention(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, causal, scale, group, layout):
+    def forward(ctx, q, k, v, causal, scale, group, layout, window):
         from ... import ops
 
         cp, r = dist.get_world_size(group), dist.get_rank(group)
@@ -185,20 +254,14 @@ class _PullAttention(torch.autograd.Function):
         outs = [None] * nq
         lses = [None] * nq
         with torch.no_grad():
-            for qi, src, kj, diag in _visible_pairs(r, cp, layout, causal):
+            for qi, src, kj, blk_causal, off in _visible_pairs(r, cp, layout, causal, window, q.shape[1] // nq):
                 kb, vb = views[src][0].chunk(nq, dim=1)[kj], views[src][1].chunk(nq, dim=1)[kj]
-                o_b, lse_b = block_attention(qs[qi], kb, vb, diag, scale)
-                if outs[qi] is None:
-                    outs[qi], lses[qi] = o_b.float(), lse_b.float()
-                else:
-                    new = torch.logaddexp(lses[qi], lse_b)
-                    outs[qi] = outs[qi] * torch.exp(lses[qi] - new).transpose(1, 2).unsqueeze(-1) + \
-                        o_b.float() * torch.exp(lse_b - new).transpose(1, 2).unsqueeze(-1)
-                    lses[qi] = new
+                o_b, lse_b = block_attention(qs[qi], kb, vb, blk_causal, scale, window, off)
+                outs[qi], lses[qi] = _merge_block(outs[qi], lses[qi], o_b, lse_b)
         out = torch.cat(outs, dim=1).to(q.dtype)
         lse = torch.cat(lses, dim=2)                                 # [B, H, S/cp]
         ctx.save_for_backward(q, k, v, out, lse)
-        ctx.causal, ctx.scale, ctx.group, ctx.layout = causal, scale, group, layout
+        ctx.causal, ctx.scale, ctx.group, ctx.layout, ctx.window = causal, scale, group, layout, window
         return out
 
     @staticmethod
@@ -207,7 +270,7 @@ class _PullAttention(torch.autograd.Function):
         from ...parallel_layers import comm
 
         q, k, v, out, lse = ctx.saved_tensors
-        group, causal, scale, layout = ctx.group, ctx.causal, ctx.scale, ctx.layout
+        group, causal, scale, layout, window = ctx.group, ctx.causal, ctx.scale, ctx.layout, ctx.window
         cp, r = dist.get_world_size(group), dist.get_rank(group)
         nq = len(_chunk_ids(r, cp, layout))
         views = ops.nvls.publish(torch.stack([k, v]).contiguous(), group)          # peers' K/V again (the slot was reused since)
@@ -216,10 +279,10 @@ class _PullAttention(torch.autograd.Function):
         qs, os_, ds = q.chunk(nq, dim=1), out.chunk(nq, dim=1), dout.contiguous().chunk(nq, dim=1)
         ls = lse.chunk(nq, dim=2)
         c = k.shape[1] // nq
-        for qi, src, kj, diag in _visible_pairs(r, cp, layout, causal):
+        for qi, src, kj, blk_causal, off in _visible_pairs(r, cp, layout, causal, window, c):
             kb, vb = views[src][0].chunk(nq, dim=1)[kj], views[src][1].chunk(nq, dim=1)[kj]
             dq_b, dk_b, dv_b = _block_backward(qs[qi].contiguous(), kb.contiguous(), vb.contiguous(), os_[qi].contiguous(),
-                                               ls[qi].contiguous(), ds[qi].contiguous(), diag, scale)
+                                               ls[qi].contiguous(), ds[qi].contiguous(), blk_causal, scale, window, off)
             dqs[qi] += dq_b.float()
             dkv[src, 0, :, kj * c:(kj + 1) * c] += dk_b.float()
             dkv[src, 1, :, kj * c:(kj + 1) * c] += dv_b.float()
@@ -230,17 +293,19 @@ class _PullAttention(torch.autograd.Function):
         else:
             mine = comm.reduce_scatter(flat, dim=0, group=group)
         mine = mine.view(dkv.shape[1:])
-        return torch.cat(dqs, dim=1).to(q.dtype), mine[0].to(k.dtype), mine[1].to(v.dtype), None, None, None, None
+        return torch.cat(dqs, dim=1).to(q.dtype), mine[0].to(k.dtype), mine[1].to(v.dtype), None, None, None, None, None
 
 
 def pull_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True, scale: Optional[float] = None,
-                   group=None, layout: str = "contiguous") -> torch.Tensor:
+                   group=None, layout: str = "contiguous", sliding_window: Optional[int] = None) -> torch.Tensor:
     """Same contract as :func:`ring_attention` (``[B, S/cp, H, D]`` slices in, local output out), no ring: see the section
     comment above.  ``layout="zigzag"``: the local slice is chunks (r, 2·cp−1−r) of the sequence (``utils.batch_utils`` cuts
     batches that way) — causal work is then balanced over the ranks.  Opt-in from the models with ``NXD_CP_PULL=1`` until the
-    symmetric-memory path has run on hardware."""
+    symmetric-memory path has run on hardware.  ``sliding_window``: as in :func:`ring_attention`; blocks wholly outside the window
+    are neither read nor computed."""
     group = group if group is not None else ps.get_context_model_parallel_group()
     scale = scale if scale is not None else 1.0 / math.sqrt(q.shape[-1])
+    window = _window_arg(sliding_window, causal)
     if dist.get_world_size(group) == 1:
-        return block_attention(q, k, v, causal, scale)[0]
-    return _PullAttention.apply(q, k, v, causal, scale, group, layout)
+        return block_attention(q, k, v, causal, scale, window)[0]
+    return _PullAttention.apply(q, k, v, causal, scale, group, layout, window)

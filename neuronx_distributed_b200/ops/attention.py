@@ -21,10 +21,11 @@ from . import _ext
 FLASH_HEAD_DIMS = (64, 80, 96, 128)
 
 
-def window_visibility(s_q: int, s_kv: int, window: Optional[int], device=None) -> torch.Tensor:
+def window_visibility(s_q: int, s_kv: int, window: Optional[int], device=None, q_offset: int = 0) -> torch.Tensor:
     """``[S_q, S_kv]`` bool: causal visibility, limited to the last ``window`` keys (query i sees i − W < j ≤ i) when
-    ``window`` is set."""
-    i = torch.arange(s_q, device=device)[:, None]
+    ``window`` is set.  ``q_offset``: global position of query row 0 minus that of key row 0 (a context-parallel block whose
+    queries come after its keys); query i then sees i + q_offset − W < j ≤ i + q_offset."""
+    i = torch.arange(s_q, device=device)[:, None] + q_offset
     j = torch.arange(s_kv, device=device)[None, :]
     vis = j <= i
     return vis if window is None else vis & (j > i - window)
@@ -115,12 +116,12 @@ class _FlashAttnLse(torch.autograd.Function):
     a gradient into LSE only shifts δ in the backward kernel (``dS = P∘(dP − (δ − g_lse))``)."""
 
     @staticmethod
-    def forward(ctx, q, k, v, causal, scale):
+    def forward(ctx, q, k, v, causal, scale, window=0, q_offset=0):
         q, k, v = _tma_view(q), _tma_view(k), _tma_view(v)
         _ext.count_launch()
-        o, lse = _ext.ext().flash_attn_fwd(q, k, v, bool(causal), float(scale), False)
+        o, lse = _ext.ext().flash_attn_fwd(q, k, v, bool(causal), float(scale), False, None, int(window), int(q_offset))
         ctx.save_for_backward(q, k, v, o, lse)
-        ctx.causal, ctx.scale = causal, scale
+        ctx.causal, ctx.scale, ctx.window, ctx.q_offset = causal, scale, window, q_offset
         return o, lse
 
     @staticmethod
@@ -129,14 +130,25 @@ class _FlashAttnLse(torch.autograd.Function):
         _ext.count_launch(3)
         go = torch.zeros_like(o) if go is None else go
         dlse = None if g_lse is None else g_lse.float().contiguous()
-        dq, dk, dv = _ext.ext().flash_attn_bwd(_tma_view(go.to(o.dtype)), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale), False, dlse)
-        return dq, dk, dv, None, None
+        dq, dk, dv = _ext.ext().flash_attn_bwd(_tma_view(go.to(o.dtype)), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale),
+                                               False, dlse, None, int(ctx.window), int(ctx.q_offset))
+        return dq, dk, dv, None, None, None, None
 
 
-def flash_attention_with_lse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool, scale: float):
-    """``(out [B,S,H,D], lse [B,H,S] fp32)`` on the own kernels, or ``None`` when they do not apply."""
+def flash_attention_with_lse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool, scale: float,
+                             sliding_window: Optional[int] = None, q_offset: int = 0):
+    """``(out [B,S,H,D], lse [B,H,S] fp32)`` on the own kernels, or ``None`` when they do not apply.
+
+    ``sliding_window`` as in :func:`flash_attention`.  ``q_offset`` ≥ 0 (causal, with a window): the global position of query
+    row 0 minus that of key row 0, as in one off-diagonal block of context-parallel attention; query i then sees keys
+    i + q_offset − W < j ≤ i + q_offset.  A row that sees no key gets O = 0 and LSE = −inf."""
+    if sliding_window is not None and not causal:
+        raise ValueError("flash_attention_with_lse: sliding_window needs causal=True")
+    window = check_window(sliding_window)
+    if q_offset < 0 or (q_offset > 0 and window == 0):
+        raise ValueError(f"flash_attention_with_lse: q_offset must be 0, or > 0 with a sliding_window; got {q_offset}")
     if flash_kernels_apply(q, k, v) and (not causal or q.shape[1] == k.shape[1]):
-        return _FlashAttnLse.apply(q, k, v, causal, scale)
+        return _FlashAttnLse.apply(q, k, v, causal, scale, window, q_offset)
     return None
 
 

@@ -1,5 +1,5 @@
 """Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
-usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window]
+usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]]
 
 --perf times forward and forward+backward of the own kernels and of SDPA in the same process, alternating, at the shapes
 the models run (BERT-large with right padding, ViT-B/16, GPT-NeoX-20B per rank at TP=8, Pythia-2.8B, Llama-2-7B).  FLOPs
@@ -9,7 +9,14 @@ triangle and a key-padding mask only the visible keys.
 --window (with --perf) times sliding-window attention instead, at the Mistral-7B per-GPU shape (B = 1, H = 32, Hkv = 8,
 D = 128, W = 4096) for S = 4k … 32k: the windowed kernels, the same kernels causal without a window, and SDPA with the windowed
 mask, all counted over the pairs the window leaves visible; then the decode kernel on a 32k cache with and without the
-window."""
+window.
+
+--window --cp N (with --perf) emulates one layer's context-parallel attention at the same shape for S = 32k, 64k and 128k on
+one GPU: the blocks the rank with the most work computes under the windowed block plan (``modules/attention/ring.py``
+``_visible_pairs``), run through ``block_attention`` and the LSE merge as ring attention runs them, against the causal plan
+(what CP computes if the window is dropped).  It reports the time, the TFLOP/s over the visible pairs and the K/V bytes each
+rank sends per layer (hops × 2·c·Hkv·D·2 B).  All ranks' blocks come from one process, so no NCCL time is measured.  Pair and
+byte counts come from shapes and are printed without a GPU too; times need one."""
 import argparse
 import json
 import math
@@ -210,6 +217,73 @@ def window_perf(e, bwd: bool, W: int = 4096):
         print(json.dumps(rec), flush=True)
 
 
+def block_pairs(c: int, causal: bool, off: int, W) -> int:
+    """Visible (query, key) pairs of one c × c CP block: all c² when dense, else i + off − W < j ≤ i + off (W None: no lower
+    bound)."""
+    if not causal:
+        return c * c
+    i = torch.arange(c, dtype=torch.int64)
+    hi = torch.clamp(i + off, max=c - 1)
+    lo = torch.zeros_like(i) if W is None else torch.clamp(i + off - W + 1, min=0)
+    return int(torch.clamp(hi - lo + 1, min=0).sum())
+
+
+def cp_window_perf(bwd: bool, cp: int, W: int = 4096):
+    """Per-rank CP attention work of the windowed and the causal block plan (contiguous split), timed on one GPU when present."""
+    from neuronx_distributed_b200.modules.attention.ring import _merge_block, _visible_pairs, block_attention, ring_hops
+
+    B, H, Hkv, D = 1, 32, 8, 128
+    scale = 1.0 / math.sqrt(D)
+    gpu = torch.cuda.is_available()
+    if gpu:
+        print(json.dumps(gpu_info()), flush=True)
+    for S in (32768, 65536, 131072):
+        c = S // cp
+        if gpu:
+            g = torch.Generator(device="cuda").manual_seed(S)
+            q, go = (torch.randn(B, c, H, D, device="cuda", generator=g).bfloat16() for _ in range(2))
+            k, v = (torch.randn(B, S, Hkv, D, device="cuda", generator=g).bfloat16() for _ in range(2))
+        for plan_name, window in (("window", W), ("causal", None)):
+            plans = [_visible_pairs(r, cp, "contiguous", True, window, c) for r in range(cp)]
+            work = [sum(block_pairs(c, bc, off, window) for _, _, _, bc, off in p) for p in plans]
+            r = max(range(cp), key=lambda i: (work[i], i))
+            hops = ring_hops(cp, c, window)
+            rec = {"bench": "mistral7b_cp_window", "plan": plan_name, "cp": cp, "S": S, "chunk": c, "B": B, "H": H, "Hkv": Hkv,
+                   "D": D, "W": W, "rank": r, "blocks": len(plans[r]), "visible_pairs": work[r] * H * B, "hops": hops,
+                   "kv_bytes_sent_per_layer": hops * 2 * B * c * Hkv * D * 2, "nccl": "not measured (one-process emulation)"}
+            fl = 4 * D * H * B * work[r]
+            if gpu:
+                qr = q.detach().requires_grad_(True)
+                kv = [(k[:, src * c:(src + 1) * c], v[:, src * c:(src + 1) * c]) for _, src, _, _, _ in plans[r]]
+
+                def fwd(plan=plans[r], kv=kv, window=window):
+                    out = lse = None
+                    for (_, _, _, bc, off), (kb, vb) in zip(plan, kv):
+                        out, lse = _merge_block(out, lse, *block_attention(qr, kb, vb, bc, scale, window, off))
+                    return out.to(q.dtype)
+
+                def fwd_only():
+                    with torch.no_grad():
+                        fwd()
+
+                def fwd_bwd():
+                    fwd().backward(go)
+
+                runs = {"fwd": fwd_only, "fwd_bwd": fwd_bwd if bwd else None}
+                for key, fn in runs.items():
+                    if fn is None:
+                        continue
+                    ms = min(time_fn(fn, 5) for _ in range(2))
+                    rec[key + "_ms"] = round(ms, 3)
+                    rec[key + "_tflops"] = round((3.5 if key == "fwd_bwd" else 1.0) * fl / ms / 1e9, 1)
+            else:
+                rec["fwd_ms"] = rec["fwd_bwd_ms"] = "not measured"
+            print(json.dumps(rec), flush=True)
+        if gpu:
+            del q, go, k, v
+            torch.cuda.empty_cache()
+
+
 def time_fn(fn, iters=20):
     for _ in range(3):
         fn()
@@ -228,8 +302,12 @@ def main():
     ap.add_argument("--perf", action="store_true")
     ap.add_argument("--bwd", action="store_true")
     ap.add_argument("--window", action="store_true", help="with --perf: the sliding-window table instead of the model shapes")
+    ap.add_argument("--cp", type=int, default=0, help="with --perf --window: the context-parallel block schedule at this CP size")
     ap.add_argument("--head-dim", type=int, default=128, choices=attention.FLASH_HEAD_DIMS)
     a = ap.parse_args()
+    if a.perf and a.window and a.cp > 1 and not torch.cuda.is_available():
+        cp_window_perf(a.bwd, a.cp)                   # shapes only: pair and byte counts, times "not measured"
+        return
     dev = torch.device("cuda")
     e = _ext.ext()
     ok_all = True
@@ -285,7 +363,10 @@ def main():
             ok_all &= ok
             print(json.dumps({"check": f"fa_bwd_{tag}", "ok": ok, **res}), flush=True)
     if a.perf:
-        (window_perf if a.window else perf)(e, a.bwd)
+        if a.window and a.cp > 1:
+            cp_window_perf(a.bwd, a.cp)
+        else:
+            (window_perf if a.window else perf)(e, a.bwd)
     print(json.dumps({"all_ok": ok_all}))
     sys.exit(0 if ok_all else 1)
 
