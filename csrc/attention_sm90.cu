@@ -12,18 +12,17 @@
 //   dQ     one CTA per (64-query tile, head, batch), loops over the key tiles: S, P, dP = dO·Vᵀ, dS, dQ += dS·K
 //   Every gradient element is owned by one thread of one CTA (no atomics), so the backward is bit-reproducible.
 // Every kernel is a template on the head dimension HD; the tile shapes (64 query / key rows) are the same for all of them.
-// Optional key-padding mask (template flag MASK, uint8 [B, S_kv], key j of batch b visible iff mask[b, j] != 0): a masked
-// key is treated like a key past S_kv, so it contributes nothing and its dK / dV are exactly 0.  The forward and dQ kernels
-// stage each key tile's 64 flags in shared memory next to K / V; a dK/dV thread owns two fixed key rows and reads their
-// flags once.  A query row that sees no key gets O = 0, LSE = −inf and dQ = 0.
-// Optional sliding window (template flag WINDOW, causal only): query i sees key j iff i − W < j ≤ i.  The forward and dQ
-// kernels start their key-tile loop at the first tile that holds a key inside the window of the tile's first query row; the
-// dK/dV kernel stops its query-tile loop at the last tile whose rows can still see the key tile.  The per-element predicate
-// removes the rest.  W ≥ S computes exactly what the causal kernels compute.
-// Query offset (WINDOW kernels only): `q_offset` = off ≥ 0 is the global position of query row 0 minus that of key row 0, so
-// query i sees key j iff i + off − W < j ≤ i + off.  This is one off-diagonal block of context-parallel attention, whose
-// queries sit `off` positions after its keys.  Whole query rows (and tiles) of such a block can see no key: they get O = 0,
-// LSE = −inf and dQ = 0, and keys no row sees get dK = dV = 0.  off = 0 is the diagonal rule above.
+// Visibility: query row i < S_q sees key j < S_kv iff
+//   - MASK (key-padding mask, uint8 [B, S_kv]): mask[b, j] != 0;
+//   - causal: j ≤ i + off;
+//   - WINDOW (sliding window W, causal only): j > i + off − W.
+// off = q_offset ≥ 0 (WINDOW kernels only, 0 otherwise) is the global position of query row 0 minus that of key row 0: one
+// off-diagonal block of context-parallel attention, whose queries sit `off` positions after its keys.  W ≥ S_kv + off is
+// plain causal attention.  The mask term is tested at each call site (the forward and dQ kernels stage each key tile's 64
+// flags in shared memory, a dK/dV thread reads the flags of its two key rows once); the causal / window / offset terms are
+// `sees`, and the tiles a CTA visits are `key_tiles` / `query_tiles`, which skip only tiles that hold no visible pair.
+// An invisible pair contributes nothing: a query row that sees no key gets O = 0, LSE = −inf and dQ = 0, and a key no row
+// sees gets dK = dV = 0.
 #include <cuda.h>
 
 #include <algorithm>
@@ -163,15 +162,57 @@ NXD_DEVICE void store_rows(const float (&c)[HD / 8][4], bf16* base, long ss, int
   }
 }
 
-struct FwdParams {
+// the fields every kernel reads
+struct Params {
   View q, k, v;
-  bf16* o; long o_sb, o_ss, o_sh;
-  float* lse;
   int B, H, Hkv, S_q, S_kv, causal;
   float scale_log2;
   const uint8_t* mask; long mask_sb;            // key-padding mask [B, S_kv] (MASK kernels only)
   int window;                                   // sliding window W, 1 ≤ W ≤ S_kv + q_offset (WINDOW kernels only)
   int q_offset;                                 // query row 0 minus key row 0 in global positions (WINDOW kernels only)
+};
+
+// the causal / window / offset terms of the visibility rule: query row i sees key j
+template <bool WINDOW>
+NXD_DEVICE bool sees(const Params& p, int i, int j) {
+  const int off = WINDOW ? p.q_offset : 0;
+  return !(p.causal && j > i + off) && !(WINDOW && j <= i + off - p.window);
+}
+
+// Tiles lo ≤ t < hi a CTA visits (none when hi ≤ lo); tile t holds rows [64t, 64t + 64).
+// key_tiles: the rows of query tile [q0, q0 + 64) see keys q0 + off − W < j (its first row's window start) up to
+// j ≤ q0 + 63 + off (causal: its last row's diagonal), so every visible key lies in the tiles returned.
+template <bool WINDOW>
+NXD_DEVICE void key_tiles(const Params& p, int q0, int& lo, int& hi) {
+  const int off = WINDOW ? p.q_offset : 0, n = (p.S_kv + BT - 1) / BT;
+  lo = WINDOW ? max(0, q0 + off - p.window + 1) / BT : 0;
+  hi = p.causal ? min(n, (q0 + BT - 1 + off) / BT + 1) : n;
+}
+// query_tiles: the keys of key tile [k0, k0 + 64) are seen by rows i ≥ k0 − off (causal: the first key's diagonal) up to
+// i ≤ k0 + 63 + W − 1 − off (the last key's window end), so every row that sees one of them lies in the tiles returned.  A
+// negative last row leaves the range empty.
+template <bool WINDOW>
+NXD_DEVICE void query_tiles(const Params& p, int k0, int& lo, int& hi) {
+  const int off = WINDOW ? p.q_offset : 0, n = (p.S_q + BT - 1) / BT;
+  lo = p.causal ? max(0, k0 - off) / BT : 0;
+  hi = WINDOW ? min(n, (k0 + 2 * BT - 2 + p.window - off) / BT) : n;
+}
+
+// K / V tile t of one (batch, kv head) and, with the mask, its key flags → buffer t & 1 of the double-buffered sK, sV, sM
+// (forward and dQ)
+template <int HD, bool MASK>
+NXD_DEVICE void load_kv(bf16* sK, bf16* sV, uint8_t* sM, const bf16* kb, const bf16* vb, const uint8_t* mb, const Params& p,
+                        int t) {
+  const int buf = t & 1;
+  load_tile<HD>(sK + buf * kTile<HD>, kb, p.k.ss, t * BT, p.S_kv);
+  load_tile<HD>(sV + buf * kTile<HD>, vb, p.v.ss, t * BT, p.S_kv);
+  cp_async_commit();
+  if (MASK) load_flags(sM + buf * BT, mb, t * BT, p.S_kv);
+}
+
+struct FwdParams : Params {
+  bf16* o; long o_sb, o_ss, o_sh;
+  float* lse;
 };
 
 template <int HD, bool MASK, bool WINDOW>
@@ -190,19 +231,11 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
   const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
   const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
-  const int off = WINDOW ? p.q_offset : 0;
-  // causal: the tile's last row sees keys up to q0 + 63 + off
-  const int n_kv =
-      p.causal ? min((p.S_kv + BT - 1) / BT, WINDOW ? (q0 + BT - 1 + off) / BT + 1 : qt + 1) : (p.S_kv + BT - 1) / BT;
-  // window: keys ≤ q0 + off − W are outside the window of every row of the tile, so whole tiles of them are skipped
-  const int t_lo = WINDOW ? max(0, q0 + off - p.window + 1) / BT : 0;
-  const int b_lo = t_lo & 1;
+  int t_lo, n_kv;
+  key_tiles<WINDOW>(p, q0, t_lo, n_kv);
 
   load_tile<HD>(sQ, qb, p.q.ss, q0, p.S_q);
-  load_tile<HD>(sK + b_lo * kTl, kb, p.k.ss, t_lo * BT, p.S_kv);
-  load_tile<HD>(sV + b_lo * kTl, vb, p.v.ss, t_lo * BT, p.S_kv);
-  cp_async_commit();
-  if (MASK) load_flags(sM + b_lo * BT, mb, t_lo * BT, p.S_kv);
+  load_kv<HD, MASK>(sK, sV, sM, kb, vb, mb, p, t_lo);
 
   float o[HD / 8][4];
 #pragma unroll
@@ -213,10 +246,7 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
   for (int t = t_lo; t < n_kv; ++t) {
     const int buf = t & 1;
     if (t + 1 < n_kv) {
-      load_tile<HD>(sK + (buf ^ 1) * kTl, kb, p.k.ss, (t + 1) * BT, p.S_kv);
-      load_tile<HD>(sV + (buf ^ 1) * kTl, vb, p.v.ss, (t + 1) * BT, p.S_kv);
-      cp_async_commit();
-      if (MASK) load_flags(sM + (buf ^ 1) * BT, mb, (t + 1) * BT, p.S_kv);
+      load_kv<HD, MASK>(sK, sV, sM, kb, vb, mb, p, t + 1);
       cp_async_wait<1>();
     } else {
       cp_async_wait<0>();
@@ -231,10 +261,8 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int key = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
-        float x = s[j][e] * p.scale_log2;
-        if (key >= p.S_kv || (p.causal && key > row[e >> 1] + off) || (MASK && !fl[j * 8 + 2 * (lane & 3) + (e & 1)]) ||
-            (WINDOW && key <= row[e >> 1] + off - p.window))
-          x = -INFINITY;
+        const bool vis = key < p.S_kv && (!MASK || fl[j * 8 + 2 * (lane & 3) + (e & 1)]) && sees<WINDOW>(p, row[e >> 1], key);
+        const float x = vis ? s[j][e] * p.scale_log2 : -INFINITY;
         s[j][e] = x;
         mx[e >> 1] = fmaxf(mx[e >> 1], x);
       }
@@ -311,16 +339,12 @@ __global__ void fa_bwd_prep_kernel(const bf16* __restrict__ o, const bf16* __res
   if (lane == 0) delta[w] = acc - (dlse ? dlse[w] : 0.f);
 }
 
-struct BwdParams {
-  View q, k, v, g;
+struct BwdParams : Params {
+  View g;
   bf16 *dq, *dk, *dv;
   long dq_sb, dq_ss, dq_sh, dk_sb, dk_ss, dk_sh, dv_sb, dv_ss, dv_sh;
   const float *lse, *delta;
-  int B, H, Hkv, S_q, S_kv, causal;
-  float scale, scale_log2;
-  const uint8_t* mask; long mask_sb;            // key-padding mask [B, S_kv] (MASK kernels only)
-  int window;                                   // sliding window W, 1 ≤ W ≤ S_kv + q_offset (WINDOW kernels only)
-  int q_offset;                                 // query row 0 minus key row 0 in global positions (WINDOW kernels only)
+  float scale;
 };
 
 template <int HD, bool MASK, bool WINDOW>
@@ -337,12 +361,8 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
   const int G = p.H / p.Hkv;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k0 = kt * BT;
-  const int n_qt = (p.S_q + BT - 1) / BT;
-  const int off = WINDOW ? p.q_offset : 0;
-  // causal: S_q == S_kv, query rows before k0 − off see none of the key tile
-  const int qt0 = p.causal ? (WINDOW ? max(0, k0 - off) / BT : kt) : 0;
-  // window: the last query row that sees key k0 + 63 is k0 + 63 + W − 1 − off (a negative bound leaves the range empty)
-  const int qt_end = WINDOW ? min(n_qt, (k0 + 2 * BT - 2 + p.window - off) / BT) : n_qt;
+  int qt0, qt_end;
+  query_tiles<WINDOW>(p, k0, qt0, qt_end);
   const int per_head = qt_end > qt0 ? qt_end - qt0 : 0;
   const int n_it = G * per_head;
 
@@ -398,8 +418,7 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
       for (int e = 0; e < 4; ++e) {
         const int qc = j * 8 + 2 * (lane & 3) + (e & 1);
         const int qi = q0 + qc;
-        const bool vis = qi < p.S_q && !(p.causal && key[e >> 1] > qi + off) && (!MASK || kvis[e >> 1]) &&
-                         !(WINDOW && qi + off >= key[e >> 1] + p.window);
+        const bool vis = qi < p.S_q && sees<WINDOW>(p, qi, key[e >> 1]) && (!MASK || kvis[e >> 1]);
         pt[j][e] = vis ? exp2f(pt[j][e] * p.scale_log2 - L[qc]) : 0.f;
       }
     }
@@ -446,18 +465,12 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) 
   const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
   const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
-  const int off = WINDOW ? p.q_offset : 0;
-  const int n_kv =
-      p.causal ? min((p.S_kv + BT - 1) / BT, WINDOW ? (q0 + BT - 1 + off) / BT + 1 : qt + 1) : (p.S_kv + BT - 1) / BT;
-  const int t_lo = WINDOW ? max(0, q0 + off - p.window + 1) / BT : 0;     // as in the forward
-  const int b_lo = t_lo & 1;
+  int t_lo, n_kv;
+  key_tiles<WINDOW>(p, q0, t_lo, n_kv);
 
   load_tile<HD>(sQ, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
   load_tile<HD>(sG, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
-  load_tile<HD>(sK + b_lo * kTl, kb, p.k.ss, t_lo * BT, p.S_kv);
-  load_tile<HD>(sV + b_lo * kTl, vb, p.v.ss, t_lo * BT, p.S_kv);
-  cp_async_commit();
-  if (MASK) load_flags(sM + b_lo * BT, mb, t_lo * BT, p.S_kv);
+  load_kv<HD, MASK>(sK, sV, sM, kb, vb, mb, p, t_lo);
 
   const int row[2] = {q0 + warp * 16 + (lane >> 2), q0 + warp * 16 + (lane >> 2) + 8};
   float L[2], D[2];
@@ -474,10 +487,7 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) 
   for (int t = t_lo; t < n_kv; ++t) {
     const int buf = t & 1;
     if (t + 1 < n_kv) {
-      load_tile<HD>(sK + (buf ^ 1) * kTl, kb, p.k.ss, (t + 1) * BT, p.S_kv);
-      load_tile<HD>(sV + (buf ^ 1) * kTl, vb, p.v.ss, (t + 1) * BT, p.S_kv);
-      cp_async_commit();
-      if (MASK) load_flags(sM + (buf ^ 1) * BT, mb, (t + 1) * BT, p.S_kv);
+      load_kv<HD, MASK>(sK, sV, sM, kb, vb, mb, p, t + 1);
       cp_async_wait<1>();
     } else {
       cp_async_wait<0>();
@@ -493,8 +503,7 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) 
       for (int e = 0; e < 4; ++e) {
         const int kc = t * BT + j * 8 + 2 * (lane & 3) + (e & 1);
         const int r = row[e >> 1];
-        const bool vis = kc < p.S_kv && r < p.S_q && !(p.causal && kc > r + off) && (!MASK || fl[j * 8 + 2 * (lane & 3) + (e & 1)]) &&
-                         !(WINDOW && kc <= r + off - p.window);
+        const bool vis = kc < p.S_kv && r < p.S_q && sees<WINDOW>(p, r, kc) && (!MASK || fl[j * 8 + 2 * (lane & 3) + (e & 1)]);
         s[j][e] = vis ? exp2f(s[j][e] * p.scale_log2 - L[e >> 1]) : 0.f;
       }
     }
@@ -565,37 +574,36 @@ static void launch_bwd(const BwdParams& p, cudaStream_t st) {
   fa_bwd_dq_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem_dq, st>>>(p);
 }
 
-static void check_args(int S_q, int S_kv, bool causal, int window, int q_offset) {
+// checks the arguments and fills the fields every kernel reads
+static void set_params(Params& p, const void* q, const void* k, const void* v, const long* qs, const long* ks, const long* vs,
+                       int B, int S_q, int S_kv, int H, int Hkv, float scale, bool causal, const void* kpm, long kpm_sb,
+                       long window, long q_offset) {
   if (causal && S_q != S_kv) nxd_throw("attention: causal needs S_q == S_kv", __FILE__, __LINE__);
   if (window < 0) nxd_throw("attention: window must be >= 0 (0 = none)", __FILE__, __LINE__);
   if (window > 0 && !causal) nxd_throw("attention: a sliding window needs causal attention", __FILE__, __LINE__);
   if (q_offset < 0) nxd_throw("attention: q_offset must be >= 0", __FILE__, __LINE__);
   if (q_offset > 0 && window == 0) nxd_throw("attention: q_offset needs a sliding window", __FILE__, __LINE__);
   // tile bounds reach 2·S + q_offset + 2·64 in 32-bit arithmetic
-  if (2L * S_kv + q_offset + 2 * BT > INT32_MAX) nxd_throw("attention: q_offset too large", __FILE__, __LINE__);
-}
-
-// W ≥ S_kv + q_offset sees every causal key; the clamp keeps tile bounds in range
-static int clamp_window(int window, int S_kv, int q_offset) {
-  return (int)std::min<long>(window, (long)S_kv + q_offset);
+  if (q_offset > INT32_MAX - 2L * S_kv - 2 * BT) nxd_throw("attention: q_offset too large", __FILE__, __LINE__);
+  p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs);
+  p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
+  p.scale_log2 = scale * kLog2e;
+  p.mask = (const uint8_t*)kpm; p.mask_sb = kpm_sb;
+  // W ≥ S_kv + q_offset sees every causal key; the clamp keeps the tile bounds in range
+  p.window = (int)std::min(window, S_kv + q_offset);
+  p.q_offset = (int)q_offset;
 }
 
 }  // namespace fa
 
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
                     int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    const void* kpm, long kpm_sb, int window, int q_offset, cudaStream_t st) {
+                    const void* kpm, long kpm_sb, long window, long q_offset, cudaStream_t st) {
   using namespace fa;
-  check_args(S_q, S_kv, causal, window, q_offset);
   FwdParams p;
-  p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs);
+  set_params(p, q, k, v, qs, ks, vs, B, S_q, S_kv, H, Hkv, scale, causal, kpm, kpm_sb, window, q_offset);
   p.o = (bf16*)out; p.o_sb = os[0]; p.o_ss = os[1]; p.o_sh = os[2];
   p.lse = lse;
-  p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
-  p.scale_log2 = scale * kLog2e;
-  p.mask = (const uint8_t*)kpm; p.mask_sb = kpm_sb;
-  p.window = clamp_window(window, S_kv, q_offset);
-  p.q_offset = q_offset;
   dispatch(D, kpm != nullptr, window > 0, [&](auto hd, auto mk, auto wd) {
     launch_fwd<decltype(hd)::value, decltype(mk)::value, decltype(wd)::value>(p, st);
   });
@@ -605,22 +613,18 @@ void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, floa
 void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
                     int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
-                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, int window,
-                    int q_offset, cudaStream_t st) {
+                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, long window,
+                    long q_offset, cudaStream_t st) {
   using namespace fa;
-  check_args(S_q, S_kv, causal, window, q_offset);
   BwdParams p;
-  p.q = view(q, qs); p.k = view(k, ks); p.v = view(v, vs); p.g = view(go, gs);
+  set_params(p, q, k, v, qs, ks, vs, B, S_q, S_kv, H, Hkv, scale, causal, kpm, kpm_sb, window, q_offset);
+  p.g = view(go, gs);
   p.dq = (bf16*)dq; p.dk = (bf16*)dk; p.dv = (bf16*)dv;
   p.dq_sb = dqs[0]; p.dq_ss = dqs[1]; p.dq_sh = dqs[2];
   p.dk_sb = dks[0]; p.dk_ss = dks[1]; p.dk_sh = dks[2];
   p.dv_sb = dvs[0]; p.dv_ss = dvs[1]; p.dv_sh = dvs[2];
   p.lse = lse; p.delta = delta;
-  p.B = B; p.H = H; p.Hkv = Hkv; p.S_q = S_q; p.S_kv = S_kv; p.causal = causal ? 1 : 0;
-  p.scale = scale; p.scale_log2 = scale * kLog2e;
-  p.mask = (const uint8_t*)kpm; p.mask_sb = kpm_sb;
-  p.window = clamp_window(window, S_kv, q_offset);
-  p.q_offset = q_offset;
+  p.scale = scale;
   dispatch(D, kpm != nullptr, window > 0, [&](auto hd, auto mk, auto wd) {
     constexpr int HD = decltype(hd)::value;
     const long rows = (long)B * H * S_q;

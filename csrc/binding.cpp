@@ -462,18 +462,6 @@ static const void* check_kpm(const c10::optional<Tensor>& m, const Tensor& q, in
   *sb = m->stride(0);
   return m->data_ptr();
 }
-// sliding window W (query i sees keys i + q_offset − W < j ≤ i + q_offset), 0 = none; causal attention only.  q_offset: global
-// position of query row 0 minus that of key row 0 (one off-diagonal block of context-parallel attention), windowed only.
-// Returns W clamped to S_kv + q_offset, the kernels' form.
-static int check_window(int64_t window, int64_t q_offset, bool causal, int64_t Skv) {
-  TORCH_CHECK(window >= 0, "window must be >= 0 (0 = none)");
-  TORCH_CHECK(window == 0 || causal, "a sliding window needs causal attention");
-  TORCH_CHECK(q_offset >= 0, "q_offset must be >= 0");
-  TORCH_CHECK(q_offset == 0 || window > 0, "q_offset needs a sliding window");
-  TORCH_CHECK(q_offset == 0 || causal, "q_offset needs causal attention");
-  TORCH_CHECK(2 * Skv + q_offset + 128 <= INT32_MAX, "q_offset too large");
-  return (int)std::min<int64_t>(window, Skv + q_offset);
-}
 // returns (out [B,S,H,D] view — memory laid out [S,B,H,D] when sbhd_out —, lse [B,H,S] fp32)
 static std::vector<Tensor> flash_attn_fwd(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
                                           bool sbhd_out, const c10::optional<Tensor>& key_padding_mask, int64_t window,
@@ -482,7 +470,6 @@ static std::vector<Tensor> flash_attn_fwd(const Tensor& q, const Tensor& k, cons
   const int B = q.size(0), S = q.size(1), H = q.size(2), D = q.size(3), Skv = k.size(1), Hkv = k.size(2);
   TORCH_CHECK(k.size(0) == B && v.size(0) == B && v.size(1) == Skv && v.size(2) == Hkv && H % Hkv == 0);
   TORCH_CHECK(k.size(3) == D && v.size(3) == D, "q, k and v must have the same head_dim");
-  const int w = check_window(window, q_offset, causal, Skv);
   long kpm_sb;
   const void* kpm = check_kpm(key_padding_mask, q, B, Skv, &kpm_sb);
   c10::cuda::CUDAGuard guard(q.device());
@@ -491,7 +478,7 @@ static std::vector<Tensor> flash_attn_fwd(const Tensor& q, const Tensor& k, cons
   const long qs[3] = {q.stride(0), q.stride(1), q.stride(2)}, ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   const long vs[3] = {v.stride(0), v.stride(1), v.stride(2)}, os[3] = {out.stride(0), out.stride(1), out.stride(2)};
   nxd::flash_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, Skv, H, Hkv, D,
-                      qs, ks, vs, os, (float)scale, causal, kpm, kpm_sb, w, (int)q_offset, stream());
+                      qs, ks, vs, os, (float)scale, causal, kpm, kpm_sb, window, q_offset, stream());
   return {out, lse};
 }
 
@@ -504,7 +491,6 @@ static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, con
   TORCH_CHECK(k.size(3) == D && v.size(3) == D && go.size(3) == D && o.size(3) == D,
               "q, k, v, out and grad_out must have the same head_dim");
   TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * H * S);
-  const int w = check_window(window, q_offset, causal, Skv);
   long kpm_sb;
   const void* kpm = check_kpm(key_padding_mask, q, B, Skv, &kpm_sb);
   c10::cuda::CUDAGuard guard(q.device());
@@ -523,7 +509,7 @@ static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, con
   }
   nxd::flash_attn_bwd(go.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), dlse_p,
                       dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr<float>(), B, S, Skv, H, Hkv, D, gs, qs, ks,
-                      vs, os, dqs, dks, dvs, (float)scale, causal, kpm, kpm_sb, w, (int)q_offset, stream());
+                      vs, os, dqs, dks, dvs, (float)scale, causal, kpm, kpm_sb, window, q_offset, stream());
   return {dq, dk, dv};
 }
 

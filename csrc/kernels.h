@@ -146,13 +146,13 @@ void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int 
 // position of query row 0 minus that of key row 0, so query i sees keys i + q_offset − W < j ≤ i + q_offset.
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
                     int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    const void* kpm, long kpm_sb, int window, int q_offset, cudaStream_t st);
+                    const void* kpm, long kpm_sb, long window, long q_offset, cudaStream_t st);
 
 // delta: fp32 scratch [B, H, S_q]; dlse may be null
 void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
                     int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
-                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, int window,
-                    int q_offset, cudaStream_t st);
+                    const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, long window,
+                    long q_offset, cudaStream_t st);
 
 }  // namespace nxd

@@ -8,7 +8,7 @@ Layout convention of ``nki_flash_attn_func`` (same as the reference):
 
 The result is ``[B, H, S, D]`` in both cases.  The math runs in ``ops.attention.flash_attention`` (own forward /
 backward kernels for bf16 with head_dim 64, 80, 96 or 128, library flash attention otherwise), which wants ``[B, S, H, D]``
-*views* — the transposes below are stride changes consumed by strided TMA descriptors, not copies."""
+*views* — the transposes below are stride changes the kernels' strided ``cp.async`` tile loads consume, not copies."""
 from __future__ import annotations
 
 from typing import Optional
@@ -24,7 +24,10 @@ def get_flash_attn_kernels(use_sharded: bool = False):
     a GPU whose two dies are one device."""
     from .. import ops
 
-    return ops.attention._FlashAttn.apply, None
+    def forward(q, k, v, causal, scale):
+        return ops.attention._FlashAttn.apply(q, k, v, causal, scale, None, 0, 0, True)[0]
+
+    return forward, None
 
 
 class NKIAttnFunc(torch.autograd.Function):

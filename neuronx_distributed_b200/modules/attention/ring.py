@@ -178,13 +178,8 @@ def _block_backward(q, k, v, out, lse, dout, causal: bool, scale: float, window:
     if q.is_cuda:
         from ... import ops
 
-        if ops.attention.flash_kernels_apply(q, k, v) and (not causal or q.shape[1] == k.shape[1]):
-            e = ops._ext.ext()
-            ops._ext.count_launch(4)
-            tv = ops.attention._tma_view
-            dq, dk, dv = e.flash_attn_bwd(tv(dout.to(out.dtype)), tv(q), tv(k), tv(v), tv(out), lse.contiguous(), bool(causal),
-                                          float(scale), False, None, None, ops.attention.check_window(window), int(q_offset))
-            return dq, dk, dv
+        if ops.attention.flash_kernels_apply(q, k, v, causal):
+            return ops.attention._flash_backward(dout, q, k, v, out, lse, causal, scale, None, window or 0, q_offset)
     hq, hkv = q.shape[2], k.shape[2]
     g = hq // hkv
     qt, dot, ot = q.transpose(1, 2).float(), dout.transpose(1, 2).float(), out.transpose(1, 2).float()     # [B,H,S,D]

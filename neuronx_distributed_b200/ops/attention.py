@@ -54,15 +54,15 @@ def _sdpa(q, k, v, causal: bool, scale: Optional[float], key_padding_mask: Optio
     return o.transpose(1, 2)
 
 
-def flash_kernels_apply(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor) -> bool:
+def flash_kernels_apply(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = False) -> bool:
     """True when the own flash kernels handle these tensors: bf16 CUDA, 4-D ``[B, S, H, D]`` with D in
-    :data:`FLASH_HEAD_DIMS` (the same for q, k and v), and the extension loaded.  ``NXD_DISABLE_OWN_ATTENTION=1`` turns
-    them off (the SDPA path is then used, e.g. as a comparison baseline)."""
+    :data:`FLASH_HEAD_DIMS` (the same for q, k and v), S_q == S_kv when ``causal``, and the extension loaded.
+    ``NXD_DISABLE_OWN_ATTENTION=1`` turns them off (the SDPA path is then used, e.g. as a comparison baseline)."""
     if os.environ.get("NXD_DISABLE_OWN_ATTENTION", "0") == "1":
         return False
     if not (q.is_cuda and q.dtype == torch.bfloat16 and k.dtype == torch.bfloat16 and v.dtype == torch.bfloat16
             and q.dim() == 4 and k.dim() == 4 and v.dim() == 4 and q.shape[-1] in FLASH_HEAD_DIMS
-            and k.shape[-1] == q.shape[-1] and v.shape[-1] == q.shape[-1]):
+            and k.shape[-1] == q.shape[-1] and v.shape[-1] == q.shape[-1] and (not causal or q.shape[1] == k.shape[1])):
         return False
     e = _ext.ext()
     return e is not None and hasattr(e, "flash_attn_fwd") and hasattr(e, "flash_attn_bwd")
@@ -78,61 +78,58 @@ def _kernel_mask(m: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
 
 
 def _tma_view(t: torch.Tensor) -> torch.Tensor:
-    """The kernels address q/k/v as ``base + b·sb + s·ss + h·sh + d`` with 16-byte row loads: head_dim must be contiguous, the
-    base 16-byte aligned and the (b, s, h) strides multiples of 8 elements (true for [B,S,H,D], [S,B,H,D], [B,H,S,D] memory
-    and for slices of a fused projection output); anything else is copied once."""
+    """The kernels address q/k/v as ``base + b·sb + s·ss + h·sh + d`` with 16-byte ``cp.async`` row loads: head_dim must be
+    contiguous, the base 16-byte aligned and the (b, s, h) strides multiples of 8 elements (true for [B,S,H,D], [S,B,H,D],
+    [B,H,S,D] memory and for slices of a fused projection output); anything else is copied once."""
     if t.stride(3) != 1 or t.data_ptr() % 16 or any(t.stride(i) % 8 for i in range(3)):
         return t.contiguous()
     return t
 
 
+def _flash_backward(go, q, k, v, o, lse, causal: bool, scale: float, mask=None, window: int = 0, q_offset: int = 0,
+                    sbhd_out: bool = False, dlse=None):
+    """``(dq, dk, dv)`` of the flash kernels for the rows' output ``o`` and log-normaliser ``lse``: a δ pre-pass, a dK/dV
+    kernel and a dQ kernel.  ``dlse``: the gradient into ``lse``, or None."""
+    _ext.count_launch(3)
+    tv = _tma_view
+    return _ext.ext().flash_attn_bwd(tv(go.to(o.dtype)), tv(q), tv(k), tv(v), tv(o), lse.contiguous(), bool(causal),
+                                     float(scale), sbhd_out, dlse, mask, int(window), int(q_offset))
+
+
 class _FlashAttn(torch.autograd.Function):
-    """Flash attention (``csrc/attention_sm90.cu``): forward saves (q, k, v, o, lse); backward is a dK/dV kernel and a dQ
-    kernel.  Outputs/gradients are laid out ``[S,B,H,D]`` in memory (returned as ``[B,S,H,D]`` views) so the
-    model's ``[S,B,H·D]`` reshape is free."""
+    """Flash attention (``csrc/attention_sm90.cu``) → ``(o, lse)``; forward saves (q, k, v, o, lse, mask).  LSE is a
+    differentiable output: ring attention merges per-block results through their LSEs, and a gradient into LSE only shifts
+    δ in the backward kernel (``dS = P∘(dP − (δ − g_lse))``).  ``sbhd_out``: outputs and gradients are laid out ``[S,B,H,D]``
+    in memory (returned as ``[B,S,H,D]`` views), so a model's ``[S,B,H·D]`` reshape is free."""
 
     @staticmethod
-    def forward(ctx, q, k, v, causal, scale, mask=None, window=0):
-        e = _ext.ext()
+    def forward(ctx, q, k, v, causal, scale, mask, window, q_offset, sbhd_out):
+        ctx.set_materialize_grads(False)
         q, k, v = _tma_view(q), _tma_view(k), _tma_view(v)
         _ext.count_launch()
-        o, lse = e.flash_attn_fwd(q, k, v, bool(causal), float(scale), True, mask, int(window))
+        o, lse = _ext.ext().flash_attn_fwd(q, k, v, bool(causal), float(scale), sbhd_out, mask, int(window), int(q_offset))
         ctx.save_for_backward(q, k, v, o, lse, mask)
-        ctx.causal, ctx.scale, ctx.window = causal, scale, window
-        return o
-
-    @staticmethod
-    def backward(ctx, go):
-        q, k, v, o, lse, mask = ctx.saved_tensors
-        e = _ext.ext()
-        _ext.count_launch(3)   # δ prep + dK/dV + dQ
-        dq, dk, dv = e.flash_attn_bwd(_tma_view(go), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale), True, None, mask,
-                                      int(ctx.window))
-        return dq, dk, dv, None, None, None, None
-
-
-class _FlashAttnLse(torch.autograd.Function):
-    """Same kernels, but LSE is a differentiable output: ring attention merges per-block results through their LSEs, and
-    a gradient into LSE only shifts δ in the backward kernel (``dS = P∘(dP − (δ − g_lse))``)."""
-
-    @staticmethod
-    def forward(ctx, q, k, v, causal, scale, window=0, q_offset=0):
-        q, k, v = _tma_view(q), _tma_view(k), _tma_view(v)
-        _ext.count_launch()
-        o, lse = _ext.ext().flash_attn_fwd(q, k, v, bool(causal), float(scale), False, None, int(window), int(q_offset))
-        ctx.save_for_backward(q, k, v, o, lse)
-        ctx.causal, ctx.scale, ctx.window, ctx.q_offset = causal, scale, window, q_offset
+        ctx.args = (causal, scale, window, q_offset, sbhd_out)
         return o, lse
 
     @staticmethod
     def backward(ctx, go, g_lse):
-        q, k, v, o, lse = ctx.saved_tensors
-        _ext.count_launch(3)
+        q, k, v, o, lse, mask = ctx.saved_tensors
+        causal, scale, window, q_offset, sbhd_out = ctx.args
         go = torch.zeros_like(o) if go is None else go
         dlse = None if g_lse is None else g_lse.float().contiguous()
-        dq, dk, dv = _ext.ext().flash_attn_bwd(_tma_view(go.to(o.dtype)), q, k, v, o, lse, bool(ctx.causal), float(ctx.scale),
-                                               False, dlse, None, int(ctx.window), int(ctx.q_offset))
-        return dq, dk, dv, None, None, None, None
+        dq, dk, dv = _flash_backward(go, q, k, v, o, lse, causal, scale, mask, window, q_offset, sbhd_out, dlse)
+        return dq, dk, dv, None, None, None, None, None, None
+
+
+def _window_args(name: str, causal: bool, sliding_window: Optional[int], q_offset: int = 0) -> int:
+    """Checks ``sliding_window`` / ``q_offset`` and returns the kernels' integer window (0 = none)."""
+    if sliding_window is not None and not causal:
+        raise ValueError(f"{name}: sliding_window needs causal=True")
+    window = check_window(sliding_window)
+    if q_offset < 0 or (q_offset > 0 and window == 0):
+        raise ValueError(f"{name}: q_offset must be 0, or > 0 with a sliding_window; got {q_offset}")
+    return window
 
 
 def flash_attention_with_lse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool, scale: float,
@@ -142,13 +139,9 @@ def flash_attention_with_lse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, 
     ``sliding_window`` as in :func:`flash_attention`.  ``q_offset`` ≥ 0 (causal, with a window): the global position of query
     row 0 minus that of key row 0, as in one off-diagonal block of context-parallel attention; query i then sees keys
     i + q_offset − W < j ≤ i + q_offset.  A row that sees no key gets O = 0 and LSE = −inf."""
-    if sliding_window is not None and not causal:
-        raise ValueError("flash_attention_with_lse: sliding_window needs causal=True")
-    window = check_window(sliding_window)
-    if q_offset < 0 or (q_offset > 0 and window == 0):
-        raise ValueError(f"flash_attention_with_lse: q_offset must be 0, or > 0 with a sliding_window; got {q_offset}")
-    if flash_kernels_apply(q, k, v) and (not causal or q.shape[1] == k.shape[1]):
-        return _FlashAttnLse.apply(q, k, v, causal, scale, window, q_offset)
+    window = _window_args("flash_attention_with_lse", causal, sliding_window, q_offset)
+    if flash_kernels_apply(q, k, v, causal):
+        return _FlashAttn.apply(q, k, v, causal, scale, None, window, q_offset, False)
     return None
 
 
@@ -167,12 +160,10 @@ def flash_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: b
     On the own kernels a masked key contributes nothing and gets dK = dV = 0, and a query row that sees no key at all gets
     O = 0 and dQ = 0.  The SDPA fallback (CPU, other dtypes or head sizes) follows SDPA's rule for such a row, which is NaN
     on some SDPA backends and versions."""
-    if sliding_window is not None and not causal:
-        raise ValueError("flash_attention: sliding_window needs causal=True")
-    window = check_window(sliding_window)
+    window = _window_args("flash_attention", causal, sliding_window)
     scale = scale if scale is not None else 1.0 / math.sqrt(q.shape[-1])
-    if flash_kernels_apply(q, k, v) and (not causal or q.shape[1] == k.shape[1]):
-        return _FlashAttn.apply(q, k, v, causal, scale, _kernel_mask(key_padding_mask), window)
+    if flash_kernels_apply(q, k, v, causal):
+        return _FlashAttn.apply(q, k, v, causal, scale, _kernel_mask(key_padding_mask), window, 0, True)[0]
     return _sdpa(q, k, v, causal, scale, key_padding_mask, window or None)
 
 
