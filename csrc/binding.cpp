@@ -1,6 +1,7 @@
 // pybind11 bindings: tensor checks + raw-pointer extraction; all math lives in the .cu files.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
+#include <cmath>
 #include <pybind11/stl.h>
 #include <torch/extension.h>
 
@@ -251,13 +252,26 @@ static py::tuple moe_block_metadata(const Tensor& expert_index, int64_t num_expe
   return py::make_tuple(b2e, tp2id, counts);
 }
 
+// KV-cache element type of the decode kernels: bf16, or fp8 e4m3 holding k / k_scale and v / v_scale (one fp32 scale per
+// tensor, the format of inference/kv_cache.py).  Returns true for e4m3.
+static bool kv_cache_e4m3(const char* fn, const Tensor& kc, const Tensor& vc, double k_scale, double v_scale) {
+  const auto t = kc.scalar_type();
+  TORCH_CHECK(t == at::kBFloat16 || t == at::kFloat8_e4m3fn, fn, ": the KV cache must be bfloat16 or float8_e4m3fn, got ", t);
+  TORCH_CHECK(vc.scalar_type() == t, fn, ": k and v caches must have the same dtype");
+  TORCH_CHECK(k_scale > 0 && v_scale > 0 && std::isfinite(k_scale) && std::isfinite(v_scale), fn, ": scales must be finite and > 0");
+  TORCH_CHECK(t != at::kBFloat16 || (k_scale == 1.0 && v_scale == 1.0), fn, ": k_scale / v_scale apply to an fp8 cache only");
+  return t == at::kFloat8_e4m3fn;
+}
+
 // q [B,1,H,D], k/v [B,1,Hkv,D] (views of the fused QKV GEMV output), cache [B,L,Hkv,D]: rotate q → new tensor, rotate k and
-// copy v straight into the cache row positions[b]
+// copy v straight into the cache row positions[b] (an e4m3 cache gets k / k_scale and v / v_scale, rounded as the cache's
+// torch rule rounds them)
 static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions, const Tensor& cos_t,
-                             const Tensor& sin_t, Tensor kc, Tensor vc) {
+                             const Tensor& sin_t, Tensor kc, Tensor vc, double k_scale, double v_scale) {
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) == 1 && q.stride(3) == 1);
   TORCH_CHECK(k.scalar_type() == at::kBFloat16 && k.dim() == 4 && k.size(1) == 1 && k.stride(3) == 1 && v.stride(3) == 1 && v.sizes() == k.sizes());
-  TORCH_CHECK(kc.scalar_type() == at::kBFloat16 && kc.dim() == 4 && kc.stride(3) == 1 && vc.sizes() == kc.sizes() && vc.strides() == kc.strides());
+  const bool e4m3 = kv_cache_e4m3("decode_rope_kv", kc, vc, k_scale, v_scale);
+  TORCH_CHECK(kc.dim() == 4 && kc.stride(3) == 1 && vc.sizes() == kc.sizes() && vc.strides() == kc.strides());
   TORCH_CHECK(positions.scalar_type() == at::kLong && positions.is_contiguous() && positions.numel() == q.size(0));
   CHECK_IN(cos_t); CHECK_IN(sin_t);
   TORCH_CHECK(cos_t.scalar_type() == at::kFloat && cos_t.size(1) == q.size(3) / 2 && cos_t.size(0) >= kc.size(1));
@@ -266,13 +280,15 @@ static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, 
   Tensor q_out = at::empty({B, 1, H, D}, q.options());
   nxd::decode_rope_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), cos_t.data_ptr<float>(),
                       sin_t.data_ptr<float>(), q_out.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, H, Hkv, D, L, q.stride(0), q.stride(2),
-                      k.stride(0), k.stride(2), v.stride(0), v.stride(2), kc.stride(0), kc.stride(1), kc.stride(2), stream());
+                      k.stride(0), k.stride(2), v.stride(0), v.stride(2), kc.stride(0), kc.stride(1), kc.stride(2), stream(), e4m3,
+                      1.0f / (float)k_scale, 1.0f / (float)v_scale);
   return q_out;
 }
 
 // ---- decode ---------------------------------------------------------------------------------------
 // q [B,1,H,128]; k/v cache [B,L,Hkv,128] (any b/s/h strides, head_dim contiguous); positions [B] int64 (attend to ≤ pos);
-// window > 0: only the last `window` positions up to pos are visible
+// window > 0: only the last `window` positions up to pos are visible.  The cache is bf16, or e4m3 with per-tensor scales
+// (the kernel then loads 8 bytes per lane: base pointers and strides must be multiples of 8 elements, as on bf16)
 static int decode_splits(int B, int Hkv, int L, int64_t window) {
   TORCH_CHECK(window >= 0, "decode_attention: window must be >= 0 (0 = none)");
   const int rows = window > 0 && window < L ? (int)window : L;      // cache rows one sequence reads at most
@@ -280,15 +296,24 @@ static int decode_splits(int B, int Hkv, int L, int64_t window) {
   int splits = (6 * num_sms() + B * Hkv - 1) / (B * Hkv);
   return std::max(1, std::min(std::min(splits, 64), (rows + 63) / 64));
 }
-static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions, double scale,
-                               int64_t window) {
+// argument checks shared by decode_attention and decode_attention_partial; returns true for an e4m3 cache
+static bool check_decode_args(const char* fn, const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions,
+                              double k_scale, double v_scale) {
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) == 1 && q.size(3) == 128 && q.stride(3) == 1);
-  TORCH_CHECK(k.scalar_type() == at::kBFloat16 && k.dim() == 4 && k.size(3) == 128 && k.stride(3) == 1 && v.stride(3) == 1 &&
-              v.sizes() == k.sizes());
+  const bool e4m3 = kv_cache_e4m3(fn, k, v, k_scale, v_scale);
+  TORCH_CHECK(k.dim() == 4 && k.size(3) == 128 && k.stride(3) == 1 && v.stride(3) == 1 && v.sizes() == k.sizes());
   TORCH_CHECK(positions.scalar_type() == at::kLong && positions.is_cuda() && positions.is_contiguous() && positions.numel() == q.size(0));
-  const int B = q.size(0), H = q.size(2), L = k.size(1), Hkv = k.size(2);
-  TORCH_CHECK(H % Hkv == 0 && k.size(0) == B);
+  TORCH_CHECK(q.size(2) % k.size(2) == 0 && k.size(0) == q.size(0));
   TORCH_CHECK(q.stride(2) % 8 == 0 && k.stride(1) % 8 == 0 && k.stride(2) % 8 == 0 && v.stride(1) % 8 == 0 && v.stride(2) % 8 == 0);
+  TORCH_CHECK(!e4m3 || ((reinterpret_cast<uintptr_t>(k.data_ptr()) | reinterpret_cast<uintptr_t>(v.data_ptr())) % 8 == 0 &&
+                        k.stride(0) % 8 == 0 && v.stride(0) % 8 == 0),
+              fn, ": e4m3 caches are read 8 bytes at a time: their base addresses and strides must be multiples of 8");
+  return e4m3;
+}
+static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions, double scale,
+                               int64_t window, double k_scale, double v_scale) {
+  const bool e4m3 = check_decode_args("decode_attention", q, k, v, positions, k_scale, v_scale);
+  const int B = q.size(0), H = q.size(2), L = k.size(1), Hkv = k.size(2);
   c10::cuda::CUDAGuard guard(q.device());
   const int splits = decode_splits(B, Hkv, L, window);
   Tensor out = at::empty({B, 1, H, 128}, q.options());
@@ -297,21 +322,17 @@ static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v
   const long ks[3] = {k.stride(0), k.stride(1), k.stride(2)}, vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   nxd::decode_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), out.data_ptr(),
                         part_o.data_ptr<float>(), part_ml.data_ptr<float>(), B, H, Hkv, L, ks, vs, q.stride(0), q.stride(2),
-                        out.stride(0), out.stride(2), (float)scale, splits, (int)std::min<int64_t>(window, INT32_MAX), stream());
+                        out.stride(0), out.stride(2), (float)scale, splits, (int)std::min<int64_t>(window, INT32_MAX), stream(),
+                        nullptr, nullptr, e4m3, (float)k_scale, (float)v_scale);
   return out;
 }
 // This rank's contribution to distributed flash-decoding: un-normalised output (relative to the row maximum) [B,H,128] fp32 and
 // (row maximum in natural-log units, row sum) [B,H,2] fp32 over the local cache shard; ``positions`` are LOCAL (may be < 0 or
 // >= L: nothing / everything of this shard is visible).
 static std::vector<Tensor> decode_attention_partial(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions,
-                                                    double scale, int64_t window) {
-  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) == 1 && q.size(3) == 128 && q.stride(3) == 1);
-  TORCH_CHECK(k.scalar_type() == at::kBFloat16 && k.dim() == 4 && k.size(3) == 128 && k.stride(3) == 1 && v.stride(3) == 1 &&
-              v.sizes() == k.sizes());
-  TORCH_CHECK(positions.scalar_type() == at::kLong && positions.is_cuda() && positions.is_contiguous() && positions.numel() == q.size(0));
+                                                    double scale, int64_t window, double k_scale, double v_scale) {
+  const bool e4m3 = check_decode_args("decode_attention_partial", q, k, v, positions, k_scale, v_scale);
   const int B = q.size(0), H = q.size(2), L = k.size(1), Hkv = k.size(2);
-  TORCH_CHECK(H % Hkv == 0 && k.size(0) == B);
-  TORCH_CHECK(q.stride(2) % 8 == 0 && k.stride(1) % 8 == 0 && k.stride(2) % 8 == 0 && v.stride(1) % 8 == 0 && v.stride(2) % 8 == 0);
   c10::cuda::CUDAGuard guard(q.device());
   const int splits = decode_splits(B, Hkv, L, window);
   Tensor fin_o = at::empty({B, H, 128}, q.options().dtype(at::kFloat));
@@ -321,7 +342,8 @@ static std::vector<Tensor> decode_attention_partial(const Tensor& q, const Tenso
   const long ks[3] = {k.stride(0), k.stride(1), k.stride(2)}, vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   nxd::decode_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), nullptr, part_o.data_ptr<float>(),
                         part_ml.data_ptr<float>(), B, H, Hkv, L, ks, vs, q.stride(0), q.stride(2), 0, 0, (float)scale, splits,
-                        (int)std::min<int64_t>(window, INT32_MAX), stream(), fin_o.data_ptr<float>(), fin_ml.data_ptr<float>());
+                        (int)std::min<int64_t>(window, INT32_MAX), stream(), fin_o.data_ptr<float>(), fin_ml.data_ptr<float>(),
+                        e4m3, (float)k_scale, (float)v_scale);
   return {fin_o, fin_ml};
 }
 // x [T,H] bf16; gamma [H] bf16 or none; router_w [E,H] bf16; router_bias [E] fp32 or none; w_gu [El,H,2I]; w_dn [El,I,H]
@@ -764,9 +786,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gemm_bf16", &gemm_bf16);
   m.def("oneshot_allreduce", &oneshot_allreduce);
   m.def("decode_attention", &decode_attention, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"), py::arg("scale"),
-        py::arg("window") = 0);
+        py::arg("window") = 0, py::kw_only(), py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0);
   m.def("decode_attention_partial", &decode_attention_partial, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"),
-        py::arg("scale"), py::arg("window") = 0);
+        py::arg("scale"), py::arg("window") = 0, py::kw_only(), py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0);
   m.def("nvls_embedding_gather", &nvls_embedding_gather);
   m.def("nvls_publish", &nvls_publish);
   m.def("ptr_view", &ptr_view);
@@ -777,7 +799,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("moe_block_tkg_supported", [](int64_t T, int64_t H, int64_t E, int64_t I, int64_t K) {
     return nxd::moe_block_tkg_supported((int)T, (int)H, (int)E, (int)I, (int)K);
   });
-  m.def("decode_rope_kv", &decode_rope_kv);
+  m.def("decode_rope_kv", &decode_rope_kv, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"), py::arg("cos"),
+        py::arg("sin"), py::arg("k_cache"), py::arg("v_cache"), py::kw_only(), py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0);
   m.def("moe_block_metadata", &moe_block_metadata);
   m.def("row_argmax", &row_argmax);
   m.def("row_topk", &row_topk);

@@ -4,9 +4,11 @@
 //                      GQA group processed together so K/V are read once per kv head), + a combine pass over the splits.
 //                      Role of the reference's token-generation attention (modules/attention, models' TKG path).
 //                      Optional sliding window W: only cache rows positions[b] − W < j ≤ positions[b] are read.
+//                      The cache is bf16 or fp8 e4m3 with one fp32 scale per tensor (inference/kv_cache.py owns that format).
 //   gemv_bf16        : y[M≤8, N] = x[M, K] · W[N, K]ᵀ (+ optional residual) for batch-1..8 decode; every weight byte is read once
 //                      with 16-byte loads, fp32 accumulation.
 #include <cuda.h>
+#include <cuda_fp8.h>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -18,13 +20,39 @@ namespace {
 constexpr int HD = 128;
 constexpr int kDecThreads = 128;
 
-// 16 lanes share one kv position (8 dims = 16 bytes each); a warp covers 2 positions per step, the CTA 8.
-template <int G>
+// 8 consecutive elements → fp32 (bf16: one 16-byte load; e4m3: one 8-byte load and the hardware fp8x2 → f16x2 unpack)
+__device__ __forceinline__ void load8(const __nv_bfloat16* p, float (&f)[8], float mul) {
+  const uint4 a = *reinterpret_cast<const uint4*>(p);
+  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&a);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { const float2 t = __bfloat1622float2(h[i]); f[2 * i] = t.x * mul; f[2 * i + 1] = t.y * mul; }
+}
+__device__ __forceinline__ void load8(const __nv_fp8_e4m3* p, float (&f)[8], float mul) {
+  const uint2 a = *reinterpret_cast<const uint2*>(p);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const unsigned w = i < 2 ? a.x : a.y;
+    const float2 t = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w >> (16 * (i & 1))), __NV_E4M3)));
+    f[2 * i] = t.x * mul; f[2 * i + 1] = t.y * mul;
+  }
+}
+
+// 16 lanes share one kv position (8 dims each); a warp covers 2 positions per step, the CTA 8.  A bf16 lane loads 16 bytes
+// of K and of V per position and takes one position per step (P = 1).  An e4m3 lane gets 8 bytes per position, so it takes
+// P = 2 positions per step (a warp covers 4, the CTA 16): each lane still has 32 bytes of K/V in flight per step, as on bf16,
+// and keeps the bf16 kernel's per-lane softmax state (P = 1 would halve the bytes in flight of a kernel that is latency-bound
+// per CTA).  The other way to keep 16-byte loads, 8 lanes × 16 dims, doubles each lane's q and o registers: G = 8 uses 184
+// registers on bf16 already, so it would spill there.  For G ≤ 4 that mapping fits and would halve the softmax updates per
+// position (16 lanes repeat the same one here); it has not been timed against this one (DESIGN §6).
+// k_scale is folded into scale_log2 by the host; v_scale multiplies the partial o (1 on bf16).
+template <typename T, int G>
 __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
-    const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc, const __nv_bfloat16* __restrict__ vc,
+    const __nv_bfloat16* __restrict__ q, const T* __restrict__ kc, const T* __restrict__ vc,
     const long* __restrict__ positions, float* __restrict__ part_o, float* __restrict__ part_ml, int B, int H, int Hkv, int L,
     long k_sb, long k_ss, long k_sh, long v_sb, long v_ss, long v_sh, long q_sb, long q_sh, float scale_log2, int splits,
-    int window) {
+    int window, float v_scale) {
+  constexpr bool kE4M3 = sizeof(T) == 1;
+  constexpr int P = kE4M3 ? 2 : 1;                          // positions per lane per step
   const int kvh = blockIdx.x, b = blockIdx.y, split = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sub = lane >> 4, l16 = lane & 15;               // position slot within the warp step, 8-dim slice
@@ -37,12 +65,6 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
   const int per = (n_valid + splits - 1) / splits;
   const int s0 = lo + split * per, s1 = min(hi, s0 + per);
 
-  auto load8 = [](const __nv_bfloat16* p, float (&f)[8], float mul) {
-    const uint4 a = *reinterpret_cast<const uint4*>(p);
-    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&a);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { const float2 t = __bfloat1622float2(h[i]); f[2 * i] = t.x * mul; f[2 * i + 1] = t.y * mul; }
-  };
   float qf[G][8];
 #pragma unroll
   for (int g = 0; g < G; ++g) load8(q + b * q_sb + (long)(kvh * G + g) * q_sh + l16 * 8, qf[g], scale_log2);
@@ -53,35 +75,45 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
 #pragma unroll
     for (int i = 0; i < 8; ++i) o[g][i] = 0.f;
   }
-  const __nv_bfloat16* kb = kc + b * k_sb + (long)kvh * k_sh + l16 * 8;
-  const __nv_bfloat16* vb = vc + b * v_sb + (long)kvh * v_sh + l16 * 8;
-  for (int sbase = s0 + warp * 2; sbase < s1; sbase += 8) {      // warp-uniform trip count (full-mask shuffles inside)
-    const int s = sbase + sub;
-    const bool live = s < s1;
-    float kf[8], vf[8];
-    if (live) {
-      load8(kb + (long)s * k_ss, kf, 1.f);
-      load8(vb + (long)s * v_ss, vf, 1.f);
-    } else {
+  const T* kb = kc + b * k_sb + (long)kvh * k_sh + l16 * 8;
+  const T* vb = vc + b * v_sb + (long)kvh * v_sh + l16 * 8;
+  for (int sbase = s0 + warp * 2 * P; sbase < s1; sbase += 8 * P) {      // warp-uniform trip count (full-mask shuffles inside)
+    bool live[P];
+    float kf[P][8], vf[P][8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) { kf[i] = 0.f; vf[i] = 0.f; }
+    for (int j = 0; j < P; ++j) {                         // all loads of the step are issued before any math
+      const int s = sbase + 2 * j + sub;
+      live[j] = s < s1;
+      if constexpr (kE4M3) {                              // a position past s1 re-reads row s1 − 1; its score is not used
+        load8(kb + (long)min(s, s1 - 1) * k_ss, kf[j], 1.f);
+        load8(vb + (long)min(s, s1 - 1) * v_ss, vf[j], 1.f);
+      } else if (live[j]) {
+        load8(kb + (long)s * k_ss, kf[j], 1.f);
+        load8(vb + (long)s * v_ss, vf[j], 1.f);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { kf[j][i] = 0.f; vf[j][i] = 0.f; }
+      }
     }
 #pragma unroll
-    for (int g = 0; g < G; ++g) {
-      float d = 0.f;
+    for (int j = 0; j < P; ++j) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) d = fmaf(qf[g][i], kf[i], d);
-      d += __shfl_xor_sync(0xffffffffu, d, 1);
-      d += __shfl_xor_sync(0xffffffffu, d, 2);
-      d += __shfl_xor_sync(0xffffffffu, d, 4);
-      d += __shfl_xor_sync(0xffffffffu, d, 8);            // score·log2e of (position s, head g) in all 16 lanes
-      if (live) {
-        const float mn = fmaxf(m[g], d);
-        const float corr = exp2f(m[g] - mn), p = exp2f(d - mn);
-        m[g] = mn;
-        l[g] = l[g] * corr + p;
+      for (int g = 0; g < G; ++g) {
+        float d = 0.f;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) o[g][i] = fmaf(o[g][i], corr, p * vf[i]);
+        for (int i = 0; i < 8; ++i) d = fmaf(qf[g][i], kf[j][i], d);
+        d += __shfl_xor_sync(0xffffffffu, d, 1);
+        d += __shfl_xor_sync(0xffffffffu, d, 2);
+        d += __shfl_xor_sync(0xffffffffu, d, 4);
+        d += __shfl_xor_sync(0xffffffffu, d, 8);          // score·log2e of (position s, head g) in all 16 lanes
+        if (live[j]) {
+          const float mn = fmaxf(m[g], d);
+          const float corr = exp2f(m[g] - mn), p = exp2f(d - mn);
+          m[g] = mn;
+          l[g] = l[g] * corr + p;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) o[g][i] = fmaf(o[g][i], corr, p * vf[j][i]);
+        }
       }
     }
   }
@@ -120,7 +152,8 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
       ls += sm_l[w][g] * c;
     }
     const long idx = (((long)b * H + kvh * G + g) * splits + split);
-    part_o[idx * HD + d] = acc;
+    if constexpr (kE4M3) part_o[idx * HD + d] = acc * v_scale;
+    else part_o[idx * HD + d] = acc;
     if (d == 0) { part_ml[idx * 2] = mn; part_ml[idx * 2 + 1] = ls; }
   }
 }
@@ -203,16 +236,30 @@ __global__ void __launch_bounds__(256) gemv_kernel(const __nv_bfloat16* __restri
   }
 }
 
+// KVCacheManager._q on CUDA, bit for bit: x · (1/scale) in fp32 (torch divides by a Python scalar through its fp32
+// reciprocal), then torch's float → e4m3 cast.  That cast rounds to nearest even and does not saturate: a value past 464
+// (which rounds beyond 448), ±inf and NaN become the NaN byte 0x7F with the input's sign, where the hardware's satfinite
+// conversion would clamp to ±448.
+__device__ __forceinline__ __nv_fp8_e4m3 quant_e4m3(__nv_bfloat16 x, float inv) {
+  const float f = __bfloat162float(x) * inv;
+  __nv_fp8_e4m3 r;
+  r.__x = fabsf(f) <= 464.f ? __nv_cvt_float_to_fp8(f, __NV_SATFINITE, __NV_E4M3)
+                            : (__nv_fp8_storage_t)(((__float_as_uint(f) >> 24) & 0x80u) | 0x7Fu);
+  return r;
+}
+
 // Decode-time RoPE + KV-cache append in ONE launch (was ~25 tiny elementwise / index_put kernels per layer in the token-
 // generation graph): q [B,H,D] rotated into q_out, k rotated and v copied into the cache row positions[b].  One warp per head
-// row; cos/sin rows gathered by position.  HF rotate-half convention (csrc/elementwise.cu rope_kernel).
+// row; cos/sin rows gathered by position.  HF rotate-half convention (csrc/elementwise.cu rope_kernel).  An e4m3 cache gets
+// the bf16 rows a bf16 cache would hold, quantised by quant_e4m3 with k_inv = 1/k_scale and v_inv = 1/v_scale.
+template <typename T>
 __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                                             const __nv_bfloat16* __restrict__ v, const long* __restrict__ positions,
                                                             const float* __restrict__ cos_t, const float* __restrict__ sin_t,
-                                                            __nv_bfloat16* __restrict__ q_out, __nv_bfloat16* __restrict__ kc,
-                                                            __nv_bfloat16* __restrict__ vc, int B, int H, int Hkv, int D, int L,
+                                                            __nv_bfloat16* __restrict__ q_out, T* __restrict__ kc,
+                                                            T* __restrict__ vc, int B, int H, int Hkv, int D, int L,
                                                             long q_sb, long q_sh, long k_sb, long k_sh, long v_sb, long v_sh,
-                                                            long c_sb, long c_ss, long c_sh) {
+                                                            long c_sb, long c_ss, long c_sh, float k_inv, float v_inv) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int rows = B * (H + 2 * Hkv);
   if (warp >= rows) return;
@@ -224,20 +271,40 @@ __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16
     const bool is_q = r < H;
     const int h = is_q ? r : r - H;
     const __nv_bfloat16* src = is_q ? q + b * q_sb + (long)h * q_sh : k + b * k_sb + (long)h * k_sh;
-    __nv_bfloat16* dst = is_q ? q_out + ((long)b * H + h) * D : kc + b * c_sb + pos * c_ss + (long)h * c_sh;
+    __nv_bfloat16* dst = is_q ? q_out + ((long)b * H + h) * D : reinterpret_cast<__nv_bfloat16*>(kc + b * c_sb + pos * c_ss + (long)h * c_sh);
     const float* cr = cos_t + pos * half;
     const float* sr = sin_t + pos * half;
-    for (int c = lane; c < half; c += 32) {
-      const float a = __bfloat162float(src[c]), bb = __bfloat162float(src[half + c]);
-      const float cs = cr[c], sn = sr[c];
-      dst[c] = __float2bfloat16_rn(a * cs - bb * sn);
-      dst[half + c] = __float2bfloat16_rn(bb * cs + a * sn);
+    if constexpr (sizeof(T) == 2) {
+      for (int c = lane; c < half; c += 32) {
+        const float a = __bfloat162float(src[c]), bb = __bfloat162float(src[half + c]);
+        const float cs = cr[c], sn = sr[c];
+        dst[c] = __float2bfloat16_rn(a * cs - bb * sn);
+        dst[half + c] = __float2bfloat16_rn(bb * cs + a * sn);
+      }
+    } else {                                           // q rows stay bf16; k rows are rounded to bf16, then quantised
+      T* kd = reinterpret_cast<T*>(dst);
+      for (int c = lane; c < half; c += 32) {
+        const float a = __bfloat162float(src[c]), bb = __bfloat162float(src[half + c]);
+        const float cs = cr[c], sn = sr[c];
+        const __nv_bfloat16 x0 = __float2bfloat16_rn(a * cs - bb * sn), x1 = __float2bfloat16_rn(bb * cs + a * sn);
+        if (is_q) {
+          dst[c] = x0;
+          dst[half + c] = x1;
+        } else {
+          kd[c] = quant_e4m3(x0, k_inv);
+          kd[half + c] = quant_e4m3(x1, k_inv);
+        }
+      }
     }
   } else {                                             // v head: copy
     const int h = r - H - Hkv;
     const __nv_bfloat16* src = v + b * v_sb + (long)h * v_sh;
-    __nv_bfloat16* dst = vc + b * c_sb + pos * c_ss + (long)h * c_sh;
-    for (int c = lane; c < D; c += 32) dst[c] = src[c];
+    T* dst = vc + b * c_sb + pos * c_ss + (long)h * c_sh;
+    if constexpr (sizeof(T) == 2) {
+      for (int c = lane; c < D; c += 32) dst[c] = src[c];
+    } else {
+      for (int c = lane; c < D; c += 32) dst[c] = quant_e4m3(src[c], v_inv);
+    }
   }
 }
 
@@ -245,32 +312,40 @@ __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16
 
 void decode_rope_kv(const void* q, const void* k, const void* v, const long* positions, const float* cos_t, const float* sin_t,
                     void* q_out, void* kc, void* vc, int B, int H, int Hkv, int D, int L, long q_sb, long q_sh, long k_sb, long k_sh,
-                    long v_sb, long v_sh, long c_sb, long c_ss, long c_sh, cudaStream_t st) {
+                    long v_sb, long v_sh, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3, float k_inv, float v_inv) {
   const int rows = B * (H + 2 * Hkv);
   const int grid = (rows * 32 + 127) / 128;
-  decode_rope_kv_kernel<<<grid, 128, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, positions,
-                                              cos_t, sin_t, (__nv_bfloat16*)q_out, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, B, H, Hkv, D, L,
-                                              q_sb, q_sh, k_sb, k_sh, v_sb, v_sh, c_sb, c_ss, c_sh);
+#define NXD_ROPE_KV(T)                                                                                                       \
+  decode_rope_kv_kernel<T><<<grid, 128, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v,   \
+      positions, cos_t, sin_t, (__nv_bfloat16*)q_out, (T*)kc, (T*)vc, B, H, Hkv, D, L, q_sb, q_sh, k_sb, k_sh, v_sb, v_sh, c_sb, \
+      c_ss, c_sh, k_inv, v_inv)
+  if (kv_e4m3) NXD_ROPE_KV(__nv_fp8_e4m3);
+  else NXD_ROPE_KV(__nv_bfloat16);
+#undef NXD_ROPE_KV
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 
 void decode_attention(const void* q, const void* k, const void* v, const long* positions, void* out, float* part_o,
                       float* part_ml, int B, int H, int Hkv, int L, const long* ks, const long* vs, long q_sb, long q_sh,
-                      long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o, float* fin_ml) {
+                      long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o, float* fin_ml,
+                      bool kv_e4m3, float k_scale, float v_scale) {
   const int G = H / Hkv;
   dim3 grid(Hkv, B, splits);
-  const float sl2 = scale * 1.4426950408889634f;
-#define NXD_DEC(Gv)                                                                                                  \
-  decode_attn_kernel<Gv><<<grid, kDecThreads, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k,             \
-      (const __nv_bfloat16*)v, positions, part_o, part_ml, B, H, Hkv, L, ks[0], ks[1], ks[2], vs[0], vs[1], vs[2], q_sb, \
-      q_sh, sl2, splits, window)
-  switch (G) {
-    case 1: NXD_DEC(1); break;
-    case 2: NXD_DEC(2); break;
-    case 4: NXD_DEC(4); break;
-    case 8: NXD_DEC(8); break;
-    default: nxd_throw("decode_attention: unsupported GQA group size", __FILE__, __LINE__);
+  const float sl2 = scale * 1.4426950408889634f * k_scale;
+#define NXD_DEC(T, Gv)                                                                                                 \
+  decode_attn_kernel<T, Gv><<<grid, kDecThreads, 0, st>>>((const __nv_bfloat16*)q, (const T*)k, (const T*)v, positions, \
+      part_o, part_ml, B, H, Hkv, L, ks[0], ks[1], ks[2], vs[0], vs[1], vs[2], q_sb, q_sh, sl2, splits, window, v_scale)
+#define NXD_DEC_G(T)                                                                      \
+  switch (G) {                                                                            \
+    case 1: NXD_DEC(T, 1); break;                                                         \
+    case 2: NXD_DEC(T, 2); break;                                                         \
+    case 4: NXD_DEC(T, 4); break;                                                         \
+    case 8: NXD_DEC(T, 8); break;                                                         \
+    default: nxd_throw("decode_attention: unsupported GQA group size", __FILE__, __LINE__); \
   }
+  if (kv_e4m3) NXD_DEC_G(__nv_fp8_e4m3)
+  else NXD_DEC_G(__nv_bfloat16)
+#undef NXD_DEC_G
 #undef NXD_DEC
   if (fin_o != nullptr) decode_combine_partial_kernel<<<B * H, HD, 0, st>>>(part_o, part_ml, fin_o, fin_ml, splits);
   else decode_combine_kernel<<<B * H, HD, 0, st>>>(part_o, part_ml, (__nv_bfloat16*)out, splits, o_sb, o_sh, H);

@@ -132,12 +132,15 @@ void gemv_mx_grouped(const void* x, const void* w, const void* scale, const long
 // ---- decode (decode.cu)
 void decode_attention(const void* q, const void* k, const void* v, const long* positions, void* out, float* part_o,
                       float* part_ml, int B, int H, int Hkv, int L, const long* ks, const long* vs, long q_sb, long q_sh,
-                      long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o = nullptr,
-                      float* fin_ml = nullptr);   // fin_o/fin_ml: un-normalised [B*H,128] + (max, sum) [B*H,2] instead of ``out``
-                                                  // window: keys positions[b] − window < j ≤ positions[b] visible (0: no window)
+                      long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o,
+                      float* fin_ml, bool kv_e4m3, float k_scale, float v_scale);
+                      // fin_o/fin_ml: un-normalised [B*H,128] + (max, sum) [B*H,2] instead of ``out`` (nullptr: ``out``)
+                      // window: keys positions[b] − window < j ≤ positions[b] visible (0: no window)
+                      // kv_e4m3: k/v are fp8 e4m3 caches holding k / k_scale and v / v_scale (bf16: both scales 1)
 void decode_rope_kv(const void* q, const void* k, const void* v, const long* positions, const float* cos_t, const float* sin_t,
                     void* q_out, void* kc, void* vc, int B, int H, int Hkv, int D, int L, long q_sb, long q_sh, long k_sb, long k_sh,
-                    long v_sb, long v_sh, long c_sb, long c_ss, long c_sh, cudaStream_t st);
+                    long v_sb, long v_sh, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3, float k_inv,
+                    float v_inv);   // kv_e4m3: the cache stores k·k_inv and v·v_inv as e4m3 (bf16: rows as computed)
 void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, cudaStream_t st);
 
 // ---- attention (attention_sm90.cu): q [B,S_q,H,D], k/v [B,S_kv,Hkv,D] bf16 views, D ∈ {64, 80, 96, 128}; strides = (b, s, h)

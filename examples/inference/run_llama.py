@@ -6,6 +6,9 @@ reference's ``examples/inference/run_llama.py`` / ``runner.py`` (trace → load 
       --max_prompt_length 1024 --sequence_length 2048 --benchmark
   # GQA with fewer KV heads than ranks: replicas of a KV head shard its cache along the sequence (flash decoding)
   torchrun --nproc-per-node 8 examples/inference/run_llama.py --model 7b --num_kv_heads 4 --tp_degree 8 --flash_decoding
+  # KV cache stored in fp8 e4m3 (one scale per tensor): half the cache bytes, read directly by the decode kernels
+  torchrun --nproc-per-node 1 examples/inference/run_llama.py --model 7b --batch_size 16 --max_prompt_length 2048 \
+      --sequence_length 4096 --benchmark --kv_cache_quant fp8
 """
 import argparse
 import json
@@ -25,6 +28,7 @@ from neuronx_distributed_b200.trace.model_builder import ModelBuilder  # noqa: E
 from neuronx_distributed_b200.models.llama import LlamaConfig, llama2_7b_config, llama2_13b_config  # noqa: E402
 from neuronx_distributed_b200.models.llama_inference import LlamaForInference  # noqa: E402
 from neuronx_distributed_b200.parallel_layers import parallel_state as ps  # noqa: E402
+from neuronx_distributed_b200.quantization import KVQuantizationConfig  # noqa: E402
 from training_utils import init_distributed  # noqa: E402
 
 
@@ -42,6 +46,9 @@ def main():
     p.add_argument("--flash_decoding", action="store_true",
                    help="shard the KV cache along the sequence inside each KV-replica group (needs tp_degree > number of KV heads)")
     p.add_argument("--num_kv_heads", type=int, default=0, help="override the number of KV heads (GQA experiments)")
+    p.add_argument("--kv_cache_quant", default="none", choices=["none", "fp8"],
+                   help="fp8: store the KV cache in float8 e4m3 with one scale per tensor (--kv_cache_scale)")
+    p.add_argument("--kv_cache_scale", type=float, default=1.0, help="the cache stores k / scale and v / scale")
     a = p.parse_args()
     dev = init_distributed()
     ps.initialize_model_parallel(tensor_model_parallel_size=a.tp_degree)
@@ -54,8 +61,11 @@ def main():
     if a.num_kv_heads > 0:
         cfg.num_key_value_heads = a.num_kv_heads
     torch.manual_seed(0)
+    kv_quant = None
+    if a.kv_cache_quant == "fp8":
+        kv_quant = KVQuantizationConfig(quant_dtype=torch.float8_e4m3fn, dequant_dtype=dtype, scale=a.kv_cache_scale)
     model = LlamaForInference(cfg, batch_size=a.batch_size, max_seq_len=a.sequence_length,
-                              flash_decoding=a.flash_decoding).eval()
+                              flash_decoding=a.flash_decoding, kv_quant=kv_quant).eval()
     B, P = a.batch_size, a.max_prompt_length
     mb = ModelBuilder(tp_degree=a.tp_degree, use_cuda_graphs=(dev.type == "cuda" and not a.no_cuda_graphs))
     for bucket in generate_buckets(min(128, P), P):
@@ -85,6 +95,10 @@ def main():
     if a.benchmark:
         lat = Benchmark(generate, num_runs=a.num_runs).run()
         rep = generate_report(lat, a.sequence_length, B)
+        rep["generated_tokens_per_s"] = B * new_tokens / (sum(lat) / len(lat))
+        if dev.type == "cuda":
+            rep["peak_allocated_GiB"] = torch.cuda.max_memory_allocated(dev) / 2 ** 30
+            rep["kv_cache_GiB"] = sum(t.nbytes for t in model.kv.k + model.kv.v) / 2 ** 30
         if dist.get_rank() == 0:
             print(json.dumps({"e2e_model": rep, "config": vars(a)}), flush=True)
     dist.barrier()

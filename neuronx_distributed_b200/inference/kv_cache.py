@@ -8,7 +8,13 @@ from typing import List, Optional, Tuple
 
 import torch
 
-from ..quantization.quantization_config import KVQuantizationConfig
+from ..quantization.quantization_config import KVQuantizationConfig, QuantizationType
+
+
+def per_tensor(kv_quant: KVQuantizationConfig) -> bool:
+    """True when ``kv_quant`` asks for one scale per tensor, the only granularity this cache implements."""
+    return (not kv_quant.per_key and kv_quant.k_quant_method == QuantizationType.PER_TENSOR_SYMMETRIC
+            and kv_quant.v_quant_method == QuantizationType.PER_TENSOR_SYMMETRIC)
 
 
 class KVCacheManager:
@@ -55,6 +61,14 @@ class KVCacheManager:
             self.k[layer][: k.shape[0], : hi - lo].copy_(self._q(k[:, lo:hi]))
             self.v[layer][: v.shape[0], : hi - lo].copy_(self._q(v[:, lo:hi]))
 
+    def write_decode_sharded(self, layer: int, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor,
+                             shard_rank: int) -> None:
+        """Flash-decoding layout: k/v ``[B, 1, H, D]`` of global ``positions``, written only by the rank whose sequence
+        shard holds each position."""
+        from ..modules.attention.flash_decode import write_decode_sharded
+
+        write_decode_sharded(self.k[layer], self.v[layer], self._q(k), self._q(v), positions, shard_rank)
+
     def write_decode(self, layer: int, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor) -> None:
         """k/v ``[B, 1, H, D]``; ``positions`` ``[B]`` (device tensor; no host sync → graph capturable)."""
         b = torch.arange(k.shape[0], device=k.device)
@@ -80,10 +94,28 @@ class KVCacheManager:
             self.k[layer].index_put_((b, dst), self.k[layer][b, src])
             self.v[layer].index_put_((b, dst), self.v[layer][b, src])
 
-    def get(self, layer: int, length: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    def kernel_scales(self) -> Optional[Tuple[float, float]]:
+        """``(k_scale, v_scale)`` when the decode kernels (``csrc/decode.cu``) can read this cache as stored, else ``None``.
+        They read a bf16 cache (scales 1.0) and an fp8 e4m3 cache with one scale per tensor that de-quantises to bf16, on
+        CUDA; there ``stored`` holds k / k_scale and v / v_scale, rounded by ``_q``."""
+        if not self.k or not self.k[0].is_cuda:
+            return None
+        q = self.kv_quant
+        if q is None:
+            return (1.0, 1.0) if self.dtype == torch.bfloat16 else None
+        if q.quant_dtype == torch.float8_e4m3fn and per_tensor(q) and q.dequant_dtype == torch.bfloat16:
+            return (q.scale, q.scale)
+        return None
+
+    def stored(self, layer: int, length: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The cache tensors of ``layer`` as stored (fp8 when quantised), positions ``[0, length)``."""
         k, v = self.k[layer], self.v[layer]
         if length is not None:
             k, v = k[:, :length], v[:, :length]
+        return k, v
+
+    def get(self, layer: int, length: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        k, v = self.stored(layer, length)
         return self._dq(k), self._dq(v)
 
     def reset(self) -> None:

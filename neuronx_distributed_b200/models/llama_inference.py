@@ -11,16 +11,20 @@ import torch
 from torch import nn
 
 from .. import ops
-from ..inference.kv_cache import KVCacheManager
+from ..inference.kv_cache import KVCacheManager, per_tensor
+from ..quantization.quantization_config import KVQuantizationConfig
 from ..utils.sampling import Sampler
 from .llama import LlamaConfig, LlamaForCausalLM
 
 
 class LlamaForInference(nn.Module):
     def __init__(self, cfg: LlamaConfig, batch_size: int = 1, max_seq_len: int = 2048, on_device_sampling: bool = True,
-                 sampler: Optional[Sampler] = None, lm_cls=None, flash_decoding: bool = False):
+                 sampler: Optional[Sampler] = None, lm_cls=None, flash_decoding: bool = False,
+                 kv_quant: Optional[KVQuantizationConfig] = None):
         """``lm_cls``: any decoder built from Llama attention blocks (``LlamaForCausalLM`` default; ``MixtralForCausalLM`` for
-        the MoE families — its layers' ``mlp`` returns ``(y, router_logits)``, handled in ``_body``)."""
+        the MoE families — its layers' ``mlp`` returns ``(y, router_logits)``, handled in ``_body``).
+        ``kv_quant``: store the KV cache quantised, with one scale per tensor (fp8 e4m3 is read by the decode kernels
+        directly).  Prefill attention runs on the un-quantised k/v it computes; only the cache write is quantised."""
         super().__init__()
         cfg.sequence_parallel_enabled = False
         cfg.activation_checkpointing = "none"
@@ -39,8 +43,14 @@ class LlamaForInference(nn.Module):
                 "flash decoding needs replicated KV heads (tensor-parallel size > number of KV heads)"
             shards, self.kv_rank = dist.get_world_size(self.kv_group), dist.get_rank(self.kv_group)
             assert max_seq_len % shards == 0, f"max_seq_len {max_seq_len} must divide by the KV replication factor {shards}"
+        if kv_quant is not None and not per_tensor(kv_quant):
+            raise ValueError("kv_quant: the KV cache implements one scale per tensor; per-key and per-channel methods are "
+                             "not supported")
+        if kv_quant is not None and kv_quant.dequant_dtype != cfg.dtype:
+            raise ValueError(f"kv_quant.dequant_dtype ({kv_quant.dequant_dtype}) must be the model dtype ({cfg.dtype}): "
+                             "attention off the kernels reads the de-quantised cache next to the model's queries")
         self.kv = KVCacheManager(cfg.num_hidden_layers, batch_size, max_seq_len, attn0.num_kv_heads_local, cfg.head_dim,
-                                 dtype=cfg.dtype, device=cfg.device, num_cores_per_group=shards)
+                                 dtype=cfg.dtype, device=cfg.device, kv_quant=kv_quant, num_cores_per_group=shards)
         self.sampler = sampler or Sampler(top_k=1, vocab_parallel=True)
         self.on_device_sampling = on_device_sampling
         cos, sin = ops.rope.rope_tables(max_seq_len, cfg.head_dim, cfg.rope_theta, cfg.device, 0, cfg.rope_scaling_factor)
@@ -69,15 +79,20 @@ class LlamaForInference(nn.Module):
         q = q.reshape(S, B, att.num_heads_local, D).transpose(0, 1)
         k = k.reshape(S, B, att.num_kv_heads_local, D).transpose(0, 1)
         v = v.reshape(S, B, att.num_kv_heads_local, D).transpose(0, 1).contiguous()
+        # (k_scale, v_scale) when the decode kernels read the cache as stored; the defaults (1.0) are not passed on, so a bf16
+        # cache makes the calls it makes without quantisation
+        scales = self.kv.kernel_scales()
+        scale_kw = {} if scales in (None, (1.0, 1.0)) else {"k_scale": scales[0], "v_scale": scales[1]}
         if self.flash_decoding and not prefill:
             assert S == 1 and tree is None, "flash decoding serves plain token generation (no speculation window)"
-            from ..modules.attention.flash_decode import flash_decode_attention, write_decode_sharded
+            from ..modules.attention.flash_decode import flash_decode_attention
 
             cos = self.rope_cos[positions].unsqueeze(1)
             sin = self.rope_sin[positions].unsqueeze(1)
             q, k = _rope_per_batch(q, cos, sin), _rope_per_batch(k, cos, sin)
-            write_decode_sharded(self.kv.k[layer_idx], self.kv.v[layer_idx], k, v, positions, self.kv_rank)   # owner-only write
-            o = flash_decode_attention(q, self.kv.k[layer_idx], self.kv.v[layer_idx], positions, self.kv_group, sliding_window=sw)
+            self.kv.write_decode_sharded(layer_idx, k, v, positions, self.kv_rank)                  # owner-only write
+            kc, vc = self.kv.stored(layer_idx) if scales is not None else self.kv.get(layer_idx)
+            o = flash_decode_attention(q, kc, vc, positions, self.kv_group, sliding_window=sw, **scale_kw)
         elif not prefill and S > 1:
             # speculation window: W new tokens per sequence at positions p..p+W-1, causal among themselves, full cache before
             W = S
@@ -98,14 +113,14 @@ class LlamaForInference(nn.Module):
             else:
                 self.kv.write_prefill(layer_idx, k, v)
             o = ops.attention.flash_attention(q, k, v, causal=True, sliding_window=sw)
-        elif (q.is_cuda and q.dtype == torch.bfloat16 and self.kv.kv_quant is None and self.kv.seq_shards == 1
+        elif (q.is_cuda and q.dtype == torch.bfloat16 and scales is not None and self.kv.seq_shards == 1
               and ops._ext.ext() is not None and hasattr(ops._ext.ext(), "decode_rope_kv")):
             # one launch: RoPE of q and k at each sequence's position + append of k / v to the cache (csrc/decode.cu)
             ops._ext.count_launch()
             q = ops._ext.ext().decode_rope_kv(q, k, v, positions.to(torch.long).contiguous(), self.rope_cos, self.rope_sin,
-                                              self.kv.k[layer_idx], self.kv.v[layer_idx])
-            kc, vc = self.kv.get(layer_idx, kv_len)
-            o = _decode_attention(q, kc, vc, positions, sw)
+                                              self.kv.k[layer_idx], self.kv.v[layer_idx], **scale_kw)
+            kc, vc = self.kv.stored(layer_idx, kv_len)
+            o = _decode_attention(q, kc, vc, positions, sw, **scale_kw)
         else:
             # one new token per sequence at its own position
             cos = self.rope_cos[positions].unsqueeze(1)     # [B, 1, D/2] → per-batch tables
@@ -271,9 +286,11 @@ def _window_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positio
 
 
 def _decode_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor,
-                      sliding_window: Optional[int] = None) -> torch.Tensor:
+                      sliding_window: Optional[int] = None, k_scale: float = 1.0, v_scale: float = 1.0) -> torch.Tensor:
     """q [B,1,H,D] vs cache k/v [B,L,Hkv,D]; keys beyond each sequence's position (and, with ``sliding_window`` SW, keys at or
-    before position − SW) are masked."""
+    before position − SW) are masked.  An fp8 cache holds k / ``k_scale`` and v / ``v_scale``."""
+    if k.dtype in ops.attention.FP8_KV_DTYPES:
+        return ops.attention.decode_attention(q, k, v, positions, sliding_window=sliding_window, k_scale=k_scale, v_scale=v_scale)
     window = ops.attention.check_window(sliding_window)
     B, _, H, D = q.shape
     Hkv, L = k.shape[2], k.shape[1]

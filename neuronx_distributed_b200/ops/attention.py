@@ -20,6 +20,9 @@ from . import _ext
 #: head sizes the flash kernels are compiled for
 FLASH_HEAD_DIMS = (64, 80, 96, 128)
 
+#: fp8 KV-cache dtypes: stored as k / k_scale and v / v_scale, de-quantised off the kernels (the decode kernels read e4m3)
+FP8_KV_DTYPES = (torch.float8_e4m3fn, torch.float8_e5m2)
+
 
 def window_visibility(s_q: int, s_kv: int, window: Optional[int], device=None, q_offset: int = 0) -> torch.Tensor:
     """``[S_q, S_kv]`` bool: causal visibility, limited to the last ``window`` keys (query i sees i − W < j ≤ i) when
@@ -176,21 +179,43 @@ def check_window(sliding_window: Optional[int]) -> int:
     return int(sliding_window)
 
 
+def check_kv_scales(k_cache: torch.Tensor, v_cache: torch.Tensor, k_scale: float, v_scale: float) -> dict:
+    """The decode kernels' ``k_scale`` / ``v_scale`` keyword arguments: ``{}`` when both are 1.0 (what a bf16 cache always
+    has), else both.  Raises ``ValueError`` for scales other than 1.0 on a cache that is not fp8, or for k and v caches of
+    different dtypes."""
+    if k_cache.dtype != v_cache.dtype:
+        raise ValueError(f"k and v caches must have the same dtype, got {k_cache.dtype} and {v_cache.dtype}")
+    if k_scale == 1.0 and v_scale == 1.0:
+        return {}
+    if k_cache.dtype not in FP8_KV_DTYPES:
+        raise ValueError(f"k_scale / v_scale apply to fp8 caches only; got a {k_cache.dtype} cache with scales "
+                         f"({k_scale}, {v_scale})")
+    return {"k_scale": float(k_scale), "v_scale": float(v_scale)}
+
+
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, positions: torch.Tensor,
-                     scale: Optional[float] = None, sliding_window: Optional[int] = None) -> torch.Tensor:
+                     scale: Optional[float] = None, sliding_window: Optional[int] = None, k_scale: float = 1.0,
+                     v_scale: float = 1.0) -> torch.Tensor:
     """One new token per sequence against a KV cache: ``q [B,1,H,D]``, caches ``[B,L,Hkv,D]`` (any batch / sequence / head
     strides), ``positions [B]`` = cache index of the newest token (keys ≤ position are visible; with ``sliding_window`` W only
-    keys position − W < j ≤ position, and the kernel reads only those rows).  CUDA bf16 with head_dim 128: the split-KV
-    flash-decoding kernel (``csrc/decode.cu``); otherwise SDPA with a length mask."""
+    keys position − W < j ≤ position, and the kernel reads only those rows).  An fp8 cache holds k / ``k_scale`` and
+    v / ``v_scale`` (one scale per tensor, as ``inference.kv_cache.KVCacheManager`` stores it).  CUDA bf16 q with a bf16 or
+    fp8 e4m3 cache and head_dim 128: the split-KV flash-decoding kernel (``csrc/decode.cu``), which reads the e4m3 bytes
+    directly; otherwise SDPA with a length mask on the de-quantised cache."""
     B, _, H, D = q.shape
     Hkv, L = k_cache.shape[2], k_cache.shape[1]
     window = check_window(sliding_window)
+    kw = check_kv_scales(k_cache, v_cache, k_scale, v_scale)
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     e = _ext.ext() if q.is_cuda else None
-    if (e is not None and hasattr(e, "decode_attention") and D == 128 and q.dtype == torch.bfloat16 and k_cache.dtype == torch.bfloat16
-            and H // Hkv in (1, 2, 4, 8) and k_cache.stride(3) == 1 and v_cache.stride(3) == 1):
+    if (e is not None and hasattr(e, "decode_attention") and D == 128 and q.dtype == torch.bfloat16
+            and k_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn) and H // Hkv in (1, 2, 4, 8) and k_cache.stride(3) == 1
+            and v_cache.stride(3) == 1):
         _ext.count_launch(2)
-        return e.decode_attention(q.contiguous(), k_cache, v_cache, positions.to(torch.long).contiguous(), float(scale), window)
+        return e.decode_attention(q.contiguous(), k_cache, v_cache, positions.to(torch.long).contiguous(), float(scale), window,
+                                  **kw)
+    if k_cache.dtype in FP8_KV_DTYPES:
+        k_cache, v_cache = (k_cache.float() * k_scale).to(q.dtype), (v_cache.float() * v_scale).to(q.dtype)
     qt, kt, vt = q.transpose(1, 2), k_cache.transpose(1, 2), v_cache.transpose(1, 2)
     if H != Hkv:
         kt, vt = kt.repeat_interleave(H // Hkv, 1), vt.repeat_interleave(H // Hkv, 1)

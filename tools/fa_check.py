@@ -1,5 +1,5 @@
 """Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
-usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]]
+usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]] [--kv-fp8]
 
 --perf times forward and forward+backward of the own kernels and of SDPA in the same process, alternating, at the shapes
 the models run (BERT-large with right padding, ViT-B/16, GPT-NeoX-20B per rank at TP=8, Pythia-2.8B, Llama-2-7B).  FLOPs
@@ -16,7 +16,13 @@ one GPU: the blocks the rank with the most work computes under the windowed bloc
 ``_visible_pairs``), run through ``block_attention`` and the LSE merge as ring attention runs them, against the causal plan
 (what CP computes if the window is dropped).  It reports the time, the TFLOP/s over the visible pairs and the K/V bytes each
 rank sends per layer (hops × 2·c·Hkv·D·2 B).  All ranks' blocks come from one process, so no NCCL time is measured.  Pair and
-byte counts come from shapes and are printed without a GPU too; times need one."""
+byte counts come from shapes and are printed without a GPU too; times need one.
+
+--kv-fp8 (with --perf) times ``decode_attention`` on a bf16 and on an fp8 e4m3 KV cache of the same shape, alternating in one
+process: the Mistral-7B per-GPU shape (H 32, Hkv 8, D 128) on a full 32k cache at B = 1, 8 and 32, and the Llama-2-13B
+MHA shape (H = Hkv = 40) at B = 8, L = 4096.  Bytes read come from the shapes (the K and V rows and q; the fp32 split
+partials, which stay in L2, are left out); GB/s is those bytes over the time of the call (both kernels).  Both caches hold the same values (the bf16 one
+is the de-quantised e4m3 one), and the two outputs are compared."""
 import argparse
 import json
 import math
@@ -217,6 +223,44 @@ def window_perf(e, bwd: bool, W: int = 4096):
         print(json.dumps(rec), flush=True)
 
 
+KV_FP8_SHAPES = [  # name, B, L, H, Hkv
+    ("mistral7b", 1, 32768, 32, 8), ("mistral7b", 8, 32768, 32, 8), ("mistral7b", 32, 32768, 32, 8),
+    ("llama2_13b", 8, 4096, 40, 40),
+]
+
+
+def kv_fp8_perf():
+    dev = torch.device("cuda")
+    print(json.dumps(gpu_info()), flush=True)
+    D, ks, vs = 128, 0.05, 0.05
+    g = torch.Generator(device=dev).manual_seed(0)
+    for name, B, L, H, Hkv in KV_FP8_SHAPES:
+        q = torch.randn(B, 1, H, D, device=dev, generator=g).bfloat16()
+        k8, v8 = ((torch.randn(B, L, Hkv, D, device=dev, generator=g) / s).to(torch.float8_e4m3fn) for s in (ks, vs))
+        k16, v16 = (k8.float() * ks).bfloat16(), (v8.float() * vs).bfloat16()
+        pos = torch.full((B,), L - 1, device=dev, dtype=torch.long)
+        scale = 1.0 / math.sqrt(D)
+        o16 = attention.decode_attention(q, k16, v16, pos, scale)
+        o8 = attention.decode_attention(q, k8, v8, pos, scale, k_scale=ks, v_scale=vs)
+        err = ((o8.float() - o16.float()).abs().max() / o16.float().abs().max()).item()
+        t = {"bf16": [], "e4m3": []}
+        iters = max(20, 2000 // B)
+        for _ in range(3):                                     # alternate, keep each one's best
+            t["bf16"].append(time_fn(lambda: attention.decode_attention(q, k16, v16, pos, scale), iters))
+            t["e4m3"].append(time_fn(lambda: attention.decode_attention(q, k8, v8, pos, scale, k_scale=ks, v_scale=vs), iters))
+        rec = {"bench": f"{name}_decode_kv_fp8", "B": B, "L": L, "H": H, "Hkv": Hkv, "D": D, "e4m3_vs_bf16_rel_err": round(err, 5)}
+        for dt, elt in (("bf16", 2), ("e4m3", 1)):
+            ms = min(t[dt])
+            nbytes = 2 * B * L * Hkv * D * elt + B * H * D * 2   # K and V rows, q
+            rec[f"{dt}_us"] = round(ms * 1e3, 2)
+            rec[f"{dt}_bytes"] = nbytes
+            rec[f"{dt}_GBps"] = round(nbytes / ms / 1e6, 1)
+        rec["bf16_over_e4m3"] = round(rec["bf16_us"] / rec["e4m3_us"], 2)
+        print(json.dumps(rec), flush=True)
+        del q, k8, v8, k16, v16
+        torch.cuda.empty_cache()
+
+
 def block_pairs(c: int, causal: bool, off: int, W) -> int:
     """Visible (query, key) pairs of one c × c CP block: all c² when dense, else i + off − W < j ≤ i + off (W None: no lower
     bound)."""
@@ -303,6 +347,7 @@ def main():
     ap.add_argument("--bwd", action="store_true")
     ap.add_argument("--window", action="store_true", help="with --perf: the sliding-window table instead of the model shapes")
     ap.add_argument("--cp", type=int, default=0, help="with --perf --window: the context-parallel block schedule at this CP size")
+    ap.add_argument("--kv-fp8", action="store_true", help="with --perf: decode attention on bf16 vs fp8 e4m3 KV caches")
     ap.add_argument("--head-dim", type=int, default=128, choices=attention.FLASH_HEAD_DIMS)
     a = ap.parse_args()
     if a.perf and a.window and a.cp > 1 and not torch.cuda.is_available():
@@ -363,7 +408,9 @@ def main():
             ok_all &= ok
             print(json.dumps({"check": f"fa_bwd_{tag}", "ok": ok, **res}), flush=True)
     if a.perf:
-        if a.window and a.cp > 1:
+        if a.kv_fp8:
+            kv_fp8_perf()
+        elif a.window and a.cp > 1:
             cp_window_perf(a.bwd, a.cp)
         else:
             (window_perf if a.window else perf)(e, a.bwd)
