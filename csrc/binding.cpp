@@ -397,7 +397,8 @@ static Tensor gemv_mx(const Tensor& x, const Tensor& w, const Tensor& scale, int
   TORCH_CHECK(K % 32 == 0 && scale.size(1) == K / 32, "gemv_mx: scale must be [N, K/32]");
   const long row_bytes = fmt == 0 ? K / 2 : K;
   TORCH_CHECK((long)(w.numel() * w.element_size()) == (long)N * row_bytes, "gemv_mx: weight bytes do not match [N, K] in this format");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(w.data_ptr()) % 16 == 0);
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(w.data_ptr()) % 16 == 0,
+              "gemv_mx: x and w must start 16-byte aligned (the kernel loads 16-byte vectors)");
   c10::cuda::CUDAGuard guard(x.device());
   Tensor y = at::empty({M, N}, x.options());
   const void* res = nullptr;
@@ -418,6 +419,8 @@ static Tensor gemv_mx_grouped(const Tensor& x, const Tensor& w, const Tensor& sc
   TORCH_CHECK(K % 32 == 0 && scale.size(2) == K / 32, "gemv_mx_grouped: scale must be [E, N, K/32]");
   const long row_bytes = fmt == 0 ? K / 2 : K;
   TORCH_CHECK((long)(w.numel() * w.element_size()) == (long)E * N * row_bytes, "gemv_mx_grouped: weight bytes do not match [E, N, K]");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(w.data_ptr()) % 16 == 0,
+              "gemv_mx_grouped: x and w must start 16-byte aligned (the kernel loads 16-byte vectors)");
   c10::cuda::CUDAGuard guard(x.device());
   Tensor y = at::empty({S, N}, x.options());
   nxd::gemv_mx_grouped(x.data_ptr(), w.data_ptr(), scale.data_ptr(), expert.data_ptr<long>(), y.data_ptr(), S, N, K, E, (int)fmt, stream());
@@ -426,6 +429,8 @@ static Tensor gemv_mx_grouped(const Tensor& x, const Tensor& w, const Tensor& sc
 static Tensor gemv(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& residual) {
   TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && x.dim() == 2 && w.dim() == 2);
   TORCH_CHECK(x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1) && x.size(0) >= 1 && x.size(0) <= 8 && x.size(1) % 8 == 0);
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(w.data_ptr()) % 16 == 0,
+              "gemv: x and w must start 16-byte aligned (the kernel loads 16-byte vectors)");
   c10::cuda::CUDAGuard guard(x.device());
   Tensor y = at::empty({x.size(0), w.size(0)}, x.options());
   const void* res = nullptr;

@@ -228,7 +228,7 @@ def _row_linear_plus_residual(lin, inp: torch.Tensor, residual: torch.Tensor) ->
         x2 = inp.reshape(M, inp.shape[-1]).contiguous()
         r2 = residual.reshape(M, residual.shape[-1]).contiguous()
         tp = lin.tensor_model_parallel_size
-        if tp == 1 and hasattr(e, "gemv"):
+        if tp == 1 and hasattr(e, "gemv") and x2.data_ptr() % 16 == 0 and w.data_ptr() % 16 == 0:   # 16-byte vector loads
             ops._ext.count_launch()
             return e.gemv(x2, w, r2).view_as(residual)
         if tp > 1 and ops.tp_fused.get_backend() == "fused" and ops.nvls.gemv_all_reduce_eligible(x2, w):

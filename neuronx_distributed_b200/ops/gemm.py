@@ -36,6 +36,16 @@ def _eligible(a: torch.Tensor, b: torch.Tensor, M: int, N: int, K: int) -> bool:
     return M >= 1 and N % 8 == 0 and K % 8 == 0 and M % 8 == 0
 
 
+def _gemv_eligible(a: torch.Tensor, b: torch.Tensor, M: int, K: int, trans_a: bool, trans_b: bool, out, out_dtype) -> bool:
+    """``x[M <= 8, K] @ W[N, K]ᵀ`` with a bf16 result goes to the decode GEMV.  It loads 16-byte vectors of both operands,
+    so both must start 16-byte aligned: a contiguous view at an element offset that is not a multiple of 8 (a tensor cut
+    out of a flat buffer after tensors of odd sizes) is not, and takes the general path."""
+    return (M <= 8 and not trans_a and trans_b and out is None and out_dtype == torch.bfloat16 and a.is_cuda
+            and a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and K % 8 == 0 and a.is_contiguous() and b.is_contiguous()
+            and a.data_ptr() % 16 == 0 and b.data_ptr() % 16 == 0
+            and _ext.ext() is not None and hasattr(_ext.ext(), "gemv") and os.environ.get("NXD_DISABLE_TCGEN05_GEMM", "0") != "1")
+
+
 def matmul(a: torch.Tensor, b: torch.Tensor, trans_a: bool = False, trans_b: bool = False,
            out: torch.Tensor | None = None, accumulate: bool = False, out_dtype=None) -> torch.Tensor:
     """``op(a) @ op(b)`` for 2-D tensors. ``accumulate`` adds into ``out`` (fp32 or bf16)."""
@@ -43,9 +53,7 @@ def matmul(a: torch.Tensor, b: torch.Tensor, trans_a: bool = False, trans_b: boo
     K = a.shape[0] if trans_a else a.shape[1]
     N = b.shape[0] if trans_b else b.shape[1]
     out_dtype = out_dtype or (out.dtype if out is not None else a.dtype)
-    if (M <= 8 and not trans_a and trans_b and out is None and out_dtype == torch.bfloat16 and a.is_cuda
-            and a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and K % 8 == 0 and a.is_contiguous() and b.is_contiguous()
-            and _ext.ext() is not None and hasattr(_ext.ext(), "gemv") and os.environ.get("NXD_DISABLE_TCGEN05_GEMM", "0") != "1"):
+    if _gemv_eligible(a, b, M, K, trans_a, trans_b, out, out_dtype):
         # decode-time GEMV: a bandwidth problem (every weight byte read once), not a tensor-core one — csrc/decode.cu
         _ext.count_launch()
         return _ext.ext().gemv(a, b, None)

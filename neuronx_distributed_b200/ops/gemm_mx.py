@@ -152,11 +152,23 @@ def gemm_f4_eligible(M: int, N: int, K: int, *tensors: torch.Tensor) -> bool:
 
 
 def gemv_eligible(x2d: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor) -> bool:
-    if os.environ.get("NXD_GEMV_MX", "0") != "1":                 # opt-in until the kernel has run on hardware
+    """The MX GEMV loads 16-byte vectors of the activations and the codes, so both must start 16-byte aligned."""
+    if os.environ.get("NXD_GEMV_MX", "0") != "1":                 # opt-in
         return False
     return (x2d.is_cuda and x2d.dtype == torch.bfloat16 and x2d.dim() == 2 and 1 <= x2d.shape[0] <= 8 and x2d.shape[1] % 32 == 0
             and x2d.is_contiguous() and weight.is_contiguous() and scale.is_contiguous() and scale.dtype == torch.uint8
-            and scale.dim() == 2 and _ext.use_cuda(x2d, weight, scale) and hasattr(_ext.ext(), "gemv_mx"))
+            and scale.dim() == 2 and x2d.data_ptr() % 16 == 0 and weight.data_ptr() % 16 == 0
+            and _ext.use_cuda(x2d, weight, scale) and hasattr(_ext.ext(), "gemv_mx"))
+
+
+def grouped_gemv_eligible(x: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor) -> bool:
+    """As :func:`gemv_eligible` for the per-slot expert GEMV (``x [S, K]``, stacked ``[E, N, K]`` codes), given the
+    contiguous tensors the kernel will read."""
+    if os.environ.get("NXD_GEMV_MX", "0") != "1":
+        return False
+    return (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 2 and x.shape[1] % 32 == 0
+            and x.data_ptr() % 16 == 0 and weight.data_ptr() % 16 == 0
+            and _ext.use_cuda(x, weight, scale) and hasattr(_ext.ext(), "gemv_mx_grouped"))
 
 
 def grouped_linear_mx(x: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor, expert: torch.Tensor, kind: Optional[str] = None
@@ -166,10 +178,10 @@ def grouped_linear_mx(x: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor
     launch that reads only the chosen experts' codes, ids stay on the device; otherwise gather + de-quantise + batched matmul."""
     kind = kind or kind_of(weight)
     E, N = scale.shape[0], scale.shape[1]
-    if (os.environ.get("NXD_GEMV_MX", "0") == "1" and x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 2 and x.shape[1] % 32 == 0
-            and _ext.use_cuda(x, weight, scale) and hasattr(_ext.ext(), "gemv_mx_grouped")):
+    xc, wc = x.contiguous(), weight.contiguous()
+    if grouped_gemv_eligible(xc, wc, scale):
         _ext.count_launch()
-        return _ext.ext().gemv_mx_grouped(x.contiguous(), weight.contiguous(), scale.contiguous(), expert.long().contiguous(), _FMT[kind])
+        return _ext.ext().gemv_mx_grouped(xc, wc, scale.contiguous(), expert.long().contiguous(), _FMT[kind])
     wb = weight.contiguous().view(torch.uint8).reshape(E, N, -1)[expert.long()]                      # [S, N, bytes]
     w = dequantize(wb.reshape(-1, wb.shape[-1]), scale[expert.long()].reshape(-1, scale.shape[-1]), kind).view(x.shape[0], N, -1)
     return torch.einsum("sk,snk->sn", x.float(), w).to(x.dtype)

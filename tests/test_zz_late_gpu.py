@@ -398,44 +398,6 @@ def test_all_to_all_over_peer_memory_loopback():
     run_distributed(_all_to_all_loopback, 2, use_cuda="loopback", timeout=_PER_TEST_S)
 
 
-def test_gemv_mx_matches_dequantised_reference():
-    """Decode GEMV on MXFP4 / MXFP8 weights (codes decoded in registers) vs fp32 matmul on the de-quantised weights."""
-    _run("""
-        import torch
-        from neuronx_distributed_b200.ops import gemm_mx, _ext
-        from neuronx_distributed_b200.quantization.microscaling.mx_torch import quantize_mx
-        torch.manual_seed(0)
-        for kind in ("mxfp4", "mxfp8"):
-            for M, N, K in ((1, 4096, 4096), (4, 1000, 2880), (8, 512, 14336)):
-                K = K // 32 * 32
-                w = torch.randn(N, K) * 0.05
-                p, s = quantize_mx(w, kind)
-                p, s = p.cuda(), s.cuda()
-                x = torch.randn(M, K, device="cuda").bfloat16()
-                res = torch.randn(M, N, device="cuda").bfloat16()
-                assert gemm_mx.gemv_eligible(x, p, s)
-                n0 = _ext.launches()
-                y = gemm_mx.linear_mx(x, p, s, residual=res)
-                assert _ext.launches() == n0 + 1
-                ref = x.float() @ gemm_mx.dequantize(p, s, kind).t() + res.float()
-                err = ((y.float() - ref).norm() / ref.norm()).item()
-                print(kind, M, N, K, "rel err", err)
-                assert err < 1e-2, err
-            # per-slot expert selection (MoE decode): only the chosen experts' codes are read
-            E, N, K, S = 8, 1024, 2048, 6
-            w = torch.randn(E, N, K) * 0.05
-            p, s = quantize_mx(w, kind)
-            p, s = p.cuda(), s.cuda()
-            x = torch.randn(S, K, device="cuda").bfloat16()
-            ex = torch.tensor([7, 0, 3, 3, 5, 1], device="cuda")
-            y = gemm_mx.grouped_linear_mx(x, p, s, ex)
-            ref = torch.stack([x[i].float() @ gemm_mx.dequantize(p[ex[i]], s[ex[i]], kind).t() for i in range(S)])
-            err = ((y.float() - ref).norm() / ref.norm()).item()
-            print(kind, "grouped rel err", err)
-            assert err < 1e-2, err
-    """, env={"NXD_GEMV_MX": "1"})
-
-
 def _pull_attention_loopback(rank, world):
     import math
 
