@@ -23,7 +23,10 @@
 // `sees`, and the tiles a CTA visits are `key_tiles` / `query_tiles`, which skip only tiles that hold no visible pair.
 // An invisible pair contributes nothing: a query row that sees no key gets O = 0, LSE = −inf and dQ = 0, and a key no row
 // sees gets dK = dV = 0.
+// spec_attn_kernel runs the forward kernel's loop for W new tokens per sequence against a bf16 or e4m3 KV cache (speculation
+// and Medusa verification); its visibility rule is written above it.
 #include <cuda.h>
+#include <cuda_fp8.h>
 
 #include <algorithm>
 #include <cstdint>
@@ -309,6 +312,227 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
     for (int r = 0; r < 2; ++r)
       if (row[r] < p.S_q)
         p.lse[((long)b * p.H + h) * p.S_q + row[r]] = l[r] > 0.f ? (m[r] + __log2f(l[r])) / kLog2e : -INFINITY;
+  }
+}
+
+// ---- verification of W new tokens per sequence against a KV cache (speculation chains, Medusa trees) ----------------------
+// Sequence b's window holds cache slots p = positions[b] .. p + W − 1.  Window row w sits at sequence position p + d[w]
+// (d = depth, or w for a chain) and has tree-mask row M[w] (a chain: u ≤ w).  Row w sees slot c < min(p + W, L) iff
+//   - c < p (committed): with a sliding window SW, c > p + d[w] − SW;
+//   - c = p + u (window): M[w, u] and, with SW, d[u] > d[w] − SW.
+// A row that sees nothing gets O = 0.  The W·G (token w, head g of the GQA group) rows of one kv head are cut into 64-row
+// tiles (row w·G + g), and one CTA per (row tile, split, kv head, sequence) runs the forward kernel's loop over 64-slot K/V
+// tiles, so each K/V row is read once for every row of the tile.  The splits divide only the slots a row of the tile can
+// see (from p + min d − SW + 1 with a window).  An e4m3 cache is staged raw by cp.async and converted to bf16 in shared
+// memory, which is exact; k_scale is folded into the softmax scale and v_scale multiplies the partial output.  A window
+// slot no row of the tile sees gets its V row zeroed, so its bytes never reach the output (K is masked by a select).
+// Partials (o relative to the row maximum, maximum and sum in log2 units) are merged by decode.cu's combine kernel.
+constexpr int kSpecMaxW = 64;
+constexpr int kRawTile = BT * 128;                      // bytes of one staged e4m3 tile
+template <bool E4M3>
+constexpr int kSmemSpec = (E4M3 ? 3 * kTile<128> * 2 + 4 * kRawTile : kSmemFwd<128>) + kSpecMaxW * (8 + 4);
+
+struct SpecParams {
+  const bf16* q; long q_sb, q_ss, q_sh;
+  const void *k, *v; long k_sb, k_ss, k_sh, v_sb, v_ss, v_sh;
+  const long* positions;
+  const uint8_t* mask;                          // [W, W], row w sees window column u iff nonzero; null: chain
+  const long* depth;                            // [W]; null: chain (d[w] = w)
+  float *part_o, *part_ml;
+  int W, H, L, splits, row_tiles, window;
+  float scale_log2, v_scale;
+};
+
+NXD_DEVICE void cp_async8(void* dst, const void* src, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(smem_addr(dst)), "l"(src), "r"(valid ? 8 : 0) : "memory");
+}
+
+// rows [s0, s0+64) of one e4m3 (batch, kv head) slice → unpadded 128-byte shared rows; rows ≥ S are zero-filled.  8-byte
+// copies: an e4m3 cache is only required to be 8-byte aligned.
+NXD_DEVICE void load_raw_e4m3(uint8_t* sm, const uint8_t* base, long ss, int s0, int S) {
+  for (int i = threadIdx.x; i < BT * 16; i += kThreads) {
+    const int r = i >> 4, c = i & 15;
+    const bool ok = s0 + r < S;
+    cp_async8(sm + r * 128 + c * 8, base + (long)(ok ? s0 + r : 0) * ss + c * 8, ok);
+  }
+}
+
+// staged e4m3 tile → padded bf16 tile (every e4m3 value is a bf16 value)
+NXD_DEVICE void e4m3_to_bf16(bf16* dst, const uint8_t* src) {
+  for (int i = threadIdx.x; i < BT * 16; i += kThreads) {
+    const int r = i >> 4, c = i & 15;
+    const uint2 a = *(const uint2*)(src + r * 128 + c * 8);
+    uint32_t o[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const unsigned w = j < 2 ? a.x : a.y;
+      const float2 f = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w >> (16 * (j & 1))), __NV_E4M3)));
+      o[j] = pack_bf16(f.x, f.y);
+    }
+    *(uint4*)(dst + r * LDS<128> + c * 8) = make_uint4(o[0], o[1], o[2], o[3]);
+  }
+}
+
+template <int G, bool E4M3>
+__global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p) {
+  constexpr int HD = 128, kTl = kTile<HD>, kBufs = E4M3 ? 1 : 2;
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  bf16* sQ = (bf16*)smem_raw;
+  bf16* sK = sQ + kTl;                          // kBufs buffers
+  bf16* sV = sK + kBufs * kTl;                  // kBufs buffers
+  uint8_t* sRaw = (uint8_t*)(sV + kBufs * kTl); // e4m3: raw K, V × 2 buffers
+  uint64_t* sBits = (uint64_t*)(sRaw + (E4M3 ? 4 * kRawTile : 0));   // window columns row w sees
+  int* sDepth = (int*)(sBits + kSpecMaxW);
+  const int rt = blockIdx.x % p.row_tiles, split = blockIdx.x / p.row_tiles, kvh = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int W = p.W, r0 = rt * BT, n_rows = W * G;
+  const long pos = p.positions[b];
+  // p clamped to [−64, L]: the same slots are committed / window slots below L, and slot − p stays in int range
+  const int p32 = (int)min(max(pos, (long)-kSpecMaxW), (long)p.L);
+
+  if (threadIdx.x < W) sDepth[threadIdx.x] = p.depth ? (int)p.depth[threadIdx.x] : threadIdx.x;
+  __syncthreads();
+  if (threadIdx.x < W) {
+    const int w = threadIdx.x;
+    const long dw = sDepth[w];
+    uint64_t bits = 0;
+    for (int u = 0; u < W; ++u) {
+      const bool m = p.mask ? p.mask[w * W + u] != 0 : u <= w;
+      if (m && (p.window == 0 || sDepth[u] > dw - p.window)) bits |= 1ull << u;
+    }
+    sBits[w] = bits;
+  }
+  __syncthreads();
+  // tokens [w_lo, w_hi) of this row tile (G divides 64): their smallest depth and the window columns any of them sees
+  const int w_lo = r0 / G, w_hi = min((r0 + BT) / G, W);
+  int dmin = INT32_MAX;
+  uint64_t seen = 0;
+  for (int w = w_lo; w < w_hi; ++w) { dmin = min(dmin, sDepth[w]); seen |= sBits[w]; }
+  const uint64_t unseen = ~seen & (W == 64 ? ~0ull : (1ull << W) - 1);
+  // slots [lo, hi) some row of the tile sees; the splits divide them in whole 64-slot tiles
+  const long lo_l = p.window > 0 ? min(pos, pos + dmin - p.window + 1) : 0;
+  const int lo = (int)min(max(lo_l, 0L), (long)p.L);
+  const int hi = (int)max(min(pos + W, (long)p.L), (long)lo);
+  const int per = ((hi - lo + p.splits - 1) / p.splits + BT - 1) / BT * BT;
+  const int s0 = lo + split * per, s1 = min(hi, s0 + per);
+  const int n_t = s1 > s0 ? (s1 - s0 + BT - 1) / BT : 0;
+
+  // this thread's two rows: committed slots c > cmin are visible, window slot p + u iff bit u of wbits
+  int cmin[2];
+  uint64_t wbits[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = r0 + warp * 16 + (lane >> 2) + 8 * r;
+    const bool ok = row < n_rows;
+    wbits[r] = ok ? sBits[row / G] : 0;
+    const long c = p.window > 0 ? (long)p32 + sDepth[ok ? row / G : 0] - p.window : (long)INT32_MIN;
+    cmin[r] = ok ? (int)max(c, (long)INT32_MIN) : INT32_MAX;
+  }
+
+  const bf16* qb = p.q + b * p.q_sb + (long)kvh * G * p.q_sh;
+  const uint8_t* kb = (const uint8_t*)p.k + (b * p.k_sb + (long)kvh * p.k_sh) * (E4M3 ? 1 : 2);
+  const uint8_t* vb = (const uint8_t*)p.v + (b * p.v_sb + (long)kvh * p.v_sh) * (E4M3 ? 1 : 2);
+  auto issue = [&](int t) {                     // K / V tile t of the split → buffer t & 1
+    const int s = s0 + t * BT, buf = t & 1;
+    if constexpr (E4M3) {
+      load_raw_e4m3(sRaw + 2 * buf * kRawTile, kb, p.k_ss, s, s1);
+      load_raw_e4m3(sRaw + (2 * buf + 1) * kRawTile, vb, p.v_ss, s, s1);
+    } else {
+      load_tile<HD>(sK + buf * kTl, (const bf16*)kb, p.k_ss, s, s1);
+      load_tile<HD>(sV + buf * kTl, (const bf16*)vb, p.v_ss, s, s1);
+    }
+    cp_async_commit();
+  };
+  if (n_t > 0) {
+    for (int i = threadIdx.x; i < BT * 16; i += kThreads) {    // Q rows (token w, head g) of the tile; rows past W·G are 0
+      const int r = i >> 4, c = i & 15, row = r0 + r;
+      const bool ok = row < n_rows;
+      cp_async16(sQ + r * LDS<HD> + c * 8, qb + (ok ? (row / G) * p.q_ss + (row % G) * p.q_sh : 0) + c * 8, ok);
+    }
+    issue(0);
+  }
+
+  float o[HD / 8][4];
+#pragma unroll
+  for (int i = 0; i < HD / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+
+  for (int t = 0; t < n_t; ++t) {
+    const int buf = t & 1, c0 = s0 + t * BT;
+    if (t + 1 < n_t) {
+      issue(t + 1);
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    bf16* k = sK + (E4M3 ? 0 : buf * kTl);
+    bf16* v = sV + (E4M3 ? 0 : buf * kTl);
+    if constexpr (E4M3) {
+      e4m3_to_bf16(k, sRaw + 2 * buf * kRawTile);
+      e4m3_to_bf16(v, sRaw + (2 * buf + 1) * kRawTile);
+    }
+    // tile rows holding a window slot no row of the tile sees
+    const int sh = c0 - p32;
+    const uint64_t zero = sh >= 0 ? (sh < 64 ? unseen >> sh : 0) : (sh > -64 ? unseen << -sh : 0);
+    if (zero) {
+      for (int i = threadIdx.x; i < BT * 16; i += kThreads)
+        if ((zero >> (i >> 4)) & 1) *(uint4*)(v + (i >> 4) * LDS<HD> + (i & 15) * 8) = make_uint4(0, 0, 0, 0);
+    }
+    if (E4M3 || zero) __syncthreads();
+    float s[8][4];
+    mma_abt<HD>(s, sQ, warp * 16, k);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int c = c0 + j * 8 + 2 * (lane & 3) + (e & 1), r = e >> 1;
+        const bool vis = c < s1 && (c < p32 ? c > cmin[r] : (wbits[r] >> ((c - p32) & 63)) & 1);
+        const float x = vis ? s[j][e] * p.scale_log2 : -INFINITY;
+        s[j][e] = x;
+        mx[r] = fmaxf(mx[r], x);
+      }
+    }
+    float alpha[2], mu[2], rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float mn = fmaxf(m[r], mx[r]);
+      mu[r] = mn == -INFINITY ? 0.f : mn;
+      alpha[r] = exp2f(m[r] - mu[r]);
+      m[r] = mn;
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float x = exp2f(s[j][e] - mu[e >> 1]);
+        s[j][e] = x;
+        rs[e >> 1] += x;
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) l[r] = l[r] * alpha[r] + rs[r];
+#pragma unroll
+    for (int i = 0; i < HD / 8; ++i) { o[i][0] *= alpha[0]; o[i][1] *= alpha[0]; o[i][2] *= alpha[1]; o[i][3] *= alpha[1]; }
+    uint32_t pf[4][4];
+    to_a_frags(s, pf);
+    mma_pb<HD>(o, pf, v);
+    __syncthreads();                              // the buffers are refilled at the next iteration
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+    const int row = r0 + warp * 16 + (lane >> 2) + 8 * r;
+    if (row >= n_rows) continue;
+    const long idx = (((long)b * W + row / G) * p.H + kvh * G + row % G) * p.splits + split;
+#pragma unroll
+    for (int dt = 0; dt < HD / 8; ++dt)
+      *(float2*)(p.part_o + idx * HD + dt * 8 + 2 * (lane & 3)) = make_float2(o[dt][2 * r] * p.v_scale, o[dt][2 * r + 1] * p.v_scale);
+    if ((lane & 3) == 0) { p.part_ml[idx * 2] = m[r]; p.part_ml[idx * 2 + 1] = l[r]; }
   }
 }
 
@@ -633,6 +857,48 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
     launch_bwd<HD, decltype(mk)::value, decltype(wd)::value>(p, st);
   });
   NXD_CUDA_CHECK(cudaGetLastError());
+}
+
+void speculation_attention(const void* q, const void* k, const void* v, const long* positions, const void* mask,
+                           const long* depth, void* out, float* part_o, float* part_ml, int B, int W, int H, int Hkv, int L,
+                           const long* qs, const long* ks, const long* vs, float scale, int window, int splits, bool kv_e4m3,
+                           float k_scale, float v_scale, cudaStream_t st) {
+  using namespace fa;
+  const int G = H / Hkv;
+  SpecParams p;
+  p.q = (const bf16*)q; p.q_sb = qs[0]; p.q_ss = qs[1]; p.q_sh = qs[2];
+  p.k = k; p.k_sb = ks[0]; p.k_ss = ks[1]; p.k_sh = ks[2];
+  p.v = v; p.v_sb = vs[0]; p.v_ss = vs[1]; p.v_sh = vs[2];
+  p.positions = positions; p.mask = (const uint8_t*)mask; p.depth = depth;
+  p.part_o = part_o; p.part_ml = part_ml;
+  p.W = W; p.H = H; p.L = L; p.splits = splits; p.row_tiles = (W * G + BT - 1) / BT; p.window = window;
+  p.scale_log2 = scale * kLog2e * k_scale;
+  p.v_scale = v_scale;
+  const dim3 grid(p.row_tiles * splits, Hkv, B);
+  auto launch = [&](auto g, auto e4) {
+    constexpr int Gv = decltype(g)::value;
+    constexpr bool E4 = decltype(e4)::value;
+    static bool configured = false;
+    if (!configured) {
+      NXD_CUDA_CHECK(cudaFuncSetAttribute(spec_attn_kernel<Gv, E4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemSpec<E4>));
+      configured = true;
+    }
+    spec_attn_kernel<Gv, E4><<<grid, kThreads, kSmemSpec<E4>, st>>>(p);
+  };
+  auto with_cache = [&](auto g) {
+    if (kv_e4m3) launch(g, std::true_type{});
+    else launch(g, std::false_type{});
+  };
+  switch (G) {
+    case 1: with_cache(std::integral_constant<int, 1>{}); break;
+    case 2: with_cache(std::integral_constant<int, 2>{}); break;
+    case 4: with_cache(std::integral_constant<int, 4>{}); break;
+    case 8: with_cache(std::integral_constant<int, 8>{}); break;
+    default: nxd_throw("speculation_attention: unsupported GQA group size", __FILE__, __LINE__);
+  }
+  NXD_CUDA_CHECK(cudaGetLastError());
+  // row (b·W + w)·H + h of the partials → out [B, W, H, 128]
+  decode_combine(part_o, part_ml, out, B * W * H, splits, (long)H * 128, 128, H, st);
 }
 
 }  // namespace nxd

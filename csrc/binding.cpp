@@ -263,25 +263,33 @@ static bool kv_cache_e4m3(const char* fn, const Tensor& kc, const Tensor& vc, do
   return t == at::kFloat8_e4m3fn;
 }
 
-// q [B,1,H,D], k/v [B,1,Hkv,D] (views of the fused QKV GEMV output), cache [B,L,Hkv,D]: rotate q → new tensor, rotate k and
-// copy v straight into the cache row positions[b] (an e4m3 cache gets k / k_scale and v / v_scale, rounded as the cache's
-// torch rule rounds them)
+// q [B,W,H,D], k/v [B,W,Hkv,D] (views of the fused QKV projection output), cache [B,L,Hkv,D]: rotate q → new tensor, rotate
+// k and copy v straight into the cache (token w at slot positions[b] + w, rotated at positions[b] + depth[w], or + w without
+// depth; an e4m3 cache gets k / k_scale and v / v_scale, rounded as the cache's torch rule rounds them)
 static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions, const Tensor& cos_t,
-                             const Tensor& sin_t, Tensor kc, Tensor vc, double k_scale, double v_scale) {
-  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) == 1 && q.stride(3) == 1);
-  TORCH_CHECK(k.scalar_type() == at::kBFloat16 && k.dim() == 4 && k.size(1) == 1 && k.stride(3) == 1 && v.stride(3) == 1 && v.sizes() == k.sizes());
+                             const Tensor& sin_t, Tensor kc, Tensor vc, double k_scale, double v_scale,
+                             const c10::optional<Tensor>& depth) {
+  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) >= 1 && q.stride(3) == 1);
+  TORCH_CHECK(k.scalar_type() == at::kBFloat16 && k.dim() == 4 && k.size(1) == q.size(1) && k.stride(3) == 1 && v.stride(3) == 1 && v.sizes() == k.sizes());
   const bool e4m3 = kv_cache_e4m3("decode_rope_kv", kc, vc, k_scale, v_scale);
   TORCH_CHECK(kc.dim() == 4 && kc.stride(3) == 1 && vc.sizes() == kc.sizes() && vc.strides() == kc.strides());
   TORCH_CHECK(positions.scalar_type() == at::kLong && positions.is_contiguous() && positions.numel() == q.size(0));
   CHECK_IN(cos_t); CHECK_IN(sin_t);
   TORCH_CHECK(cos_t.scalar_type() == at::kFloat && cos_t.size(1) == q.size(3) / 2 && cos_t.size(0) >= kc.size(1));
+  const long* dp = nullptr;
+  if (depth.has_value()) {
+    TORCH_CHECK(depth->is_cuda() && depth->scalar_type() == at::kLong && depth->is_contiguous() && depth->numel() == q.size(1),
+                "decode_rope_kv: depth must be a contiguous int64 CUDA tensor [W]");
+    dp = depth->data_ptr<long>();
+  }
   c10::cuda::CUDAGuard g(q.device());
-  const int B = (int)q.size(0), H = (int)q.size(2), Hkv = (int)k.size(2), D = (int)q.size(3), L = (int)kc.size(1);
-  Tensor q_out = at::empty({B, 1, H, D}, q.options());
-  nxd::decode_rope_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), cos_t.data_ptr<float>(),
-                      sin_t.data_ptr<float>(), q_out.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, H, Hkv, D, L, q.stride(0), q.stride(2),
-                      k.stride(0), k.stride(2), v.stride(0), v.stride(2), kc.stride(0), kc.stride(1), kc.stride(2), stream(), e4m3,
-                      1.0f / (float)k_scale, 1.0f / (float)v_scale);
+  const int B = (int)q.size(0), W = (int)q.size(1), H = (int)q.size(2), Hkv = (int)k.size(2), D = (int)q.size(3), L = (int)kc.size(1);
+  Tensor q_out = at::empty({B, W, H, D}, q.options());
+  const long qs[3] = {q.stride(0), q.stride(1), q.stride(2)}, ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
+  const long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
+  nxd::decode_rope_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), dp, cos_t.data_ptr<float>(),
+                      sin_t.data_ptr<float>(), q_out.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, W, H, Hkv, D, L, qs, ks, vs,
+                      kc.stride(0), kc.stride(1), kc.stride(2), stream(), e4m3, 1.0f / (float)k_scale, 1.0f / (float)v_scale);
   return q_out;
 }
 
@@ -296,10 +304,12 @@ static int decode_splits(int B, int Hkv, int L, int64_t window) {
   int splits = (6 * num_sms() + B * Hkv - 1) / (B * Hkv);
   return std::max(1, std::min(std::min(splits, 64), (rows + 63) / 64));
 }
-// argument checks shared by decode_attention and decode_attention_partial; returns true for an e4m3 cache
+// argument checks shared by decode_attention, decode_attention_partial (one token per sequence) and speculation_attention
+// (max_tokens = 64); returns true for an e4m3 cache
 static bool check_decode_args(const char* fn, const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions,
-                              double k_scale, double v_scale) {
-  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) == 1 && q.size(3) == 128 && q.stride(3) == 1);
+                              double k_scale, double v_scale, int64_t max_tokens = 1) {
+  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) >= 1 && q.size(1) <= max_tokens &&
+              q.size(3) == 128 && q.stride(3) == 1);
   const bool e4m3 = kv_cache_e4m3(fn, k, v, k_scale, v_scale);
   TORCH_CHECK(k.dim() == 4 && k.size(3) == 128 && k.stride(3) == 1 && v.stride(3) == 1 && v.sizes() == k.sizes());
   TORCH_CHECK(positions.scalar_type() == at::kLong && positions.is_cuda() && positions.is_contiguous() && positions.numel() == q.size(0));
@@ -345,6 +355,50 @@ static std::vector<Tensor> decode_attention_partial(const Tensor& q, const Tenso
                         (int)std::min<int64_t>(window, INT32_MAX), stream(), fin_o.data_ptr<float>(), fin_ml.data_ptr<float>(),
                         e4m3, (float)k_scale, (float)v_scale);
   return {fin_o, fin_ml};
+}
+// q [B,W≤64,H,128] (any b/s/h strides, rows 16-byte aligned) verified against the cache as decode_attention reads it; tree_mask
+// [W,W] bool / uint8 and tree_depth [W] int64 (both or neither: a chain).  Never reads them on the host.
+static Tensor speculation_attention(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions,
+                                    const c10::optional<Tensor>& tree_mask, const c10::optional<Tensor>& tree_depth, double scale,
+                                    int64_t window, double k_scale, double v_scale) {
+  const char* fn = "speculation_attention";
+  const bool e4m3 = check_decode_args(fn, q, k, v, positions, k_scale, v_scale, 64);
+  const int B = q.size(0), W = q.size(1), H = q.size(2), L = k.size(1), Hkv = k.size(2), G = H / Hkv;
+  TORCH_CHECK(G == 1 || G == 2 || G == 4 || G == 8, fn, ": the GQA group size must be 1, 2, 4 or 8");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0 && q.stride(0) % 8 == 0 && q.stride(1) % 8 == 0,
+              fn, ": q rows must be 16-byte aligned");
+  TORCH_CHECK(e4m3 || ((reinterpret_cast<uintptr_t>(k.data_ptr()) | reinterpret_cast<uintptr_t>(v.data_ptr())) % 16 == 0 &&
+                       k.stride(0) % 8 == 0 && v.stride(0) % 8 == 0),
+              fn, ": bf16 cache rows must be 16-byte aligned");
+  TORCH_CHECK(window >= 0, fn, ": window must be >= 0 (0 = none)");
+  TORCH_CHECK(tree_mask.has_value() == tree_depth.has_value(), fn, ": tree_mask and tree_depth go together");
+  const void* mp = nullptr;
+  const long* dp = nullptr;
+  if (tree_mask.has_value()) {
+    TORCH_CHECK((tree_mask->scalar_type() == at::kBool || tree_mask->scalar_type() == at::kByte) && tree_mask->is_contiguous() &&
+                    tree_mask->dim() == 2 && tree_mask->size(0) == W && tree_mask->size(1) == W && tree_mask->device() == q.device(),
+                fn, ": tree_mask must be a contiguous bool / uint8 [W, W] tensor on q's device");
+    TORCH_CHECK(tree_depth->scalar_type() == at::kLong && tree_depth->is_contiguous() && tree_depth->numel() == W &&
+                    tree_depth->device() == q.device(),
+                fn, ": tree_depth must be a contiguous int64 [W] tensor on q's device");
+    mp = tree_mask->data_ptr();
+    dp = tree_depth->data_ptr<long>();
+  }
+  c10::cuda::CUDAGuard guard(q.device());
+  // slots one row tile reads at most; enough CTAs for ~4 per SM, at least 128 slots per split
+  const int row_tiles = (W * G + 63) / 64;
+  const int64_t rows = window > 0 ? std::min<int64_t>(L, std::min<int64_t>(window, L) + W - 1) : L;
+  const int ctas = B * Hkv * row_tiles;
+  const int splits = std::max(1, std::min({(4 * num_sms() + ctas - 1) / ctas, 64, (int)((rows + 127) / 128)}));
+  Tensor out = at::empty({B, W, H, 128}, q.options());
+  Tensor part_o = at::empty({(int64_t)B * W * H * splits, 128}, q.options().dtype(at::kFloat));
+  Tensor part_ml = at::empty({(int64_t)B * W * H * splits, 2}, q.options().dtype(at::kFloat));
+  const long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
+  const long ks[3] = {k.stride(0), k.stride(1), k.stride(2)}, vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
+  nxd::speculation_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), mp, dp, out.data_ptr(),
+                             part_o.data_ptr<float>(), part_ml.data_ptr<float>(), B, W, H, Hkv, L, qs, ks, vs, (float)scale,
+                             (int)std::min<int64_t>(window, INT32_MAX), splits, e4m3, (float)k_scale, (float)v_scale, stream());
+  return out;
 }
 // x [T,H] bf16; gamma [H] bf16 or none; router_w [E,H] bf16; router_bias [E] fp32 or none; w_gu [El,H,2I]; w_dn [El,I,H]
 // → (out [T,H] bf16 partial over this rank's experts / intermediate shard, router logits [T,E] fp32, top-k idx [T,K], top-k w [T,K])
@@ -805,7 +859,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return nxd::moe_block_tkg_supported((int)T, (int)H, (int)E, (int)I, (int)K);
   });
   m.def("decode_rope_kv", &decode_rope_kv, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"), py::arg("cos"),
-        py::arg("sin"), py::arg("k_cache"), py::arg("v_cache"), py::kw_only(), py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0);
+        py::arg("sin"), py::arg("k_cache"), py::arg("v_cache"), py::kw_only(), py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0,
+        py::arg("depth") = py::none());
+  m.def("speculation_attention", &speculation_attention, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"),
+        py::arg("tree_mask") = py::none(), py::arg("tree_depth") = py::none(), py::kw_only(), py::arg("scale"),
+        py::arg("window") = 0, py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0);
   m.def("moe_block_metadata", &moe_block_metadata);
   m.def("row_argmax", &row_argmax);
   m.def("row_topk", &row_topk);

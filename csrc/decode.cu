@@ -249,29 +249,37 @@ __device__ __forceinline__ __nv_fp8_e4m3 quant_e4m3(__nv_bfloat16 x, float inv) 
 }
 
 // Decode-time RoPE + KV-cache append in ONE launch (was ~25 tiny elementwise / index_put kernels per layer in the token-
-// generation graph): q [B,H,D] rotated into q_out, k rotated and v copied into the cache row positions[b].  One warp per head
-// row; cos/sin rows gathered by position.  HF rotate-half convention (csrc/elementwise.cu rope_kernel).  An e4m3 cache gets
-// the bf16 rows a bf16 cache would hold, quantised by quant_e4m3 with k_inv = 1/k_scale and v_inv = 1/v_scale.
+// generation graph): q [B,W,H,D] rotated into q_out, k rotated and v copied into the cache.  Token w of sequence b is
+// rotated at position positions[b] + depth[w] (no depth: + w) and written to slot positions[b] + w, both clamped to the
+// cache (W = 1: the token at positions[b]; W > 1: a speculation window or a Medusa tree).  One warp per head row; cos/sin
+// rows gathered by position.  HF rotate-half convention (csrc/elementwise.cu rope_kernel).  An e4m3 cache gets the bf16
+// rows a bf16 cache would hold, quantised by quant_e4m3 with k_inv = 1/k_scale and v_inv = 1/v_scale.
 template <typename T>
 __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                                             const __nv_bfloat16* __restrict__ v, const long* __restrict__ positions,
-                                                            const float* __restrict__ cos_t, const float* __restrict__ sin_t,
-                                                            __nv_bfloat16* __restrict__ q_out, T* __restrict__ kc,
-                                                            T* __restrict__ vc, int B, int H, int Hkv, int D, int L,
-                                                            long q_sb, long q_sh, long k_sb, long k_sh, long v_sb, long v_sh,
-                                                            long c_sb, long c_ss, long c_sh, float k_inv, float v_inv) {
+                                                            const long* __restrict__ depth, const float* __restrict__ cos_t,
+                                                            const float* __restrict__ sin_t, __nv_bfloat16* __restrict__ q_out,
+                                                            T* __restrict__ kc, T* __restrict__ vc, int B, int W, int H, int Hkv,
+                                                            int D, int L, long q_sb, long q_ss, long q_sh, long k_sb, long k_ss,
+                                                            long k_sh, long v_sb, long v_ss, long v_sh, long c_sb, long c_ss,
+                                                            long c_sh, float k_inv, float v_inv) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  const int rows = B * (H + 2 * Hkv);
+  const int rows = B * W * (H + 2 * Hkv);
   if (warp >= rows) return;
-  const int b = warp / (H + 2 * Hkv), r = warp % (H + 2 * Hkv);
-  long pos = positions[b];
+  const int bw = warp / (H + 2 * Hkv), r = warp % (H + 2 * Hkv), b = bw / W, w = bw % W;
+  const long p = positions[b];
+  long pos = p + (depth ? depth[w] : w), slot = p + w;
   pos = pos < 0 ? 0 : (pos >= L ? L - 1 : pos);
+  slot = slot < 0 ? 0 : (slot >= L ? L - 1 : slot);
+  q += b * q_sb + w * q_ss;
+  k += b * k_sb + w * k_ss;
+  v += b * v_sb + w * v_ss;
   const int half = D / 2;
   if (r < H + Hkv) {                                   // q or k head: rotate
     const bool is_q = r < H;
     const int h = is_q ? r : r - H;
-    const __nv_bfloat16* src = is_q ? q + b * q_sb + (long)h * q_sh : k + b * k_sb + (long)h * k_sh;
-    __nv_bfloat16* dst = is_q ? q_out + ((long)b * H + h) * D : reinterpret_cast<__nv_bfloat16*>(kc + b * c_sb + pos * c_ss + (long)h * c_sh);
+    const __nv_bfloat16* src = is_q ? q + (long)h * q_sh : k + (long)h * k_sh;
+    __nv_bfloat16* dst = is_q ? q_out + ((long)bw * H + h) * D : reinterpret_cast<__nv_bfloat16*>(kc + b * c_sb + slot * c_ss + (long)h * c_sh);
     const float* cr = cos_t + pos * half;
     const float* sr = sin_t + pos * half;
     if constexpr (sizeof(T) == 2) {
@@ -298,8 +306,8 @@ __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16
     }
   } else {                                             // v head: copy
     const int h = r - H - Hkv;
-    const __nv_bfloat16* src = v + b * v_sb + (long)h * v_sh;
-    T* dst = vc + b * c_sb + pos * c_ss + (long)h * c_sh;
+    const __nv_bfloat16* src = v + (long)h * v_sh;
+    T* dst = vc + b * c_sb + slot * c_ss + (long)h * c_sh;
     if constexpr (sizeof(T) == 2) {
       for (int c = lane; c < D; c += 32) dst[c] = src[c];
     } else {
@@ -310,15 +318,16 @@ __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16
 
 }  // namespace
 
-void decode_rope_kv(const void* q, const void* k, const void* v, const long* positions, const float* cos_t, const float* sin_t,
-                    void* q_out, void* kc, void* vc, int B, int H, int Hkv, int D, int L, long q_sb, long q_sh, long k_sb, long k_sh,
-                    long v_sb, long v_sh, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3, float k_inv, float v_inv) {
-  const int rows = B * (H + 2 * Hkv);
+void decode_rope_kv(const void* q, const void* k, const void* v, const long* positions, const long* depth, const float* cos_t,
+                    const float* sin_t, void* q_out, void* kc, void* vc, int B, int W, int H, int Hkv, int D, int L, const long* qs,
+                    const long* ks, const long* vs, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3, float k_inv,
+                    float v_inv) {
+  const int rows = B * W * (H + 2 * Hkv);
   const int grid = (rows * 32 + 127) / 128;
-#define NXD_ROPE_KV(T)                                                                                                       \
-  decode_rope_kv_kernel<T><<<grid, 128, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v,   \
-      positions, cos_t, sin_t, (__nv_bfloat16*)q_out, (T*)kc, (T*)vc, B, H, Hkv, D, L, q_sb, q_sh, k_sb, k_sh, v_sb, v_sh, c_sb, \
-      c_ss, c_sh, k_inv, v_inv)
+#define NXD_ROPE_KV(T)                                                                                                          \
+  decode_rope_kv_kernel<T><<<grid, 128, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v,      \
+      positions, depth, cos_t, sin_t, (__nv_bfloat16*)q_out, (T*)kc, (T*)vc, B, W, H, Hkv, D, L, qs[0], qs[1], qs[2], ks[0], ks[1], \
+      ks[2], vs[0], vs[1], vs[2], c_sb, c_ss, c_sh, k_inv, v_inv)
   if (kv_e4m3) NXD_ROPE_KV(__nv_fp8_e4m3);
   else NXD_ROPE_KV(__nv_bfloat16);
 #undef NXD_ROPE_KV
@@ -349,6 +358,12 @@ void decode_attention(const void* q, const void* k, const void* v, const long* p
 #undef NXD_DEC
   if (fin_o != nullptr) decode_combine_partial_kernel<<<B * H, HD, 0, st>>>(part_o, part_ml, fin_o, fin_ml, splits);
   else decode_combine_kernel<<<B * H, HD, 0, st>>>(part_o, part_ml, (__nv_bfloat16*)out, splits, o_sb, o_sh, H);
+  NXD_CUDA_CHECK(cudaGetLastError());
+}
+
+void decode_combine(const float* part_o, const float* part_ml, void* out, int rows, int splits, long o_sb, long o_sh, int H,
+                    cudaStream_t st) {
+  decode_combine_kernel<<<rows, HD, 0, st>>>(part_o, part_ml, (__nv_bfloat16*)out, splits, o_sb, o_sh, H);
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 

@@ -83,6 +83,9 @@ class LlamaForInference(nn.Module):
         # cache makes the calls it makes without quantisation
         scales = self.kv.kernel_scales()
         scale_kw = {} if scales in (None, (1.0, 1.0)) else {"k_scale": scales[0], "v_scale": scales[1]}
+        # RoPE + cache append in one launch (csrc/decode.cu), then attention on the cache as stored
+        fused = (q.is_cuda and q.dtype == torch.bfloat16 and scales is not None and self.kv.seq_shards == 1
+                 and ops._ext.ext() is not None and hasattr(ops._ext.ext(), "decode_rope_kv"))
         if self.flash_decoding and not prefill:
             assert S == 1 and tree is None, "flash decoding serves plain token generation (no speculation window)"
             from ..modules.attention.flash_decode import flash_decode_attention
@@ -94,17 +97,24 @@ class LlamaForInference(nn.Module):
             kc, vc = self.kv.stored(layer_idx) if scales is not None else self.kv.get(layer_idx)
             o = flash_decode_attention(q, kc, vc, positions, self.kv_group, sliding_window=sw, **scale_kw)
         elif not prefill and S > 1:
-            # speculation window: W new tokens per sequence at positions p..p+W-1, causal among themselves, full cache before
-            W = S
-            # linear window: node w sits at sequence position p+w; Medusa tree: node w sits at p+depth[w] (its cache SLOT is
-            # still p+w) and sees only its ancestors inside the window
-            depth = torch.arange(W, device=q.device) if tree is None else tree[1]
-            idx = (positions.unsqueeze(1) + depth.unsqueeze(0)).clamp(max=self.max_seq_len - 1)
-            cos, sin = self.rope_cos[idx], self.rope_sin[idx]                     # [B, W, D/2]
-            q, k = _rope_window(q, cos, sin), _rope_window(k, cos, sin)
-            self.kv.write_window(layer_idx, k, v, positions)
-            kc, vc = self.kv.get(layer_idx, kv_len)
-            o = _window_attention(q, kc, vc, positions, None if tree is None else tree[0], sw, depth)
+            # speculation window: W new tokens per sequence in cache slots p..p+W-1; linear window: token w sits at sequence
+            # position p+w; Medusa tree: node w sits at p+depth[w] and sees only its ancestors inside the window
+            # (ops.attention.speculation_attention)
+            tree_mask, depth = (None, None) if tree is None else tree
+            if fused:
+                ops._ext.count_launch()
+                q = ops._ext.ext().decode_rope_kv(q, k, v, positions.to(torch.long).contiguous(), self.rope_cos, self.rope_sin,
+                                                  self.kv.k[layer_idx], self.kv.v[layer_idx], depth=depth, **scale_kw)
+                kc, vc = self.kv.stored(layer_idx, kv_len)
+                o = ops.attention.speculation_attention(q, kc, vc, positions, tree_mask, depth, sw, **scale_kw)
+            else:
+                d = torch.arange(S, device=q.device) if depth is None else depth
+                idx = (positions.unsqueeze(1) + d.unsqueeze(0)).clamp(max=self.max_seq_len - 1)
+                cos, sin = self.rope_cos[idx], self.rope_sin[idx]                 # [B, W, D/2]
+                q, k = _rope_window(q, cos, sin), _rope_window(k, cos, sin)
+                self.kv.write_window(layer_idx, k, v, positions)
+                kc, vc = self.kv.get(layer_idx, kv_len)
+                o = ops.attention.speculation_attention_torch(q, kc, vc, positions, tree_mask, depth, sw)
         elif prefill:
             cos, sin = self.rope_cos[:S], self.rope_sin[:S]
             q, k = ops.rope.apply_rotary(q, cos, sin), ops.rope.apply_rotary(k, cos, sin)
@@ -113,9 +123,7 @@ class LlamaForInference(nn.Module):
             else:
                 self.kv.write_prefill(layer_idx, k, v)
             o = ops.attention.flash_attention(q, k, v, causal=True, sliding_window=sw)
-        elif (q.is_cuda and q.dtype == torch.bfloat16 and scales is not None and self.kv.seq_shards == 1
-              and ops._ext.ext() is not None and hasattr(ops._ext.ext(), "decode_rope_kv")):
-            # one launch: RoPE of q and k at each sequence's position + append of k / v to the cache (csrc/decode.cu)
+        elif fused:
             ops._ext.count_launch()
             q = ops._ext.ext().decode_rope_kv(q, k, v, positions.to(torch.long).contiguous(), self.rope_cos, self.rope_sin,
                                               self.kv.k[layer_idx], self.kv.v[layer_idx], **scale_kw)
@@ -195,7 +203,8 @@ class LlamaForInference(nn.Module):
         each of the W positions, ``[B, W]`` (reference ``examples/inference`` speculation model, ``speculation_length``).
         With ``tree_mask [W, W]`` (True = node row sees node column) and ``tree_depth [W]`` the window is a Medusa candidate
         tree instead of a chain.  ``return_hidden`` also returns the final hidden states ``[B, W, H]`` (Medusa heads input)."""
-        tree = None if tree_mask is None else (tree_mask.bool(), tree_depth.long())
+        dev = input_ids.device
+        tree = None if tree_mask is None else (tree_mask.to(dev, torch.bool).contiguous(), tree_depth.to(dev, torch.long).contiguous())
         h = self._body(input_ids, positions, False, kv_len, tree)                # [W, B, H]
         logits = self.lm.lm_head(h).float()                                       # [W, B, V/tp]
         W, B = logits.shape[:2]
@@ -252,37 +261,6 @@ def _rope_window(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch
     x1, x2 = xf[..., :d2], xf[..., d2:]
     c, s = cos.unsqueeze(2), sin.unsqueeze(2)
     return torch.cat([x1 * c - x2 * s, x2 * c + x1 * s], dim=-1).to(x.dtype)
-
-
-def _window_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor,
-                      tree_mask: Optional[torch.Tensor] = None, sliding_window: Optional[int] = None,
-                      depth: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """q [B,W,H,D] in cache slots p..p+W-1 vs cache k/v [B,L,Hkv,D].  Chain: token w sees slots ≤ p+w.  Tree (``tree_mask``
-    [W,W]): node w sees every slot < p (the committed sequence) and the window slots of its ancestors.
-    ``sliding_window`` SW: a token at sequence position p + ``depth[w]`` (chain: depth w) also only sees keys whose sequence
-    position is > p + depth[w] − SW; a committed slot c sits at position c, window slot p + u at p + depth[u]."""
-    B, W, H, D = q.shape
-    Hkv, L = k.shape[2], k.shape[1]
-    qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
-    if H != Hkv:
-        kt, vt = kt.repeat_interleave(H // Hkv, 1), vt.repeat_interleave(H // Hkv, 1)
-    cols = torch.arange(L, device=q.device)
-    if tree_mask is None:
-        lim = positions[:, None] + torch.arange(W, device=q.device)[None, :]                   # [B, W]
-        mask = (cols[None, None, :] <= lim[:, :, None])[:, None]                               # [B,1,W,L]
-    else:
-        rel = cols[None, :] - positions[:, None]                                               # [B, L] slot index inside the window
-        inside = (rel >= 0) & (rel < W)
-        tm = tree_mask.to(q.device)[:, rel.clamp(0, W - 1)].permute(1, 0, 2)                   # [B, W, L]
-        mask = ((rel < 0)[:, None, :] | (inside[:, None, :] & tm))[:, None]
-    if sliding_window is not None:
-        depth = torch.arange(W, device=q.device) if depth is None else depth.to(q.device)
-        rel = cols[None, :] - positions[:, None]                                               # [B, L]
-        kpos = torch.where(rel < W, positions[:, None] + depth[rel.clamp(0, W - 1)], cols[None, :])
-        kpos = torch.where(rel < 0, cols[None, :], kpos)                                       # sequence position of each slot
-        qpos = positions[:, None] + depth[None, :]                                             # [B, W]
-        mask = mask & (kpos[:, None, :] > qpos[:, :, None] - sliding_window)[:, None]
-    return torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask).transpose(1, 2)
 
 
 def _decode_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor,

@@ -223,6 +223,99 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     return torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask, scale=scale).transpose(1, 2)
 
 
+#: most new tokens per sequence the speculation kernel verifies in one call
+SPEC_MAX_TOKENS = 64
+
+
+def _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale):
+    """Argument checks of :func:`speculation_attention` → ``(window, scale kwargs)``; raises ``ValueError``."""
+    if q.dim() != 4 or k_cache.dim() != 4 or v_cache.shape != k_cache.shape:
+        raise ValueError(f"speculation_attention: expected q [B,W,H,D] and caches [B,L,Hkv,D], got {tuple(q.shape)}, "
+                         f"{tuple(k_cache.shape)} and {tuple(v_cache.shape)}")
+    B, W, H, D = q.shape
+    if k_cache.shape[0] != B or k_cache.shape[3] != D or H % k_cache.shape[2]:
+        raise ValueError(f"speculation_attention: q {tuple(q.shape)} does not match the caches {tuple(k_cache.shape)}")
+    if (tree_mask is None) != (tree_depth is None):
+        raise ValueError("speculation_attention: tree_mask and tree_depth go together")
+    if tree_mask is not None and (tuple(tree_mask.shape) != (W, W) or tuple(tree_depth.shape) != (W,)):
+        raise ValueError(f"speculation_attention: tree_mask must be [W, W] and tree_depth [W] for W = {W}, got "
+                         f"{tuple(tree_mask.shape)} and {tuple(tree_depth.shape)}")
+    return check_window(sliding_window), check_kv_scales(k_cache, v_cache, k_scale, v_scale)
+
+
+def speculation_visibility(positions: torch.Tensor, length: int, W: int, tree_mask: Optional[torch.Tensor] = None,
+                           tree_depth: Optional[torch.Tensor] = None, window: int = 0) -> torch.Tensor:
+    """``[B, W, length]`` bool: which cache slots each of W new tokens sees (the rule of :func:`speculation_attention`)."""
+    dev = positions.device
+    p = positions.long()[:, None]                                                          # [B, 1]
+    d = torch.arange(W, device=dev) if tree_depth is None else tree_depth.to(dev).long()
+    m = torch.ones(W, W, dtype=torch.bool, device=dev).tril() if tree_mask is None else tree_mask.to(dev).bool()
+    c = torch.arange(length, device=dev)[None, :]                                          # [1, L]
+    u = c - p                                                                              # [B, L] window column of slot c
+    inside = (u >= 0) & (u < W)
+    uc = u.clamp(0, W - 1)
+    vis = (u < 0)[:, None, :] | (inside[:, None, :] & m[:, uc].permute(1, 0, 2))          # [B, W, L]
+    if window > 0:
+        kpos = torch.where(inside, p + d[uc], c)                                           # sequence position of slot c
+        vis = vis & (kpos[:, None, :] > (p + d[None, :])[:, :, None] - window)
+    return vis
+
+
+def speculation_attention_torch(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, positions: torch.Tensor,
+                                tree_mask: Optional[torch.Tensor] = None, tree_depth: Optional[torch.Tensor] = None,
+                                sliding_window: Optional[int] = None, scale: Optional[float] = None, k_scale: float = 1.0,
+                                v_scale: float = 1.0) -> torch.Tensor:
+    """The torch path of :func:`speculation_attention` (any device and dtype): SDPA with a ``[B, 1, W, L]`` mask on the
+    de-quantised cache, K / V repeated over the GQA group."""
+    window, _ = _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale)
+    B, W, H, D = q.shape
+    Hkv, L = k_cache.shape[2], k_cache.shape[1]
+    if k_cache.dtype in FP8_KV_DTYPES:
+        k_cache, v_cache = (k_cache.float() * k_scale).to(q.dtype), (v_cache.float() * v_scale).to(q.dtype)
+    qt, kt, vt = q.transpose(1, 2), k_cache.transpose(1, 2), v_cache.transpose(1, 2)
+    if H != Hkv:
+        kt, vt = kt.repeat_interleave(H // Hkv, 1), vt.repeat_interleave(H // Hkv, 1)
+    mask = speculation_visibility(positions, L, W, tree_mask, tree_depth, window)[:, None]
+    return F.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask, scale=scale).transpose(1, 2)
+
+
+def speculation_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, positions: torch.Tensor,
+                          tree_mask: Optional[torch.Tensor] = None, tree_depth: Optional[torch.Tensor] = None,
+                          sliding_window: Optional[int] = None, scale: Optional[float] = None, k_scale: float = 1.0,
+                          v_scale: float = 1.0) -> torch.Tensor:
+    """W new tokens per sequence against a KV cache, as speculative decoding and Medusa verify them: ``q [B,W,H,D]``,
+    caches ``[B,L,Hkv,D]`` (any batch / sequence / head strides), ``positions [B]``.  Token w of sequence b occupies cache
+    slot p + w (p = ``positions[b]``) and sits at sequence position p + d[w], with d = ``tree_depth`` (a chain: d[w] = w).
+    Its window mask row is ``tree_mask[w]`` ([W, W], True = sees that window column; a chain: the lower triangle).
+
+    Token w sees slot c iff c < p (the committed sequence) and, with ``sliding_window`` SW, c > p + d[w] − SW; or
+    c = p + u with ``tree_mask[w, u]`` and, with SW, d[u] > d[w] − SW.  Slots ≥ p + W and ≥ L are never seen; a token that
+    sees nothing gets 0.  An fp8 cache holds k / ``k_scale`` and v / ``v_scale``.
+
+    CUDA bf16 q with head_dim 128, W ≤ 64, H / Hkv ∈ {1, 2, 4, 8} and a bf16 or fp8 e4m3 cache whose rows are aligned as
+    :func:`decode_attention` needs: the kernel in ``csrc/attention_sm90.cu``, which reads each K / V row once for all W
+    tokens and the GQA group, reads e4m3 as stored, and with a window only the slots some token can see.  ``tree_mask``
+    and ``tree_depth`` are never read on the host there, so the call can be captured in a CUDA graph.  Otherwise
+    :func:`speculation_attention_torch`."""
+    window, kw = _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale)
+    B, W, H, D = q.shape
+    scale = scale if scale is not None else 1.0 / math.sqrt(D)
+    e = _ext.ext() if q.is_cuda else None
+    align = 16 if k_cache.dtype == torch.bfloat16 else 8
+    if (e is not None and hasattr(e, "speculation_attention") and D == 128 and q.dtype == torch.bfloat16
+            and k_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn) and W <= SPEC_MAX_TOKENS
+            and H // k_cache.shape[2] in (1, 2, 4, 8)
+            and all(t.stride(3) == 1 and t.data_ptr() % align == 0 and all(s % 8 == 0 for s in t.stride()[:3])
+                    for t in (k_cache, v_cache))):
+        if tree_mask is not None:
+            tree_mask, tree_depth = tree_mask.to(q.device).contiguous(), tree_depth.to(q.device, torch.long).contiguous()
+        _ext.count_launch(2)
+        return e.speculation_attention(_tma_view(q), k_cache, v_cache, positions.to(torch.long).contiguous(), tree_mask,
+                                       tree_depth, scale=float(scale), window=window, **kw)
+    return speculation_attention_torch(q, k_cache, v_cache, positions, tree_mask, tree_depth, sliding_window, scale, k_scale,
+                                       v_scale)
+
+
 def decode_visibility(positions: torch.Tensor, length: int, window: int = 0) -> torch.Tensor:
     """``[B, length]`` bool: cache index j is visible to the token at ``positions[b]`` iff j ≤ position and, with a window
     W > 0, j > position − W."""

@@ -1,5 +1,5 @@
 """Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
-usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]] [--kv-fp8]
+usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]] [--kv-fp8] [--spec]
 
 --perf times forward and forward+backward of the own kernels and of SDPA in the same process, alternating, at the shapes
 the models run (BERT-large with right padding, ViT-B/16, GPT-NeoX-20B per rank at TP=8, Pythia-2.8B, Llama-2-7B).  FLOPs
@@ -22,7 +22,14 @@ byte counts come from shapes and are printed without a GPU too; times need one.
 process: the Mistral-7B per-GPU shape (H 32, Hkv 8, D 128) on a full 32k cache at B = 1, 8 and 32, and the Llama-2-13B
 MHA shape (H = Hkv = 40) at B = 8, L = 4096.  Bytes read come from the shapes (the K and V rows and q; the fp32 split
 partials, which stay in L2, are left out); GB/s is those bytes over the time of the call (both kernels).  Both caches hold the same values (the bf16 one
-is the de-quantised e4m3 one), and the two outputs are compared."""
+is the de-quantised e4m3 one), and the two outputs are compared.
+
+--spec (with --perf) times ``speculation_attention`` (the verification kernel and its combine) against the path it replaces
+(de-quantise the whole fp8 cache, then SDPA with a [B, 1, W, L] mask on K / V repeated over the GQA group), alternating in
+one process: Llama-2-7B (H = Hkv = 32) at L = 4096, B = 1, and Mistral-7B (H 32, Hkv 8) at L = 32768, B = 1 and 8, with and
+without a 4096 sliding window; a 5-token chain, the Medusa example's 10-node tree and a random 64-node tree; bf16 and e4m3
+caches holding the same values.  Bytes come from the shapes: the K and V rows some token can see, read once, plus q and the
+output."""
 import argparse
 import json
 import math
@@ -261,6 +268,83 @@ def kv_fp8_perf():
         torch.cuda.empty_cache()
 
 
+# name, B, L, H, Hkv, sliding window
+SPEC_SHAPES = [
+    ("llama2_7b", 1, 4096, 32, 32, None),
+    ("mistral7b", 1, 32768, 32, 8, None),
+    ("mistral7b", 1, 32768, 32, 8, 4096),
+    ("mistral7b", 8, 32768, 32, 8, None),
+    ("mistral7b", 8, 32768, 32, 8, 4096),
+]
+# the candidate tree of examples/inference/run_llama_medusa.py (10 nodes)
+MEDUSA_CHOICES = [[0], [1], [2], [0, 0], [0, 1], [1, 0], [0, 0, 0], [0, 0, 1], [0, 1, 0]]
+
+
+def spec_windows(dev):
+    """(name, tree_mask, tree_depth, W): a 5-token chain, the example's 10-node Medusa tree and a random 64-node tree."""
+    from neuronx_distributed_b200.utils.medusa_utils import generate_medusa_buffers
+
+    buf = generate_medusa_buffers(MEDUSA_CHOICES, device=dev, topk=10)
+    g = torch.Generator().manual_seed(0)
+    mask, depth = torch.eye(64, dtype=torch.bool), torch.zeros(64, dtype=torch.long)
+    for i in range(1, 64):
+        par = int(torch.randint(0, i, (1,), generator=g))
+        mask[i] |= mask[par]
+        depth[i] = depth[par] + 1
+    return [("chain5", None, None, 5), ("tree10", buf["medusa_attn_mask"][0, 0].bool(), buf["medusa_position_ids"].long(), 10),
+            ("tree64", mask.to(dev), depth.to(dev), 64)]
+
+
+def spec_perf():
+    """``speculation_attention`` (kernel) against the path it replaces (de-quantise the whole cache, then the torch path),
+    alternating in one process, on a full cache (p = L − W)."""
+    dev = torch.device("cuda")
+    print(json.dumps(gpu_info()), flush=True)
+    D, ks, vs = 128, 0.05, 0.05
+    for name, B, L, H, Hkv, sw in SPEC_SHAPES:
+        g = torch.Generator(device=dev).manual_seed(L + B)
+        k8, v8 = ((torch.randn(B, L, Hkv, D, device=dev, generator=g) / s).to(torch.float8_e4m3fn) for s in (ks, vs))
+        k16, v16 = (k8.float() * ks).bfloat16(), (v8.float() * vs).bfloat16()
+        for wname, mask, depth, W in spec_windows(dev):
+            q = torch.randn(B, W, H, D, device=dev, generator=g).bfloat16()
+            pos = torch.full((B,), L - W, device=dev, dtype=torch.long)
+            rows = L if sw is None else min(L, W + sw - 1)             # cache rows one sequence's tokens can see
+            for cache in ("bf16", "e4m3"):
+                kc, vc = (k16, v16) if cache == "bf16" else (k8, v8)
+                kw = {} if cache == "bf16" else {"k_scale": ks, "v_scale": vs}
+
+                def new():
+                    return attention.speculation_attention(q, kc, vc, pos, mask, depth, sw, **kw)
+
+                def old():
+                    kd, vd = (kc, vc) if cache == "bf16" else ((kc.float() * ks).bfloat16(), (vc.float() * vs).bfloat16())
+                    return attention.speculation_attention_torch(q, kd, vd, pos, mask, depth, sw)
+
+                n0 = _ext.launches()
+                o_new = new()
+                assert _ext.launches() == n0 + 2, "the kernel did not run"
+                o_old = old()
+                err = ((o_new.float() - o_old.float()).abs().max() / o_old.float().abs().max()).item()
+                t = {"new": [], "old": []}
+                iters = 20 if B * L <= 32768 else 5
+                for _ in range(3):                             # alternate, keep each one's best
+                    t["new"].append(time_fn(new, iters))
+                    t["old"].append(time_fn(old, iters))
+                elt = 2 if cache == "bf16" else 1
+                nbytes = 2 * B * rows * Hkv * D * elt + 2 * B * W * H * D * 2       # K and V rows read once, q and out
+                rec = {"bench": f"{name}_spec_{wname}", "cache": cache, "B": B, "L": L, "H": H, "Hkv": Hkv, "W": W,
+                       "sliding_window": sw, "bytes": nbytes, "rel_err_vs_old": round(err, 5)}
+                for key in ("new", "old"):
+                    ms = min(t[key])
+                    rec[f"{key}_us"] = round(ms * 1e3, 1)
+                    rec[f"{key}_GBps"] = round(nbytes / ms / 1e6, 1)
+                rec["speedup"] = round(rec["old_us"] / rec["new_us"], 2)
+                print(json.dumps(rec), flush=True)
+            del q
+        del k8, v8, k16, v16
+        torch.cuda.empty_cache()
+
+
 def block_pairs(c: int, causal: bool, off: int, W) -> int:
     """Visible (query, key) pairs of one c × c CP block: all c² when dense, else i + off − W < j ≤ i + off (W None: no lower
     bound)."""
@@ -348,6 +432,7 @@ def main():
     ap.add_argument("--window", action="store_true", help="with --perf: the sliding-window table instead of the model shapes")
     ap.add_argument("--cp", type=int, default=0, help="with --perf --window: the context-parallel block schedule at this CP size")
     ap.add_argument("--kv-fp8", action="store_true", help="with --perf: decode attention on bf16 vs fp8 e4m3 KV caches")
+    ap.add_argument("--spec", action="store_true", help="with --perf: speculation / Medusa verification attention")
     ap.add_argument("--head-dim", type=int, default=128, choices=attention.FLASH_HEAD_DIMS)
     a = ap.parse_args()
     if a.perf and a.window and a.cp > 1 and not torch.cuda.is_available():
@@ -410,6 +495,8 @@ def main():
     if a.perf:
         if a.kv_fp8:
             kv_fp8_perf()
+        elif a.spec:
+            spec_perf()
         elif a.window and a.cp > 1:
             cp_window_perf(a.bwd, a.cp)
         else:
