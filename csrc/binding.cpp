@@ -416,9 +416,13 @@ static std::vector<Tensor> moe_block_tkg(const Tensor& x, const c10::optional<Te
   const int T = x.size(0), H = x.size(1), E = router_w.size(0), El = w_gu.size(0), I = w_dn.size(1), K = top_k;
   TORCH_CHECK(nxd::moe_block_tkg_supported(T, H, E, I, K), "moe_block_tkg: unsupported shape");
   TORCH_CHECK(e0 >= 0 && e0 + El <= E);
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(x.data_ptr()) | reinterpret_cast<uintptr_t>(router_w.data_ptr()) |
+               reinterpret_cast<uintptr_t>(w_gu.data_ptr()) | reinterpret_cast<uintptr_t>(w_dn.data_ptr())) % 16 == 0,
+              "moe_block_tkg: x, router_w, w_gu and w_dn must start 16-byte aligned (the kernel loads 16-byte vectors)");
   const void* g = nullptr;
   if (gamma.has_value()) {
     TORCH_CHECK(gamma->scalar_type() == at::kBFloat16 && gamma->is_contiguous() && gamma->numel() == H);
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(gamma->data_ptr()) % 16 == 0, "moe_block_tkg: gamma must start 16-byte aligned");
     g = gamma->data_ptr();
   }
   const float* rb = nullptr;

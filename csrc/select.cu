@@ -1,13 +1,18 @@
 // Row-wise selection kernels for on-device sampling (roles of the reference's NKI `cascaded_max` K10, `nkilib.core.topk`
 // K11 and the torch_neuronx TopK / Argmax custom calls K12 — operators/argmax.py:129, operators/topk.py:17-21,
-// utils/sampling.py:50-60).  A vocab(-shard) row is a one-pass HBM-bound reduction: one CTA per row, 16-byte loads,
-// ties resolved to the smallest index (torch.argmax / torch.topk order on equal values is unspecified; the distributed
-// wrappers in operators/ rely on "smallest global index wins").
+// utils/sampling.py:50-60).  A vocab(-shard) row is a one-pass HBM-bound reduction: one CTA per row, 16-byte loads.
 //   row_argmax   x [R, V] → value fp32 [R], index int64 [R] (+ index_offset: global id of this rank's first column)
 //   row_topk     x [R, V] → values fp32 [R, k], indices int64 [R, k], sorted descending; k <= 128, V*4 bytes <= 200 KB:
-//                the row is staged once in shared memory as fp32 and k block-wide arg-max passes pick the winners.
-#include <cfloat>
-
+//                the row is staged once in shared memory as order keys and k block-wide arg-max passes pick the winners.
+//
+// Selection rule (torch's, and what the distributed wrappers in operators/ rely on): descending order; NaN ranks above
+// +inf; -0 and +0 are equal; among equal values the smaller index comes first (torch leaves that order unspecified, the
+// wrappers need "smallest global index wins").  top-k returns k distinct indices and the values x[idx] in fp32, -inf and
+// NaN included; the arg-max of an all -inf row is index 0 with value -inf.
+// Every element is ranked by a 32-bit order key (the fp32 bit pattern made monotonic as an unsigned integer, NaN mapped to
+// the top key).  The smallest real key is that of -inf, 0x007fffff, so key 0 is free: it marks a top-k entry already taken
+// and "nothing seen yet", and can never win against a real element.  Key and index travel as one 64-bit word
+// (key << 32 | ~index), so "larger word" is exactly the rule above.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -15,38 +20,38 @@ namespace nxd {
 
 namespace {
 
-struct ValIdx { float v; int i; };
-
-NXD_DEVICE ValIdx better(ValIdx a, ValIdx b) {           // larger value, then smaller index
-  return (b.v > a.v || (b.v == a.v && b.i < a.i)) ? b : a;
+NXD_DEVICE uint32_t order_key(float f) {
+  uint32_t u = __float_as_uint(f);
+  if ((u & 0x7fffffffu) > 0x7f800000u) return 0xffffffffu;      // any NaN: above +inf (0xff800000)
+  if (u == 0x80000000u) u = 0u;                                 // -0 ranks equal to +0
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
-NXD_DEVICE ValIdx warp_best(ValIdx x) {
+NXD_DEVICE unsigned long long pack_key(uint32_t key, int i) { return (unsigned long long)key << 32 | (uint32_t)~i; }
+NXD_DEVICE int packed_index(unsigned long long p) { return (int)~(uint32_t)p; }
+
+NXD_DEVICE unsigned long long warp_best(unsigned long long x) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
-    ValIdx y;
-    y.v = __shfl_xor_sync(0xffffffffu, x.v, o);
-    y.i = __shfl_xor_sync(0xffffffffu, x.i, o);
-    x = better(x, y);
+    const unsigned long long y = __shfl_xor_sync(0xffffffffu, x, o);
+    x = y > x ? y : x;
   }
   return x;
 }
-NXD_DEVICE ValIdx block_best(ValIdx x, ValIdx* smem) {    // smem: >= 32 entries; result valid in all threads
+NXD_DEVICE unsigned long long block_best(unsigned long long x, unsigned long long* smem) {   // smem: >= 32 entries; all threads
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
   x = warp_best(x);
   __syncthreads();
   if (lane == 0) smem[warp] = x;
   __syncthreads();
-  ValIdx r = lane < nw ? smem[lane] : ValIdx{-FLT_MAX, 0x7fffffff};
-  r = warp_best(r);
-  return r;
+  return warp_best(lane < nw ? smem[lane] : 0ull);
 }
 
 template <typename T>
 __global__ void __launch_bounds__(256) row_argmax_kernel(const T* __restrict__ x, float* __restrict__ val, long* __restrict__ idx,
                                                          int V, long row_stride, long index_offset) {
-  __shared__ ValIdx red[32];
+  __shared__ unsigned long long red[32];
   const T* row = x + (long)blockIdx.x * row_stride;
-  ValIdx best{-FLT_MAX, 0x7fffffff};
+  unsigned long long best = 0ull;                               // below every real element (V >= 1)
   constexpr int N = 16 / sizeof(T);
   const bool vec_ok = ((uintptr_t)row % 16 == 0);
   const int nvec = vec_ok ? V / N : 0;
@@ -54,29 +59,43 @@ __global__ void __launch_bounds__(256) row_argmax_kernel(const T* __restrict__ x
     Pack16<T> p;
     p.load(row + (long)v * N);
 #pragma unroll
-    for (int j = 0; j < N; ++j) best = better(best, ValIdx{p.f(j), v * N + j});
+    for (int j = 0; j < N; ++j) {
+      const unsigned long long c = pack_key(order_key(p.f(j)), v * N + j);
+      best = c > best ? c : best;
+    }
   }
-  for (int c = nvec * N + threadIdx.x; c < V; c += blockDim.x) best = better(best, ValIdx{to_f32<T>(row[c]), c});
+  for (int c = nvec * N + threadIdx.x; c < V; c += blockDim.x) {
+    const unsigned long long q = pack_key(order_key(to_f32<T>(row[c])), c);
+    best = q > best ? q : best;
+  }
   best = block_best(best, red);
-  if (threadIdx.x == 0) { val[blockIdx.x] = best.v; idx[blockIdx.x] = (long)best.i + index_offset; }
+  if (threadIdx.x == 0) {
+    const int i = packed_index(best);
+    val[blockIdx.x] = to_f32<T>(row[i]);
+    idx[blockIdx.x] = (long)i + index_offset;
+  }
 }
 
 template <typename T>
 __global__ void __launch_bounds__(256) row_topk_kernel(const T* __restrict__ x, float* __restrict__ vals, long* __restrict__ idxs,
                                                        int V, int k, long row_stride, long index_offset) {
-  extern __shared__ float srow[];
-  __shared__ ValIdx red[32];
+  extern __shared__ uint32_t skey[];
+  __shared__ unsigned long long red[32];
   const T* row = x + (long)blockIdx.x * row_stride;
-  for (int c = threadIdx.x; c < V; c += blockDim.x) srow[c] = to_f32<T>(row[c]);
+  for (int c = threadIdx.x; c < V; c += blockDim.x) skey[c] = order_key(to_f32<T>(row[c]));
   __syncthreads();
-  for (int j = 0; j < k; ++j) {
-    ValIdx best{-FLT_MAX, 0x7fffffff};
-    for (int c = threadIdx.x; c < V; c += blockDim.x) best = better(best, ValIdx{srow[c], c});
+  for (int j = 0; j < k; ++j) {                                 // k <= V: an untaken real element always wins
+    unsigned long long best = 0ull;
+    for (int c = threadIdx.x; c < V; c += blockDim.x) {
+      const unsigned long long q = pack_key(skey[c], c);
+      best = q > best ? q : best;
+    }
     best = block_best(best, red);
     if (threadIdx.x == 0) {
-      vals[(long)blockIdx.x * k + j] = best.v;
-      idxs[(long)blockIdx.x * k + j] = (long)best.i + index_offset;
-      if (best.i < V) srow[best.i] = -FLT_MAX;
+      const int i = packed_index(best);
+      vals[(long)blockIdx.x * k + j] = to_f32<T>(row[i]);
+      idxs[(long)blockIdx.x * k + j] = (long)i + index_offset;
+      skey[i] = 0u;                                             // taken
     }
     __syncthreads();
   }
@@ -86,6 +105,7 @@ __global__ void __launch_bounds__(256) row_topk_kernel(const T* __restrict__ x, 
 
 void row_argmax(const void* x, float* val, long* idx, int rows, int V, long row_stride, long index_offset, int dt, cudaStream_t st) {
   if (rows == 0) return;
+  if (V < 1) nxd_throw("row_argmax: a row needs at least one element", __FILE__, __LINE__);
   if (dt == kBF16) row_argmax_kernel<__nv_bfloat16><<<rows, 256, 0, st>>>((const __nv_bfloat16*)x, val, idx, V, row_stride, index_offset);
   else if (dt == kF16) row_argmax_kernel<__half><<<rows, 256, 0, st>>>((const __half*)x, val, idx, V, row_stride, index_offset);
   else row_argmax_kernel<float><<<rows, 256, 0, st>>>((const float*)x, val, idx, V, row_stride, index_offset);

@@ -81,12 +81,16 @@ def moe_block_tkg_reference(x, gamma, router_w, router_bias, w_gu, w_dn, e0: int
     return out.to(dt), logits, idx, w
 
 
-def kernel_eligible(x: torch.Tensor, router_w: torch.Tensor, w_gu: torch.Tensor, w_dn: torch.Tensor, top_k: int) -> bool:
+def kernel_eligible(x: torch.Tensor, router_w: torch.Tensor, w_gu: torch.Tensor, w_dn: torch.Tensor, top_k: int,
+                    gamma: Optional[torch.Tensor] = None) -> bool:
     if not (_ext.use_cuda(x, router_w, w_gu, w_dn) and hasattr(_ext.ext(), "moe_block_tkg")):
         return False
-    if os.environ.get("NXD_MOE_TKG_KERNEL", "0") != "1":      # opt-in until the kernel has run on hardware (tests/test_zz_late_gpu.py)
-        return False
+    if os.environ.get("NXD_MOE_TKG_KERNEL", "0") != "1":      # opt-in until a decode timing against the composed path
+        return False                                           # (numerics: tests/test_moe_tkg_gpu.py)
     if not all(t.dtype == torch.bfloat16 and t.is_contiguous() for t in (x, router_w, w_gu, w_dn)):
+        return False
+    # the kernel loads x, gamma and the weights as 16-byte vectors: a view at an odd storage offset takes the reference
+    if any(t is not None and t.data_ptr() % 16 for t in (x, gamma, router_w, w_gu, w_dn)):
         return False
     return bool(_ext.ext().moe_block_tkg_supported(x.shape[0], x.shape[1], router_w.shape[0], w_dn.shape[1], int(top_k)))
 
@@ -94,13 +98,14 @@ def kernel_eligible(x: torch.Tensor, router_w: torch.Tensor, w_gu: torch.Tensor,
 def moe_block_tkg(x, gamma, router_w, router_bias, w_gu, w_dn, e0: int, top_k: int, eps: float = 1e-6, router_act: int = 0,
                   act_over_topk: bool = False, normalize: bool = True, pre_scale: bool = False, round_logits: bool = True,
                   act: int = 0, act_alpha: float = 1.0, act_beta: float = 0.0, clamps=(-_INF, _INF, -_INF, _INF)):
-    if kernel_eligible(x, router_w, w_gu, w_dn, top_k):
+    g = None if gamma is None else gamma.contiguous()
+    if kernel_eligible(x, router_w, w_gu, w_dn, top_k, g):
         _ext.count_launch()
         c = [(-3.0e38 if math.isinf(v) and v < 0 else 3.0e38 if math.isinf(v) else float(v)) for v in clamps]
         coop = os.environ.get("NXD_MOE_TKG_COOP", "1") == "1"
         rb = None if router_bias is None else router_bias.float().contiguous()
         out, logits, idx, w = _ext.ext().moe_block_tkg(
-            x, None if gamma is None else gamma.contiguous(), router_w, rb, w_gu, w_dn, int(e0), int(top_k), float(eps),
+            x, g, router_w, rb, w_gu, w_dn, int(e0), int(top_k), float(eps),
             int(router_act), bool(act_over_topk), bool(normalize), bool(pre_scale), bool(round_logits), int(act), float(act_alpha),
             float(act_beta), c[0], c[1], c[2], c[3], coop)
         return out, logits, idx, w

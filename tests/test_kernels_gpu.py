@@ -240,28 +240,6 @@ def test_decode_rope_kv_fused_vs_separate_ops():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
-def test_row_argmax_and_topk_kernels_vs_torch(dtype):
-    from neuronx_distributed_b200.ops import select
-
-    dev = torch.device("cuda")
-    torch.manual_seed(1)
-    for rows, V in ((3, 4000), (2, 32016), (5, 1001)):
-        x = torch.randn(rows, V, device=dev).to(dtype)
-        v, i = select.row_max(x, index_offset=7)
-        rv, ri = torch.max(x.float(), dim=-1)
-        torch.testing.assert_close(v, rv)
-        assert torch.equal(x.float().gather(1, (i - 7).unsqueeze(1)).squeeze(1), rv)      # an index of the maximum …
-        first = (x.float() == rv.unsqueeze(1)).float().argmax(dim=1)
-        assert torch.equal(i - 7, first)                                                   # … the smallest one
-        for k in (1, 8, 50):
-            tv, ti = select.row_topk(x, k)
-            rtv, _ = torch.topk(x.float(), k, dim=-1)
-            torch.testing.assert_close(tv, rtv)
-            assert torch.equal(x.float().gather(1, ti), tv)
-
-
-@pytest.mark.gpu
 def test_moe_block_metadata_kernel_matches_sort_based_build():
     import os
 
