@@ -68,15 +68,23 @@ NXD_DEVICE void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "m
 template <int N>
 NXD_DEVICE void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// rows [s0, s0+64) of one (batch, head) slice → padded shared tile; rows ≥ S are zero-filled
-template <int HD>
-NXD_DEVICE void load_tile(bf16* sm, const bf16* base, long ss, int s0, int S) {
+// row (s0 + r) mod L of a ring of L rows, from w0 = s0 mod L (computed once per tile): r < 64, so one subtraction when L ≥ 64
+NXD_DEVICE int ring_row(int w0, int r, int L) {
+  const int x = w0 + r;
+  return x < L ? x : (L >= BT ? x - L : x % L);
+}
+
+// rows [s0, s0+64) of one (batch, head) slice → padded shared tile; rows ≥ S are zero-filled.  ROLL: the slice is a ring of
+// L rows and row s is read at s mod L.
+template <int HD, bool ROLL = false>
+NXD_DEVICE void load_tile(bf16* sm, const bf16* base, long ss, int s0, int S, int L = 0) {
   constexpr int kChunks = HD / 8;                                   // 16-byte chunks per row
   constexpr bool kPow2 = (kChunks & (kChunks - 1)) == 0;
+  const int w0 = ROLL ? s0 % L : 0;
   for (int i = threadIdx.x; i < BT * kChunks; i += kThreads) {
     const int r = kPow2 ? i >> (kChunks == 16 ? 4 : 3) : i / kChunks, c = kPow2 ? i & (kChunks - 1) : i % kChunks;
     const bool ok = s0 + r < S;
-    cp_async16(sm + r * LDS<HD> + c * 8, base + (long)(ok ? s0 + r : 0) * ss + c * 8, ok);
+    cp_async16(sm + r * LDS<HD> + c * 8, base + (long)(ok ? (ROLL ? ring_row(w0, r, L) : s0 + r) : 0) * ss + c * 8, ok);
   }
 }
 
@@ -327,6 +335,10 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
 // memory, which is exact; k_scale is folded into the softmax scale and v_scale multiplies the partial output.  A window
 // slot no row of the tile sees gets its V row zeroed, so its bytes never reach the output (K is masked by a select).
 // Partials (o relative to the row maximum, maximum and sum in log2 units) are merged by decode.cu's combine kernel.
+// ROLL: the cache is a ring of L rows and slot c (a logical position) lives in row c mod L.  Everything above stays in
+// logical positions, without the upper clamp at L; only the row address of a tile load wraps, per row, because a 64-row
+// tile can straddle the end of the ring.  The host guarantees window > 0 and window + W − 1 ≤ L, so the slots a tile reads
+// (at most p + dmin − window + 1 … p + W − 1) map to distinct rows.
 constexpr int kSpecMaxW = 64;
 constexpr int kRawTile = BT * 128;                      // bytes of one staged e4m3 tile
 template <bool E4M3>
@@ -348,12 +360,14 @@ NXD_DEVICE void cp_async8(void* dst, const void* src, bool valid) {
 }
 
 // rows [s0, s0+64) of one e4m3 (batch, kv head) slice → unpadded 128-byte shared rows; rows ≥ S are zero-filled.  8-byte
-// copies: an e4m3 cache is only required to be 8-byte aligned.
-NXD_DEVICE void load_raw_e4m3(uint8_t* sm, const uint8_t* base, long ss, int s0, int S) {
+// copies: an e4m3 cache is only required to be 8-byte aligned.  ROLL as in load_tile.
+template <bool ROLL>
+NXD_DEVICE void load_raw_e4m3(uint8_t* sm, const uint8_t* base, long ss, int s0, int S, int L) {
+  const int w0 = ROLL ? s0 % L : 0;
   for (int i = threadIdx.x; i < BT * 16; i += kThreads) {
     const int r = i >> 4, c = i & 15;
     const bool ok = s0 + r < S;
-    cp_async8(sm + r * 128 + c * 8, base + (long)(ok ? s0 + r : 0) * ss + c * 8, ok);
+    cp_async8(sm + r * 128 + c * 8, base + (long)(ok ? (ROLL ? ring_row(w0, r, L) : s0 + r) : 0) * ss + c * 8, ok);
   }
 }
 
@@ -373,7 +387,7 @@ NXD_DEVICE void e4m3_to_bf16(bf16* dst, const uint8_t* src) {
   }
 }
 
-template <int G, bool E4M3>
+template <int G, bool E4M3, bool ROLL>
 __global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p) {
   constexpr int HD = 128, kTl = kTile<HD>, kBufs = E4M3 ? 1 : 2;
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -387,8 +401,9 @@ __global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int W = p.W, r0 = rt * BT, n_rows = W * G;
   const long pos = p.positions[b];
-  // p clamped to [−64, L]: the same slots are committed / window slots below L, and slot − p stays in int range
-  const int p32 = (int)min(max(pos, (long)-kSpecMaxW), (long)p.L);
+  // p clamped to [−64, L] (ROLL: to ≥ −64): the same slots are committed / window slots below L, and slot − p stays in int
+  // range
+  const int p32 = ROLL ? (int)max(pos, (long)-kSpecMaxW) : (int)min(max(pos, (long)-kSpecMaxW), (long)p.L);
 
   if (threadIdx.x < W) sDepth[threadIdx.x] = p.depth ? (int)p.depth[threadIdx.x] : threadIdx.x;
   __syncthreads();
@@ -411,8 +426,8 @@ __global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p)
   const uint64_t unseen = ~seen & (W == 64 ? ~0ull : (1ull << W) - 1);
   // slots [lo, hi) some row of the tile sees; the splits divide them in whole 64-slot tiles
   const long lo_l = p.window > 0 ? min(pos, pos + dmin - p.window + 1) : 0;
-  const int lo = (int)min(max(lo_l, 0L), (long)p.L);
-  const int hi = (int)max(min(pos + W, (long)p.L), (long)lo);
+  const int lo = ROLL ? (int)max(lo_l, 0L) : (int)min(max(lo_l, 0L), (long)p.L);
+  const int hi = ROLL ? (int)max(pos + W, (long)lo) : (int)max(min(pos + W, (long)p.L), (long)lo);
   const int per = ((hi - lo + p.splits - 1) / p.splits + BT - 1) / BT * BT;
   const int s0 = lo + split * per, s1 = min(hi, s0 + per);
   const int n_t = s1 > s0 ? (s1 - s0 + BT - 1) / BT : 0;
@@ -435,11 +450,11 @@ __global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p)
   auto issue = [&](int t) {                     // K / V tile t of the split → buffer t & 1
     const int s = s0 + t * BT, buf = t & 1;
     if constexpr (E4M3) {
-      load_raw_e4m3(sRaw + 2 * buf * kRawTile, kb, p.k_ss, s, s1);
-      load_raw_e4m3(sRaw + (2 * buf + 1) * kRawTile, vb, p.v_ss, s, s1);
+      load_raw_e4m3<ROLL>(sRaw + 2 * buf * kRawTile, kb, p.k_ss, s, s1, p.L);
+      load_raw_e4m3<ROLL>(sRaw + (2 * buf + 1) * kRawTile, vb, p.v_ss, s, s1, p.L);
     } else {
-      load_tile<HD>(sK + buf * kTl, (const bf16*)kb, p.k_ss, s, s1);
-      load_tile<HD>(sV + buf * kTl, (const bf16*)vb, p.v_ss, s, s1);
+      load_tile<HD, ROLL>(sK + buf * kTl, (const bf16*)kb, p.k_ss, s, s1, p.L);
+      load_tile<HD, ROLL>(sV + buf * kTl, (const bf16*)vb, p.v_ss, s, s1, p.L);
     }
     cp_async_commit();
   };
@@ -862,7 +877,7 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
 void speculation_attention(const void* q, const void* k, const void* v, const long* positions, const void* mask,
                            const long* depth, void* out, float* part_o, float* part_ml, int B, int W, int H, int Hkv, int L,
                            const long* qs, const long* ks, const long* vs, float scale, int window, int splits, bool kv_e4m3,
-                           float k_scale, float v_scale, cudaStream_t st) {
+                           float k_scale, float v_scale, bool rolling, cudaStream_t st) {
   using namespace fa;
   const int G = H / Hkv;
   SpecParams p;
@@ -875,19 +890,23 @@ void speculation_attention(const void* q, const void* k, const void* v, const lo
   p.scale_log2 = scale * kLog2e * k_scale;
   p.v_scale = v_scale;
   const dim3 grid(p.row_tiles * splits, Hkv, B);
-  auto launch = [&](auto g, auto e4) {
+  auto launch = [&](auto g, auto e4, auto roll) {
     constexpr int Gv = decltype(g)::value;
-    constexpr bool E4 = decltype(e4)::value;
+    constexpr bool E4 = decltype(e4)::value, R = decltype(roll)::value;
     static bool configured = false;
     if (!configured) {
-      NXD_CUDA_CHECK(cudaFuncSetAttribute(spec_attn_kernel<Gv, E4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemSpec<E4>));
+      NXD_CUDA_CHECK(cudaFuncSetAttribute(spec_attn_kernel<Gv, E4, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemSpec<E4>));
       configured = true;
     }
-    spec_attn_kernel<Gv, E4><<<grid, kThreads, kSmemSpec<E4>, st>>>(p);
+    spec_attn_kernel<Gv, E4, R><<<grid, kThreads, kSmemSpec<E4>, st>>>(p);
+  };
+  auto with_roll = [&](auto g, auto e4) {
+    if (rolling) launch(g, e4, std::true_type{});
+    else launch(g, e4, std::false_type{});
   };
   auto with_cache = [&](auto g) {
-    if (kv_e4m3) launch(g, std::true_type{});
-    else launch(g, std::false_type{});
+    if (kv_e4m3) with_roll(g, std::true_type{});
+    else with_roll(g, std::false_type{});
   };
   switch (G) {
     case 1: with_cache(std::integral_constant<int, 1>{}); break;

@@ -265,10 +265,12 @@ static bool kv_cache_e4m3(const char* fn, const Tensor& kc, const Tensor& vc, do
 
 // q [B,W,H,D], k/v [B,W,Hkv,D] (views of the fused QKV projection output), cache [B,L,Hkv,D]: rotate q → new tensor, rotate
 // k and copy v straight into the cache (token w at slot positions[b] + w, rotated at positions[b] + depth[w], or + w without
-// depth; an e4m3 cache gets k / k_scale and v / v_scale, rounded as the cache's torch rule rounds them)
+// depth; an e4m3 cache gets k / k_scale and v / v_scale, rounded as the cache's torch rule rounds them).  rolling: the cache is
+// a ring of L rows, token w goes to row (positions[b] + w) mod L, and the rotation position is clamped to the table length
+// instead of L.
 static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions, const Tensor& cos_t,
                              const Tensor& sin_t, Tensor kc, Tensor vc, double k_scale, double v_scale,
-                             const c10::optional<Tensor>& depth) {
+                             const c10::optional<Tensor>& depth, bool rolling) {
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) >= 1 && q.stride(3) == 1);
   TORCH_CHECK(k.scalar_type() == at::kBFloat16 && k.dim() == 4 && k.size(1) == q.size(1) && k.stride(3) == 1 && v.stride(3) == 1 && v.sizes() == k.sizes());
   const bool e4m3 = kv_cache_e4m3("decode_rope_kv", kc, vc, k_scale, v_scale);
@@ -276,6 +278,9 @@ static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, 
   TORCH_CHECK(positions.scalar_type() == at::kLong && positions.is_contiguous() && positions.numel() == q.size(0));
   CHECK_IN(cos_t); CHECK_IN(sin_t);
   TORCH_CHECK(cos_t.scalar_type() == at::kFloat && cos_t.size(1) == q.size(3) / 2 && cos_t.size(0) >= kc.size(1));
+  // rolling: positions run past the ring, up to the table length, which bounds the rotation instead of L (both tables are
+  // read, so the shorter one bounds it).  The W slots of one call are distinct rows when W <= L, which the caller keeps
+  // (LlamaForInference: W <= 64 < L).
   const long* dp = nullptr;
   if (depth.has_value()) {
     TORCH_CHECK(depth->is_cuda() && depth->scalar_type() == at::kLong && depth->is_contiguous() && depth->numel() == q.size(1),
@@ -287,9 +292,11 @@ static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, 
   Tensor q_out = at::empty({B, W, H, D}, q.options());
   const long qs[3] = {q.stride(0), q.stride(1), q.stride(2)}, ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   const long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
+  const int n_pos = rolling ? (int)std::min<int64_t>(std::min(cos_t.size(0), sin_t.size(0)), INT32_MAX) : L;
   nxd::decode_rope_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), dp, cos_t.data_ptr<float>(),
-                      sin_t.data_ptr<float>(), q_out.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, W, H, Hkv, D, L, qs, ks, vs,
-                      kc.stride(0), kc.stride(1), kc.stride(2), stream(), e4m3, 1.0f / (float)k_scale, 1.0f / (float)v_scale);
+                      sin_t.data_ptr<float>(), q_out.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, W, H, Hkv, D, L, n_pos, qs, ks,
+                      vs, kc.stride(0), kc.stride(1), kc.stride(2), stream(), e4m3, 1.0f / (float)k_scale, 1.0f / (float)v_scale,
+                      rolling);
   return q_out;
 }
 
@@ -320,10 +327,14 @@ static bool check_decode_args(const char* fn, const Tensor& q, const Tensor& k, 
               fn, ": e4m3 caches are read 8 bytes at a time: their base addresses and strides must be multiples of 8");
   return e4m3;
 }
+// rolling: the cache is a ring of L rows holding position j in row j mod L; only a sliding window shorter than the ring
+// keeps every visible position in its own row
 static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions, double scale,
-                               int64_t window, double k_scale, double v_scale) {
+                               int64_t window, double k_scale, double v_scale, bool rolling) {
   const bool e4m3 = check_decode_args("decode_attention", q, k, v, positions, k_scale, v_scale);
   const int B = q.size(0), H = q.size(2), L = k.size(1), Hkv = k.size(2);
+  TORCH_CHECK(!rolling || (window > 0 && window < L), "decode_attention: a rolling cache needs 0 < window < L (",
+                    L, " rows), got window ", window);
   c10::cuda::CUDAGuard guard(q.device());
   const int splits = decode_splits(B, Hkv, L, window);
   Tensor out = at::empty({B, 1, H, 128}, q.options());
@@ -333,7 +344,7 @@ static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v
   nxd::decode_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), out.data_ptr(),
                         part_o.data_ptr<float>(), part_ml.data_ptr<float>(), B, H, Hkv, L, ks, vs, q.stride(0), q.stride(2),
                         out.stride(0), out.stride(2), (float)scale, splits, (int)std::min<int64_t>(window, INT32_MAX), stream(),
-                        nullptr, nullptr, e4m3, (float)k_scale, (float)v_scale);
+                        nullptr, nullptr, e4m3, (float)k_scale, (float)v_scale, rolling);
   return out;
 }
 // This rank's contribution to distributed flash-decoding: un-normalised output (relative to the row maximum) [B,H,128] fp32 and
@@ -357,10 +368,11 @@ static std::vector<Tensor> decode_attention_partial(const Tensor& q, const Tenso
   return {fin_o, fin_ml};
 }
 // q [B,W≤64,H,128] (any b/s/h strides, rows 16-byte aligned) verified against the cache as decode_attention reads it; tree_mask
-// [W,W] bool / uint8 and tree_depth [W] int64 (both or neither: a chain).  Never reads them on the host.
+// [W,W] bool / uint8 and tree_depth [W] int64 (both or neither: a chain).  Never reads them on the host.  rolling: a ring of L
+// rows, as in decode_attention.
 static Tensor speculation_attention(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions,
                                     const c10::optional<Tensor>& tree_mask, const c10::optional<Tensor>& tree_depth, double scale,
-                                    int64_t window, double k_scale, double v_scale) {
+                                    int64_t window, double k_scale, double v_scale, bool rolling) {
   const char* fn = "speculation_attention";
   const bool e4m3 = check_decode_args(fn, q, k, v, positions, k_scale, v_scale, 64);
   const int B = q.size(0), W = q.size(1), H = q.size(2), L = k.size(1), Hkv = k.size(2), G = H / Hkv;
@@ -371,6 +383,10 @@ static Tensor speculation_attention(const Tensor& q, const Tensor& k, const Tens
                        k.stride(0) % 8 == 0 && v.stride(0) % 8 == 0),
               fn, ": bf16 cache rows must be 16-byte aligned");
   TORCH_CHECK(window >= 0, fn, ": window must be >= 0 (0 = none)");
+  // token w writes row (p + w) mod L over position p + w − L, which no token of the window may see: every token sees only
+  // positions > p − window, so p + W − 1 − L ≤ p − window
+  TORCH_CHECK(!rolling || (window > 0 && window + W - 1 <= L), fn, ": a rolling cache needs window > 0 and window + W - 1 "
+                    "<= L, got window ", window, ", W ", W, ", L ", L);
   TORCH_CHECK(tree_mask.has_value() == tree_depth.has_value(), fn, ": tree_mask and tree_depth go together");
   const void* mp = nullptr;
   const long* dp = nullptr;
@@ -397,7 +413,8 @@ static Tensor speculation_attention(const Tensor& q, const Tensor& k, const Tens
   const long ks[3] = {k.stride(0), k.stride(1), k.stride(2)}, vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   nxd::speculation_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), mp, dp, out.data_ptr(),
                              part_o.data_ptr<float>(), part_ml.data_ptr<float>(), B, W, H, Hkv, L, qs, ks, vs, (float)scale,
-                             (int)std::min<int64_t>(window, INT32_MAX), splits, e4m3, (float)k_scale, (float)v_scale, stream());
+                             (int)std::min<int64_t>(window, INT32_MAX), splits, e4m3, (float)k_scale, (float)v_scale, rolling,
+                             stream());
   return out;
 }
 // x [T,H] bf16; gamma [H] bf16 or none; router_w [E,H] bf16; router_bias [E] fp32 or none; w_gu [El,H,2I]; w_dn [El,I,H]
@@ -849,7 +866,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gemm_bf16", &gemm_bf16);
   m.def("oneshot_allreduce", &oneshot_allreduce);
   m.def("decode_attention", &decode_attention, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"), py::arg("scale"),
-        py::arg("window") = 0, py::kw_only(), py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0);
+        py::arg("window") = 0, py::kw_only(), py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0, py::arg("rolling") = false);
   m.def("decode_attention_partial", &decode_attention_partial, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"),
         py::arg("scale"), py::arg("window") = 0, py::kw_only(), py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0);
   m.def("nvls_embedding_gather", &nvls_embedding_gather);
@@ -864,10 +881,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   });
   m.def("decode_rope_kv", &decode_rope_kv, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"), py::arg("cos"),
         py::arg("sin"), py::arg("k_cache"), py::arg("v_cache"), py::kw_only(), py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0,
-        py::arg("depth") = py::none());
+        py::arg("depth") = py::none(), py::arg("rolling") = false);
   m.def("speculation_attention", &speculation_attention, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("positions"),
         py::arg("tree_mask") = py::none(), py::arg("tree_depth") = py::none(), py::kw_only(), py::arg("scale"),
-        py::arg("window") = 0, py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0);
+        py::arg("window") = 0, py::arg("k_scale") = 1.0, py::arg("v_scale") = 1.0, py::arg("rolling") = false);
   m.def("moe_block_metadata", &moe_block_metadata);
   m.def("row_argmax", &row_argmax);
   m.def("row_topk", &row_topk);

@@ -45,7 +45,10 @@ __device__ __forceinline__ void load8(const __nv_fp8_e4m3* p, float (&f)[8], flo
 // registers on bf16 already, so it would spill there.  For G ≤ 4 that mapping fits and would halve the softmax updates per
 // position (16 lanes repeat the same one here); it has not been timed against this one (DESIGN §6).
 // k_scale is folded into scale_log2 by the host; v_scale multiplies the partial o (1 on bf16).
-template <typename T, int G>
+// ROLL: the cache is a ring of L rows (inference/kv_cache.py, rolling mode) and logical position s lives in row s mod L.  The
+// visible range stays in logical positions and is not clipped to L; the host guarantees 0 < window < L, so it spans fewer
+// than L positions and row(s) = s − wrap0, minus L once past the end, with wrap0 = lo − lo mod L.
+template <typename T, int G, bool ROLL>
 __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
     const __nv_bfloat16* __restrict__ q, const T* __restrict__ kc, const T* __restrict__ vc,
     const long* __restrict__ positions, float* __restrict__ part_o, float* __restrict__ part_ml, int B, int H, int Hkv, int L,
@@ -59,11 +62,17 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
   // visible rows [lo, hi): the splits divide this range.  Positions may lie outside [0, L) (the local positions of a sequence
   // shard); then the range is clipped to the cache, and it is empty when the window ends before row 0 or starts past L.
   const long pos = positions[b];
-  const int hi = (int)min(pos + 1, (long)L);
-  const int lo = window > 0 ? (int)min(max(pos - window + 1, 0L), (long)L) : 0;
+  const int hi = ROLL ? (int)(pos + 1) : (int)min(pos + 1, (long)L);
+  const int lo = ROLL ? (int)max(pos - window + 1, 0L) : window > 0 ? (int)min(max(pos - window + 1, 0L), (long)L) : 0;
   const int n_valid = max(hi - lo, 0);
   const int per = (n_valid + splits - 1) / splits;
   const int s0 = lo + split * per, s1 = min(hi, s0 + per);
+  const int wrap0 = ROLL ? lo - lo % L : 0;
+  auto row = [&](int s) {
+    int r = s - wrap0;
+    if (ROLL && r >= L) r -= L;
+    return r;
+  };
 
   float qf[G][8];
 #pragma unroll
@@ -85,11 +94,11 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
       const int s = sbase + 2 * j + sub;
       live[j] = s < s1;
       if constexpr (kE4M3) {                              // a position past s1 re-reads row s1 − 1; its score is not used
-        load8(kb + (long)min(s, s1 - 1) * k_ss, kf[j], 1.f);
-        load8(vb + (long)min(s, s1 - 1) * v_ss, vf[j], 1.f);
+        load8(kb + (long)row(min(s, s1 - 1)) * k_ss, kf[j], 1.f);
+        load8(vb + (long)row(min(s, s1 - 1)) * v_ss, vf[j], 1.f);
       } else if (live[j]) {
-        load8(kb + (long)s * k_ss, kf[j], 1.f);
-        load8(vb + (long)s * v_ss, vf[j], 1.f);
+        load8(kb + (long)row(s) * k_ss, kf[j], 1.f);
+        load8(vb + (long)row(s) * v_ss, vf[j], 1.f);
       } else {
 #pragma unroll
         for (int i = 0; i < 8; ++i) { kf[j][i] = 0.f; vf[j][i] = 0.f; }
@@ -250,27 +259,33 @@ __device__ __forceinline__ __nv_fp8_e4m3 quant_e4m3(__nv_bfloat16 x, float inv) 
 
 // Decode-time RoPE + KV-cache append in ONE launch (was ~25 tiny elementwise / index_put kernels per layer in the token-
 // generation graph): q [B,W,H,D] rotated into q_out, k rotated and v copied into the cache.  Token w of sequence b is
-// rotated at position positions[b] + depth[w] (no depth: + w) and written to slot positions[b] + w, both clamped to the
-// cache (W = 1: the token at positions[b]; W > 1: a speculation window or a Medusa tree).  One warp per head row; cos/sin
-// rows gathered by position.  HF rotate-half convention (csrc/elementwise.cu rope_kernel).  An e4m3 cache gets the bf16
-// rows a bf16 cache would hold, quantised by quant_e4m3 with k_inv = 1/k_scale and v_inv = 1/v_scale.
-template <typename T>
+// rotated at position positions[b] + depth[w] (no depth: + w), clamped to [0, n_pos), and written to slot positions[b] + w,
+// clamped to the cache (W = 1: the token at positions[b]; W > 1: a speculation window or a Medusa tree).  ROLL: the cache is
+// a ring of L rows and the slot is (positions[b] + w) mod L.  One warp per head row; cos/sin rows gathered by position.
+// HF rotate-half convention (csrc/elementwise.cu rope_kernel).  An e4m3 cache gets the bf16 rows a bf16 cache would hold,
+// quantised by quant_e4m3 with k_inv = 1/k_scale and v_inv = 1/v_scale.
+template <typename T, bool ROLL>
 __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                                             const __nv_bfloat16* __restrict__ v, const long* __restrict__ positions,
                                                             const long* __restrict__ depth, const float* __restrict__ cos_t,
                                                             const float* __restrict__ sin_t, __nv_bfloat16* __restrict__ q_out,
                                                             T* __restrict__ kc, T* __restrict__ vc, int B, int W, int H, int Hkv,
-                                                            int D, int L, long q_sb, long q_ss, long q_sh, long k_sb, long k_ss,
-                                                            long k_sh, long v_sb, long v_ss, long v_sh, long c_sb, long c_ss,
-                                                            long c_sh, float k_inv, float v_inv) {
+                                                            int D, int L, int n_pos, long q_sb, long q_ss, long q_sh, long k_sb,
+                                                            long k_ss, long k_sh, long v_sb, long v_ss, long v_sh, long c_sb,
+                                                            long c_ss, long c_sh, float k_inv, float v_inv) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int rows = B * W * (H + 2 * Hkv);
   if (warp >= rows) return;
   const int bw = warp / (H + 2 * Hkv), r = warp % (H + 2 * Hkv), b = bw / W, w = bw % W;
   const long p = positions[b];
   long pos = p + (depth ? depth[w] : w), slot = p + w;
-  pos = pos < 0 ? 0 : (pos >= L ? L - 1 : pos);
-  slot = slot < 0 ? 0 : (slot >= L ? L - 1 : slot);
+  pos = pos < 0 ? 0 : (pos >= n_pos ? n_pos - 1 : pos);
+  if constexpr (ROLL) {
+    slot %= L;
+    if (slot < 0) slot += L;
+  } else {
+    slot = slot < 0 ? 0 : (slot >= L ? L - 1 : slot);
+  }
   q += b * q_sb + w * q_ss;
   k += b * k_sb + w * k_ss;
   v += b * v_sb + w * v_ss;
@@ -319,17 +334,22 @@ __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16
 }  // namespace
 
 void decode_rope_kv(const void* q, const void* k, const void* v, const long* positions, const long* depth, const float* cos_t,
-                    const float* sin_t, void* q_out, void* kc, void* vc, int B, int W, int H, int Hkv, int D, int L, const long* qs,
-                    const long* ks, const long* vs, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3, float k_inv,
-                    float v_inv) {
+                    const float* sin_t, void* q_out, void* kc, void* vc, int B, int W, int H, int Hkv, int D, int L, int n_pos,
+                    const long* qs, const long* ks, const long* vs, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3,
+                    float k_inv, float v_inv, bool rolling) {
   const int rows = B * W * (H + 2 * Hkv);
   const int grid = (rows * 32 + 127) / 128;
-#define NXD_ROPE_KV(T)                                                                                                          \
-  decode_rope_kv_kernel<T><<<grid, 128, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v,      \
-      positions, depth, cos_t, sin_t, (__nv_bfloat16*)q_out, (T*)kc, (T*)vc, B, W, H, Hkv, D, L, qs[0], qs[1], qs[2], ks[0], ks[1], \
-      ks[2], vs[0], vs[1], vs[2], c_sb, c_ss, c_sh, k_inv, v_inv)
-  if (kv_e4m3) NXD_ROPE_KV(__nv_fp8_e4m3);
-  else NXD_ROPE_KV(__nv_bfloat16);
+#define NXD_ROPE_KV(T, R)                                                                                                     \
+  decode_rope_kv_kernel<T, R><<<grid, 128, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, \
+      positions, depth, cos_t, sin_t, (__nv_bfloat16*)q_out, (T*)kc, (T*)vc, B, W, H, Hkv, D, L, n_pos, qs[0], qs[1], qs[2],   \
+      ks[0], ks[1], ks[2], vs[0], vs[1], vs[2], c_sb, c_ss, c_sh, k_inv, v_inv)
+  if (kv_e4m3) {
+    if (rolling) NXD_ROPE_KV(__nv_fp8_e4m3, true);
+    else NXD_ROPE_KV(__nv_fp8_e4m3, false);
+  } else {
+    if (rolling) NXD_ROPE_KV(__nv_bfloat16, true);
+    else NXD_ROPE_KV(__nv_bfloat16, false);
+  }
 #undef NXD_ROPE_KV
   NXD_CUDA_CHECK(cudaGetLastError());
 }
@@ -337,24 +357,28 @@ void decode_rope_kv(const void* q, const void* k, const void* v, const long* pos
 void decode_attention(const void* q, const void* k, const void* v, const long* positions, void* out, float* part_o,
                       float* part_ml, int B, int H, int Hkv, int L, const long* ks, const long* vs, long q_sb, long q_sh,
                       long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o, float* fin_ml,
-                      bool kv_e4m3, float k_scale, float v_scale) {
+                      bool kv_e4m3, float k_scale, float v_scale, bool rolling) {
   const int G = H / Hkv;
   dim3 grid(Hkv, B, splits);
   const float sl2 = scale * 1.4426950408889634f * k_scale;
-#define NXD_DEC(T, Gv)                                                                                                 \
-  decode_attn_kernel<T, Gv><<<grid, kDecThreads, 0, st>>>((const __nv_bfloat16*)q, (const T*)k, (const T*)v, positions, \
+#define NXD_DEC(T, Gv, R)                                                                                                 \
+  decode_attn_kernel<T, Gv, R><<<grid, kDecThreads, 0, st>>>((const __nv_bfloat16*)q, (const T*)k, (const T*)v, positions, \
       part_o, part_ml, B, H, Hkv, L, ks[0], ks[1], ks[2], vs[0], vs[1], vs[2], q_sb, q_sh, sl2, splits, window, v_scale)
+#define NXD_DEC_R(T, Gv)             \
+  if (rolling) NXD_DEC(T, Gv, true); \
+  else NXD_DEC(T, Gv, false)
 #define NXD_DEC_G(T)                                                                      \
   switch (G) {                                                                            \
-    case 1: NXD_DEC(T, 1); break;                                                         \
-    case 2: NXD_DEC(T, 2); break;                                                         \
-    case 4: NXD_DEC(T, 4); break;                                                         \
-    case 8: NXD_DEC(T, 8); break;                                                         \
+    case 1: NXD_DEC_R(T, 1); break;                                                       \
+    case 2: NXD_DEC_R(T, 2); break;                                                       \
+    case 4: NXD_DEC_R(T, 4); break;                                                       \
+    case 8: NXD_DEC_R(T, 8); break;                                                       \
     default: nxd_throw("decode_attention: unsupported GQA group size", __FILE__, __LINE__); \
   }
   if (kv_e4m3) NXD_DEC_G(__nv_fp8_e4m3)
   else NXD_DEC_G(__nv_bfloat16)
 #undef NXD_DEC_G
+#undef NXD_DEC_R
 #undef NXD_DEC
   if (fin_o != nullptr) decode_combine_partial_kernel<<<B * H, HD, 0, st>>>(part_o, part_ml, fin_o, fin_ml, splits);
   else decode_combine_kernel<<<B * H, HD, 0, st>>>(part_o, part_ml, (__nv_bfloat16*)out, splits, o_sb, o_sh, H);

@@ -133,16 +133,17 @@ void gemv_mx_grouped(const void* x, const void* w, const void* scale, const long
 void decode_attention(const void* q, const void* k, const void* v, const long* positions, void* out, float* part_o,
                       float* part_ml, int B, int H, int Hkv, int L, const long* ks, const long* vs, long q_sb, long q_sh,
                       long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o,
-                      float* fin_ml, bool kv_e4m3, float k_scale, float v_scale);
+                      float* fin_ml, bool kv_e4m3, float k_scale, float v_scale, bool rolling = false);
                       // fin_o/fin_ml: un-normalised [B*H,128] + (max, sum) [B*H,2] instead of ``out`` (nullptr: ``out``)
                       // window: keys positions[b] − window < j ≤ positions[b] visible (0: no window)
                       // kv_e4m3: k/v are fp8 e4m3 caches holding k / k_scale and v / v_scale (bf16: both scales 1)
-// q/k/v [B,W,·,D] (strides qs/ks/vs = (b, s, h)); token w is rotated at positions[b] + depth[w] (depth null: + w) and written to
-// slot positions[b] + w, both clamped to [0, L)
+                      // rolling: the cache is a ring of L rows, position j in row j mod L (needs 0 < window < L)
+// q/k/v [B,W,·,D] (strides qs/ks/vs = (b, s, h)); token w is rotated at positions[b] + depth[w] (depth null: + w), clamped to
+// [0, n_pos) (n_pos: rows of cos_t / sin_t), and written to slot positions[b] + w, clamped to [0, L) (rolling: mod L)
 void decode_rope_kv(const void* q, const void* k, const void* v, const long* positions, const long* depth, const float* cos_t,
-                    const float* sin_t, void* q_out, void* kc, void* vc, int B, int W, int H, int Hkv, int D, int L, const long* qs,
-                    const long* ks, const long* vs, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3, float k_inv,
-                    float v_inv);   // kv_e4m3: the cache stores k·k_inv and v·v_inv as e4m3 (bf16: rows as computed)
+                    const float* sin_t, void* q_out, void* kc, void* vc, int B, int W, int H, int Hkv, int D, int L, int n_pos,
+                    const long* qs, const long* ks, const long* vs, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3,
+                    float k_inv, float v_inv, bool rolling);   // kv_e4m3: the cache stores k·k_inv and v·v_inv as e4m3
 // merge of per-split decode partials [rows·splits, 128] + (max, sum) → bf16 row r at out + (r / H)·o_sb + (r % H)·o_sh
 void decode_combine(const float* part_o, const float* part_ml, void* out, int rows, int splits, long o_sb, long o_sh, int H,
                     cudaStream_t st);
@@ -166,9 +167,10 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
 // W ≤ 64 new tokens per sequence against a KV cache (speculation / Medusa verification): q [B,W,H,128] bf16, k/v caches
 // [B,L,Hkv,128] bf16 or e4m3 (kv_e4m3), H/Hkv ∈ {1,2,4,8}; mask uint8 [W,W] and depth int64 [W] (both null: a chain);
 // window: sliding window (0: none).  part_o [B·W·H·splits, 128] / part_ml [B·W·H·splits, 2] fp32 scratch; out [B,W,H,128].
+// rolling: the cache is a ring of L rows, position j in row j mod L (needs window > 0 and window + W − 1 ≤ L).
 void speculation_attention(const void* q, const void* k, const void* v, const long* positions, const void* mask,
                            const long* depth, void* out, float* part_o, float* part_ml, int B, int W, int H, int Hkv, int L,
                            const long* qs, const long* ks, const long* vs, float scale, int window, int splits, bool kv_e4m3,
-                           float k_scale, float v_scale, cudaStream_t st);
+                           float k_scale, float v_scale, bool rolling, cudaStream_t st);
 
 }  // namespace nxd

@@ -9,6 +9,9 @@ reference's ``examples/inference/run_llama.py`` / ``runner.py`` (trace → load 
   # KV cache stored in fp8 e4m3 (one scale per tensor): half the cache bytes, read directly by the decode kernels
   torchrun --nproc-per-node 1 examples/inference/run_llama.py --model 7b --batch_size 16 --max_prompt_length 2048 \
       --sequence_length 4096 --benchmark --kv_cache_quant fp8
+  # Mistral-7B geometry (sliding window 4096): a rolling KV cache keeps 4096 + 64 rows per sequence instead of 8192
+  torchrun --nproc-per-node 1 examples/inference/run_llama.py --model mistral-7b --batch_size 16 --max_prompt_length 2048 \
+      --sequence_length 8192 --benchmark --num_runs 1 --rolling_kv_cache
 """
 import argparse
 import json
@@ -32,9 +35,15 @@ from neuronx_distributed_b200.quantization import KVQuantizationConfig  # noqa: 
 from training_utils import init_distributed  # noqa: E402
 
 
+def mistral_7b_config(**kw) -> LlamaConfig:
+    """Mistral-7B geometry: GQA with 8 KV heads and a 4096-token sliding window."""
+    return LlamaConfig(vocab_size=32000, hidden_size=4096, intermediate_size=14336, num_hidden_layers=32, num_attention_heads=32,
+                       num_key_value_heads=8, sliding_window=4096, **kw)
+
+
 def main():
     p = argparse.ArgumentParser()
-    p.add_argument("--model", default="tiny", choices=["tiny", "7b", "13b"])
+    p.add_argument("--model", default="tiny", choices=["tiny", "7b", "13b", "mistral-7b"])
     p.add_argument("--tp_degree", type=int, default=1)
     p.add_argument("--batch_size", type=int, default=1)
     p.add_argument("--max_prompt_length", type=int, default=128)
@@ -49,12 +58,16 @@ def main():
     p.add_argument("--kv_cache_quant", default="none", choices=["none", "fp8"],
                    help="fp8: store the KV cache in float8 e4m3 with one scale per tensor (--kv_cache_scale)")
     p.add_argument("--kv_cache_scale", type=float, default=1.0, help="the cache stores k / scale and v / scale")
+    p.add_argument("--rolling_kv_cache", action="store_true",
+                   help="sliding-window models: keep only the last window + 64 positions of each sequence in a ring")
+    p.add_argument("--max_new_tokens", type=int, default=0,
+                   help="tokens generated per sequence (default: fill the sequence); the cache size is set by --sequence_length")
     a = p.parse_args()
     dev = init_distributed()
     ps.initialize_model_parallel(tensor_model_parallel_size=a.tp_degree)
     dtype = torch.bfloat16 if dev.type == "cuda" else torch.float32
     kw = dict(dtype=dtype, device=dev, max_position_embeddings=a.sequence_length)
-    cfg = {"7b": llama2_7b_config, "13b": llama2_13b_config}.get(a.model, lambda **k: LlamaConfig(
+    cfg = {"7b": llama2_7b_config, "13b": llama2_13b_config, "mistral-7b": mistral_7b_config}.get(a.model, lambda **k: LlamaConfig(
         vocab_size=4096, hidden_size=512, intermediate_size=1408, num_hidden_layers=4, num_attention_heads=8, **k))(**kw)
     if a.num_layers > 0:
         cfg.num_hidden_layers = a.num_layers
@@ -65,7 +78,7 @@ def main():
     if a.kv_cache_quant == "fp8":
         kv_quant = KVQuantizationConfig(quant_dtype=torch.float8_e4m3fn, dequant_dtype=dtype, scale=a.kv_cache_scale)
     model = LlamaForInference(cfg, batch_size=a.batch_size, max_seq_len=a.sequence_length,
-                              flash_decoding=a.flash_decoding, kv_quant=kv_quant).eval()
+                              flash_decoding=a.flash_decoding, kv_quant=kv_quant, rolling_kv_cache=a.rolling_kv_cache).eval()
     B, P = a.batch_size, a.max_prompt_length
     mb = ModelBuilder(tp_degree=a.tp_degree, use_cuda_graphs=(dev.type == "cuda" and not a.no_cuda_graphs))
     for bucket in generate_buckets(min(128, P), P):
@@ -77,7 +90,7 @@ def main():
            step_fn=lambda m, i, pos: m.token_generation(i, pos))
     nxd_model = mb.trace()
     prompt = torch.randint(0, cfg.vocab_size, (B, P), device=dev)
-    new_tokens = a.sequence_length - P
+    new_tokens = min(a.max_new_tokens, a.sequence_length - P) if a.max_new_tokens > 0 else a.sequence_length - P
 
     def generate():
         tok = nxd_model(prompt, torch.full((B,), P - 1, dtype=torch.long, device=dev)).clone()
@@ -99,6 +112,7 @@ def main():
         if dev.type == "cuda":
             rep["peak_allocated_GiB"] = torch.cuda.max_memory_allocated(dev) / 2 ** 30
             rep["kv_cache_GiB"] = sum(t.nbytes for t in model.kv.k + model.kv.v) / 2 ** 30
+            rep["kv_cache_rows"], rep["kv_cache_rolling"] = model.kv.rows, model.kv.rolling
         if dist.get_rank() == 0:
             print(json.dumps({"e2e_model": rep, "config": vars(a)}), flush=True)
     dist.barrier()

@@ -1,13 +1,21 @@
 """KV-cache manager (role of reference ``examples/inference/modules/kvcache/kv_cache_manager.py:60-199``):
 persistent per-layer K/V buffers ``[B, S_max, H_kv_local, D]`` allocated once (CUDA-graph safe), prefill writes a
 whole prompt, decode scatters one position per sequence; optional fp8 storage (``KVQuantizationConfig``) and
-flash-decoding layout where the sequence axis is additionally sharded inside a KV-replica group."""
+flash-decoding layout where the sequence axis is additionally sharded inside a KV-replica group.
+
+Rolling mode (``rolling_window`` = the model's sliding window SW): the cache keeps R = min(max_seq_len, SW + 64) rows and
+logical position t lives in row t mod R.  64 is ``ops.attention.SPEC_MAX_TOKENS``: a verification window of W ≤ 64 tokens
+at position p writes row (p + w) mod R over position p + w − R ≤ p − SW, and no token of the window sees a position
+≤ p − SW (each sees committed positions > p + d − SW ≥ p − SW), so R ≥ SW + W − 1 keeps every visible position in the
+ring.  Positions stay bounded by max_seq_len (the RoPE tables).  When R == max_seq_len the layout is the linear one and
+the cache is not rolling.  This class is the only place that maps positions to rows."""
 from __future__ import annotations
 
 from typing import List, Optional, Tuple
 
 import torch
 
+from ..ops.attention import SPEC_MAX_TOKENS
 from ..quantization.quantization_config import KVQuantizationConfig, QuantizationType
 
 
@@ -20,13 +28,22 @@ def per_tensor(kv_quant: KVQuantizationConfig) -> bool:
 class KVCacheManager:
     def __init__(self, num_layers: int, batch_size: int, max_seq_len: int, num_kv_heads_local: int, head_dim: int,
                  dtype: torch.dtype = torch.bfloat16, device=None, kv_quant: Optional[KVQuantizationConfig] = None,
-                 num_cores_per_group: int = 1):
+                 num_cores_per_group: int = 1, rolling_window: Optional[int] = None):
+        """``rolling_window``: keep a ring of ``min(max_seq_len, rolling_window + 64)`` rows (module docstring); ``rolling``
+        is True when that is shorter than ``max_seq_len``, and ``rows`` is the row count either way."""
         self.num_layers, self.batch_size, self.max_seq_len = num_layers, batch_size, max_seq_len
         self.kv_quant = kv_quant
         self.seq_shards = num_cores_per_group
         store = kv_quant.quant_dtype if kv_quant is not None else dtype
         self.dtype = dtype
         s_local = max_seq_len // num_cores_per_group
+        if rolling_window is not None:
+            if int(rolling_window) < 1 or num_cores_per_group != 1:
+                raise ValueError(f"rolling_window must be >= 1 on an unsharded cache, got {rolling_window} with "
+                                 f"{num_cores_per_group} sequence shards")
+            s_local = min(max_seq_len, int(rolling_window) + SPEC_MAX_TOKENS)
+        self.rows = s_local
+        self.rolling = rolling_window is not None and s_local < max_seq_len
         shape = (batch_size, s_local, num_kv_heads_local, head_dim)
         self.k: List[torch.Tensor] = [torch.zeros(shape, dtype=store, device=device) for _ in range(num_layers)]
         self.v: List[torch.Tensor] = [torch.zeros(shape, dtype=store, device=device) for _ in range(num_layers)]
@@ -41,9 +58,35 @@ class KVCacheManager:
             return x
         return (x.float() * self.kv_quant.scale).to(self.kv_quant.dequant_dtype)
 
-    def write_prefill(self, layer: int, k: torch.Tensor, v: torch.Tensor, seq_ids: Optional[torch.Tensor] = None) -> None:
-        """k/v ``[B, S, H, D]`` → cache rows ``seq_ids`` (default 0..B-1), positions 0..S-1."""
+    def _row(self, positions: torch.Tensor) -> torch.Tensor:
+        """Cache row of each position (the identity unless rolling)."""
+        return positions % self.rows if self.rolling else positions
+
+    def _ring(self, cache: torch.Tensor, x: torch.Tensor, lengths: Optional[torch.Tensor]) -> torch.Tensor:
+        """Rolling prefill of ``cache [B, R, H, D]`` from ``x [B, S, H, D]``: ring row j of sequence b takes the newest prompt
+        position t < lengths[b] (default S) with t ≡ j (mod R) and keeps its content when there is none.  One gather of
+        static shape, no host sync: right-padding past a prompt never reaches the ring."""
+        B, S = x.shape[:2]
+        R = self.rows
+        last = (torch.full((B,), S, device=x.device, dtype=torch.long) if lengths is None
+                else lengths.to(x.device, torch.long)).clamp(max=S)[:, None] - 1
+        t = last - (last - torch.arange(R, device=x.device)[None, :]) % R          # [B, R]
+        src = self._q(x.gather(1, t.clamp(min=0)[:, :, None, None].expand(B, R, *x.shape[2:])))
+        keep = (t < 0)[:, :, None, None]
+        if src.element_size() == 1:                                                 # where() has no fp8 kernels
+            return torch.where(keep, cache.view(torch.uint8), src.view(torch.uint8)).view(cache.dtype)
+        return torch.where(keep, cache, src)
+
+    def write_prefill(self, layer: int, k: torch.Tensor, v: torch.Tensor, seq_ids: Optional[torch.Tensor] = None,
+                      lengths: Optional[torch.Tensor] = None) -> None:
+        """k/v ``[B, S, H, D]`` → cache rows ``seq_ids`` (default 0..B-1), positions 0..S-1.  ``lengths`` ``[B]``: the
+        prompt lengths (the rest is right-padding); only a rolling cache uses them (:meth:`_ring`)."""
         S = k.shape[1]
+        if self.rolling:
+            rows = slice(0, k.shape[0]) if seq_ids is None else seq_ids
+            for cache, x in ((self.k[layer], k), (self.v[layer], v)):
+                cache[rows] = self._ring(cache[rows], x, lengths)
+            return
         if seq_ids is None:
             self.k[layer][: k.shape[0], :S].copy_(self._q(k))
             self.v[layer][: v.shape[0], :S].copy_(self._q(v))
@@ -54,6 +97,7 @@ class KVCacheManager:
     def write_prefill_sharded(self, layer: int, k: torch.Tensor, v: torch.Tensor, shard_rank: int) -> None:
         """Flash-decoding layout: this rank keeps prompt positions ``[shard_rank·L_local, (shard_rank+1)·L_local)`` of the
         k/v ``[B, S, H, D]`` every member of the KV-replica group computed (reference ``kv_cache_manager.py:60-88``)."""
+        self._not_rolling("write_prefill_sharded")
         l_local = self.k[layer].shape[1]
         lo = shard_rank * l_local
         hi = min(k.shape[1], lo + l_local)
@@ -67,19 +111,25 @@ class KVCacheManager:
         shard holds each position."""
         from ..modules.attention.flash_decode import write_decode_sharded
 
+        self._not_rolling("write_decode_sharded")
         write_decode_sharded(self.k[layer], self.v[layer], self._q(k), self._q(v), positions, shard_rank)
+
+    def _not_rolling(self, name: str) -> None:
+        if self.rolling:
+            raise ValueError(f"KVCacheManager.{name}: the flash-decoding layout does not take a rolling cache")
 
     def write_decode(self, layer: int, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor) -> None:
         """k/v ``[B, 1, H, D]``; ``positions`` ``[B]`` (device tensor; no host sync → graph capturable)."""
         b = torch.arange(k.shape[0], device=k.device)
-        self.k[layer].index_put_((b, positions), self._q(k[:, 0]))
-        self.v[layer].index_put_((b, positions), self._q(v[:, 0]))
+        self.k[layer].index_put_((b, self._row(positions)), self._q(k[:, 0]))
+        self.v[layer].index_put_((b, self._row(positions)), self._q(v[:, 0]))
 
     def write_window(self, layer: int, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor) -> None:
         """k/v ``[B, W, H, D]`` written at positions ``positions[b] + 0..W-1`` (speculative verification / chunked prefill)."""
         B, W = k.shape[0], k.shape[1]
         b = torch.arange(B, device=k.device).unsqueeze(1).expand(B, W)
-        pos = (positions.unsqueeze(1) + torch.arange(W, device=k.device).unsqueeze(0)).clamp(max=self.k[layer].shape[1] - 1)
+        pos = positions.unsqueeze(1) + torch.arange(W, device=k.device).unsqueeze(0)
+        pos = self._row(pos) if self.rolling else pos.clamp(max=self.k[layer].shape[1] - 1)
         self.k[layer].index_put_((b, pos), self._q(k))
         self.v[layer].index_put_((b, pos), self._q(v))
 
@@ -88,8 +138,8 @@ class KVCacheManager:
         ``positions[b] + i`` for every layer, so the accepted path becomes a contiguous continuation of the sequence."""
         B, n = src_offsets.shape
         b = torch.arange(B, device=positions.device).unsqueeze(1).expand(B, n)
-        src = positions.unsqueeze(1) + src_offsets
-        dst = positions.unsqueeze(1) + torch.arange(n, device=positions.device).unsqueeze(0)
+        src = self._row(positions.unsqueeze(1) + src_offsets)
+        dst = self._row(positions.unsqueeze(1) + torch.arange(n, device=positions.device).unsqueeze(0))
         for layer in range(self.num_layers):
             self.k[layer].index_put_((b, dst), self.k[layer][b, src])
             self.v[layer].index_put_((b, dst), self.v[layer][b, src])
@@ -108,8 +158,11 @@ class KVCacheManager:
         return None
 
     def stored(self, layer: int, length: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
-        """The cache tensors of ``layer`` as stored (fp8 when quantised), positions ``[0, length)``."""
+        """The cache tensors of ``layer`` as stored (fp8 when quantised), positions ``[0, length)`` (a rolling cache has no
+        prefix of positions: ``length`` must be None)."""
         k, v = self.k[layer], self.v[layer]
+        if length is not None and self.rolling:
+            raise ValueError("KVCacheManager.stored: a rolling cache has no prefix of positions; pass length=None")
         if length is not None:
             k, v = k[:, :length], v[:, :length]
         return k, v

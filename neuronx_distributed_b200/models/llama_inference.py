@@ -20,12 +20,19 @@ from .llama import LlamaConfig, LlamaForCausalLM
 class LlamaForInference(nn.Module):
     def __init__(self, cfg: LlamaConfig, batch_size: int = 1, max_seq_len: int = 2048, on_device_sampling: bool = True,
                  sampler: Optional[Sampler] = None, lm_cls=None, flash_decoding: bool = False,
-                 kv_quant: Optional[KVQuantizationConfig] = None):
+                 kv_quant: Optional[KVQuantizationConfig] = None, rolling_kv_cache: bool = False):
         """``lm_cls``: any decoder built from Llama attention blocks (``LlamaForCausalLM`` default; ``MixtralForCausalLM`` for
         the MoE families — its layers' ``mlp`` returns ``(y, router_logits)``, handled in ``_body``).
         ``kv_quant``: store the KV cache quantised, with one scale per tensor (fp8 e4m3 is read by the decode kernels
-        directly).  Prefill attention runs on the un-quantised k/v it computes; only the cache write is quantised."""
+        directly).  Prefill attention runs on the un-quantised k/v it computes; only the cache write is quantised.
+        ``rolling_kv_cache`` (needs ``cfg.sliding_window``): keep only the last ``sliding_window + 64`` positions of each
+        sequence in a ring (``inference.kv_cache``), so cache memory no longer grows with ``max_seq_len``.  The model then
+        computes what it computes on the full cache; ``kv_len`` must be None."""
         super().__init__()
+        if rolling_kv_cache and cfg.sliding_window is None:
+            raise ValueError("rolling_kv_cache needs a model with a sliding window (cfg.sliding_window)")
+        if rolling_kv_cache and flash_decoding:
+            raise ValueError("rolling_kv_cache does not combine with flash_decoding")
         cfg.sequence_parallel_enabled = False
         cfg.activation_checkpointing = "none"
         self.cfg = cfg
@@ -50,7 +57,8 @@ class LlamaForInference(nn.Module):
             raise ValueError(f"kv_quant.dequant_dtype ({kv_quant.dequant_dtype}) must be the model dtype ({cfg.dtype}): "
                              "attention off the kernels reads the de-quantised cache next to the model's queries")
         self.kv = KVCacheManager(cfg.num_hidden_layers, batch_size, max_seq_len, attn0.num_kv_heads_local, cfg.head_dim,
-                                 dtype=cfg.dtype, device=cfg.device, kv_quant=kv_quant, num_cores_per_group=shards)
+                                 dtype=cfg.dtype, device=cfg.device, kv_quant=kv_quant, num_cores_per_group=shards,
+                                 rolling_window=cfg.sliding_window if rolling_kv_cache else None)
         self.sampler = sampler or Sampler(top_k=1, vocab_parallel=True)
         self.on_device_sampling = on_device_sampling
         cos, sin = ops.rope.rope_tables(max_seq_len, cfg.head_dim, cfg.rope_theta, cfg.device, 0, cfg.rope_scaling_factor)
@@ -69,9 +77,10 @@ class LlamaForInference(nn.Module):
 
     # ------------------------------------------------------------------ shared pieces
     def _attn_block(self, layer_idx: int, layer, x: torch.Tensor, positions: Optional[torch.Tensor], prefill: bool,
-                    kv_len: Optional[int], tree=None) -> torch.Tensor:
+                    kv_len: Optional[int], tree=None, prompt_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
         att = layer.self_attn
         sw = self.cfg.sliding_window                       # Mistral / Mixtral window (None: full causal attention)
+        roll = {"rolling": True} if self.kv.rolling else {}   # ring cache: the kernels and torch paths map positions to rows
         h = layer.input_layernorm(x)
         q, k, v = att.qkv_proj(h)                          # [S, B, h*D]
         S, B = q.shape[0], q.shape[1]
@@ -104,9 +113,9 @@ class LlamaForInference(nn.Module):
             if fused:
                 ops._ext.count_launch()
                 q = ops._ext.ext().decode_rope_kv(q, k, v, positions.to(torch.long).contiguous(), self.rope_cos, self.rope_sin,
-                                                  self.kv.k[layer_idx], self.kv.v[layer_idx], depth=depth, **scale_kw)
+                                                  self.kv.k[layer_idx], self.kv.v[layer_idx], depth=depth, **scale_kw, **roll)
                 kc, vc = self.kv.stored(layer_idx, kv_len)
-                o = ops.attention.speculation_attention(q, kc, vc, positions, tree_mask, depth, sw, **scale_kw)
+                o = ops.attention.speculation_attention(q, kc, vc, positions, tree_mask, depth, sw, **scale_kw, **roll)
             else:
                 d = torch.arange(S, device=q.device) if depth is None else depth
                 idx = (positions.unsqueeze(1) + d.unsqueeze(0)).clamp(max=self.max_seq_len - 1)
@@ -114,21 +123,21 @@ class LlamaForInference(nn.Module):
                 q, k = _rope_window(q, cos, sin), _rope_window(k, cos, sin)
                 self.kv.write_window(layer_idx, k, v, positions)
                 kc, vc = self.kv.get(layer_idx, kv_len)
-                o = ops.attention.speculation_attention_torch(q, kc, vc, positions, tree_mask, depth, sw)
+                o = ops.attention.speculation_attention_torch(q, kc, vc, positions, tree_mask, depth, sw, **roll)
         elif prefill:
             cos, sin = self.rope_cos[:S], self.rope_sin[:S]
             q, k = ops.rope.apply_rotary(q, cos, sin), ops.rope.apply_rotary(k, cos, sin)
             if self.flash_decoding:
                 self.kv.write_prefill_sharded(layer_idx, k, v, self.kv_rank)
             else:
-                self.kv.write_prefill(layer_idx, k, v)
+                self.kv.write_prefill(layer_idx, k, v, lengths=prompt_lens)
             o = ops.attention.flash_attention(q, k, v, causal=True, sliding_window=sw)
         elif fused:
             ops._ext.count_launch()
             q = ops._ext.ext().decode_rope_kv(q, k, v, positions.to(torch.long).contiguous(), self.rope_cos, self.rope_sin,
-                                              self.kv.k[layer_idx], self.kv.v[layer_idx], **scale_kw)
+                                              self.kv.k[layer_idx], self.kv.v[layer_idx], **scale_kw, **roll)
             kc, vc = self.kv.stored(layer_idx, kv_len)
-            o = _decode_attention(q, kc, vc, positions, sw, **scale_kw)
+            o = _decode_attention(q, kc, vc, positions, sw, **scale_kw, **roll)
         else:
             # one new token per sequence at its own position
             cos = self.rope_cos[positions].unsqueeze(1)     # [B, 1, D/2] → per-batch tables
@@ -136,7 +145,7 @@ class LlamaForInference(nn.Module):
             q, k = _rope_per_batch(q, cos, sin), _rope_per_batch(k, cos, sin)
             self.kv.write_decode(layer_idx, k, v, positions)
             kc, vc = self.kv.get(layer_idx, kv_len)
-            o = _decode_attention(q, kc, vc, positions, sw)
+            o = _decode_attention(q, kc, vc, positions, sw, **roll)
         o = o.transpose(0, 1).reshape(S, B, att.num_heads_local * D)
         return _row_linear_plus_residual(att.o_proj, o, x)
 
@@ -153,11 +162,14 @@ class LlamaForInference(nn.Module):
                                             tensor_model_parallel_group=getattr(mlp, "tensor_parallel_group", None)).eval()
         return blocks[layer_idx]
 
-    def _body(self, input_ids: torch.Tensor, positions: Optional[torch.Tensor], prefill: bool, kv_len: Optional[int], tree=None):
+    def _body(self, input_ids: torch.Tensor, positions: Optional[torch.Tensor], prefill: bool, kv_len: Optional[int], tree=None,
+              prompt_lens: Optional[torch.Tensor] = None):
+        if kv_len is not None and self.kv.rolling:
+            raise ValueError("kv_len must be None with a rolling KV cache: a prefix of a ring holds no prefix of positions")
         core = self._core
         x = core.embed_tokens(input_ids).transpose(0, 1).contiguous()               # [S, B, H]
         for i, layer in enumerate(core.layers):
-            x = self._attn_block(i, layer, x, positions, prefill, kv_len, tree)
+            x = self._attn_block(i, layer, x, positions, prefill, kv_len, tree, prompt_lens)
             mlp = layer.mlp
             if hasattr(mlp, "gate_up_proj") and hasattr(mlp, "down_proj") and not prefill and x.shape[0] * x.shape[1] <= 8:
                 # dense decode MLP: the residual add rides in the down-projection's GEMV(+all-reduce) epilogue
@@ -179,7 +191,8 @@ class LlamaForInference(nn.Module):
     @torch.no_grad()
     def context_encoding(self, input_ids: torch.Tensor, last_token_index: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``input_ids`` [B, S_bucket] (right-padded) → next token ids [B] (or vocab-parallel logits)."""
-        h = self._body(input_ids, None, True, None)                              # [S, B, H]
+        lens = None if last_token_index is None else last_token_index + 1        # a rolling cache keeps no right-padding
+        h = self._body(input_ids, None, True, None, prompt_lens=lens)            # [S, B, H]
         B = input_ids.shape[0]
         if last_token_index is None:
             last = h[-1]
@@ -264,11 +277,14 @@ def _rope_window(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch
 
 
 def _decode_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor,
-                      sliding_window: Optional[int] = None, k_scale: float = 1.0, v_scale: float = 1.0) -> torch.Tensor:
+                      sliding_window: Optional[int] = None, k_scale: float = 1.0, v_scale: float = 1.0,
+                      rolling: bool = False) -> torch.Tensor:
     """q [B,1,H,D] vs cache k/v [B,L,Hkv,D]; keys beyond each sequence's position (and, with ``sliding_window`` SW, keys at or
-    before position − SW) are masked.  An fp8 cache holds k / ``k_scale`` and v / ``v_scale``."""
-    if k.dtype in ops.attention.FP8_KV_DTYPES:
-        return ops.attention.decode_attention(q, k, v, positions, sliding_window=sliding_window, k_scale=k_scale, v_scale=v_scale)
+    before position − SW) are masked.  An fp8 cache holds k / ``k_scale`` and v / ``v_scale``; ``rolling``: a ring cache
+    (``ops.attention.decode_attention``)."""
+    if k.dtype in ops.attention.FP8_KV_DTYPES or rolling:
+        return ops.attention.decode_attention(q, k, v, positions, sliding_window=sliding_window, k_scale=k_scale, v_scale=v_scale,
+                                              rolling=rolling)
     window = ops.attention.check_window(sliding_window)
     B, _, H, D = q.shape
     Hkv, L = k.shape[2], k.shape[1]

@@ -193,19 +193,37 @@ def check_kv_scales(k_cache: torch.Tensor, v_cache: torch.Tensor, k_scale: float
     return {"k_scale": float(k_scale), "v_scale": float(v_scale)}
 
 
+def check_rolling(name: str, rolling: bool, window: int, length: int, W: Optional[int] = None) -> None:
+    """A rolling cache of L = ``length`` rows (position t in row t mod L) needs a sliding window: 0 < window < L for one
+    token per sequence (``W`` None), window + W − 1 ≤ L for W verified tokens.  Token w of a window writes row (p + w) mod L
+    over position p + w − L, which must be invisible to every token of the window, and each sees only positions
+    > p − window.  Raises ``ValueError``."""
+    if not rolling:
+        return
+    if W is None and not 0 < window < length:
+        raise ValueError(f"{name}: a rolling cache of {length} rows needs 0 < sliding_window < {length}, got {window or None}")
+    if W is not None and not (window > 0 and window + W - 1 <= length):
+        raise ValueError(f"{name}: a rolling cache of {length} rows needs a sliding_window with sliding_window + W - 1 <= "
+                         f"{length} for W = {W} tokens, got {window or None}")
+
+
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, positions: torch.Tensor,
                      scale: Optional[float] = None, sliding_window: Optional[int] = None, k_scale: float = 1.0,
-                     v_scale: float = 1.0) -> torch.Tensor:
+                     v_scale: float = 1.0, rolling: bool = False) -> torch.Tensor:
     """One new token per sequence against a KV cache: ``q [B,1,H,D]``, caches ``[B,L,Hkv,D]`` (any batch / sequence / head
     strides), ``positions [B]`` = cache index of the newest token (keys ≤ position are visible; with ``sliding_window`` W only
     keys position − W < j ≤ position, and the kernel reads only those rows).  An fp8 cache holds k / ``k_scale`` and
-    v / ``v_scale`` (one scale per tensor, as ``inference.kv_cache.KVCacheManager`` stores it).  CUDA bf16 q with a bf16 or
-    fp8 e4m3 cache and head_dim 128: the split-KV flash-decoding kernel (``csrc/decode.cu``), which reads the e4m3 bytes
-    directly; otherwise SDPA with a length mask on the de-quantised cache."""
+    v / ``v_scale`` (one scale per tensor, as ``inference.kv_cache.KVCacheManager`` stores it).  ``rolling``: the cache is a
+    ring of L rows holding position j in row j mod L (``KVCacheManager`` in rolling mode); needs 0 < W < L.  CUDA bf16 q
+    with a bf16 or fp8 e4m3 cache and head_dim 128: the split-KV flash-decoding kernel (``csrc/decode.cu``), which reads the
+    e4m3 bytes directly; otherwise SDPA with a length mask on the de-quantised cache."""
     B, _, H, D = q.shape
     Hkv, L = k_cache.shape[2], k_cache.shape[1]
     window = check_window(sliding_window)
+    check_rolling("decode_attention", rolling, window, L)
     kw = check_kv_scales(k_cache, v_cache, k_scale, v_scale)
+    if rolling:
+        kw["rolling"] = True
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     e = _ext.ext() if q.is_cuda else None
     if (e is not None and hasattr(e, "decode_attention") and D == 128 and q.dtype == torch.bfloat16
@@ -219,7 +237,7 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     qt, kt, vt = q.transpose(1, 2), k_cache.transpose(1, 2), v_cache.transpose(1, 2)
     if H != Hkv:
         kt, vt = kt.repeat_interleave(H // Hkv, 1), vt.repeat_interleave(H // Hkv, 1)
-    mask = decode_visibility(positions, L, window)[:, None, None, :]
+    mask = decode_visibility(positions, L, window, rolling)[:, None, None, :]
     return torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask, scale=scale).transpose(1, 2)
 
 
@@ -227,7 +245,7 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
 SPEC_MAX_TOKENS = 64
 
 
-def _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale):
+def _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale, rolling=False):
     """Argument checks of :func:`speculation_attention` → ``(window, scale kwargs)``; raises ``ValueError``."""
     if q.dim() != 4 or k_cache.dim() != 4 or v_cache.shape != k_cache.shape:
         raise ValueError(f"speculation_attention: expected q [B,W,H,D] and caches [B,L,Hkv,D], got {tuple(q.shape)}, "
@@ -240,23 +258,34 @@ def _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window,
     if tree_mask is not None and (tuple(tree_mask.shape) != (W, W) or tuple(tree_depth.shape) != (W,)):
         raise ValueError(f"speculation_attention: tree_mask must be [W, W] and tree_depth [W] for W = {W}, got "
                          f"{tuple(tree_mask.shape)} and {tuple(tree_depth.shape)}")
-    return check_window(sliding_window), check_kv_scales(k_cache, v_cache, k_scale, v_scale)
+    window = check_window(sliding_window)
+    check_rolling("speculation_attention", rolling, window, k_cache.shape[1], W)
+    return window, check_kv_scales(k_cache, v_cache, k_scale, v_scale)
 
 
 def speculation_visibility(positions: torch.Tensor, length: int, W: int, tree_mask: Optional[torch.Tensor] = None,
-                           tree_depth: Optional[torch.Tensor] = None, window: int = 0) -> torch.Tensor:
-    """``[B, W, length]`` bool: which cache slots each of W new tokens sees (the rule of :func:`speculation_attention`)."""
+                           tree_depth: Optional[torch.Tensor] = None, window: int = 0, rolling: bool = False) -> torch.Tensor:
+    """``[B, W, length]`` bool: which cache slots each of W new tokens sees (the rule of :func:`speculation_attention`).
+    ``rolling``: slot c is a row of a ring of ``length`` rows: window column (c − p) mod length when that is < W, else the
+    newest committed position p − 1 − ((p − 1 − c) mod length), which is seen only when ≥ 0."""
     dev = positions.device
     p = positions.long()[:, None]                                                          # [B, 1]
     d = torch.arange(W, device=dev) if tree_depth is None else tree_depth.to(dev).long()
     m = torch.ones(W, W, dtype=torch.bool, device=dev).tril() if tree_mask is None else tree_mask.to(dev).bool()
     c = torch.arange(length, device=dev)[None, :]                                          # [1, L]
-    u = c - p                                                                              # [B, L] window column of slot c
-    inside = (u >= 0) & (u < W)
+    if rolling:
+        u = (c - p) % length                                                               # [B, L] window column of slot c
+        inside = u < W
+        cpos = p - 1 - (p - 1 - c) % length                                                # committed position of slot c
+        committed = ~inside & (cpos >= 0)
+    else:
+        u = c - p
+        inside = (u >= 0) & (u < W)
+        cpos, committed = c, u < 0
     uc = u.clamp(0, W - 1)
-    vis = (u < 0)[:, None, :] | (inside[:, None, :] & m[:, uc].permute(1, 0, 2))          # [B, W, L]
+    vis = committed[:, None, :] | (inside[:, None, :] & m[:, uc].permute(1, 0, 2))        # [B, W, L]
     if window > 0:
-        kpos = torch.where(inside, p + d[uc], c)                                           # sequence position of slot c
+        kpos = torch.where(inside, p + d[uc], cpos)                                        # sequence position of slot c
         vis = vis & (kpos[:, None, :] > (p + d[None, :])[:, :, None] - window)
     return vis
 
@@ -264,10 +293,10 @@ def speculation_visibility(positions: torch.Tensor, length: int, W: int, tree_ma
 def speculation_attention_torch(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, positions: torch.Tensor,
                                 tree_mask: Optional[torch.Tensor] = None, tree_depth: Optional[torch.Tensor] = None,
                                 sliding_window: Optional[int] = None, scale: Optional[float] = None, k_scale: float = 1.0,
-                                v_scale: float = 1.0) -> torch.Tensor:
+                                v_scale: float = 1.0, rolling: bool = False) -> torch.Tensor:
     """The torch path of :func:`speculation_attention` (any device and dtype): SDPA with a ``[B, 1, W, L]`` mask on the
     de-quantised cache, K / V repeated over the GQA group."""
-    window, _ = _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale)
+    window, _ = _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale, rolling)
     B, W, H, D = q.shape
     Hkv, L = k_cache.shape[2], k_cache.shape[1]
     if k_cache.dtype in FP8_KV_DTYPES:
@@ -275,14 +304,14 @@ def speculation_attention_torch(q: torch.Tensor, k_cache: torch.Tensor, v_cache:
     qt, kt, vt = q.transpose(1, 2), k_cache.transpose(1, 2), v_cache.transpose(1, 2)
     if H != Hkv:
         kt, vt = kt.repeat_interleave(H // Hkv, 1), vt.repeat_interleave(H // Hkv, 1)
-    mask = speculation_visibility(positions, L, W, tree_mask, tree_depth, window)[:, None]
+    mask = speculation_visibility(positions, L, W, tree_mask, tree_depth, window, rolling)[:, None]
     return F.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask, scale=scale).transpose(1, 2)
 
 
 def speculation_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, positions: torch.Tensor,
                           tree_mask: Optional[torch.Tensor] = None, tree_depth: Optional[torch.Tensor] = None,
                           sliding_window: Optional[int] = None, scale: Optional[float] = None, k_scale: float = 1.0,
-                          v_scale: float = 1.0) -> torch.Tensor:
+                          v_scale: float = 1.0, rolling: bool = False) -> torch.Tensor:
     """W new tokens per sequence against a KV cache, as speculative decoding and Medusa verify them: ``q [B,W,H,D]``,
     caches ``[B,L,Hkv,D]`` (any batch / sequence / head strides), ``positions [B]``.  Token w of sequence b occupies cache
     slot p + w (p = ``positions[b]``) and sits at sequence position p + d[w], with d = ``tree_depth`` (a chain: d[w] = w).
@@ -290,14 +319,18 @@ def speculation_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch
 
     Token w sees slot c iff c < p (the committed sequence) and, with ``sliding_window`` SW, c > p + d[w] − SW; or
     c = p + u with ``tree_mask[w, u]`` and, with SW, d[u] > d[w] − SW.  Slots ≥ p + W and ≥ L are never seen; a token that
-    sees nothing gets 0.  An fp8 cache holds k / ``k_scale`` and v / ``v_scale``.
+    sees nothing gets 0.  An fp8 cache holds k / ``k_scale`` and v / ``v_scale``.  ``rolling``: the cache is a ring of L
+    rows holding slot c in row c mod L (``KVCacheManager`` in rolling mode); needs SW > 0 and SW + W − 1 ≤ L, and the rule
+    above then applies to logical slots without the bound at L.
 
     CUDA bf16 q with head_dim 128, W ≤ 64, H / Hkv ∈ {1, 2, 4, 8} and a bf16 or fp8 e4m3 cache whose rows are aligned as
     :func:`decode_attention` needs: the kernel in ``csrc/attention_sm90.cu``, which reads each K / V row once for all W
     tokens and the GQA group, reads e4m3 as stored, and with a window only the slots some token can see.  ``tree_mask``
     and ``tree_depth`` are never read on the host there, so the call can be captured in a CUDA graph.  Otherwise
     :func:`speculation_attention_torch`."""
-    window, kw = _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale)
+    window, kw = _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale, rolling)
+    if rolling:
+        kw["rolling"] = True
     B, W, H, D = q.shape
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     e = _ext.ext() if q.is_cuda else None
@@ -313,13 +346,18 @@ def speculation_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch
         return e.speculation_attention(_tma_view(q), k_cache, v_cache, positions.to(torch.long).contiguous(), tree_mask,
                                        tree_depth, scale=float(scale), window=window, **kw)
     return speculation_attention_torch(q, k_cache, v_cache, positions, tree_mask, tree_depth, sliding_window, scale, k_scale,
-                                       v_scale)
+                                       v_scale, rolling)
 
 
-def decode_visibility(positions: torch.Tensor, length: int, window: int = 0) -> torch.Tensor:
+def decode_visibility(positions: torch.Tensor, length: int, window: int = 0, rolling: bool = False) -> torch.Tensor:
     """``[B, length]`` bool: cache index j is visible to the token at ``positions[b]`` iff j ≤ position and, with a window
-    W > 0, j > position − W."""
+    W > 0, j > position − W.  ``rolling``: j is a row of a ring of ``length`` rows, holding the newest position
+    c_j = position − ((position − j) mod length), which is visible iff c_j ≥ 0 and, with W > 0, c_j > position − W."""
     j = torch.arange(length, device=positions.device)[None, :]
     p = positions[:, None]
-    vis = j <= p
+    if rolling:
+        j = p - (p - j) % length
+        vis = j >= 0
+    else:
+        vis = j <= p
     return vis if window <= 0 else vis & (j > p - window)

@@ -1,5 +1,5 @@
 """Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
-usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]] [--kv-fp8] [--spec]
+usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]] [--kv-fp8] [--spec] [--rolling]
 
 --perf times forward and forward+backward of the own kernels and of SDPA in the same process, alternating, at the shapes
 the models run (BERT-large with right padding, ViT-B/16, GPT-NeoX-20B per rank at TP=8, Pythia-2.8B, Llama-2-7B).  FLOPs
@@ -29,7 +29,12 @@ is the de-quantised e4m3 one), and the two outputs are compared.
 one process: Llama-2-7B (H = Hkv = 32) at L = 4096, B = 1, and Mistral-7B (H 32, Hkv 8) at L = 32768, B = 1 and 8, with and
 without a 4096 sliding window; a 5-token chain, the Medusa example's 10-node tree and a random 64-node tree; bf16 and e4m3
 caches holding the same values.  Bytes come from the shapes: the K and V rows some token can see, read once, plus q and the
-output."""
+output.
+
+--rolling (with --perf) times ``decode_attention`` and ``speculation_attention`` on a rolling KV cache (SW + 64 = 4160 rows,
+position t in row t mod 4160) against the linear 32k cache holding the same history, alternating in one process: Mistral-7B
+(H 32, Hkv 8, SW 4096) at B = 1, 8 and 32, position 32767 − W, decode and the chain5 / tree10 / tree64 windows, bf16 and
+e4m3.  Both read the same rows, so the times should match; the outputs are checked bit for bit."""
 import argparse
 import json
 import math
@@ -345,6 +350,60 @@ def spec_perf():
         torch.cuda.empty_cache()
 
 
+def _ring_of(lin: torch.Tensor, rows: int, end: int) -> torch.Tensor:
+    """The rolling cache (``inference.kv_cache``) of ``rows`` rows holding positions < ``end`` of the linear cache ``lin``."""
+    j = torch.arange(rows, device=lin.device)
+    t = (end - 1 - (end - 1 - j) % rows).clamp(min=0)
+    return lin[:, t].contiguous()
+
+
+def rolling_perf(sw: int = 4096):
+    """``decode_attention`` and ``speculation_attention`` on a rolling cache of SW + 64 rows against the linear 32k cache
+    holding the same history, alternating in one process; outputs must be bit-identical."""
+    dev = torch.device("cuda")
+    print(json.dumps(gpu_info()), flush=True)
+    D, H, Hkv, L, ks, vs = 128, 32, 8, 32768, 0.05, 0.05
+    R = sw + attention.SPEC_MAX_TOKENS
+    for B in (1, 8, 32):
+        g = torch.Generator(device=dev).manual_seed(B)
+        k8, v8 = ((torch.randn(B, L, Hkv, D, device=dev, generator=g) / s).to(torch.float8_e4m3fn) for s in (ks, vs))
+        for cache in ("bf16", "e4m3"):
+            kl, vl = (k8, v8) if cache == "e4m3" else ((k8.float() * ks).bfloat16(), (v8.float() * vs).bfloat16())
+            kw = {} if cache == "bf16" else {"k_scale": ks, "v_scale": vs}
+            elt = 2 if cache == "bf16" else 1
+            for wname, mask, depth, W in [("decode", None, None, 1)] + spec_windows(dev):
+                pos = torch.full((B,), L - W, device=dev, dtype=torch.long)
+                kr, vr = _ring_of(kl, R, L), _ring_of(vl, R, L)
+                q = torch.randn(B, W, H, D, device=dev, generator=g).bfloat16()
+                if W == 1:
+                    def call(kc, vc, roll):
+                        return attention.decode_attention(q, kc, vc, pos, sliding_window=sw, rolling=roll, **kw)
+                else:
+                    def call(kc, vc, roll):
+                        return attention.speculation_attention(q, kc, vc, pos, mask, depth, sw, rolling=roll, **kw)
+                n0 = _ext.launches()
+                equal = torch.equal(call(kl, vl, False), call(kr, vr, True))
+                assert _ext.launches() == n0 + 4, "a kernel did not run"
+                t = {"linear": [], "rolling": []}
+                iters = max(20, 2000 // B)
+                for _ in range(3):                             # alternate, keep each one's best
+                    t["linear"].append(time_fn(lambda: call(kl, vl, False), iters))
+                    t["rolling"].append(time_fn(lambda: call(kr, vr, True), iters))
+                nbytes = 2 * B * (sw + W - 1) * Hkv * D * elt + 2 * B * W * H * D * 2    # visible K / V rows, q and out
+                rec = {"bench": f"mistral7b_rolling_{wname}", "cache": cache, "B": B, "position": L - W, "W": W,
+                       "sliding_window": sw, "linear_rows": L, "rolling_rows": R, "bit_equal": equal, "bytes": nbytes}
+                for key in ("linear", "rolling"):
+                    ms = min(t[key])
+                    rec[f"{key}_us"] = round(ms * 1e3, 2)
+                    rec[f"{key}_GBps"] = round(nbytes / ms / 1e6, 1)
+                rec["rolling_over_linear"] = round(rec["rolling_us"] / rec["linear_us"], 3)
+                print(json.dumps(rec), flush=True)
+                del kr, vr
+            del kl, vl
+        del k8, v8
+        torch.cuda.empty_cache()
+
+
 def block_pairs(c: int, causal: bool, off: int, W) -> int:
     """Visible (query, key) pairs of one c × c CP block: all c² when dense, else i + off − W < j ≤ i + off (W None: no lower
     bound)."""
@@ -433,6 +492,7 @@ def main():
     ap.add_argument("--cp", type=int, default=0, help="with --perf --window: the context-parallel block schedule at this CP size")
     ap.add_argument("--kv-fp8", action="store_true", help="with --perf: decode attention on bf16 vs fp8 e4m3 KV caches")
     ap.add_argument("--spec", action="store_true", help="with --perf: speculation / Medusa verification attention")
+    ap.add_argument("--rolling", action="store_true", help="with --perf: decode / verification on rolling vs linear KV caches")
     ap.add_argument("--head-dim", type=int, default=128, choices=attention.FLASH_HEAD_DIMS)
     a = ap.parse_args()
     if a.perf and a.window and a.cp > 1 and not torch.cuda.is_available():
@@ -497,6 +557,8 @@ def main():
             kv_fp8_perf()
         elif a.spec:
             spec_perf()
+        elif a.rolling:
+            rolling_perf()
         elif a.window and a.cp > 1:
             cp_window_perf(a.bwd, a.cp)
         else:
