@@ -118,14 +118,9 @@ class KVCacheManager:
         if self.rolling:
             raise ValueError(f"KVCacheManager.{name}: the flash-decoding layout does not take a rolling cache")
 
-    def write_decode(self, layer: int, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor) -> None:
-        """k/v ``[B, 1, H, D]``; ``positions`` ``[B]`` (device tensor; no host sync → graph capturable)."""
-        b = torch.arange(k.shape[0], device=k.device)
-        self.k[layer].index_put_((b, self._row(positions)), self._q(k[:, 0]))
-        self.v[layer].index_put_((b, self._row(positions)), self._q(v[:, 0]))
-
     def write_window(self, layer: int, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor) -> None:
-        """k/v ``[B, W, H, D]`` written at positions ``positions[b] + 0..W-1`` (speculative verification / chunked prefill)."""
+        """k/v ``[B, W, H, D]`` written at positions ``positions[b] + 0..W-1`` (decode at W = 1, speculative verification,
+        chunked prefill); ``positions`` ``[B]`` is a device tensor (no host sync → graph capturable)."""
         B, W = k.shape[0], k.shape[1]
         b = torch.arange(B, device=k.device).unsqueeze(1).expand(B, W)
         pos = positions.unsqueeze(1) + torch.arange(W, device=k.device).unsqueeze(0)

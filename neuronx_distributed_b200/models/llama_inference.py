@@ -4,7 +4,6 @@ on-device sampling — role of reference ``examples/inference`` (``NeuronBaseMod
 No sequence parallelism at inference: Row-parallel outputs are all-reduced."""
 from __future__ import annotations
 
-import math
 from typing import Optional
 
 import torch
@@ -92,39 +91,7 @@ class LlamaForInference(nn.Module):
         # cache makes the calls it makes without quantisation
         scales = self.kv.kernel_scales()
         scale_kw = {} if scales in (None, (1.0, 1.0)) else {"k_scale": scales[0], "v_scale": scales[1]}
-        # RoPE + cache append in one launch (csrc/decode.cu), then attention on the cache as stored
-        fused = (q.is_cuda and q.dtype == torch.bfloat16 and scales is not None and self.kv.seq_shards == 1
-                 and ops._ext.ext() is not None and hasattr(ops._ext.ext(), "decode_rope_kv"))
-        if self.flash_decoding and not prefill:
-            assert S == 1 and tree is None, "flash decoding serves plain token generation (no speculation window)"
-            from ..modules.attention.flash_decode import flash_decode_attention
-
-            cos = self.rope_cos[positions].unsqueeze(1)
-            sin = self.rope_sin[positions].unsqueeze(1)
-            q, k = _rope_per_batch(q, cos, sin), _rope_per_batch(k, cos, sin)
-            self.kv.write_decode_sharded(layer_idx, k, v, positions, self.kv_rank)                  # owner-only write
-            kc, vc = self.kv.stored(layer_idx) if scales is not None else self.kv.get(layer_idx)
-            o = flash_decode_attention(q, kc, vc, positions, self.kv_group, sliding_window=sw, **scale_kw)
-        elif not prefill and S > 1:
-            # speculation window: W new tokens per sequence in cache slots p..p+W-1; linear window: token w sits at sequence
-            # position p+w; Medusa tree: node w sits at p+depth[w] and sees only its ancestors inside the window
-            # (ops.attention.speculation_attention)
-            tree_mask, depth = (None, None) if tree is None else tree
-            if fused:
-                ops._ext.count_launch()
-                q = ops._ext.ext().decode_rope_kv(q, k, v, positions.to(torch.long).contiguous(), self.rope_cos, self.rope_sin,
-                                                  self.kv.k[layer_idx], self.kv.v[layer_idx], depth=depth, **scale_kw, **roll)
-                kc, vc = self.kv.stored(layer_idx, kv_len)
-                o = ops.attention.speculation_attention(q, kc, vc, positions, tree_mask, depth, sw, **scale_kw, **roll)
-            else:
-                d = torch.arange(S, device=q.device) if depth is None else depth
-                idx = (positions.unsqueeze(1) + d.unsqueeze(0)).clamp(max=self.max_seq_len - 1)
-                cos, sin = self.rope_cos[idx], self.rope_sin[idx]                 # [B, W, D/2]
-                q, k = _rope_window(q, cos, sin), _rope_window(k, cos, sin)
-                self.kv.write_window(layer_idx, k, v, positions)
-                kc, vc = self.kv.get(layer_idx, kv_len)
-                o = ops.attention.speculation_attention_torch(q, kc, vc, positions, tree_mask, depth, sw, **roll)
-        elif prefill:
+        if prefill:
             cos, sin = self.rope_cos[:S], self.rope_sin[:S]
             q, k = ops.rope.apply_rotary(q, cos, sin), ops.rope.apply_rotary(k, cos, sin)
             if self.flash_decoding:
@@ -132,20 +99,43 @@ class LlamaForInference(nn.Module):
             else:
                 self.kv.write_prefill(layer_idx, k, v, lengths=prompt_lens)
             o = ops.attention.flash_attention(q, k, v, causal=True, sliding_window=sw)
-        elif fused:
-            ops._ext.count_launch()
-            q = ops._ext.ext().decode_rope_kv(q, k, v, positions.to(torch.long).contiguous(), self.rope_cos, self.rope_sin,
-                                              self.kv.k[layer_idx], self.kv.v[layer_idx], **scale_kw, **roll)
-            kc, vc = self.kv.stored(layer_idx, kv_len)
-            o = _decode_attention(q, kc, vc, positions, sw, **scale_kw, **roll)
-        else:
-            # one new token per sequence at its own position
-            cos = self.rope_cos[positions].unsqueeze(1)     # [B, 1, D/2] → per-batch tables
+        elif self.flash_decoding:
+            assert S == 1 and tree is None, "flash decoding serves plain token generation (no speculation window)"
+            from ..modules.attention.flash_decode import flash_decode_attention
+
+            cos = self.rope_cos[positions].unsqueeze(1)     # [B, 1, D/2]
             sin = self.rope_sin[positions].unsqueeze(1)
-            q, k = _rope_per_batch(q, cos, sin), _rope_per_batch(k, cos, sin)
-            self.kv.write_decode(layer_idx, k, v, positions)
-            kc, vc = self.kv.get(layer_idx, kv_len)
-            o = _decode_attention(q, kc, vc, positions, sw, **roll)
+            q, k = ops.rope.rotate(q, cos, sin), ops.rope.rotate(k, cos, sin)
+            self.kv.write_decode_sharded(layer_idx, k, v, positions, self.kv_rank)                  # owner-only write
+            kc, vc = self.kv.stored(layer_idx) if scales is not None else self.kv.get(layer_idx)
+            o = flash_decode_attention(q, kc, vc, positions, self.kv_group, sliding_window=sw, **scale_kw)
+        else:
+            # generation: W = S new tokens per sequence in cache slots p..p+W-1.  A chain puts token w at sequence position
+            # p+w; a Medusa tree puts node w at p+depth[w], seeing only its ancestors inside the window
+            # (ops.attention.speculation_attention).  One token (W = 1) is plain decode, whatever tree comes with it.
+            tree_mask, depth = (None, None) if tree is None or S == 1 else tree
+            fused = (q.is_cuda and q.dtype == torch.bfloat16 and scales is not None and self.kv.seq_shards == 1
+                     and ops._ext.ext() is not None and hasattr(ops._ext.ext(), "decode_rope_kv"))
+            if fused:
+                # RoPE + cache append in one launch (csrc/decode.cu), then attention on the cache as stored
+                ops._ext.count_launch()
+                q = ops._ext.ext().decode_rope_kv(q, k, v, positions.to(torch.long).contiguous(), self.rope_cos, self.rope_sin,
+                                                  self.kv.k[layer_idx], self.kv.v[layer_idx], depth=depth, **scale_kw, **roll)
+                kc, vc = self.kv.stored(layer_idx, kv_len)
+            else:
+                d = torch.arange(S, device=q.device) if depth is None else depth
+                idx = (positions.unsqueeze(1) + d.unsqueeze(0)).clamp(max=self.max_seq_len - 1)
+                cos, sin = self.rope_cos[idx], self.rope_sin[idx]                 # [B, W, D/2]
+                q, k = ops.rope.rotate(q, cos, sin), ops.rope.rotate(k, cos, sin)
+                self.kv.write_window(layer_idx, k, v, positions)
+                kc, vc = self.kv.get(layer_idx, kv_len)
+                scale_kw = {}                                                     # kv.get de-quantised the cache
+            if S == 1:
+                o = ops.attention.decode_attention(q, kc, vc, positions, sliding_window=sw, **scale_kw, **roll)
+            elif fused:
+                o = ops.attention.speculation_attention(q, kc, vc, positions, tree_mask, depth, sw, **scale_kw, **roll)
+            else:
+                o = ops.attention.speculation_attention_torch(q, kc, vc, positions, tree_mask, depth, sw, **roll)
         o = o.transpose(0, 1).reshape(S, B, att.num_heads_local * D)
         return _row_linear_plus_residual(att.o_proj, o, x)
 
@@ -256,48 +246,3 @@ def _row_linear_plus_residual(lin, inp: torch.Tensor, residual: torch.Tensor) ->
         if tp > 1 and ops.tp_fused.get_backend() == "fused" and ops.nvls.gemv_all_reduce_eligible(x2, w):
             return ops.nvls.gemv_all_reduce(x2, w, lin.tensor_parallel_group, residual=r2).view_as(residual)
     return residual + lin(inp)
-
-
-def _rope_per_batch(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch.Tensor:
-    """x [B,1,H,D]; cos/sin [B,1,D/2] — tiny decode-time rotation (elementwise, graph-capturable)."""
-    d2 = x.shape[-1] // 2
-    xf = x.float()
-    x1, x2 = xf[..., :d2], xf[..., d2:]
-    c, s = cos.unsqueeze(2), sin.unsqueeze(2)
-    return torch.cat([x1 * c - x2 * s, x2 * c + x1 * s], dim=-1).to(x.dtype)
-
-
-def _rope_window(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch.Tensor:
-    """x [B,W,H,D]; cos/sin [B,W,D/2]."""
-    d2 = x.shape[-1] // 2
-    xf = x.float()
-    x1, x2 = xf[..., :d2], xf[..., d2:]
-    c, s = cos.unsqueeze(2), sin.unsqueeze(2)
-    return torch.cat([x1 * c - x2 * s, x2 * c + x1 * s], dim=-1).to(x.dtype)
-
-
-def _decode_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positions: torch.Tensor,
-                      sliding_window: Optional[int] = None, k_scale: float = 1.0, v_scale: float = 1.0,
-                      rolling: bool = False) -> torch.Tensor:
-    """q [B,1,H,D] vs cache k/v [B,L,Hkv,D]; keys beyond each sequence's position (and, with ``sliding_window`` SW, keys at or
-    before position − SW) are masked.  An fp8 cache holds k / ``k_scale`` and v / ``v_scale``; ``rolling``: a ring cache
-    (``ops.attention.decode_attention``)."""
-    if k.dtype in ops.attention.FP8_KV_DTYPES or rolling:
-        return ops.attention.decode_attention(q, k, v, positions, sliding_window=sliding_window, k_scale=k_scale, v_scale=v_scale,
-                                              rolling=rolling)
-    window = ops.attention.check_window(sliding_window)
-    B, _, H, D = q.shape
-    Hkv, L = k.shape[2], k.shape[1]
-    e = ops._ext.ext() if q.is_cuda else None
-    if (e is not None and hasattr(e, "decode_attention") and D == 128 and q.dtype == torch.bfloat16 and k.dtype == torch.bfloat16
-            and H // Hkv in (1, 2, 4, 8) and k.stride(3) == 1 and v.stride(3) == 1):
-        # flash-decoding kernel (csrc/decode.cu): split over the cache length, GQA group shares each K/V read
-        ops._ext.count_launch(2)
-        return e.decode_attention(q.contiguous(), k, v, positions.to(torch.long).contiguous(), 1.0 / math.sqrt(D), window)
-    qt = q.transpose(1, 2)                                   # [B,H,1,D]
-    kt, vt = k.transpose(1, 2), v.transpose(1, 2)
-    if H != Hkv:
-        kt, vt = kt.repeat_interleave(H // Hkv, 1), vt.repeat_interleave(H // Hkv, 1)
-    mask = ops.attention.decode_visibility(positions, L, window)[:, None, None, :]
-    o = torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask)
-    return o.transpose(1, 2)

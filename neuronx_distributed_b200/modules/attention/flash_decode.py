@@ -56,7 +56,7 @@ def _local_partial(q_all: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Te
     CUDA / bf16 q / bf16 or e4m3 cache / head_dim 128: the split-KV decode kernel (``csrc/decode.cu`` ``decode_attn_kernel`` +
     the partial combine): K/V are read once per KV head for the whole GQA group.  Otherwise fp32 torch math."""
     from ...ops import _ext
-    from ...ops.attention import check_kv_scales, check_window, decode_visibility
+    from ...ops.attention import check_kv_scales, check_window, speculation_visibility
 
     window = check_window(sliding_window)
     kw = check_kv_scales(k_cache, v_cache, k_scale, v_scale)
@@ -72,7 +72,7 @@ def _local_partial(q_all: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Te
     kf = (k_cache.float() * k_scale if kw else k_cache.float()).repeat_interleave(g, dim=2)    # [B, L_local, H, D]
     vf = (v_cache.float() * v_scale if kw else v_cache.float()).repeat_interleave(g, dim=2)
     s = torch.einsum("bhd,blhd->bhl", q_all[:, 0].float(), kf) * scale  # [B, H, L_local]
-    valid = decode_visibility(local_pos, l_local, window)                                        # [B, L_local]
+    valid = speculation_visibility(local_pos, l_local, 1, window=window)[:, 0]                  # [B, L_local]
     s = s.masked_fill(~valid[:, None, :], float("-inf"))
     m = s.max(dim=-1).values                                            # [B, H]  (−inf if this shard has nothing yet)
     p = torch.exp(s - torch.where(torch.isinf(m), torch.zeros_like(m), m).unsqueeze(-1))

@@ -214,9 +214,12 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     strides), ``positions [B]`` = cache index of the newest token (keys ≤ position are visible; with ``sliding_window`` W only
     keys position − W < j ≤ position, and the kernel reads only those rows).  An fp8 cache holds k / ``k_scale`` and
     v / ``v_scale`` (one scale per tensor, as ``inference.kv_cache.KVCacheManager`` stores it).  ``rolling``: the cache is a
-    ring of L rows holding position j in row j mod L (``KVCacheManager`` in rolling mode); needs 0 < W < L.  CUDA bf16 q
-    with a bf16 or fp8 e4m3 cache and head_dim 128: the split-KV flash-decoding kernel (``csrc/decode.cu``), which reads the
-    e4m3 bytes directly; otherwise SDPA with a length mask on the de-quantised cache."""
+    ring of L rows holding position j in row j mod L (``KVCacheManager`` in rolling mode); needs 0 < W < L.
+
+    This is the W = 1 chain of :func:`speculation_attention` (one token in slot p = position, seeing slots ≤ p), with the
+    stricter ring condition of a single token.  CUDA bf16 q with a bf16 or fp8 e4m3 cache and head_dim 128: the split-KV
+    flash-decoding kernel (``csrc/decode.cu``), which reads the e4m3 bytes directly; otherwise
+    :func:`speculation_attention_torch`."""
     B, _, H, D = q.shape
     Hkv, L = k_cache.shape[2], k_cache.shape[1]
     window = check_window(sliding_window)
@@ -232,13 +235,8 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
         _ext.count_launch(2)
         return e.decode_attention(q.contiguous(), k_cache, v_cache, positions.to(torch.long).contiguous(), float(scale), window,
                                   **kw)
-    if k_cache.dtype in FP8_KV_DTYPES:
-        k_cache, v_cache = (k_cache.float() * k_scale).to(q.dtype), (v_cache.float() * v_scale).to(q.dtype)
-    qt, kt, vt = q.transpose(1, 2), k_cache.transpose(1, 2), v_cache.transpose(1, 2)
-    if H != Hkv:
-        kt, vt = kt.repeat_interleave(H // Hkv, 1), vt.repeat_interleave(H // Hkv, 1)
-    mask = decode_visibility(positions, L, window, rolling)[:, None, None, :]
-    return torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, attn_mask=mask, scale=scale).transpose(1, 2)
+    return speculation_attention_torch(q, k_cache, v_cache, positions, sliding_window=sliding_window, scale=scale,
+                                       k_scale=k_scale, v_scale=v_scale, rolling=rolling)
 
 
 #: most new tokens per sequence the speculation kernel verifies in one call
@@ -265,9 +263,10 @@ def _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window,
 
 def speculation_visibility(positions: torch.Tensor, length: int, W: int, tree_mask: Optional[torch.Tensor] = None,
                            tree_depth: Optional[torch.Tensor] = None, window: int = 0, rolling: bool = False) -> torch.Tensor:
-    """``[B, W, length]`` bool: which cache slots each of W new tokens sees (the rule of :func:`speculation_attention`).
-    ``rolling``: slot c is a row of a ring of ``length`` rows: window column (c − p) mod length when that is < W, else the
-    newest committed position p − 1 − ((p − 1 − c) mod length), which is seen only when ≥ 0."""
+    """``[B, W, length]`` bool: which cache slots each of W new tokens sees (the rule of :func:`speculation_attention`; at
+    W = 1 that of one-token decode: slot c is seen iff c ≤ p and, with a window, c > p − window).  ``rolling``: slot c is a
+    row of a ring of ``length`` rows: window column (c − p) mod length when that is < W, else the newest committed position
+    p − 1 − ((p − 1 − c) mod length), which is seen only when ≥ 0."""
     dev = positions.device
     p = positions.long()[:, None]                                                          # [B, 1]
     d = torch.arange(W, device=dev) if tree_depth is None else tree_depth.to(dev).long()
@@ -347,17 +346,3 @@ def speculation_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch
                                        tree_depth, scale=float(scale), window=window, **kw)
     return speculation_attention_torch(q, k_cache, v_cache, positions, tree_mask, tree_depth, sliding_window, scale, k_scale,
                                        v_scale, rolling)
-
-
-def decode_visibility(positions: torch.Tensor, length: int, window: int = 0, rolling: bool = False) -> torch.Tensor:
-    """``[B, length]`` bool: cache index j is visible to the token at ``positions[b]`` iff j ≤ position and, with a window
-    W > 0, j > position − W.  ``rolling``: j is a row of a ring of ``length`` rows, holding the newest position
-    c_j = position − ((position − j) mod length), which is visible iff c_j ≥ 0 and, with W > 0, c_j > position − W."""
-    j = torch.arange(length, device=positions.device)[None, :]
-    p = positions[:, None]
-    if rolling:
-        j = p - (p - j) % length
-        vis = j >= 0
-    else:
-        vis = j <= p
-    return vis if window <= 0 else vis & (j > p - window)

@@ -12,13 +12,15 @@ import torch
 from . import _ext
 
 
-def _rope_ref(x, cos, sin, sign):
-    # x [B,S,H,D]; cos/sin [S, D/2]
+def rotate(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, sign: float = 1.0) -> torch.Tensor:
+    """Rotate-half RoPE in fp32 torch math (the reference of the kernel, and the decode-time rotation off the kernels):
+    x ``[B, S, H, D]``; cos/sin ``[S, D/2]`` shared by the batch, or ``[B, S, D/2]`` per row (each sequence at its own
+    positions).  ``sign`` −1 rotates backwards (the gradient)."""
     d2 = x.shape[-1] // 2
     xf = x.float()
     x1, x2 = xf[..., :d2], xf[..., d2:]
-    c = cos[None, :, None, :].float()
-    s = sin[None, :, None, :].float() * sign
+    c = cos.unsqueeze(-2).float()
+    s = sin.unsqueeze(-2).float() * sign
     return torch.cat([x1 * c - x2 * s, x2 * c + x1 * s], dim=-1).to(x.dtype)
 
 
@@ -32,7 +34,7 @@ class _Rope(torch.autograd.Function):
             _ext.count_launch()
             return _ext.ext().rope_apply(x, cos.contiguous().float(), sin.contiguous().float(), 1.0)
         ctx.cuda = False
-        return _rope_ref(x, cos, sin, 1.0)
+        return rotate(x, cos, sin)
 
     @staticmethod
     def backward(ctx, g):
@@ -40,7 +42,7 @@ class _Rope(torch.autograd.Function):
         if ctx.cuda:
             _ext.count_launch()
             return _ext.ext().rope_apply(g, cos.contiguous().float(), sin.contiguous().float(), -1.0), None, None
-        return _rope_ref(g, cos, sin, -1.0), None, None
+        return rotate(g, cos, sin, -1.0), None, None
 
 
 def apply_rotary(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch.Tensor:

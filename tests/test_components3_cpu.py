@@ -46,7 +46,7 @@ def _quant_moe(rank, world):
     kk = torch.randn(2, 5, 2, 4, generator=torch.Generator().manual_seed(2)); vv = torch.randn(2, 5, 2, 4, generator=torch.Generator().manual_seed(3))
     kv.write_prefill(1, kk, vv)
     k_new = torch.randn(2, 1, 2, 4, generator=torch.Generator().manual_seed(4))
-    kv.write_decode(1, k_new, k_new, torch.tensor([5, 6]))
+    kv.write_window(1, k_new, k_new, torch.tensor([5, 6]))
     kc, vc = kv.get(1, 8)
     assert kv.k[1].dtype == torch.float8_e4m3fn and kc.dtype == torch.float32
     assert (kc[:, :5] - kk).abs().max() < 0.25 and (vc[:, :5] - vv).abs().max() < 0.25

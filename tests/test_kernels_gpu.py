@@ -214,7 +214,6 @@ def test_fused_add_rmsnorm_vs_fp32_reference(dtype):
 def test_decode_rope_kv_fused_vs_separate_ops():
     """RoPE of q/k at per-sequence positions + KV-cache append in one launch vs the eager composition."""
     from neuronx_distributed_b200 import ops
-    from neuronx_distributed_b200.models.llama_inference import _rope_per_batch
 
     e = ops._ext.ext()
     dev = torch.device("cuda")
@@ -230,8 +229,8 @@ def test_decode_rope_kv_fused_vs_separate_ops():
     kc = torch.zeros(B, L, Hkv, D, device=dev, dtype=torch.bfloat16)
     vc = torch.zeros_like(kc)
     q_out = e.decode_rope_kv(q, k, v, pos, cos, sin, kc, vc)
-    q_ref = _rope_per_batch(q, cos[pos].unsqueeze(1), sin[pos].unsqueeze(1))
-    k_ref = _rope_per_batch(k, cos[pos].unsqueeze(1), sin[pos].unsqueeze(1))
+    q_ref = ops.rope.rotate(q, cos[pos].unsqueeze(1), sin[pos].unsqueeze(1))
+    k_ref = ops.rope.rotate(k, cos[pos].unsqueeze(1), sin[pos].unsqueeze(1))
     torch.testing.assert_close(q_out.float(), q_ref.float(), atol=2e-2, rtol=2e-2)
     b = torch.arange(B, device=dev)
     torch.testing.assert_close(kc[b, pos].float(), k_ref[:, 0].float(), atol=2e-2, rtol=2e-2)

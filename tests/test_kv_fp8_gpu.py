@@ -199,7 +199,6 @@ def test_mistral_shaped_fp8_cache_graph_torch_path_and_bf16_cache(_ext, monkeypa
     - the CUDA-graph replay of a decode step gives the eager logits bit for bit;
     - attention forced through fp32 torch math on the same quantised cache agrees (rel. error < 5e-2, confident tokens);
     - the bf16-cache model agrees within a bound set by e4m3's relative step (below)."""
-    from neuronx_distributed_b200.models import llama_inference
     from neuronx_distributed_b200.models.llama_inference import LlamaForInference
     from neuronx_distributed_b200.ops import attention
     from neuronx_distributed_b200.quantization import KVQuantizationConfig
@@ -265,9 +264,10 @@ def test_mistral_shaped_fp8_cache_graph_torch_path_and_bf16_cache(_ext, monkeypa
     # fp32 torch attention over the same quantised cache (prefill through SDPA, decode through the de-quantising fallback)
     with monkeypatch.context() as mp:
         mp.setenv("NXD_DISABLE_OWN_ATTENTION", "1")
-        mp.setattr(llama_inference, "_decode_attention",
-                   lambda q, k, v, p, sw, k_scale=1.0, v_scale=1.0: attention.decode_attention(
-                       q.float(), k, v, p, sliding_window=sw, k_scale=k_scale, v_scale=v_scale).to(q.dtype))
+        orig = attention.decode_attention
+        mp.setattr(attention, "decode_attention",
+                   lambda q, k, v, p, sliding_window, k_scale=1.0, v_scale=1.0: orig(
+                       q.float(), k, v, p, sliding_window=sliding_window, k_scale=k_scale, v_scale=v_scale).to(q.dtype))
         ref_logits = teacher_forced(m)
     for i, (a, r) in enumerate(zip(eager_logits, ref_logits)):
         assert _rel(a.float(), r.double()) < 5e-2, (i, _rel(a.float(), r.double()))

@@ -94,7 +94,7 @@ def test_decode_window_and_compact_wrap():
     for step in range(steps):
         kd, vd = torch.randn(B, 1, 2, 4, generator=g), torch.randn(B, 1, 2, 4, generator=g)
         for m in (ring, lin):
-            m.write_decode(0, kd, vd, pos + step)
+            m.write_window(0, kd, vd, pos + step)
     p = pos + steps
     _same_history(ring, lin, p.tolist())
     W = 10
@@ -112,11 +112,14 @@ def test_decode_window_and_compact_wrap():
 
 
 def test_decode_visibility_matches_linear_rule_on_unrolled_history():
+    """One decode token is the W = 1 chain of the verification rule: ``speculation_visibility(…, 1, …)[:, 0]``."""
     for L, sw in ((20, 7), (20, 19), (33, 1)):
         pos = torch.tensor([0, 5, L - 1, L, L + 3, 3 * L + 11])
-        vr = attention.decode_visibility(pos, L, sw, rolling=True)
+        vr = attention.speculation_visibility(pos, L, 1, window=sw, rolling=True)[:, 0]
         T = int(pos.max()) + 1
-        vl = attention.decode_visibility(pos, T, sw)
+        vl = attention.speculation_visibility(pos, T, 1, window=sw)[:, 0]
+        t = torch.arange(T)[None, :]
+        assert torch.equal(vl, (t <= pos[:, None]) & (t > pos[:, None] - sw))   # the plain decode rule
         j = torch.arange(L)
         for b, p in enumerate(pos.tolist()):
             c = p - (p - j) % L                                             # logical position of row j

@@ -292,8 +292,8 @@ def test_mistral_shaped_training_matches_sdpa(_ext, monkeypatch):
 def test_mistral_shaped_inference_graph_and_sdpa(_ext, monkeypatch):
     """Prefill past the window and decode steps past it: the CUDA-graph replay of a decode step gives the eager logits bit for
     bit, and a run with attention on SDPA (teacher-forced on the same tokens) agrees on every confident greedy token."""
-    from neuronx_distributed_b200.models import llama_inference
     from neuronx_distributed_b200.models.llama_inference import LlamaForInference
+    from neuronx_distributed_b200.ops import attention
 
     _one_rank_model_parallel()
     W, P, N = 64, 160, 24
@@ -337,9 +337,9 @@ def test_mistral_shaped_inference_graph_and_sdpa(_ext, monkeypatch):
 
     # SDPA run on the eager tokens: prefill through NXD_DISABLE_OWN_ATTENTION, decode through the fp32 SDPA branch
     monkeypatch.setenv("NXD_DISABLE_OWN_ATTENTION", "1")
-    orig = llama_inference._decode_attention
-    monkeypatch.setattr(llama_inference, "_decode_attention",
-                        lambda q, k, v, p, sw: orig(q.float(), k.float(), v.float(), p, sw).to(q.dtype))
+    orig = attention.decode_attention
+    monkeypatch.setattr(attention, "decode_attention", lambda q, k, v, p, sliding_window: orig(
+        q.float(), k.float(), v.float(), p, sliding_window=sliding_window).to(q.dtype))
     ref_logits = [m.context_encoding(ids, last)]
     pos = last + 1
     for i in range(N):

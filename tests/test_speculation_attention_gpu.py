@@ -154,7 +154,7 @@ def test_append_tree_matches_torch_path_and_e4m3_rule(_ext, scale):
     """Tree depths: token w is rotated at p + depth[w] and written to slot p + w.  Slots as the torch path writes them,
     rows within one bf16 ulp of its fp32 rotation, and the e4m3 bytes are ``KVCacheManager._q`` of the bf16 rows."""
     from neuronx_distributed_b200.inference.kv_cache import KVCacheManager
-    from neuronx_distributed_b200.models.llama_inference import _rope_window
+    from neuronx_distributed_b200.ops.rope import rotate
     from neuronx_distributed_b200.quantization import KVQuantizationConfig
 
     e = _ext.ext()
@@ -169,7 +169,7 @@ def test_append_tree_matches_torch_path_and_e4m3_rule(_ext, scale):
     q8 = e.decode_rope_kv(q, k, v, pos, cos, sin, k8, v8, k_scale=scale, v_scale=scale, depth=depth)
     assert torch.equal(qb, q8)
     idx = pos[:, None] + depth[None, :]
-    qt, kt = _rope_window(q, cos[idx], sin[idx]), _rope_window(k, cos[idx], sin[idx])
+    qt, kt = rotate(q, cos[idx], sin[idx]), rotate(k, cos[idx], sin[idx])
     slots = pos[:, None] + torch.arange(W, device="cuda")
     b = torch.arange(B, device="cuda")[:, None]
     assert ((qb.float() - qt.float()).abs() <= _ulp(qt)).all()

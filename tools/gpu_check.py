@@ -83,14 +83,14 @@ def check_elementwise():
     base = torch.randn(S, B, Hh * D, device=dev, dtype=torch.bfloat16)
     q = base.view(S, B, Hh, D).transpose(0, 1)
     cos, sin = ops.rope.rope_tables(S, D, device=dev)
-    from neuronx_distributed_b200.ops.rope import _rope_ref
+    from neuronx_distributed_b200.ops.rope import rotate
     qq = q.detach().clone().requires_grad_(True)
     out = ops.rope.apply_rotary(qq, cos, sin)
-    ref = _rope_ref(q.float(), cos, sin, 1.0)
+    ref = rotate(q.float(), cos, sin)
     report("rope_fwd", relerr(out, ref) < 2e-2, err=relerr(out, ref))
     g = torch.randn_like(out)
     out.backward(g)
-    refb = _rope_ref(g.float(), cos, sin, -1.0)
+    refb = rotate(g.float(), cos, sin, -1.0)
     report("rope_bwd", relerr(qq.grad, refb) < 2e-2, err=relerr(qq.grad, refb))
     # cross entropy
     for V, dt in ((4000, torch.bfloat16), (32000, torch.float32)):
