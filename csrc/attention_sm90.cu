@@ -340,9 +340,9 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
 // tile can straddle the end of the ring.  The host guarantees window > 0 and window + W − 1 ≤ L, so the slots a tile reads
 // (at most p + dmin − window + 1 … p + W − 1) map to distinct rows.
 constexpr int kSpecMaxW = 64;
-constexpr int kRawTile = BT * 128;                      // bytes of one staged e4m3 tile
-template <bool E4M3>
-constexpr int kSmemSpec = (E4M3 ? 3 * kTile<128> * 2 + 4 * kRawTile : kSmemFwd<128>) + kSpecMaxW * (8 + 4);
+template <int HD> constexpr int kRawTile = BT * HD;     // bytes of one staged e4m3 tile
+template <int HD, bool E4M3>
+constexpr int kSmemSpec = (E4M3 ? 3 * kTile<HD> * 2 + 4 * kRawTile<HD> : kSmemFwd<HD>) + kSpecMaxW * (8 + 4);
 
 struct SpecParams {
   const bf16* q; long q_sb, q_ss, q_sh;
@@ -359,23 +359,28 @@ NXD_DEVICE void cp_async8(void* dst, const void* src, bool valid) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(smem_addr(dst)), "l"(src), "r"(valid ? 8 : 0) : "memory");
 }
 
-// rows [s0, s0+64) of one e4m3 (batch, kv head) slice → unpadded 128-byte shared rows; rows ≥ S are zero-filled.  8-byte
-// copies: an e4m3 cache is only required to be 8-byte aligned.  ROLL as in load_tile.
-template <bool ROLL>
+// rows [s0, s0+64) of one e4m3 (batch, kv head) slice → unpadded HD-byte shared rows; rows ≥ S are zero-filled.  HD / 8
+// copies of 8 bytes per row: an e4m3 cache is only required to be 8-byte aligned (so are 80-byte rows).  ROLL as in load_tile.
+template <int HD, bool ROLL>
 NXD_DEVICE void load_raw_e4m3(uint8_t* sm, const uint8_t* base, long ss, int s0, int S, int L) {
+  constexpr int kChunks = HD / 8;                                   // 8-byte chunks per row
+  constexpr bool kPow2 = (kChunks & (kChunks - 1)) == 0;
   const int w0 = ROLL ? s0 % L : 0;
-  for (int i = threadIdx.x; i < BT * 16; i += kThreads) {
-    const int r = i >> 4, c = i & 15;
+  for (int i = threadIdx.x; i < BT * kChunks; i += kThreads) {
+    const int r = kPow2 ? i >> (kChunks == 16 ? 4 : 3) : i / kChunks, c = kPow2 ? i & (kChunks - 1) : i % kChunks;
     const bool ok = s0 + r < S;
-    cp_async8(sm + r * 128 + c * 8, base + (long)(ok ? (ROLL ? ring_row(w0, r, L) : s0 + r) : 0) * ss + c * 8, ok);
+    cp_async8(sm + r * HD + c * 8, base + (long)(ok ? (ROLL ? ring_row(w0, r, L) : s0 + r) : 0) * ss + c * 8, ok);
   }
 }
 
 // staged e4m3 tile → padded bf16 tile (every e4m3 value is a bf16 value)
+template <int HD>
 NXD_DEVICE void e4m3_to_bf16(bf16* dst, const uint8_t* src) {
-  for (int i = threadIdx.x; i < BT * 16; i += kThreads) {
-    const int r = i >> 4, c = i & 15;
-    const uint2 a = *(const uint2*)(src + r * 128 + c * 8);
+  constexpr int kChunks = HD / 8;
+  constexpr bool kPow2 = (kChunks & (kChunks - 1)) == 0;
+  for (int i = threadIdx.x; i < BT * kChunks; i += kThreads) {
+    const int r = kPow2 ? i >> (kChunks == 16 ? 4 : 3) : i / kChunks, c = kPow2 ? i & (kChunks - 1) : i % kChunks;
+    const uint2 a = *(const uint2*)(src + r * HD + c * 8);
     uint32_t o[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -383,19 +388,21 @@ NXD_DEVICE void e4m3_to_bf16(bf16* dst, const uint8_t* src) {
       const float2 f = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w >> (16 * (j & 1))), __NV_E4M3)));
       o[j] = pack_bf16(f.x, f.y);
     }
-    *(uint4*)(dst + r * LDS<128> + c * 8) = make_uint4(o[0], o[1], o[2], o[3]);
+    *(uint4*)(dst + r * LDS<HD> + c * 8) = make_uint4(o[0], o[1], o[2], o[3]);
   }
 }
 
-template <int G, bool E4M3, bool ROLL>
+template <int HD, int G, bool E4M3, bool ROLL>
 __global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p) {
-  constexpr int HD = 128, kTl = kTile<HD>, kBufs = E4M3 ? 1 : 2;
+  constexpr int kTl = kTile<HD>, kBufs = E4M3 ? 1 : 2;
+  constexpr int kChunks = HD / 8;                               // 16-byte chunks of a bf16 row
+  constexpr bool kPow2 = (kChunks & (kChunks - 1)) == 0;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   bf16* sQ = (bf16*)smem_raw;
   bf16* sK = sQ + kTl;                          // kBufs buffers
   bf16* sV = sK + kBufs * kTl;                  // kBufs buffers
   uint8_t* sRaw = (uint8_t*)(sV + kBufs * kTl); // e4m3: raw K, V × 2 buffers
-  uint64_t* sBits = (uint64_t*)(sRaw + (E4M3 ? 4 * kRawTile : 0));   // window columns row w sees
+  uint64_t* sBits = (uint64_t*)(sRaw + (E4M3 ? 4 * kRawTile<HD> : 0));   // window columns row w sees
   int* sDepth = (int*)(sBits + kSpecMaxW);
   const int rt = blockIdx.x % p.row_tiles, split = blockIdx.x / p.row_tiles, kvh = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -450,8 +457,8 @@ __global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p)
   auto issue = [&](int t) {                     // K / V tile t of the split → buffer t & 1
     const int s = s0 + t * BT, buf = t & 1;
     if constexpr (E4M3) {
-      load_raw_e4m3<ROLL>(sRaw + 2 * buf * kRawTile, kb, p.k_ss, s, s1, p.L);
-      load_raw_e4m3<ROLL>(sRaw + (2 * buf + 1) * kRawTile, vb, p.v_ss, s, s1, p.L);
+      load_raw_e4m3<HD, ROLL>(sRaw + 2 * buf * kRawTile<HD>, kb, p.k_ss, s, s1, p.L);
+      load_raw_e4m3<HD, ROLL>(sRaw + (2 * buf + 1) * kRawTile<HD>, vb, p.v_ss, s, s1, p.L);
     } else {
       load_tile<HD, ROLL>(sK + buf * kTl, (const bf16*)kb, p.k_ss, s, s1, p.L);
       load_tile<HD, ROLL>(sV + buf * kTl, (const bf16*)vb, p.v_ss, s, s1, p.L);
@@ -459,8 +466,9 @@ __global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p)
     cp_async_commit();
   };
   if (n_t > 0) {
-    for (int i = threadIdx.x; i < BT * 16; i += kThreads) {    // Q rows (token w, head g) of the tile; rows past W·G are 0
-      const int r = i >> 4, c = i & 15, row = r0 + r;
+    for (int i = threadIdx.x; i < BT * kChunks; i += kThreads) {   // Q rows (token w, head g) of the tile; rows past W·G are 0
+      const int r = kPow2 ? i >> (kChunks == 16 ? 4 : 3) : i / kChunks, c = kPow2 ? i & (kChunks - 1) : i % kChunks;
+      const int row = r0 + r;
       const bool ok = row < n_rows;
       cp_async16(sQ + r * LDS<HD> + c * 8, qb + (ok ? (row / G) * p.q_ss + (row % G) * p.q_sh : 0) + c * 8, ok);
     }
@@ -484,15 +492,17 @@ __global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p)
     bf16* k = sK + (E4M3 ? 0 : buf * kTl);
     bf16* v = sV + (E4M3 ? 0 : buf * kTl);
     if constexpr (E4M3) {
-      e4m3_to_bf16(k, sRaw + 2 * buf * kRawTile);
-      e4m3_to_bf16(v, sRaw + (2 * buf + 1) * kRawTile);
+      e4m3_to_bf16<HD>(k, sRaw + 2 * buf * kRawTile<HD>);
+      e4m3_to_bf16<HD>(v, sRaw + (2 * buf + 1) * kRawTile<HD>);
     }
     // tile rows holding a window slot no row of the tile sees
     const int sh = c0 - p32;
     const uint64_t zero = sh >= 0 ? (sh < 64 ? unseen >> sh : 0) : (sh > -64 ? unseen << -sh : 0);
     if (zero) {
-      for (int i = threadIdx.x; i < BT * 16; i += kThreads)
-        if ((zero >> (i >> 4)) & 1) *(uint4*)(v + (i >> 4) * LDS<HD> + (i & 15) * 8) = make_uint4(0, 0, 0, 0);
+      for (int i = threadIdx.x; i < BT * kChunks; i += kThreads) {
+        const int r = kPow2 ? i >> (kChunks == 16 ? 4 : 3) : i / kChunks, c = kPow2 ? i & (kChunks - 1) : i % kChunks;
+        if ((zero >> r) & 1) *(uint4*)(v + r * LDS<HD> + c * 8) = make_uint4(0, 0, 0, 0);
+      }
     }
     if (E4M3 || zero) __syncthreads();
     float s[8][4];
@@ -780,13 +790,7 @@ static void dispatch(int D, bool mask, bool window, F&& f) {
     if (mask) with_window(hd, std::true_type{});
     else with_window(hd, std::false_type{});
   };
-  switch (D) {
-    case 64: with_mask(std::integral_constant<int, 64>{}); break;
-    case 80: with_mask(std::integral_constant<int, 80>{}); break;
-    case 96: with_mask(std::integral_constant<int, 96>{}); break;
-    case 128: with_mask(std::integral_constant<int, 128>{}); break;
-    default: nxd_throw("attention: head_dim must be 64, 80, 96 or 128", __FILE__, __LINE__);
-  }
+  dispatch_head_dim(D, "attention", with_mask);
 }
 
 template <int HD, bool MASK, bool WINDOW>
@@ -875,8 +879,8 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
 }
 
 void speculation_attention(const void* q, const void* k, const void* v, const long* positions, const void* mask,
-                           const long* depth, void* out, float* part_o, float* part_ml, int B, int W, int H, int Hkv, int L,
-                           const long* qs, const long* ks, const long* vs, float scale, int window, int splits, bool kv_e4m3,
+                           const long* depth, void* out, float* part_o, float* part_ml, int B, int W, int H, int Hkv, int D,
+                           int L, const long* qs, const long* ks, const long* vs, float scale, int window, int splits, bool kv_e4m3,
                            float k_scale, float v_scale, bool rolling, cudaStream_t st) {
   using namespace fa;
   const int G = H / Hkv;
@@ -890,34 +894,38 @@ void speculation_attention(const void* q, const void* k, const void* v, const lo
   p.scale_log2 = scale * kLog2e * k_scale;
   p.v_scale = v_scale;
   const dim3 grid(p.row_tiles * splits, Hkv, B);
-  auto launch = [&](auto g, auto e4, auto roll) {
-    constexpr int Gv = decltype(g)::value;
+  // the shared-memory attribute is set once per (HD, G, E4M3, ROLL) instantiation, before its first launch
+  auto launch = [&](auto hd, auto g, auto e4, auto roll) {
+    constexpr int HD = decltype(hd)::value, Gv = decltype(g)::value;
     constexpr bool E4 = decltype(e4)::value, R = decltype(roll)::value;
     static bool configured = false;
     if (!configured) {
-      NXD_CUDA_CHECK(cudaFuncSetAttribute(spec_attn_kernel<Gv, E4, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemSpec<E4>));
+      NXD_CUDA_CHECK(cudaFuncSetAttribute(spec_attn_kernel<HD, Gv, E4, R>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          kSmemSpec<HD, E4>));
       configured = true;
     }
-    spec_attn_kernel<Gv, E4, R><<<grid, kThreads, kSmemSpec<E4>, st>>>(p);
+    spec_attn_kernel<HD, Gv, E4, R><<<grid, kThreads, kSmemSpec<HD, E4>, st>>>(p);
   };
-  auto with_roll = [&](auto g, auto e4) {
-    if (rolling) launch(g, e4, std::true_type{});
-    else launch(g, e4, std::false_type{});
+  auto with_roll = [&](auto hd, auto g, auto e4) {
+    if (rolling) launch(hd, g, e4, std::true_type{});
+    else launch(hd, g, e4, std::false_type{});
   };
-  auto with_cache = [&](auto g) {
-    if (kv_e4m3) with_roll(g, std::true_type{});
-    else with_roll(g, std::false_type{});
+  auto with_cache = [&](auto hd, auto g) {
+    if (kv_e4m3) with_roll(hd, g, std::true_type{});
+    else with_roll(hd, g, std::false_type{});
   };
-  switch (G) {
-    case 1: with_cache(std::integral_constant<int, 1>{}); break;
-    case 2: with_cache(std::integral_constant<int, 2>{}); break;
-    case 4: with_cache(std::integral_constant<int, 4>{}); break;
-    case 8: with_cache(std::integral_constant<int, 8>{}); break;
-    default: nxd_throw("speculation_attention: unsupported GQA group size", __FILE__, __LINE__);
-  }
+  dispatch_head_dim(D, "speculation_attention", [&](auto hd) {
+    switch (G) {
+      case 1: with_cache(hd, std::integral_constant<int, 1>{}); break;
+      case 2: with_cache(hd, std::integral_constant<int, 2>{}); break;
+      case 4: with_cache(hd, std::integral_constant<int, 4>{}); break;
+      case 8: with_cache(hd, std::integral_constant<int, 8>{}); break;
+      default: nxd_throw("speculation_attention: unsupported GQA group size", __FILE__, __LINE__);
+    }
+  });
   NXD_CUDA_CHECK(cudaGetLastError());
-  // row (b·W + w)·H + h of the partials → out [B, W, H, 128]
-  decode_combine(part_o, part_ml, out, B * W * H, splits, (long)H * 128, 128, H, st);
+  // row (b·W + w)·H + h of the partials → out [B, W, H, D]
+  decode_combine(part_o, part_ml, out, B * W * H, splits, D, (long)H * D, D, H, st);
 }
 
 }  // namespace nxd

@@ -301,7 +301,7 @@ static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, 
 }
 
 // ---- decode ---------------------------------------------------------------------------------------
-// q [B,1,H,128]; k/v cache [B,L,Hkv,128] (any b/s/h strides, head_dim contiguous); positions [B] int64 (attend to ≤ pos);
+// q [B,1,H,D]; k/v cache [B,L,Hkv,D], D ∈ {64, 80, 96, 128} (any b/s/h strides, head_dim contiguous); positions [B] int64 (attend to ≤ pos);
 // window > 0: only the last `window` positions up to pos are visible.  The cache is bf16, or e4m3 with per-tensor scales
 // (the kernel then loads 8 bytes per lane: base pointers and strides must be multiples of 8 elements, as on bf16)
 static int decode_splits(int B, int Hkv, int L, int64_t window) {
@@ -312,13 +312,17 @@ static int decode_splits(int B, int Hkv, int L, int64_t window) {
   return std::max(1, std::min(std::min(splits, 64), (rows + 63) / 64));
 }
 // argument checks shared by decode_attention, decode_attention_partial (one token per sequence) and speculation_attention
-// (max_tokens = 64); returns true for an e4m3 cache
+// (max_tokens = 64); returns true for an e4m3 cache.  The head sizes are those of the flash kernels (check_qkv).
 static bool check_decode_args(const char* fn, const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions,
                               double k_scale, double v_scale, int64_t max_tokens = 1) {
+  const int64_t d = q.dim() == 4 ? q.size(3) : 0;
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.size(1) >= 1 && q.size(1) <= max_tokens &&
-              q.size(3) == 128 && q.stride(3) == 1);
+                  (d == 64 || d == 80 || d == 96 || d == 128) && q.stride(3) == 1,
+              fn, ": expected a bf16 CUDA q [B,W,H,D] view (W = 1; verification: W <= 64) with D in {64, 80, 96, 128} and "
+              "contiguous head_dim");
   const bool e4m3 = kv_cache_e4m3(fn, k, v, k_scale, v_scale);
-  TORCH_CHECK(k.dim() == 4 && k.size(3) == 128 && k.stride(3) == 1 && v.stride(3) == 1 && v.sizes() == k.sizes());
+  TORCH_CHECK(k.dim() == 4 && k.size(3) == d && k.stride(3) == 1 && v.stride(3) == 1 && v.sizes() == k.sizes(),
+              fn, ": expected k / v caches [B,L,Hkv,D] of one shape, with q's D and contiguous head_dim");
   TORCH_CHECK(positions.scalar_type() == at::kLong && positions.is_cuda() && positions.is_contiguous() && positions.numel() == q.size(0));
   TORCH_CHECK(q.size(2) % k.size(2) == 0 && k.size(0) == q.size(0));
   TORCH_CHECK(q.stride(2) % 8 == 0 && k.stride(1) % 8 == 0 && k.stride(2) % 8 == 0 && v.stride(1) % 8 == 0 && v.stride(2) % 8 == 0);
@@ -332,42 +336,42 @@ static bool check_decode_args(const char* fn, const Tensor& q, const Tensor& k, 
 static Tensor decode_attention(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions, double scale,
                                int64_t window, double k_scale, double v_scale, bool rolling) {
   const bool e4m3 = check_decode_args("decode_attention", q, k, v, positions, k_scale, v_scale);
-  const int B = q.size(0), H = q.size(2), L = k.size(1), Hkv = k.size(2);
+  const int B = q.size(0), H = q.size(2), D = q.size(3), L = k.size(1), Hkv = k.size(2);
   TORCH_CHECK(!rolling || (window > 0 && window < L), "decode_attention: a rolling cache needs 0 < window < L (",
                     L, " rows), got window ", window);
   c10::cuda::CUDAGuard guard(q.device());
   const int splits = decode_splits(B, Hkv, L, window);
-  Tensor out = at::empty({B, 1, H, 128}, q.options());
-  Tensor part_o = at::empty({B * H * splits, 128}, q.options().dtype(at::kFloat));
+  Tensor out = at::empty({B, 1, H, D}, q.options());
+  Tensor part_o = at::empty({B * H * splits, D}, q.options().dtype(at::kFloat));
   Tensor part_ml = at::empty({B * H * splits, 2}, q.options().dtype(at::kFloat));
   const long ks[3] = {k.stride(0), k.stride(1), k.stride(2)}, vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   nxd::decode_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), out.data_ptr(),
-                        part_o.data_ptr<float>(), part_ml.data_ptr<float>(), B, H, Hkv, L, ks, vs, q.stride(0), q.stride(2),
+                        part_o.data_ptr<float>(), part_ml.data_ptr<float>(), B, H, Hkv, D, L, ks, vs, q.stride(0), q.stride(2),
                         out.stride(0), out.stride(2), (float)scale, splits, (int)std::min<int64_t>(window, INT32_MAX), stream(),
                         nullptr, nullptr, e4m3, (float)k_scale, (float)v_scale, rolling);
   return out;
 }
-// This rank's contribution to distributed flash-decoding: un-normalised output (relative to the row maximum) [B,H,128] fp32 and
+// This rank's contribution to distributed flash-decoding: un-normalised output (relative to the row maximum) [B,H,D] fp32 and
 // (row maximum in natural-log units, row sum) [B,H,2] fp32 over the local cache shard; ``positions`` are LOCAL (may be < 0 or
 // >= L: nothing / everything of this shard is visible).
 static std::vector<Tensor> decode_attention_partial(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions,
                                                     double scale, int64_t window, double k_scale, double v_scale) {
   const bool e4m3 = check_decode_args("decode_attention_partial", q, k, v, positions, k_scale, v_scale);
-  const int B = q.size(0), H = q.size(2), L = k.size(1), Hkv = k.size(2);
+  const int B = q.size(0), H = q.size(2), D = q.size(3), L = k.size(1), Hkv = k.size(2);
   c10::cuda::CUDAGuard guard(q.device());
   const int splits = decode_splits(B, Hkv, L, window);
-  Tensor fin_o = at::empty({B, H, 128}, q.options().dtype(at::kFloat));
+  Tensor fin_o = at::empty({B, H, D}, q.options().dtype(at::kFloat));
   Tensor fin_ml = at::empty({B, H, 2}, q.options().dtype(at::kFloat));
-  Tensor part_o = at::empty({B * H * splits, 128}, q.options().dtype(at::kFloat));
+  Tensor part_o = at::empty({B * H * splits, D}, q.options().dtype(at::kFloat));
   Tensor part_ml = at::empty({B * H * splits, 2}, q.options().dtype(at::kFloat));
   const long ks[3] = {k.stride(0), k.stride(1), k.stride(2)}, vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   nxd::decode_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), nullptr, part_o.data_ptr<float>(),
-                        part_ml.data_ptr<float>(), B, H, Hkv, L, ks, vs, q.stride(0), q.stride(2), 0, 0, (float)scale, splits,
+                        part_ml.data_ptr<float>(), B, H, Hkv, D, L, ks, vs, q.stride(0), q.stride(2), 0, 0, (float)scale, splits,
                         (int)std::min<int64_t>(window, INT32_MAX), stream(), fin_o.data_ptr<float>(), fin_ml.data_ptr<float>(),
                         e4m3, (float)k_scale, (float)v_scale);
   return {fin_o, fin_ml};
 }
-// q [B,W≤64,H,128] (any b/s/h strides, rows 16-byte aligned) verified against the cache as decode_attention reads it; tree_mask
+// q [B,W≤64,H,D] (any b/s/h strides, rows 16-byte aligned) verified against the cache as decode_attention reads it; tree_mask
 // [W,W] bool / uint8 and tree_depth [W] int64 (both or neither: a chain).  Never reads them on the host.  rolling: a ring of L
 // rows, as in decode_attention.
 static Tensor speculation_attention(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& positions,
@@ -375,7 +379,7 @@ static Tensor speculation_attention(const Tensor& q, const Tensor& k, const Tens
                                     int64_t window, double k_scale, double v_scale, bool rolling) {
   const char* fn = "speculation_attention";
   const bool e4m3 = check_decode_args(fn, q, k, v, positions, k_scale, v_scale, 64);
-  const int B = q.size(0), W = q.size(1), H = q.size(2), L = k.size(1), Hkv = k.size(2), G = H / Hkv;
+  const int B = q.size(0), W = q.size(1), H = q.size(2), D = q.size(3), L = k.size(1), Hkv = k.size(2), G = H / Hkv;
   TORCH_CHECK(G == 1 || G == 2 || G == 4 || G == 8, fn, ": the GQA group size must be 1, 2, 4 or 8");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0 && q.stride(0) % 8 == 0 && q.stride(1) % 8 == 0,
               fn, ": q rows must be 16-byte aligned");
@@ -406,13 +410,13 @@ static Tensor speculation_attention(const Tensor& q, const Tensor& k, const Tens
   const int64_t rows = window > 0 ? std::min<int64_t>(L, std::min<int64_t>(window, L) + W - 1) : L;
   const int ctas = B * Hkv * row_tiles;
   const int splits = std::max(1, std::min({(4 * num_sms() + ctas - 1) / ctas, 64, (int)((rows + 127) / 128)}));
-  Tensor out = at::empty({B, W, H, 128}, q.options());
-  Tensor part_o = at::empty({(int64_t)B * W * H * splits, 128}, q.options().dtype(at::kFloat));
+  Tensor out = at::empty({B, W, H, D}, q.options());
+  Tensor part_o = at::empty({(int64_t)B * W * H * splits, D}, q.options().dtype(at::kFloat));
   Tensor part_ml = at::empty({(int64_t)B * W * H * splits, 2}, q.options().dtype(at::kFloat));
   const long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
   const long ks[3] = {k.stride(0), k.stride(1), k.stride(2)}, vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   nxd::speculation_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), mp, dp, out.data_ptr(),
-                             part_o.data_ptr<float>(), part_ml.data_ptr<float>(), B, W, H, Hkv, L, qs, ks, vs, (float)scale,
+                             part_o.data_ptr<float>(), part_ml.data_ptr<float>(), B, W, H, Hkv, D, L, qs, ks, vs, (float)scale,
                              (int)std::min<int64_t>(window, INT32_MAX), splits, e4m3, (float)k_scale, (float)v_scale, rolling,
                              stream());
   return out;

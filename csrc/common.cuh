@@ -23,9 +23,23 @@
 inline void nxd_throw(const std::string& msg, const char* file, int line) {
   throw std::runtime_error(msg + " (" + file + ":" + std::to_string(line) + ")");
 }
+#include <type_traits>
 #endif
 
 namespace nxd {
+
+// f(std::integral_constant<int, HD>{}) for a runtime head dimension: the head sizes every attention kernel (flash forward and
+// backward, decode, verification) is instantiated for.  `fn` names the caller in the error for any other size.
+template <class F>
+inline void dispatch_head_dim(int D, const char* fn, F&& f) {
+  switch (D) {
+    case 64: f(std::integral_constant<int, 64>{}); break;
+    case 80: f(std::integral_constant<int, 80>{}); break;
+    case 96: f(std::integral_constant<int, 96>{}); break;
+    case 128: f(std::integral_constant<int, 128>{}); break;
+    default: nxd_throw(std::string(fn) + ": head_dim must be 64, 80, 96 or 128", __FILE__, __LINE__);
+  }
+}
 
 // ---------------------------------------------------------------- type helpers
 template <typename T> struct Vec8;  // 8 elements of a 16-bit type = 16 bytes

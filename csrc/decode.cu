@@ -17,8 +17,10 @@ namespace nxd {
 
 namespace {
 
-constexpr int HD = 128;
 constexpr int kDecThreads = 128;
+// Without a minimum-blocks hint ptxas held three HD ≠ 128 instantiations (G = 2) to 64 or 80 registers, which spilled; a
+// floor of one CTA per SM lets it allocate what they need.  0 (no hint) keeps the HD = 128 instantiations as they were.
+template <int HD> constexpr int kDecMinBlocks = HD == 128 ? 0 : 1;
 
 // 8 consecutive elements → fp32 (bf16: one 16-byte load; e4m3: one 8-byte load and the hardware fp8x2 → f16x2 unpack)
 __device__ __forceinline__ void load8(const __nv_bfloat16* p, float (&f)[8], float mul) {
@@ -37,28 +39,38 @@ __device__ __forceinline__ void load8(const __nv_fp8_e4m3* p, float (&f)[8], flo
   }
 }
 
-// 16 lanes share one kv position (8 dims each); a warp covers 2 positions per step, the CTA 8.  A bf16 lane loads 16 bytes
-// of K and of V per position and takes one position per step (P = 1).  An e4m3 lane gets 8 bytes per position, so it takes
-// P = 2 positions per step (a warp covers 4, the CTA 16): each lane still has 32 bytes of K/V in flight per step, as on bf16,
-// and keeps the bf16 kernel's per-lane softmax state (P = 1 would halve the bytes in flight of a kernel that is latency-bound
-// per CTA).  The other way to keep 16-byte loads, 8 lanes × 16 dims, doubles each lane's q and o registers: G = 8 uses 184
-// registers on bf16 already, so it would spill there.  For G ≤ 4 that mapping fits and would halve the softmax updates per
-// position (16 lanes repeat the same one here); it has not been timed against this one (DESIGN §6).
+// HD = 128: 16 lanes share one kv position (8 dims each); a warp covers 2 positions per step, the CTA 8.  A bf16 lane loads
+// 16 bytes of K and of V per position and takes one position per step (P = 1).  An e4m3 lane gets 8 bytes per position, so
+// it takes P = 2 positions per step (a warp covers 4, the CTA 16): each lane still has 32 bytes of K/V in flight per step, as
+// on bf16, and keeps the bf16 kernel's per-lane softmax state (P = 1 would halve the bytes in flight of a kernel that is
+// latency-bound per CTA).  The other way to keep 16-byte loads, 8 lanes × 16 dims, doubles each lane's q and o registers:
+// G = 8 uses 184 registers on bf16 already, so it would spill there.  For G ≤ 4 that mapping fits and would halve the softmax
+// updates per position (16 lanes repeat the same one here); it has not been timed against this one (DESIGN §6).
+// Other head sizes keep 8 dims (16 bytes of bf16, 8 of e4m3) and the same softmax state per lane:
+//   HD = 64: 8 lanes per position, so a warp covers 4 positions per step (8 on e4m3); the dot product reduces over xor 1, 2
+//            and 4, and the 4 position slots of a warp merge over xor 8 and 16 before the merge across the 4 warps.
+//   HD = 80 / 96: 16-lane groups of which HD / 8 = 10 / 12 lanes hold dims.  The others load nothing, hold zeros and still
+//            take part in the shuffles; they idle 37.5 % (80) / 25 % (96) of the load slots.  5- or 6-dim lanes would not
+//            keep 16-byte loads.
 // k_scale is folded into scale_log2 by the host; v_scale multiplies the partial o (1 on bf16).
 // ROLL: the cache is a ring of L rows (inference/kv_cache.py, rolling mode) and logical position s lives in row s mod L.  The
 // visible range stays in logical positions and is not clipped to L; the host guarantees 0 < window < L, so it spans fewer
 // than L positions and row(s) = s − wrap0, minus L once past the end, with wrap0 = lo − lo mod L.
-template <typename T, int G, bool ROLL>
-__global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
+template <int HD, typename T, int G, bool ROLL>
+__global__ void __launch_bounds__(kDecThreads, kDecMinBlocks<HD>) decode_attn_kernel(
     const __nv_bfloat16* __restrict__ q, const T* __restrict__ kc, const T* __restrict__ vc,
     const long* __restrict__ positions, float* __restrict__ part_o, float* __restrict__ part_ml, int B, int H, int Hkv, int L,
     long k_sb, long k_ss, long k_sh, long v_sb, long v_ss, long v_sh, long q_sb, long q_sh, float scale_log2, int splits,
     int window, float v_scale) {
   constexpr bool kE4M3 = sizeof(T) == 1;
   constexpr int P = kE4M3 ? 2 : 1;                          // positions per lane per step
+  constexpr int kLaneBits = HD == 64 ? 3 : 4;               // lanes per position = 1 << kLaneBits
+  constexpr int kLanes = 1 << kLaneBits, kSlots = 32 / kLanes;   // position slots of a warp step
+  static_assert(HD % 8 == 0 && HD / 8 <= kLanes && HD <= kDecThreads, "decode_attn_kernel: unsupported head_dim");
   const int kvh = blockIdx.x, b = blockIdx.y, split = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int sub = lane >> 4, l16 = lane & 15;               // position slot within the warp step, 8-dim slice
+  const int sub = lane >> kLaneBits, l16 = lane & (kLanes - 1);   // position slot within the warp step, 8-dim slice
+  const bool act = HD / 8 == kLanes || l16 < HD / 8;        // the lane holds dims (HD = 80 / 96: 10 / 12 of 16 lanes do)
   // visible rows [lo, hi): the splits divide this range.  Positions may lie outside [0, L) (the local positions of a sequence
   // shard); then the range is clipped to the cache, and it is empty when the window ends before row 0 or starts past L.
   const long pos = positions[b];
@@ -76,7 +88,14 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
 
   float qf[G][8];
 #pragma unroll
-  for (int g = 0; g < G; ++g) load8(q + b * q_sb + (long)(kvh * G + g) * q_sh + l16 * 8, qf[g], scale_log2);
+  for (int g = 0; g < G; ++g) {
+    if (act) {
+      load8(q + b * q_sb + (long)(kvh * G + g) * q_sh + l16 * 8, qf[g], scale_log2);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) qf[g][i] = 0.f;
+    }
+  }
   float m[G], l[G], o[G][8];
 #pragma unroll
   for (int g = 0; g < G; ++g) {
@@ -86,17 +105,17 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
   }
   const T* kb = kc + b * k_sb + (long)kvh * k_sh + l16 * 8;
   const T* vb = vc + b * v_sb + (long)kvh * v_sh + l16 * 8;
-  for (int sbase = s0 + warp * 2 * P; sbase < s1; sbase += 8 * P) {      // warp-uniform trip count (full-mask shuffles inside)
+  for (int sbase = s0 + warp * kSlots * P; sbase < s1; sbase += 4 * kSlots * P) {   // warp-uniform trip count (full-mask shuffles inside)
     bool live[P];
     float kf[P][8], vf[P][8];
 #pragma unroll
     for (int j = 0; j < P; ++j) {                         // all loads of the step are issued before any math
-      const int s = sbase + 2 * j + sub;
+      const int s = sbase + kSlots * j + sub;
       live[j] = s < s1;
-      if constexpr (kE4M3) {                              // a position past s1 re-reads row s1 − 1; its score is not used
+      if (kE4M3 && act) {                                 // a position past s1 re-reads row s1 − 1; its score is not used
         load8(kb + (long)row(min(s, s1 - 1)) * k_ss, kf[j], 1.f);
         load8(vb + (long)row(min(s, s1 - 1)) * v_ss, vf[j], 1.f);
-      } else if (live[j]) {
+      } else if (!kE4M3 && live[j] && act) {
         load8(kb + (long)row(s) * k_ss, kf[j], 1.f);
         load8(vb + (long)row(s) * v_ss, vf[j], 1.f);
       } else {
@@ -114,7 +133,8 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
         d += __shfl_xor_sync(0xffffffffu, d, 1);
         d += __shfl_xor_sync(0xffffffffu, d, 2);
         d += __shfl_xor_sync(0xffffffffu, d, 4);
-        d += __shfl_xor_sync(0xffffffffu, d, 8);          // score·log2e of (position s, head g) in all 16 lanes
+        if constexpr (kLanes == 16) d += __shfl_xor_sync(0xffffffffu, d, 8);
+        // d: score·log2e of (position s, head g) in all lanes of the position
         if (live[j]) {
           const float mn = fmaxf(m[g], d);
           const float corr = exp2f(m[g] - mn), p = exp2f(d - mn);
@@ -126,30 +146,37 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
       }
     }
   }
-  // merge the 2 position slots of the warp (lanes l16, l16+16), then the 4 warps through smem
+  // merge the position slots of the warp (HD = 64: lanes l16 + 8·sub over xor 8 and 16; else l16, l16 + 16 over xor 16),
+  // then the 4 warps through smem
   __shared__ float sm_o[4][G][HD];
   __shared__ float sm_m[4][G], sm_l[4][G];
 #pragma unroll
   for (int g = 0; g < G; ++g) {
-    const float m2 = __shfl_xor_sync(0xffffffffu, m[g], 16), l2 = __shfl_xor_sync(0xffffffffu, l[g], 16);
-    const float mn = fmaxf(m[g], m2);
-    const float c1 = mn == -INFINITY ? 0.f : exp2f(m[g] - mn), c2 = mn == -INFINITY ? 0.f : exp2f(m2 - mn);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float o2 = __shfl_xor_sync(0xffffffffu, o[g][i], 16);
-      o[g][i] = o[g][i] * c1 + o2 * c2;
+    for (int x = kLanes; x < 32; x *= 2) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, m[g], x), l2 = __shfl_xor_sync(0xffffffffu, l[g], x);
+      const float mn = fmaxf(m[g], m2);
+      const float c1 = mn == -INFINITY ? 0.f : exp2f(m[g] - mn), c2 = mn == -INFINITY ? 0.f : exp2f(m2 - mn);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float o2 = __shfl_xor_sync(0xffffffffu, o[g][i], x);
+        o[g][i] = o[g][i] * c1 + o2 * c2;
+      }
+      l[g] = l[g] * c1 + l2 * c2;
+      m[g] = mn;
     }
-    l[g] = l[g] * c1 + l2 * c2;
-    m[g] = mn;
     if (sub == 0) {
+      if (act) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) sm_o[warp][g][l16 * 8 + i] = o[g][i];
+        for (int i = 0; i < 8; ++i) sm_o[warp][g][l16 * 8 + i] = o[g][i];
+      }
       if (l16 == 0) { sm_m[warp][g] = m[g]; sm_l[warp][g] = l[g]; }
     }
   }
   __syncthreads();
-  // thread t = dim; loop over heads of the group
+  // thread t = dim (threads ≥ HD write nothing); loop over heads of the group
   const int d = threadIdx.x;
+  if (HD < kDecThreads && d >= HD) return;
 #pragma unroll
   for (int g = 0; g < G; ++g) {
     float mn = fmaxf(fmaxf(sm_m[0][g], sm_m[1][g]), fmaxf(sm_m[2][g], sm_m[3][g]));
@@ -167,6 +194,8 @@ __global__ void __launch_bounds__(kDecThreads) decode_attn_kernel(
   }
 }
 
+// one CTA of HD threads per output row; partial rows [rows·splits, HD]
+template <int HD>
 __global__ void __launch_bounds__(HD) decode_combine_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml,
                                                             __nv_bfloat16* __restrict__ out, int splits, long o_sb, long o_sh,
                                                             int H) {
@@ -187,6 +216,7 @@ __global__ void __launch_bounds__(HD) decode_combine_kernel(const float* __restr
 // Same merge over the splits, but the result stays un-normalised: o (relative to the row maximum), the maximum (natural-log
 // units) and the row sum — what a rank contributes to distributed flash-decoding, where the final normalisation happens after
 // the cross-rank log-sum-exp merge (modules/attention/flash_decode.py).
+template <int HD>
 __global__ void __launch_bounds__(HD) decode_combine_partial_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml,
                                                                     float* __restrict__ fin_o, float* __restrict__ fin_ml, int splits) {
   const int bh = blockIdx.x, d = threadIdx.x;
@@ -355,14 +385,16 @@ void decode_rope_kv(const void* q, const void* k, const void* v, const long* pos
 }
 
 void decode_attention(const void* q, const void* k, const void* v, const long* positions, void* out, float* part_o,
-                      float* part_ml, int B, int H, int Hkv, int L, const long* ks, const long* vs, long q_sb, long q_sh,
+                      float* part_ml, int B, int H, int Hkv, int D, int L, const long* ks, const long* vs, long q_sb, long q_sh,
                       long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o, float* fin_ml,
                       bool kv_e4m3, float k_scale, float v_scale, bool rolling) {
   const int G = H / Hkv;
   dim3 grid(Hkv, B, splits);
   const float sl2 = scale * 1.4426950408889634f * k_scale;
-#define NXD_DEC(T, Gv, R)                                                                                                 \
-  decode_attn_kernel<T, Gv, R><<<grid, kDecThreads, 0, st>>>((const __nv_bfloat16*)q, (const T*)k, (const T*)v, positions, \
+  dispatch_head_dim(D, "decode_attention", [&](auto hd) {
+    constexpr int HD = decltype(hd)::value;
+#define NXD_DEC(T, Gv, R)                                                                                                     \
+  decode_attn_kernel<HD, T, Gv, R><<<grid, kDecThreads, 0, st>>>((const __nv_bfloat16*)q, (const T*)k, (const T*)v, positions, \
       part_o, part_ml, B, H, Hkv, L, ks[0], ks[1], ks[2], vs[0], vs[1], vs[2], q_sb, q_sh, sl2, splits, window, v_scale)
 #define NXD_DEC_R(T, Gv)             \
   if (rolling) NXD_DEC(T, Gv, true); \
@@ -375,19 +407,23 @@ void decode_attention(const void* q, const void* k, const void* v, const long* p
     case 8: NXD_DEC_R(T, 8); break;                                                       \
     default: nxd_throw("decode_attention: unsupported GQA group size", __FILE__, __LINE__); \
   }
-  if (kv_e4m3) NXD_DEC_G(__nv_fp8_e4m3)
-  else NXD_DEC_G(__nv_bfloat16)
+    if (kv_e4m3) NXD_DEC_G(__nv_fp8_e4m3)
+    else NXD_DEC_G(__nv_bfloat16)
 #undef NXD_DEC_G
 #undef NXD_DEC_R
 #undef NXD_DEC
-  if (fin_o != nullptr) decode_combine_partial_kernel<<<B * H, HD, 0, st>>>(part_o, part_ml, fin_o, fin_ml, splits);
-  else decode_combine_kernel<<<B * H, HD, 0, st>>>(part_o, part_ml, (__nv_bfloat16*)out, splits, o_sb, o_sh, H);
+    if (fin_o != nullptr) decode_combine_partial_kernel<HD><<<B * H, HD, 0, st>>>(part_o, part_ml, fin_o, fin_ml, splits);
+    else decode_combine_kernel<HD><<<B * H, HD, 0, st>>>(part_o, part_ml, (__nv_bfloat16*)out, splits, o_sb, o_sh, H);
+  });
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 
-void decode_combine(const float* part_o, const float* part_ml, void* out, int rows, int splits, long o_sb, long o_sh, int H,
-                    cudaStream_t st) {
-  decode_combine_kernel<<<rows, HD, 0, st>>>(part_o, part_ml, (__nv_bfloat16*)out, splits, o_sb, o_sh, H);
+void decode_combine(const float* part_o, const float* part_ml, void* out, int rows, int splits, int D, long o_sb, long o_sh,
+                    int H, cudaStream_t st) {
+  dispatch_head_dim(D, "decode_combine", [&](auto hd) {
+    constexpr int HD = decltype(hd)::value;
+    decode_combine_kernel<HD><<<rows, HD, 0, st>>>(part_o, part_ml, (__nv_bfloat16*)out, splits, o_sb, o_sh, H);
+  });
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 

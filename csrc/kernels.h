@@ -131,10 +131,11 @@ void gemv_mx_grouped(const void* x, const void* w, const void* scale, const long
 
 // ---- decode (decode.cu)
 void decode_attention(const void* q, const void* k, const void* v, const long* positions, void* out, float* part_o,
-                      float* part_ml, int B, int H, int Hkv, int L, const long* ks, const long* vs, long q_sb, long q_sh,
-                      long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o,
+                      float* part_ml, int B, int H, int Hkv, int D, int L, const long* ks, const long* vs, long q_sb,
+                      long q_sh, long o_sb, long o_sh, float scale, int splits, int window, cudaStream_t st, float* fin_o,
                       float* fin_ml, bool kv_e4m3, float k_scale, float v_scale, bool rolling = false);
-                      // fin_o/fin_ml: un-normalised [B*H,128] + (max, sum) [B*H,2] instead of ``out`` (nullptr: ``out``)
+                      // q [B,1,H,D], k/v [B,L,Hkv,D] with D ∈ {64, 80, 96, 128}; part_o [B*H*splits, D]
+                      // fin_o/fin_ml: un-normalised [B*H,D] + (max, sum) [B*H,2] instead of ``out`` (nullptr: ``out``)
                       // window: keys positions[b] − window < j ≤ positions[b] visible (0: no window)
                       // kv_e4m3: k/v are fp8 e4m3 caches holding k / k_scale and v / v_scale (bf16: both scales 1)
                       // rolling: the cache is a ring of L rows, position j in row j mod L (needs 0 < window < L)
@@ -144,9 +145,9 @@ void decode_rope_kv(const void* q, const void* k, const void* v, const long* pos
                     const float* sin_t, void* q_out, void* kc, void* vc, int B, int W, int H, int Hkv, int D, int L, int n_pos,
                     const long* qs, const long* ks, const long* vs, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3,
                     float k_inv, float v_inv, bool rolling);   // kv_e4m3: the cache stores k·k_inv and v·v_inv as e4m3
-// merge of per-split decode partials [rows·splits, 128] + (max, sum) → bf16 row r at out + (r / H)·o_sb + (r % H)·o_sh
-void decode_combine(const float* part_o, const float* part_ml, void* out, int rows, int splits, long o_sb, long o_sh, int H,
-                    cudaStream_t st);
+// merge of per-split decode partials [rows·splits, D] + (max, sum) → bf16 row r at out + (r / H)·o_sb + (r % H)·o_sh
+void decode_combine(const float* part_o, const float* part_ml, void* out, int rows, int splits, int D, long o_sb, long o_sh,
+                    int H, cudaStream_t st);
 void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, cudaStream_t st);
 
 // ---- attention (attention_sm90.cu): q [B,S_q,H,D], k/v [B,S_kv,Hkv,D] bf16 views, D ∈ {64, 80, 96, 128}; strides = (b, s, h)
@@ -164,13 +165,14 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
                     const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, long window,
                     long q_offset, cudaStream_t st);
 
-// W ≤ 64 new tokens per sequence against a KV cache (speculation / Medusa verification): q [B,W,H,128] bf16, k/v caches
-// [B,L,Hkv,128] bf16 or e4m3 (kv_e4m3), H/Hkv ∈ {1,2,4,8}; mask uint8 [W,W] and depth int64 [W] (both null: a chain);
-// window: sliding window (0: none).  part_o [B·W·H·splits, 128] / part_ml [B·W·H·splits, 2] fp32 scratch; out [B,W,H,128].
+// W ≤ 64 new tokens per sequence against a KV cache (speculation / Medusa verification): q [B,W,H,D] bf16, k/v caches
+// [B,L,Hkv,D] bf16 or e4m3 (kv_e4m3), D ∈ {64, 80, 96, 128}, H/Hkv ∈ {1,2,4,8}; mask uint8 [W,W] and depth int64 [W] (both
+// null: a chain); window: sliding window (0: none).  part_o [B·W·H·splits, D] / part_ml [B·W·H·splits, 2] fp32 scratch; out
+// [B,W,H,D].
 // rolling: the cache is a ring of L rows, position j in row j mod L (needs window > 0 and window + W − 1 ≤ L).
 void speculation_attention(const void* q, const void* k, const void* v, const long* positions, const void* mask,
-                           const long* depth, void* out, float* part_o, float* part_ml, int B, int W, int H, int Hkv, int L,
-                           const long* qs, const long* ks, const long* vs, float scale, int window, int splits, bool kv_e4m3,
+                           const long* depth, void* out, float* part_o, float* part_ml, int B, int W, int H, int Hkv, int D,
+                           int L, const long* qs, const long* ks, const long* vs, float scale, int window, int splits, bool kv_e4m3,
                            float k_scale, float v_scale, bool rolling, cudaStream_t st);
 
 }  // namespace nxd

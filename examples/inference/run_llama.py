@@ -12,6 +12,9 @@ reference's ``examples/inference/run_llama.py`` / ``runner.py`` (trace → load 
   # Mistral-7B geometry (sliding window 4096): a rolling KV cache keeps 4096 + 64 rows per sequence instead of 8192
   torchrun --nproc-per-node 1 examples/inference/run_llama.py --model mistral-7b --batch_size 16 --max_prompt_length 2048 \
       --sequence_length 8192 --benchmark --num_runs 1 --rolling_kv_cache
+  # Llama-3.2-1B geometry (head_dim 64, 4 query heads per KV head) with random weights
+  torchrun --nproc-per-node 1 examples/inference/run_llama.py --model llama3.2-1b --batch_size 16 --max_prompt_length 2048 \
+      --sequence_length 4096 --benchmark
 """
 import argparse
 import json
@@ -41,9 +44,17 @@ def mistral_7b_config(**kw) -> LlamaConfig:
                        num_key_value_heads=8, sliding_window=4096, **kw)
 
 
+def llama3_2_1b_config(**kw) -> LlamaConfig:
+    """Llama-3.2-1B geometry: head_dim 2048 / 32 = 64, 8 KV heads (GQA group 4), rope_theta 500000.  Llama-3's rope
+    frequency scaling is not applied, so real Llama-3.2 weights would not reproduce the reference logits."""
+    return LlamaConfig(vocab_size=128256, hidden_size=2048, intermediate_size=8192, num_hidden_layers=16, num_attention_heads=32,
+                       num_key_value_heads=8, rope_theta=500000.0, **kw)
+
+
 def main():
     p = argparse.ArgumentParser()
-    p.add_argument("--model", default="tiny", choices=["tiny", "7b", "13b", "mistral-7b"])
+    p.add_argument("--model", default="tiny", choices=["tiny", "7b", "13b", "mistral-7b", "llama3.2-1b"],
+                   help="model geometry, random weights; llama3.2-1b runs without Llama-3 rope scaling")
     p.add_argument("--tp_degree", type=int, default=1)
     p.add_argument("--batch_size", type=int, default=1)
     p.add_argument("--max_prompt_length", type=int, default=128)
@@ -67,7 +78,8 @@ def main():
     ps.initialize_model_parallel(tensor_model_parallel_size=a.tp_degree)
     dtype = torch.bfloat16 if dev.type == "cuda" else torch.float32
     kw = dict(dtype=dtype, device=dev, max_position_embeddings=a.sequence_length)
-    cfg = {"7b": llama2_7b_config, "13b": llama2_13b_config, "mistral-7b": mistral_7b_config}.get(a.model, lambda **k: LlamaConfig(
+    cfg = {"7b": llama2_7b_config, "13b": llama2_13b_config, "mistral-7b": mistral_7b_config,
+           "llama3.2-1b": llama3_2_1b_config}.get(a.model, lambda **k: LlamaConfig(
         vocab_size=4096, hidden_size=512, intermediate_size=1408, num_hidden_layers=4, num_attention_heads=8, **k))(**kw)
     if a.num_layers > 0:
         cfg.num_hidden_layers = a.num_layers

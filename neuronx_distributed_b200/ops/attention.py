@@ -217,9 +217,9 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     ring of L rows holding position j in row j mod L (``KVCacheManager`` in rolling mode); needs 0 < W < L.
 
     This is the W = 1 chain of :func:`speculation_attention` (one token in slot p = position, seeing slots ≤ p), with the
-    stricter ring condition of a single token.  CUDA bf16 q with a bf16 or fp8 e4m3 cache and head_dim 128: the split-KV
-    flash-decoding kernel (``csrc/decode.cu``), which reads the e4m3 bytes directly; otherwise
-    :func:`speculation_attention_torch`."""
+    stricter ring condition of a single token.  CUDA bf16 q with a bf16 or fp8 e4m3 cache and a head_dim in
+    :data:`FLASH_HEAD_DIMS`: the split-KV flash-decoding kernel (``csrc/decode.cu``), which reads the e4m3 bytes directly;
+    otherwise :func:`speculation_attention_torch`."""
     B, _, H, D = q.shape
     Hkv, L = k_cache.shape[2], k_cache.shape[1]
     window = check_window(sliding_window)
@@ -229,7 +229,7 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
         kw["rolling"] = True
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     e = _ext.ext() if q.is_cuda else None
-    if (e is not None and hasattr(e, "decode_attention") and D == 128 and q.dtype == torch.bfloat16
+    if (e is not None and hasattr(e, "decode_attention") and D in FLASH_HEAD_DIMS and q.dtype == torch.bfloat16
             and k_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn) and H // Hkv in (1, 2, 4, 8) and k_cache.stride(3) == 1
             and v_cache.stride(3) == 1):
         _ext.count_launch(2)
@@ -322,10 +322,10 @@ def speculation_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch
     rows holding slot c in row c mod L (``KVCacheManager`` in rolling mode); needs SW > 0 and SW + W − 1 ≤ L, and the rule
     above then applies to logical slots without the bound at L.
 
-    CUDA bf16 q with head_dim 128, W ≤ 64, H / Hkv ∈ {1, 2, 4, 8} and a bf16 or fp8 e4m3 cache whose rows are aligned as
-    :func:`decode_attention` needs: the kernel in ``csrc/attention_sm90.cu``, which reads each K / V row once for all W
-    tokens and the GQA group, reads e4m3 as stored, and with a window only the slots some token can see.  ``tree_mask``
-    and ``tree_depth`` are never read on the host there, so the call can be captured in a CUDA graph.  Otherwise
+    CUDA bf16 q with a head_dim in :data:`FLASH_HEAD_DIMS`, W ≤ 64, H / Hkv ∈ {1, 2, 4, 8} and a bf16 or fp8 e4m3 cache whose
+    rows are aligned as :func:`decode_attention` needs: the kernel in ``csrc/attention_sm90.cu``, which reads each K / V
+    row once for all W tokens and the GQA group, reads e4m3 as stored, and with a window only the slots some token can see.
+    ``tree_mask`` and ``tree_depth`` are never read on the host there, so the call can be captured in a CUDA graph.  Otherwise
     :func:`speculation_attention_torch`."""
     window, kw = _check_spec_args(q, k_cache, v_cache, tree_mask, tree_depth, sliding_window, k_scale, v_scale, rolling)
     if rolling:
@@ -334,7 +334,7 @@ def speculation_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     e = _ext.ext() if q.is_cuda else None
     align = 16 if k_cache.dtype == torch.bfloat16 else 8
-    if (e is not None and hasattr(e, "speculation_attention") and D == 128 and q.dtype == torch.bfloat16
+    if (e is not None and hasattr(e, "speculation_attention") and D in FLASH_HEAD_DIMS and q.dtype == torch.bfloat16
             and k_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn) and W <= SPEC_MAX_TOKENS
             and H // k_cache.shape[2] in (1, 2, 4, 8)
             and all(t.stride(3) == 1 and t.data_ptr() % align == 0 and all(s % 8 == 0 for s in t.stride()[:3])

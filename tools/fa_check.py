@@ -1,5 +1,6 @@
 """Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
 usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]] [--kv-fp8] [--spec] [--rolling]
+                                [--decode-dims]
 
 --perf times forward and forward+backward of the own kernels and of SDPA in the same process, alternating, at the shapes
 the models run (BERT-large with right padding, ViT-B/16, GPT-NeoX-20B per rank at TP=8, Pythia-2.8B, Llama-2-7B).  FLOPs
@@ -34,7 +35,16 @@ output.
 --rolling (with --perf) times ``decode_attention`` and ``speculation_attention`` on a rolling KV cache (SW + 64 = 4160 rows,
 position t in row t mod 4160) against the linear 32k cache holding the same history, alternating in one process: Mistral-7B
 (H 32, Hkv 8, SW 4096) at B = 1, 8 and 32, position 32767 − W, decode and the chain5 / tree10 / tree64 windows, bf16 and
-e4m3.  Both read the same rows, so the times should match; the outputs are checked bit for bit."""
+e4m3.  Both read the same rows, so the times should match; the outputs are checked bit for bit.
+
+--decode-dims (with --perf) times token generation at head_dim 64, 80 and 96 on the kernels against the path those head
+sizes took before the kernels took them (``speculation_attention_torch`` on the de-quantised cache for decode and
+verification, ``_local_partial``'s fp32 torch math for flash decoding's partial), alternating in one process: Llama-3.2-1B
+attention (H 32, Hkv 8, D 64), Phi-3-mini (H = Hkv = 32, D 96) and Pythia-2.8B heads (H = Hkv = 32, D 80), with the D = 128
+kernel on a Mistral-7B head geometry (H 32, Hkv 8) as the control; B = 1, 8, 32, L = 4096 and 32768 (pairs that fit the
+card), bf16 and e4m3 caches holding the same values, one-token decode, a 5-token chain and a random 64-node tree.  GB/s is
+the K and V bytes of the visible cache rows (from the shapes) over the time of the call.  The D = 128 control's torch path
+is timed only at B = 1 (it is the one the kernels have replaced since they exist).  The partial at B = 8, L = 4096."""
 import argparse
 import json
 import math
@@ -350,6 +360,107 @@ def spec_perf():
         torch.cuda.empty_cache()
 
 
+# name, H, Hkv, D
+DECODE_DIM_SHAPES = [
+    ("llama3.2_1b", 32, 8, 64),
+    ("phi3_mini", 32, 32, 96),
+    ("pythia2.8b", 32, 32, 80),
+    ("mistral7b_control", 32, 8, 128),
+]
+
+
+def decode_dims_perf():
+    """Decode, verification and flash decoding's partial at head_dim 64 / 80 / 96 (and the D = 128 control) on the kernels
+    against the torch paths those head sizes took before, alternating in one process, on a full cache (p = L − W)."""
+    from neuronx_distributed_b200.modules.attention.flash_decode import _local_partial
+
+    dev = torch.device("cuda")
+    print(json.dumps(gpu_info()), flush=True)
+    ks, vs = 0.05, 0.05
+    windows = [(n, m, d, W) for n, m, d, W in spec_windows(dev) if n != "tree10"]
+    for name, H, Hkv, D in DECODE_DIM_SHAPES:
+        for L in (4096, 32768):
+            for B in (1, 8, 32):
+                if 2 * B * L * Hkv * D * 2 > 24 * 2 ** 30:                 # bf16 + e4m3 + de-quantised copies must fit
+                    continue
+                g = torch.Generator(device=dev).manual_seed(L + B + D)
+                k8, v8 = ((torch.randn(B, L, Hkv, D, device=dev, generator=g) / s).to(torch.float8_e4m3fn) for s in (ks, vs))
+                k16, v16 = (k8.float() * ks).bfloat16(), (v8.float() * vs).bfloat16()
+                for wname, mask, depth, W in [("decode", None, None, 1)] + windows:
+                    q = torch.randn(B, W, H, D, device=dev, generator=g).bfloat16()
+                    pos = torch.full((B,), L - W, device=dev, dtype=torch.long)
+                    for cache in ("bf16", "e4m3"):
+                        kc, vc = (k16, v16) if cache == "bf16" else (k8, v8)
+                        kw = {} if cache == "bf16" else {"k_scale": ks, "v_scale": vs}
+                        if W == 1:
+                            def new():
+                                return attention.decode_attention(q, kc, vc, pos, **kw)
+                        else:
+                            def new():
+                                return attention.speculation_attention(q, kc, vc, pos, mask, depth, **kw)
+
+                        def old():
+                            kd, vd = (kc, vc) if cache == "bf16" else ((kc.float() * ks).bfloat16(), (vc.float() * vs).bfloat16())
+                            return attention.speculation_attention_torch(q, kd, vd, pos, mask, depth)
+
+                        n0 = _ext.launches()
+                        o_new = new()
+                        assert _ext.launches() == n0 + 2, "the kernel did not run"
+                        time_old = D != 128 or B == 1
+                        t = {"new": [], "old": []}
+                        iters = 20 if B * L <= 32768 else 5
+                        rec = {"bench": f"{name}_{wname}", "cache": cache, "B": B, "L": L, "H": H, "Hkv": Hkv, "D": D, "W": W}
+                        if time_old:
+                            o_old = old()
+                            rec["rel_err_vs_old"] = round(((o_new.float() - o_old.float()).abs().max()
+                                                           / o_old.float().abs().max()).item(), 5)
+                            del o_old
+                        for _ in range(3):                         # alternate, keep each one's best
+                            t["new"].append(time_fn(new, iters))
+                            if time_old:
+                                t["old"].append(time_fn(old, iters))
+                        elt = 2 if cache == "bf16" else 1
+                        rec["kv_bytes"] = nbytes = 2 * B * L * Hkv * D * elt        # K and V rows, each read once
+                        for key in ("new", "old"):
+                            if not t[key]:
+                                rec[f"{key}_us"] = "not measured"
+                                continue
+                            ms = min(t[key])
+                            rec[f"{key}_us"] = round(ms * 1e3, 1)
+                            rec[f"{key}_GBps"] = round(nbytes / ms / 1e6, 1)
+                        if t["old"]:
+                            rec["speedup"] = round(rec["old_us"] / rec["new_us"], 2)
+                        print(json.dumps(rec), flush=True)
+                    del q
+                if L == 4096 and B == 8:                           # flash decoding's local partial: kernel vs fp32 torch math
+                    q = torch.randn(B, 1, H, D, device=dev, generator=g).bfloat16()
+                    local = torch.full((B,), L - 1, device=dev, dtype=torch.long)
+                    for cache in ("bf16", "e4m3"):
+                        kc, vc = (k16, v16) if cache == "bf16" else (k8, v8)
+                        sc = (1.0, 1.0) if cache == "bf16" else (ks, vs)
+                        new = lambda: _local_partial(q, kc, vc, local, 1.0 / math.sqrt(D), None, *sc)  # noqa: E731
+                        old = lambda: _local_partial(q.float(), kc, vc, local, 1.0 / math.sqrt(D), None, *sc)  # noqa: E731
+                        n0 = _ext.launches()
+                        new()
+                        assert _ext.launches() == n0 + 2, "the kernel did not run"
+                        t = {"new": [], "old": []}
+                        for _ in range(3):
+                            t["new"].append(time_fn(new, 20))
+                            t["old"].append(time_fn(old, 20))
+                        nbytes = 2 * B * L * Hkv * D * (2 if cache == "bf16" else 1)
+                        rec = {"bench": f"{name}_flash_decode_partial", "cache": cache, "B": B, "L": L, "H": H, "Hkv": Hkv, "D": D,
+                               "kv_bytes": nbytes}
+                        for key in ("new", "old"):
+                            ms = min(t[key])
+                            rec[f"{key}_us"] = round(ms * 1e3, 1)
+                            rec[f"{key}_GBps"] = round(nbytes / ms / 1e6, 1)
+                        rec["speedup"] = round(rec["old_us"] / rec["new_us"], 2)
+                        print(json.dumps(rec), flush=True)
+                    del q
+                del k8, v8, k16, v16
+                torch.cuda.empty_cache()
+
+
 def _ring_of(lin: torch.Tensor, rows: int, end: int) -> torch.Tensor:
     """The rolling cache (``inference.kv_cache``) of ``rows`` rows holding positions < ``end`` of the linear cache ``lin``."""
     j = torch.arange(rows, device=lin.device)
@@ -493,6 +604,8 @@ def main():
     ap.add_argument("--kv-fp8", action="store_true", help="with --perf: decode attention on bf16 vs fp8 e4m3 KV caches")
     ap.add_argument("--spec", action="store_true", help="with --perf: speculation / Medusa verification attention")
     ap.add_argument("--rolling", action="store_true", help="with --perf: decode / verification on rolling vs linear KV caches")
+    ap.add_argument("--decode-dims", action="store_true",
+                    help="with --perf: decode / verification / flash-decoding partial at head_dim 64, 80, 96 vs the torch path")
     ap.add_argument("--head-dim", type=int, default=128, choices=attention.FLASH_HEAD_DIMS)
     a = ap.parse_args()
     if a.perf and a.window and a.cp > 1 and not torch.cuda.is_available():
@@ -559,6 +672,8 @@ def main():
             spec_perf()
         elif a.rolling:
             rolling_perf()
+        elif a.decode_dims:
+            decode_dims_perf()
         elif a.window and a.cp > 1:
             cp_window_perf(a.bwd, a.cp)
         else:
