@@ -1,17 +1,21 @@
-// Flash attention for sm_90a (head_dim 64, 80, 96 or 128, bf16): warp-level bf16 tensor-core MMAs (mma.sync m16n8k16, ldmatrix operand
-// loads from padded shared memory, cp.async double-buffered tiles), fp32 online softmax.  Role parity: reference
+// Flash attention for sm_90a (head_dim 64, 80, 96 or 128, bf16): warpgroup tensor-core MMAs (wgmma.mma_async) on
+// 128B-swizzled shared-memory tiles filled by cp.async (double-buffered), fp32 online softmax.  Role parity: reference
 // kernels/flash_attn.py:162-212 (nki_flash_attn_func → flash_fwd / flash_attn_bwd) and modules/attention call sites.
 //
-// Forward, one CTA per (64-query tile, head, batch), 4 warps, warp w owns query rows 16w..16w+15 of the tile:
-//   S = Q·K_jᵀ (fp32 fragments), running max / sum in registers, P packed to bf16 straight from the S fragments into the
-//   A operand of O += P·V_j.  Outputs: O (bf16, arbitrary b/s/h strides) and LSE (fp32 [B, H, S], natural log).
+// Every kernel runs two warpgroups per CTA; warpgroup g owns rows 64g..64g+63 of the CTA's 128-row tile, and warp w of it
+// rows 16w..16w+15 of those, in the register layout of the mma.sync m16n8 fragments (which is the wgmma m64 layout).
+// Forward, one CTA per (128-query tile, head, batch), looping over 64-key tiles:
+//   S = Q·K_jᵀ (SS wgmma), running max / sum in registers, P packed to bf16 straight from the S fragments into the A
+//   operand of O += P·V_j (RS wgmma).  Outputs: O (bf16, arbitrary b/s/h strides) and LSE (fp32 [B, H, S], natural log).
 // Backward, three launches:
 //   prep   δ = rowsum(dO ∘ O) − dLSE                                         (one warp per query row)
-//   dK/dV  one CTA per (64-key tile, kv head, batch), loops over the query tiles of every query head of the group:
-//          Sᵀ = K·Qᵀ, Pᵀ = exp(Sᵀ − LSE), dV += Pᵀ·dO, dPᵀ = V·dOᵀ, dSᵀ = Pᵀ∘(dPᵀ − δ), dK += dSᵀ·Q
-//   dQ     one CTA per (64-query tile, head, batch), loops over the key tiles: S, P, dP = dO·Vᵀ, dS, dQ += dS·K
+//   dK/dV  one CTA per (128-key tile, kv head, batch), loops over the 64-query tiles of every query head of the group:
+//          Sᵀ = K·Qᵀ, dPᵀ = V·dOᵀ (SS), Pᵀ = exp(Sᵀ − LSE), dSᵀ = Pᵀ∘(dPᵀ − δ), dV += Pᵀ·dO, dK += dSᵀ·Q (RS)
+//   dQ     one CTA per (128-query tile, head, batch), loops over the 64-key tiles: S, dP = dO·Vᵀ (SS), P, dS, dQ += dS·K (RS)
 //   Every gradient element is owned by one thread of one CTA (no atomics), so the backward is bit-reproducible.
-// Every kernel is a template on the head dimension HD; the tile shapes (64 query / key rows) are the same for all of them.
+// Every kernel is a template on the head dimension HD with the same tiles and the same MMA sequence for all of them: the
+// products with k = HD take HD/16 k-steps, and those with n = HD always compute 64 columns per 64-column panel (the
+// columns past HD are discarded), so a D < 128 run equals the first D columns of a D = 128 run on zero-padded inputs.
 // Visibility: query row i < S_q sees key j < S_kv iff
 //   - MASK (key-padding mask, uint8 [B, S_kv]): mask[b, j] != 0;
 //   - causal: j ≤ i + off;
@@ -20,11 +24,13 @@
 // off-diagonal block of context-parallel attention, whose queries sit `off` positions after its keys.  W ≥ S_kv + off is
 // plain causal attention.  The mask term is tested at each call site (the forward and dQ kernels stage each key tile's 64
 // flags in shared memory, a dK/dV thread reads the flags of its two key rows once); the causal / window / offset terms are
-// `sees`, and the tiles a CTA visits are `key_tiles` / `query_tiles`, which skip only tiles that hold no visible pair.
+// `sees`, and the tiles a CTA visits are the union of `key_tiles` / `query_tiles` over its two 64-row halves, which skip
+// only tiles that hold no visible pair.
 // An invisible pair contributes nothing: a query row that sees no key gets O = 0, LSE = −inf and dQ = 0, and a key no row
-// sees gets dK = dV = 0.
-// spec_attn_kernel runs the forward kernel's loop for W new tokens per sequence against a bf16 or e4m3 KV cache (speculation
-// and Medusa verification); its visibility rule is written above it.
+// sees gets dK = dV = 0.  A tile one warpgroup sees nothing of adds exact zeros to its accumulators.
+// spec_attn_kernel runs a forward loop on warp-level mma.sync (m16n8k16, ldmatrix from padded shared memory, 4 warps per
+// 64-row tile) for W new tokens per sequence against a bf16 or e4m3 KV cache (speculation and Medusa verification); its
+// visibility rule is written above it.
 #include <cuda.h>
 #include <cuda_fp8.h>
 
@@ -34,19 +40,27 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "sm90_ptx.cuh"
 
 namespace nxd {
 namespace fa {
 
 constexpr int BT = 64;                       // rows of a query or key tile
-constexpr int kThreads = 128;
-// padded shared-memory row (elements): 144 / 176 / 208 / 272 B for HD = 64 / 80 / 96 / 128.  Each stride is 16 B more than
-// a multiple of 32 B, so the 8 row addresses of one ldmatrix 8x8 matrix start in distinct 4-bank groups (conflict-free).
+constexpr int kThreads = 128;                // spec_attn_kernel
+constexpr int kWgThreads = 256;              // flash kernels: two warpgroups
+// padded shared-memory row of spec_attn_kernel (elements): 144 / 176 / 208 / 272 B for HD = 64 / 80 / 96 / 128.  Each
+// stride is 16 B more than a multiple of 32 B, so the 8 row addresses of one ldmatrix 8x8 matrix start in distinct 4-bank
+// groups (conflict-free).
 template <int HD> constexpr int LDS = HD + 8;
 template <int HD> constexpr int kTile = BT * LDS<HD>;              // elements of one staged tile
-template <int HD> constexpr int kSmemFwd = 5 * kTile<HD> * 2;                      // Q, K×2, V×2
-template <int HD> constexpr int kSmemDkv = 6 * kTile<HD> * 2 + 4 * BT * 4;         // K, V, Q×2, dO×2, LSE×2, δ×2
-template <int HD> constexpr int kSmemDq = 6 * kTile<HD> * 2;                       // Q, dO, K×2, V×2
+// wgmma operand tiles of the flash kernels: R rows × HD columns staged as kPanels [R × 64] bf16 panels in the 128-byte
+// swizzle (row r of a panel is 128 B at r·128, its 16-byte chunk c sits at chunk c ^ (r & 7)); panels start 1 KB aligned.
+template <int HD> constexpr int kPanels = (HD + 63) / 64;
+template <int R, int HD> constexpr int kPTile = R * 64 * kPanels<HD>;           // elements
+template <int HD> constexpr int kSmemFwd = (kPTile<2 * BT, HD> + 4 * kPTile<BT, HD>) * 2 + 1024;      // Q, K×2, V×2
+template <int HD> constexpr int kSmemDkv = (2 * kPTile<2 * BT, HD> + 4 * kPTile<BT, HD>) * 2 + 4 * BT * 4 + 1024;
+                                                                             // K, V, Q×2, dO×2, LSE×2, δ×2
+template <int HD> constexpr int kSmemDq = (2 * kPTile<2 * BT, HD> + 4 * kPTile<BT, HD>) * 2 + 1024;   // Q, dO, K×2, V×2
 constexpr int kSmemFlags = 2 * BT;                                                 // key-mask flags ×2 (MASK kernels)
 constexpr float kLog2e = 1.4426950408889634f;
 
@@ -86,6 +100,32 @@ NXD_DEVICE void load_tile(bf16* sm, const bf16* base, long ss, int s0, int S, in
     const bool ok = s0 + r < S;
     cp_async16(sm + r * LDS<HD> + c * 8, base + (long)(ok ? (ROLL ? ring_row(w0, r, L) : s0 + r) : 0) * ss + c * 8, ok);
   }
+}
+
+// rows [s0, s0+R) of one (batch, head) slice → swizzled panels; rows ≥ S are zero-filled.  NT threads share the copies.
+template <int R, int HD, int NT = kWgThreads>
+NXD_DEVICE void load_panels(bf16* sm, const bf16* base, long ss, int s0, int S) {
+  constexpr int kChunks = HD / 8;                                   // 16-byte chunks per row
+  for (int i = threadIdx.x; i < R * kChunks; i += NT) {
+    const int r = i / kChunks, c = i - r * kChunks;
+    const bool ok = s0 + r < S;
+    cp_async16(sm + (c >> 3) * (R * 64) + r * 64 + (((c ^ r) & 7) << 3), base + (long)(ok ? s0 + r : 0) * ss + c * 8, ok);
+  }
+}
+
+// aligns the dynamic shared memory to the 1 KB the 128-byte swizzle needs (the kernels request 1 KB of slack)
+NXD_DEVICE bf16* panel_base(uint8_t* smem) { return (bf16*)(((uintptr_t)smem + 1023) & ~(uintptr_t)1023); }
+
+// wgmma descriptor of a K-major operand (k = HD contiguous): rows [r0, r0 + 64) of an R-row panel tile, k-step ks
+// (16 columns: panel ks / 4, 32 B into its rows)
+template <int R>
+NXD_DEVICE uint64_t desc_k(const bf16* tile, int r0, int ks) {
+  return make_smem_desc(smem_u32(tile + (ks >> 2) * (R * 64) + r0 * 64) + (ks & 3) * 32, 16, 1024);
+}
+// wgmma descriptor of an MN-major operand (n = HD contiguous) of a 64-row panel tile: k rows [16ks, 16ks + 16), every
+// panel (LBO = one panel)
+NXD_DEVICE uint64_t desc_mn(const bf16* tile, int ks) {
+  return make_smem_desc(smem_u32(tile + ks * 16 * 64), BT * 128, 1024);
 }
 
 // visibility flags of keys [s0, s0+64) (1 = visible; keys ≥ S are 0) → shared memory.  Plain loads: the mask row has no
@@ -160,9 +200,9 @@ NXD_DEVICE void to_a_frags(const float (&c)[8][4], uint32_t (&p)[4][4]) {
   }
 }
 
-// 16 x HD fp32 fragments (rows row0 + lane/4 and +8) × scale → bf16 rows of a [B,S,H,HD] view
-template <int HD>
-NXD_DEVICE void store_rows(const float (&c)[HD / 8][4], bf16* base, long ss, int row0, int S, float scale0, float scale1) {
+// the first HD columns of 16 x NB·8 fp32 fragments (rows row0 + lane/4 and +8) × scale → bf16 rows of a [B,S,H,HD] view
+template <int HD, int NB>
+NXD_DEVICE void store_rows(const float (&c)[NB][4], bf16* base, long ss, int row0, int S, float scale0, float scale1) {
   const int lane = threadIdx.x & 31;
   const int r0 = row0 + (lane >> 2), r1 = r0 + 8;
 #pragma unroll
@@ -215,8 +255,8 @@ template <int HD, bool MASK>
 NXD_DEVICE void load_kv(bf16* sK, bf16* sV, uint8_t* sM, const bf16* kb, const bf16* vb, const uint8_t* mb, const Params& p,
                         int t) {
   const int buf = t & 1;
-  load_tile<HD>(sK + buf * kTile<HD>, kb, p.k.ss, t * BT, p.S_kv);
-  load_tile<HD>(sV + buf * kTile<HD>, vb, p.v.ss, t * BT, p.S_kv);
+  load_panels<BT, HD>(sK + buf * kPTile<BT, HD>, kb, p.k.ss, t * BT, p.S_kv);
+  load_panels<BT, HD>(sV + buf * kPTile<BT, HD>, vb, p.v.ss, t * BT, p.S_kv);
   cp_async_commit();
   if (MASK) load_flags(sM + buf * BT, mb, t * BT, p.S_kv);
 }
@@ -227,32 +267,33 @@ struct FwdParams : Params {
 };
 
 template <int HD, bool MASK, bool WINDOW>
-__global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
-  constexpr int kTl = kTile<HD>;
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  bf16* sQ = (bf16*)smem_raw;
-  bf16* sK = sQ + kTl;          // 2 buffers
-  bf16* sV = sK + 2 * kTl;      // 2 buffers
-  uint8_t* sM = (uint8_t*)(sV + 2 * kTl);       // 2 × 64 key flags (MASK)
+__global__ void __launch_bounds__(kWgThreads) fa_fwd_kernel(const FwdParams p) {
+  constexpr int kT = kPTile<BT, HD>, kNB = 8 * kPanels<HD>;
+  extern __shared__ uint8_t smem_raw[];
+  bf16* sQ = panel_base(smem_raw);              // 128 rows
+  bf16* sK = sQ + kPTile<2 * BT, HD>;           // 2 buffers
+  bf16* sV = sK + 2 * kT;                       // 2 buffers
+  uint8_t* sM = (uint8_t*)(sV + 2 * kT);        // 2 × 64 key flags (MASK)
   // causal: the last query tiles see the most keys, so they are scheduled first
   const int qt = gridDim.x - 1 - blockIdx.x, h = blockIdx.y, b = blockIdx.z, hk = h / (p.H / p.Hkv);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = qt * BT;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int q0 = qt * 2 * BT, r0 = q0 + wg * BT + warp * 16;
   const bf16* qb = p.q.p + b * p.q.sb + h * p.q.sh;
   const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
   const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
-  int t_lo, n_kv;
-  key_tiles<WINDOW>(p, q0, t_lo, n_kv);
+  int t_lo, n_kv, lo1, hi0;                     // the key tiles of either 64-row half (monotone in the first row)
+  key_tiles<WINDOW>(p, q0, t_lo, hi0);
+  key_tiles<WINDOW>(p, q0 + BT, lo1, n_kv);
 
-  load_tile<HD>(sQ, qb, p.q.ss, q0, p.S_q);
+  load_panels<2 * BT, HD>(sQ, qb, p.q.ss, q0, p.S_q);
   load_kv<HD, MASK>(sK, sV, sM, kb, vb, mb, p, t_lo);
 
-  float o[HD / 8][4];
+  float o[kNB][4];
 #pragma unroll
-  for (int i = 0; i < HD / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  for (int i = 0; i < kNB; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-  const int row[2] = {q0 + warp * 16 + (lane >> 2), q0 + warp * 16 + (lane >> 2) + 8};
+  const int row[2] = {r0 + (lane >> 2), r0 + (lane >> 2) + 8};
 
   for (int t = t_lo; t < n_kv; ++t) {
     const int buf = t & 1;
@@ -262,10 +303,17 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
     } else {
       cp_async_wait<0>();
     }
+    fence_proxy_async_smem();
     __syncthreads();
     const uint8_t* fl = sM + buf * BT;
     float s[8][4];
-    mma_abt<HD>(s, sQ, warp * 16, sK + buf * kTl);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks)
+      wgmma_m64n64k16_ss(s, desc_k<2 * BT>(sQ, wg * BT, ks), desc_k<BT>(sK + buf * kT, 0, ks), ks > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(s);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -300,10 +348,15 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
 #pragma unroll
     for (int r = 0; r < 2; ++r) l[r] = l[r] * alpha[r] + rs[r];
 #pragma unroll
-    for (int i = 0; i < HD / 8; ++i) { o[i][0] *= alpha[0]; o[i][1] *= alpha[0]; o[i][2] *= alpha[1]; o[i][3] *= alpha[1]; }
+    for (int i = 0; i < kNB; ++i) { o[i][0] *= alpha[0]; o[i][1] *= alpha[0]; o[i][2] *= alpha[1]; o[i][3] *= alpha[1]; }
     uint32_t pf[4][4];
     to_a_frags(s, pf);
-    mma_pb<HD>(o, pf, sV + buf * kTl);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < BT / 16; ++ks) wgmma_m64k16_rs(o, pf[ks], desc_mn(sV + buf * kT, ks));
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(o);
     __syncthreads();                              // buffer `buf` is refilled at the next iteration
   }
   if (WINDOW) cp_async_wait<0>();                 // an offset tile that sees no key skips the loop with its first loads in flight
@@ -314,7 +367,7 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
     l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
     inv[r] = l[r] > 0.f ? 1.f / l[r] : 0.f;
   }
-  store_rows<HD>(o, p.o + b * p.o_sb + h * p.o_sh, p.o_ss, q0 + warp * 16, p.S_q, inv[0], inv[1]);
+  store_rows<HD>(o, p.o + b * p.o_sb + h * p.o_sh, p.o_ss, r0, p.S_q, inv[0], inv[1]);
   if ((lane & 3) == 0) {
 #pragma unroll
     for (int r = 0; r < 2; ++r)
@@ -342,7 +395,7 @@ __global__ void __launch_bounds__(kThreads) fa_fwd_kernel(const FwdParams p) {
 constexpr int kSpecMaxW = 64;
 template <int HD> constexpr int kRawTile = BT * HD;     // bytes of one staged e4m3 tile
 template <int HD, bool E4M3>
-constexpr int kSmemSpec = (E4M3 ? 3 * kTile<HD> * 2 + 4 * kRawTile<HD> : kSmemFwd<HD>) + kSpecMaxW * (8 + 4);
+constexpr int kSmemSpec = (E4M3 ? 3 * kTile<HD> * 2 + 4 * kRawTile<HD> : 5 * kTile<HD> * 2) + kSpecMaxW * (8 + 4);
 
 struct SpecParams {
   const bf16* q; long q_sb, q_ss, q_sh;
@@ -597,30 +650,31 @@ struct BwdParams : Params {
 };
 
 template <int HD, bool MASK, bool WINDOW>
-__global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParams p) {
-  constexpr int kTl = kTile<HD>;
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  bf16* sK = (bf16*)smem_raw;
-  bf16* sV = sK + kTl;
-  bf16* sQ = sV + kTl;          // 2 buffers
-  bf16* sG = sQ + 2 * kTl;      // 2 buffers
-  float* sL = (float*)(sG + 2 * kTl);     // 2 × 64 LSE (log2 units)
-  float* sD = sL + 2 * BT;                // 2 × 64 δ
+__global__ void __launch_bounds__(kWgThreads, 1) fa_bwd_dkdv_kernel(const BwdParams p) {
+  constexpr int kT = kPTile<BT, HD>, kNB = 8 * kPanels<HD>;
+  extern __shared__ uint8_t smem_raw[];
+  bf16* sK = panel_base(smem_raw);              // 128 rows
+  bf16* sV = sK + kPTile<2 * BT, HD>;           // 128 rows
+  bf16* sQ = sV + kPTile<2 * BT, HD>;           // 2 buffers
+  bf16* sG = sQ + 2 * kT;                       // 2 buffers
+  float* sL = (float*)(sG + 2 * kT);            // 2 × 64 LSE (log2 units)
+  float* sD = sL + 2 * BT;                      // 2 × 64 δ
   const int kt = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
   const int G = p.H / p.Hkv;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int k0 = kt * BT;
-  int qt0, qt_end;
-  query_tiles<WINDOW>(p, k0, qt0, qt_end);
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int k0 = kt * 2 * BT, r0 = k0 + wg * BT + warp * 16;
+  int qt0, qt_end, lo1, hi0;                    // the query tiles of either 64-key half (monotone in the first key)
+  query_tiles<WINDOW>(p, k0, qt0, hi0);
+  query_tiles<WINDOW>(p, k0 + BT, lo1, qt_end);
   const int per_head = qt_end > qt0 ? qt_end - qt0 : 0;
   const int n_it = G * per_head;
 
-  load_tile<HD>(sK, p.k.p + b * p.k.sb + hk * p.k.sh, p.k.ss, k0, p.S_kv);
-  load_tile<HD>(sV, p.v.p + b * p.v.sb + hk * p.v.sh, p.v.ss, k0, p.S_kv);
+  load_panels<2 * BT, HD>(sK, p.k.p + b * p.k.sb + hk * p.k.sh, p.k.ss, k0, p.S_kv);
+  load_panels<2 * BT, HD>(sV, p.v.p + b * p.v.sb + hk * p.v.sh, p.v.ss, k0, p.S_kv);
   auto issue = [&](int it, int buf) {
     const int h = hk * G + it / per_head, q0 = (qt0 + it % per_head) * BT;
-    load_tile<HD>(sQ + buf * kTl, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
-    load_tile<HD>(sG + buf * kTl, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
+    load_panels<BT, HD>(sQ + buf * kT, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
+    load_panels<BT, HD>(sG + buf * kT, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
     if (threadIdx.x < BT) {
       const int s = q0 + threadIdx.x;
       const long i = ((long)b * p.H + h) * p.S_q + s;
@@ -631,13 +685,13 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
   if (n_it > 0) issue(0, 0);
   cp_async_commit();
 
-  float dk[HD / 8][4], dv[HD / 8][4];
+  float dk[kNB][4], dv[kNB][4];
 #pragma unroll
-  for (int i = 0; i < HD / 8; ++i) {
+  for (int i = 0; i < kNB; ++i) {
     dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = 0.f;
     dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f;
   }
-  const int key[2] = {k0 + warp * 16 + (lane >> 2), k0 + warp * 16 + (lane >> 2) + 8};
+  const int key[2] = {r0 + (lane >> 2), r0 + (lane >> 2) + 8};
   bool kvis[2] = {true, true};                       // this thread's two key rows are not masked
   if (MASK) {
 #pragma unroll
@@ -654,13 +708,22 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
     } else {
       cp_async_wait<0>();
     }
+    fence_proxy_async_smem();
     __syncthreads();
-    const bf16* q = sQ + buf * kTl;
-    const bf16* g = sG + buf * kTl;
+    const bf16* q = sQ + buf * kT;
+    const bf16* g = sG + buf * kT;
     const float* L = sL + buf * BT;
     const float* D = sD + buf * BT;
-    float pt[8][4];
-    mma_abt<HD>(pt, sK, warp * 16, q);               // Sᵀ: rows = keys, columns = queries
+    float pt[8][4], dpt[8][4];                       // Sᵀ, dPᵀ: rows = keys, columns = queries
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) wgmma_m64n64k16_ss(pt, desc_k<2 * BT>(sK, wg * BT, ks), desc_k<BT>(q, 0, ks), ks > 0);
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) wgmma_m64n64k16_ss(dpt, desc_k<2 * BT>(sV, wg * BT, ks), desc_k<BT>(g, 0, ks), ks > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(pt);
+    fence_acc(dpt);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
@@ -671,11 +734,12 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
         pt[j][e] = vis ? exp2f(pt[j][e] * p.scale_log2 - L[qc]) : 0.f;
       }
     }
-    uint32_t pf[4][4];
+    uint32_t pf[4][4], sf[4][4];
     to_a_frags(pt, pf);
-    mma_pb<HD>(dv, pf, g);                           // dV += Pᵀ·dO
-    float dpt[8][4];
-    mma_abt<HD>(dpt, sV, warp * 16, g);              // dPᵀ = V·dOᵀ
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < BT / 16; ++ks) wgmma_m64k16_rs(dv, pf[ks], desc_mn(g, ks));     // dV += Pᵀ·dO
+    wgmma_commit();
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
@@ -684,44 +748,46 @@ __global__ void __launch_bounds__(kThreads, 1) fa_bwd_dkdv_kernel(const BwdParam
         dpt[j][e] = pt[j][e] * (dpt[j][e] - D[qc]);
       }
     }
-    to_a_frags(dpt, pf);
-    mma_pb<HD>(dk, pf, q);                           // dK += dSᵀ·Q
+    to_a_frags(dpt, sf);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < BT / 16; ++ks) wgmma_m64k16_rs(dk, sf[ks], desc_mn(q, ks));     // dK += dSᵀ·Q
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(dv);
+    fence_acc(dk);
     __syncthreads();
   }
   if (WINDOW) cp_async_wait<0>();                    // a key tile no offset query sees skips the loop with K / V in flight
-  store_rows<HD>(dk, p.dk + b * p.dk_sb + hk * p.dk_sh, p.dk_ss, k0 + warp * 16, p.S_kv, p.scale, p.scale);
-  store_rows<HD>(dv, p.dv + b * p.dv_sb + hk * p.dv_sh, p.dv_ss, k0 + warp * 16, p.S_kv, 1.f, 1.f);
+  store_rows<HD>(dk, p.dk + b * p.dk_sb + hk * p.dk_sh, p.dk_ss, r0, p.S_kv, p.scale, p.scale);
+  store_rows<HD>(dv, p.dv + b * p.dv_sb + hk * p.dv_sh, p.dv_ss, r0, p.S_kv, 1.f, 1.f);
 }
 
-// CTAs per SM the dQ kernel is compiled for (0: no bound).  Left to itself ptxas spills at HD = 80 / 96, and at 64 with the
-// mask or the window, to reach an occupancy the shared memory does not allow (Q, dO, K×2, V×2 tiles: 54 / 66 / 78 / 102 KB).
-// EXTRA: the kernel has the mask or window predicate (a few more live registers).
-template <int HD, bool EXTRA> constexpr int kDqMinBlocks = HD == 64 ? (EXTRA ? 3 : 4) : HD == 128 ? 0 : 2;
-
 template <int HD, bool MASK, bool WINDOW>
-__global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) fa_bwd_dq_kernel(const BwdParams p) {
-  constexpr int kTl = kTile<HD>;
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  bf16* sQ = (bf16*)smem_raw;
-  bf16* sG = sQ + kTl;
-  bf16* sK = sG + kTl;          // 2 buffers
-  bf16* sV = sK + 2 * kTl;      // 2 buffers
-  uint8_t* sM = (uint8_t*)(sV + 2 * kTl);       // 2 × 64 key flags (MASK)
+__global__ void __launch_bounds__(kWgThreads, 1) fa_bwd_dq_kernel(const BwdParams p) {
+  constexpr int kT = kPTile<BT, HD>, kNB = 8 * kPanels<HD>;
+  extern __shared__ uint8_t smem_raw[];
+  bf16* sQ = panel_base(smem_raw);              // 128 rows
+  bf16* sG = sQ + kPTile<2 * BT, HD>;           // 128 rows
+  bf16* sK = sG + kPTile<2 * BT, HD>;           // 2 buffers
+  bf16* sV = sK + 2 * kT;                       // 2 buffers
+  uint8_t* sM = (uint8_t*)(sV + 2 * kT);        // 2 × 64 key flags (MASK)
   // causal: the last query tiles see the most keys, so they are scheduled first
   const int qt = gridDim.x - 1 - blockIdx.x, h = blockIdx.y, b = blockIdx.z, hk = h / (p.H / p.Hkv);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = qt * BT;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int q0 = qt * 2 * BT, r0 = q0 + wg * BT + warp * 16;
   const bf16* kb = p.k.p + b * p.k.sb + hk * p.k.sh;
   const bf16* vb = p.v.p + b * p.v.sb + hk * p.v.sh;
   const uint8_t* mb = MASK ? p.mask + b * p.mask_sb : nullptr;
-  int t_lo, n_kv;
-  key_tiles<WINDOW>(p, q0, t_lo, n_kv);
+  int t_lo, n_kv, lo1, hi0;                     // as in the forward
+  key_tiles<WINDOW>(p, q0, t_lo, hi0);
+  key_tiles<WINDOW>(p, q0 + BT, lo1, n_kv);
 
-  load_tile<HD>(sQ, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
-  load_tile<HD>(sG, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
+  load_panels<2 * BT, HD>(sQ, p.q.p + b * p.q.sb + h * p.q.sh, p.q.ss, q0, p.S_q);
+  load_panels<2 * BT, HD>(sG, p.g.p + b * p.g.sb + h * p.g.sh, p.g.ss, q0, p.S_q);
   load_kv<HD, MASK>(sK, sV, sM, kb, vb, mb, p, t_lo);
 
-  const int row[2] = {q0 + warp * 16 + (lane >> 2), q0 + warp * 16 + (lane >> 2) + 8};
+  const int row[2] = {r0 + (lane >> 2), r0 + (lane >> 2) + 8};
   float L[2], D[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -729,9 +795,9 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) 
     L[r] = row[r] < p.S_q ? p.lse[i] * kLog2e : 0.f;
     D[r] = row[r] < p.S_q ? p.delta[i] : 0.f;
   }
-  float dq[HD / 8][4];
+  float dq[kNB][4];
 #pragma unroll
-  for (int i = 0; i < HD / 8; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
+  for (int i = 0; i < kNB; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
 
   for (int t = t_lo; t < n_kv; ++t) {
     const int buf = t & 1;
@@ -741,11 +807,21 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) 
     } else {
       cp_async_wait<0>();
     }
+    fence_proxy_async_smem();
     __syncthreads();
-    const bf16* k = sK + buf * kTl;
+    const bf16* k = sK + buf * kT;
     const uint8_t* fl = sM + buf * BT;
-    float s[8][4];
-    mma_abt<HD>(s, sQ, warp * 16, k);
+    float s[8][4], dp[8][4];
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) wgmma_m64n64k16_ss(s, desc_k<2 * BT>(sQ, wg * BT, ks), desc_k<BT>(k, 0, ks), ks > 0);
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks)                                                    // dP = dO·Vᵀ
+      wgmma_m64n64k16_ss(dp, desc_k<2 * BT>(sG, wg * BT, ks), desc_k<BT>(sV + buf * kT, 0, ks), ks > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(s);
+    fence_acc(dp);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
@@ -754,22 +830,21 @@ __global__ void __launch_bounds__(kThreads, (kDqMinBlocks<HD, MASK || WINDOW>)) 
         const int r = row[e >> 1];
         const bool vis = kc < p.S_kv && r < p.S_q && sees<WINDOW>(p, r, kc) && (!MASK || fl[j * 8 + 2 * (lane & 3) + (e & 1)]);
         s[j][e] = vis ? exp2f(s[j][e] * p.scale_log2 - L[e >> 1]) : 0.f;
+        dp[j][e] = s[j][e] * (dp[j][e] - D[e >> 1]);
       }
-    }
-    float dp[8][4];
-    mma_abt<HD>(dp, sG, warp * 16, sV + buf * kTl);  // dP = dO·Vᵀ
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) dp[j][e] = s[j][e] * (dp[j][e] - D[e >> 1]);
     }
     uint32_t pf[4][4];
     to_a_frags(dp, pf);
-    mma_pb<HD>(dq, pf, k);                           // dQ += dS·K
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < BT / 16; ++ks) wgmma_m64k16_rs(dq, pf[ks], desc_mn(k, ks));      // dQ += dS·K
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(dq);
     __syncthreads();
   }
   if (WINDOW) cp_async_wait<0>();                    // as in the forward
-  store_rows<HD>(dq, p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, q0 + warp * 16, p.S_q, p.scale, p.scale);
+  store_rows<HD>(dq, p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, r0, p.S_q, p.scale, p.scale);
 }
 
 static View view(const void* ptr, const long* s) {
@@ -801,7 +876,7 @@ static void launch_fwd(const FwdParams& p, cudaStream_t st) {
     NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_fwd_kernel<HD, MASK, WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
-  fa_fwd_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem, st>>>(p);
+  fa_fwd_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + 2 * BT - 1) / (2 * BT), p.H, p.B), kWgThreads, smem, st>>>(p);
 }
 
 template <int HD, bool MASK, bool WINDOW>
@@ -813,8 +888,8 @@ static void launch_bwd(const BwdParams& p, cudaStream_t st) {
     NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dq_kernel<HD, MASK, WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dq));
     configured = true;
   }
-  fa_bwd_dkdv_kernel<HD, MASK, WINDOW><<<dim3((p.S_kv + BT - 1) / BT, p.Hkv, p.B), kThreads, smem_dkv, st>>>(p);
-  fa_bwd_dq_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + BT - 1) / BT, p.H, p.B), kThreads, smem_dq, st>>>(p);
+  fa_bwd_dkdv_kernel<HD, MASK, WINDOW><<<dim3((p.S_kv + 2 * BT - 1) / (2 * BT), p.Hkv, p.B), kWgThreads, smem_dkv, st>>>(p);
+  fa_bwd_dq_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + 2 * BT - 1) / (2 * BT), p.H, p.B), kWgThreads, smem_dq, st>>>(p);
 }
 
 // checks the arguments and fills the fields every kernel reads
