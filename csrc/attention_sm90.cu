@@ -28,6 +28,10 @@
 // only tiles that hold no visible pair.
 // An invisible pair contributes nothing: a query row that sees no key gets O = 0, LSE = −inf and dQ = 0, and a key no row
 // sees gets dK = dV = 0.  A tile one warpgroup sees nothing of adds exact zeros to its accumulators.
+// DROPOUT kernels apply attention dropout with the rule written above `Dropout`: the forward zeroes the dropped entries of
+// P before O += P·V (the row sums, the running max and the LSE use the undropped P, so the LSE equals that of p = 0) and
+// folds 1/(1 − p) into the final normalisation; the backward uses dV += (P∘Z)ᵀ·dO / (1 − p) and dS = P∘(dP∘Z/(1 − p) − δ),
+// where δ = rowsum(dO∘O) of the dropped output is unchanged.
 // spec_attn_kernel runs a forward loop on warp-level mma.sync (m16n8k16, ldmatrix from padded shared memory, 4 warps per
 // 64-row tile) for W new tokens per sequence against a bf16 or e4m3 KV cache (speculation and Medusa verification); its
 // visibility rule is written above it.
@@ -35,6 +39,7 @@
 #include <cuda_fp8.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <type_traits>
 
@@ -230,6 +235,62 @@ NXD_DEVICE bool sees(const Params& p, int i, int j) {
   return !(p.causal && j > i + off) && !(WINDOW && j <= i + off - p.window);
 }
 
+// Attention dropout.  Element (b, h, i, j) — query row i, key row j, h the global query head (head_offset + the head index
+// of this call) — is kept iff word 2·((i >> 3) & 1) + ((j >> 3) & 1) of Philox4x32-10 with key (seed low word, seed high
+// word) and counter (j & ~8, i & ~8, h, b) is below keep_threshold = round((1 − p)·2³²) (at most 2³² − 1), and a kept
+// element is scaled by 1/(1 − p).  The rule depends on nothing but these coordinates (not on tiling, head size, layout,
+// GQA grouping or the head count, so tensor-parallel shards with their head offsets drop what one unsharded run drops).
+// One Philox call decides the 2×2 block {i0, i0 + 8} × {j0, j0 + 8}, which one thread holds whole in the accumulator
+// fragments of all three kernels (rows r, r + 8 and columns c, c + 8).  ops.attention.attention_dropout_keep is the same
+// rule on the host.
+struct Dropout {
+  const void* seed; int seed64;                 // the seed: one int64 (seed64) or int32 in device memory
+  uint32_t keep_threshold;
+  float rscale;                                 // 1 / (1 − p)
+  int head_offset;
+};
+
+NXD_DEVICE uint2 dropout_key(const Dropout& d) {
+  const uint64_t s = d.seed64 ? *(const unsigned long long*)d.seed : (uint64_t)(int64_t)*(const int*)d.seed;
+  return make_uint2((uint32_t)s, (uint32_t)(s >> 32));
+}
+
+NXD_DEVICE uint4 philox4x32_10(uint2 key, uint4 c) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) { key.x += 0x9E3779B9u; key.y += 0xBB67AE85u; }
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ key.x, lo1, hi0 ^ c.w ^ key.y, lo0);
+  }
+  return c;
+}
+
+// keep flags of the block {i0, i0 + 8} × {j0, j0 + 8} (bit 3 of i0 and j0 clear): bit 2·(i ≠ i0) + (j ≠ j0)
+NXD_DEVICE uint32_t keep_bits(const Dropout& d, uint2 key, int b, int h, int i0, int j0) {
+  const uint4 w = philox4x32_10(key, make_uint4((uint32_t)j0, (uint32_t)i0, (uint32_t)(h + d.head_offset), (uint32_t)b));
+  const uint32_t t = d.keep_threshold;
+  return (uint32_t)(w.x < t) | (uint32_t)(w.y < t) << 1 | (uint32_t)(w.z < t) << 2 | (uint32_t)(w.w < t) << 3;
+}
+
+// the dropout of a [16 × 64] fragment with query rows {i, i + 8} and key columns j0(jj, c) + {0, 8} (forward, dQ): f(x, keep)
+// for every element x of c[8][4]
+template <class F>
+NXD_DEVICE void drop_rows(const Dropout& d, uint2 key, int b, int h, int i, int k0, float (&c)[8][4], F&& f) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int jj = 0; jj < 8; jj += 2) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const uint32_t z = keep_bits(d, key, b, h, i, k0 + jj * 8 + 2 * (lane & 3) + e);
+      f(c[jj][e], z & 1);
+      f(c[jj + 1][e], z & 2);
+      f(c[jj][2 + e], z & 4);
+      f(c[jj + 1][2 + e], z & 8);
+    }
+  }
+}
+
 // Tiles lo ≤ t < hi a CTA visits (none when hi ≤ lo); tile t holds rows [64t, 64t + 64).
 // key_tiles: the rows of query tile [q0, q0 + 64) see keys q0 + off − W < j (its first row's window start) up to
 // j ≤ q0 + 63 + off (causal: its last row's diagonal), so every visible key lies in the tiles returned.
@@ -264,9 +325,10 @@ NXD_DEVICE void load_kv(bf16* sK, bf16* sV, uint8_t* sM, const bf16* kb, const b
 struct FwdParams : Params {
   bf16* o; long o_sb, o_ss, o_sh;
   float* lse;
+  Dropout drop;                                 // DROPOUT kernels only
 };
 
-template <int HD, bool MASK, bool WINDOW>
+template <int HD, bool MASK, bool WINDOW, bool DROPOUT>
 __global__ void __launch_bounds__(kWgThreads) fa_fwd_kernel(const FwdParams p) {
   constexpr int kT = kPTile<BT, HD>, kNB = 8 * kPanels<HD>;
   extern __shared__ uint8_t smem_raw[];
@@ -294,6 +356,7 @@ __global__ void __launch_bounds__(kWgThreads) fa_fwd_kernel(const FwdParams p) {
   for (int i = 0; i < kNB; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const int row[2] = {r0 + (lane >> 2), r0 + (lane >> 2) + 8};
+  const uint2 dkey = DROPOUT ? dropout_key(p.drop) : make_uint2(0, 0);
 
   for (int t = t_lo; t < n_kv; ++t) {
     const int buf = t & 1;
@@ -349,6 +412,7 @@ __global__ void __launch_bounds__(kWgThreads) fa_fwd_kernel(const FwdParams p) {
     for (int r = 0; r < 2; ++r) l[r] = l[r] * alpha[r] + rs[r];
 #pragma unroll
     for (int i = 0; i < kNB; ++i) { o[i][0] *= alpha[0]; o[i][1] *= alpha[0]; o[i][2] *= alpha[1]; o[i][3] *= alpha[1]; }
+    if constexpr (DROPOUT) drop_rows(p.drop, dkey, b, h, row[0], t * BT, s, [](float& x, bool keep) { x = keep ? x : 0.f; });
     uint32_t pf[4][4];
     to_a_frags(s, pf);
     wgmma_fence();
@@ -365,7 +429,7 @@ __global__ void __launch_bounds__(kWgThreads) fa_fwd_kernel(const FwdParams p) {
   for (int r = 0; r < 2; ++r) {
     l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
     l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
-    inv[r] = l[r] > 0.f ? 1.f / l[r] : 0.f;
+    inv[r] = l[r] > 0.f ? (DROPOUT ? p.drop.rscale : 1.f) / l[r] : 0.f;
   }
   store_rows<HD>(o, p.o + b * p.o_sb + h * p.o_sh, p.o_ss, r0, p.S_q, inv[0], inv[1]);
   if ((lane & 3) == 0) {
@@ -647,9 +711,10 @@ struct BwdParams : Params {
   long dq_sb, dq_ss, dq_sh, dk_sb, dk_ss, dk_sh, dv_sb, dv_ss, dv_sh;
   const float *lse, *delta;
   float scale;
+  Dropout drop;                                 // DROPOUT kernels only
 };
 
-template <int HD, bool MASK, bool WINDOW>
+template <int HD, bool MASK, bool WINDOW, bool DROPOUT>
 __global__ void __launch_bounds__(kWgThreads, 1) fa_bwd_dkdv_kernel(const BwdParams p) {
   constexpr int kT = kPTile<BT, HD>, kNB = 8 * kPanels<HD>;
   extern __shared__ uint8_t smem_raw[];
@@ -697,6 +762,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) fa_bwd_dkdv_kernel(const BwdPar
 #pragma unroll
     for (int r = 0; r < 2; ++r) kvis[r] = key[r] < p.S_kv && p.mask[b * p.mask_sb + key[r]] != 0;
   }
+  const uint2 dkey = DROPOUT ? dropout_key(p.drop) : make_uint2(0, 0);
 
   for (int it = 0; it < n_it; ++it) {
     const int buf = it & 1;
@@ -735,20 +801,54 @@ __global__ void __launch_bounds__(kWgThreads, 1) fa_bwd_dkdv_kernel(const BwdPar
       }
     }
     uint32_t pf[4][4], sf[4][4];
-    to_a_frags(pt, pf);
+    if constexpr (DROPOUT) {
+      // dSᵀ = Pᵀ∘(dPᵀ∘Z/(1 − p) − δ) and Pᵀ∘Z for dV (its 1/(1 − p) is applied at the store), packed to bf16 one k-step at
+      // a time so the fp32 fragments die early.  Rows are keys and columns queries here: the block of query columns
+      // qc, qc + 8 and key rows key[0], key[1] is bits 0, 2 | 1, 3.
+      const int h = hk * G + it / per_head;
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const int jj = 2 * ks;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int qc = jj * 8 + 2 * (lane & 3) + e;
+          const uint32_t z = keep_bits(p.drop, dkey, b, h, q0 + qc, key[0]);
+          auto f = [&](float& x, float& dx, bool keep, float delta) {
+            dx = x * (keep ? dx * p.drop.rscale - delta : -delta);
+            x = keep ? x : 0.f;
+          };
+          f(pt[jj][e], dpt[jj][e], z & 1, D[qc]);
+          f(pt[jj][2 + e], dpt[jj][2 + e], z & 2, D[qc]);
+          f(pt[jj + 1][e], dpt[jj + 1][e], z & 4, D[qc + 8]);
+          f(pt[jj + 1][2 + e], dpt[jj + 1][2 + e], z & 8, D[qc + 8]);
+        }
+        pf[ks][0] = pack_bf16(pt[jj][0], pt[jj][1]);
+        pf[ks][1] = pack_bf16(pt[jj][2], pt[jj][3]);
+        pf[ks][2] = pack_bf16(pt[jj + 1][0], pt[jj + 1][1]);
+        pf[ks][3] = pack_bf16(pt[jj + 1][2], pt[jj + 1][3]);
+        sf[ks][0] = pack_bf16(dpt[jj][0], dpt[jj][1]);
+        sf[ks][1] = pack_bf16(dpt[jj][2], dpt[jj][3]);
+        sf[ks][2] = pack_bf16(dpt[jj + 1][0], dpt[jj + 1][1]);
+        sf[ks][3] = pack_bf16(dpt[jj + 1][2], dpt[jj + 1][3]);
+      }
+    } else {
+      to_a_frags(pt, pf);
+    }
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < BT / 16; ++ks) wgmma_m64k16_rs(dv, pf[ks], desc_mn(g, ks));     // dV += Pᵀ·dO
     wgmma_commit();
+    if constexpr (!DROPOUT) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
+      for (int j = 0; j < 8; ++j) {
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int qc = j * 8 + 2 * (lane & 3) + (e & 1);
-        dpt[j][e] = pt[j][e] * (dpt[j][e] - D[qc]);
+        for (int e = 0; e < 4; ++e) {
+          const int qc = j * 8 + 2 * (lane & 3) + (e & 1);
+          dpt[j][e] = pt[j][e] * (dpt[j][e] - D[qc]);
+        }
       }
+      to_a_frags(dpt, sf);
     }
-    to_a_frags(dpt, sf);
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < BT / 16; ++ks) wgmma_m64k16_rs(dk, sf[ks], desc_mn(q, ks));     // dK += dSᵀ·Q
@@ -760,10 +860,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) fa_bwd_dkdv_kernel(const BwdPar
   }
   if (WINDOW) cp_async_wait<0>();                    // a key tile no offset query sees skips the loop with K / V in flight
   store_rows<HD>(dk, p.dk + b * p.dk_sb + hk * p.dk_sh, p.dk_ss, r0, p.S_kv, p.scale, p.scale);
-  store_rows<HD>(dv, p.dv + b * p.dv_sb + hk * p.dv_sh, p.dv_ss, r0, p.S_kv, 1.f, 1.f);
+  const float dv_scale = DROPOUT ? p.drop.rscale : 1.f;
+  store_rows<HD>(dv, p.dv + b * p.dv_sb + hk * p.dv_sh, p.dv_ss, r0, p.S_kv, dv_scale, dv_scale);
 }
 
-template <int HD, bool MASK, bool WINDOW>
+template <int HD, bool MASK, bool WINDOW, bool DROPOUT>
 __global__ void __launch_bounds__(kWgThreads, 1) fa_bwd_dq_kernel(const BwdParams p) {
   constexpr int kT = kPTile<BT, HD>, kNB = 8 * kPanels<HD>;
   extern __shared__ uint8_t smem_raw[];
@@ -798,6 +899,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) fa_bwd_dq_kernel(const BwdParam
   float dq[kNB][4];
 #pragma unroll
   for (int i = 0; i < kNB; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
+  const uint2 dkey = DROPOUT ? dropout_key(p.drop) : make_uint2(0, 0);
 
   for (int t = t_lo; t < n_kv; ++t) {
     const int buf = t & 1;
@@ -822,6 +924,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) fa_bwd_dq_kernel(const BwdParam
     wgmma_wait<0>();
     fence_acc(s);
     fence_acc(dp);
+    // dS = P∘(dP∘Z/(1 − p) − δ)
+    if constexpr (DROPOUT)
+      drop_rows(p.drop, dkey, b, h, row[0], t * BT, dp, [&](float& x, bool keep) { x = keep ? x * p.drop.rscale : 0.f; });
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
@@ -853,13 +958,17 @@ static View view(const void* ptr, const long* s) {
   return View{(const bf16*)ptr, s[0], s[1], s[2]};
 }
 
-// f(std::integral_constant<int, HD>, std::integral_constant<bool, MASK>, std::integral_constant<bool, WINDOW>) for the runtime
-// head dimension, mask flag and window flag
+// f(std::integral_constant<int, HD>, std::integral_constant<bool, MASK>, std::integral_constant<bool, WINDOW>,
+// std::integral_constant<bool, DROPOUT>) for the runtime head dimension, mask, window and dropout flags
 template <class F>
-static void dispatch(int D, bool mask, bool window, F&& f) {
+static void dispatch(int D, bool mask, bool window, bool dropout, F&& f) {
+  auto with_dropout = [&](auto hd, auto mk, auto wd) {
+    if (dropout) f(hd, mk, wd, std::true_type{});
+    else f(hd, mk, wd, std::false_type{});
+  };
   auto with_window = [&](auto hd, auto mk) {
-    if (window) f(hd, mk, std::true_type{});
-    else f(hd, mk, std::false_type{});
+    if (window) with_dropout(hd, mk, std::true_type{});
+    else with_dropout(hd, mk, std::false_type{});
   };
   auto with_mask = [&](auto hd) {
     if (mask) with_window(hd, std::true_type{});
@@ -868,28 +977,32 @@ static void dispatch(int D, bool mask, bool window, F&& f) {
   dispatch_head_dim(D, "attention", with_mask);
 }
 
-template <int HD, bool MASK, bool WINDOW>
+template <int HD, bool MASK, bool WINDOW, bool DROPOUT>
 static void launch_fwd(const FwdParams& p, cudaStream_t st) {
   constexpr int smem = kSmemFwd<HD> + (MASK ? kSmemFlags : 0);
   static bool configured = false;
   if (!configured) {
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_fwd_kernel<HD, MASK, WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_fwd_kernel<HD, MASK, WINDOW, DROPOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        smem));
     configured = true;
   }
-  fa_fwd_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + 2 * BT - 1) / (2 * BT), p.H, p.B), kWgThreads, smem, st>>>(p);
+  fa_fwd_kernel<HD, MASK, WINDOW, DROPOUT><<<dim3((p.S_q + 2 * BT - 1) / (2 * BT), p.H, p.B), kWgThreads, smem, st>>>(p);
 }
 
-template <int HD, bool MASK, bool WINDOW>
+template <int HD, bool MASK, bool WINDOW, bool DROPOUT>
 static void launch_bwd(const BwdParams& p, cudaStream_t st) {
   constexpr int smem_dkv = kSmemDkv<HD>, smem_dq = kSmemDq<HD> + (MASK ? kSmemFlags : 0);
   static bool configured = false;
   if (!configured) {
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dkdv_kernel<HD, MASK, WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dkv));
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dq_kernel<HD, MASK, WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dq));
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dkdv_kernel<HD, MASK, WINDOW, DROPOUT>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, smem_dkv));
+    NXD_CUDA_CHECK(cudaFuncSetAttribute(fa_bwd_dq_kernel<HD, MASK, WINDOW, DROPOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        smem_dq));
     configured = true;
   }
-  fa_bwd_dkdv_kernel<HD, MASK, WINDOW><<<dim3((p.S_kv + 2 * BT - 1) / (2 * BT), p.Hkv, p.B), kWgThreads, smem_dkv, st>>>(p);
-  fa_bwd_dq_kernel<HD, MASK, WINDOW><<<dim3((p.S_q + 2 * BT - 1) / (2 * BT), p.H, p.B), kWgThreads, smem_dq, st>>>(p);
+  fa_bwd_dkdv_kernel<HD, MASK, WINDOW, DROPOUT><<<dim3((p.S_kv + 2 * BT - 1) / (2 * BT), p.Hkv, p.B), kWgThreads, smem_dkv,
+                                                   st>>>(p);
+  fa_bwd_dq_kernel<HD, MASK, WINDOW, DROPOUT><<<dim3((p.S_q + 2 * BT - 1) / (2 * BT), p.H, p.B), kWgThreads, smem_dq, st>>>(p);
 }
 
 // checks the arguments and fills the fields every kernel reads
@@ -912,18 +1025,34 @@ static void set_params(Params& p, const void* q, const void* k, const void* v, c
   p.q_offset = (int)q_offset;
 }
 
+// checks the dropout arguments and fills `Dropout`; returns whether the DROPOUT kernels run (p > 0)
+static bool set_dropout(Dropout& d, double dropout_p, const void* seed, bool seed64, long head_offset, int H) {
+  if (!(dropout_p >= 0.0 && dropout_p < 1.0)) nxd_throw("attention: dropout_p must be in [0, 1)", __FILE__, __LINE__);
+  if (head_offset < 0 || head_offset > INT32_MAX - H) nxd_throw("attention: head_offset out of range", __FILE__, __LINE__);
+  d = Dropout{seed, seed64 ? 1 : 0, 0u, 1.f, (int)head_offset};
+  if (dropout_p == 0.0) return false;
+  if (!seed) nxd_throw("attention: dropout_p > 0 needs a seed", __FILE__, __LINE__);
+  // the same double arithmetic as ops.attention.attention_dropout_keep
+  const double t = std::floor((1.0 - dropout_p) * 4294967296.0 + 0.5);
+  d.keep_threshold = (uint32_t)std::min(t, 4294967295.0);
+  d.rscale = (float)(1.0 / (1.0 - dropout_p));
+  return true;
+}
+
 }  // namespace fa
 
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
                     int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    const void* kpm, long kpm_sb, long window, long q_offset, cudaStream_t st) {
+                    const void* kpm, long kpm_sb, long window, long q_offset, double dropout_p, const void* seed,
+                    bool seed64, long head_offset, cudaStream_t st) {
   using namespace fa;
   FwdParams p;
   set_params(p, q, k, v, qs, ks, vs, B, S_q, S_kv, H, Hkv, scale, causal, kpm, kpm_sb, window, q_offset);
+  const bool dropout = set_dropout(p.drop, dropout_p, seed, seed64, head_offset, H);
   p.o = (bf16*)out; p.o_sb = os[0]; p.o_ss = os[1]; p.o_sh = os[2];
   p.lse = lse;
-  dispatch(D, kpm != nullptr, window > 0, [&](auto hd, auto mk, auto wd) {
-    launch_fwd<decltype(hd)::value, decltype(mk)::value, decltype(wd)::value>(p, st);
+  dispatch(D, kpm != nullptr, window > 0, dropout, [&](auto hd, auto mk, auto wd, auto dr) {
+    launch_fwd<decltype(hd)::value, decltype(mk)::value, decltype(wd)::value, decltype(dr)::value>(p, st);
   });
   NXD_CUDA_CHECK(cudaGetLastError());
 }
@@ -932,10 +1061,11 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
                     int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
                     const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, long window,
-                    long q_offset, cudaStream_t st) {
+                    long q_offset, double dropout_p, const void* seed, bool seed64, long head_offset, cudaStream_t st) {
   using namespace fa;
   BwdParams p;
   set_params(p, q, k, v, qs, ks, vs, B, S_q, S_kv, H, Hkv, scale, causal, kpm, kpm_sb, window, q_offset);
+  const bool dropout = set_dropout(p.drop, dropout_p, seed, seed64, head_offset, H);
   p.g = view(go, gs);
   p.dq = (bf16*)dq; p.dk = (bf16*)dk; p.dv = (bf16*)dv;
   p.dq_sb = dqs[0]; p.dq_ss = dqs[1]; p.dq_sh = dqs[2];
@@ -943,12 +1073,12 @@ void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v,
   p.dv_sb = dvs[0]; p.dv_ss = dvs[1]; p.dv_sh = dvs[2];
   p.lse = lse; p.delta = delta;
   p.scale = scale;
-  dispatch(D, kpm != nullptr, window > 0, [&](auto hd, auto mk, auto wd) {
+  dispatch(D, kpm != nullptr, window > 0, dropout, [&](auto hd, auto mk, auto wd, auto dr) {
     constexpr int HD = decltype(hd)::value;
     const long rows = (long)B * H * S_q;
     fa_bwd_prep_kernel<HD><<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(
         (const bf16*)o, (const bf16*)go, dlse, delta, B, S_q, H, os[0], os[1], os[2], gs[0], gs[1], gs[2]);
-    launch_bwd<HD, decltype(mk)::value, decltype(wd)::value>(p, st);
+    launch_bwd<HD, decltype(mk)::value, decltype(wd)::value, decltype(dr)::value>(p, st);
   });
   NXD_CUDA_CHECK(cudaGetLastError());
 }

@@ -568,30 +568,48 @@ static const void* check_kpm(const c10::optional<Tensor>& m, const Tensor& q, in
   *sb = m->stride(0);
   return m->data_ptr();
 }
+// attention dropout arguments: 0 ≤ dropout_p < 1; with dropout_p > 0 a one-element int32 / int64 seed on q's device →
+// (data, seed is int64), else (null, false)
+static const void* check_dropout(double dropout_p, const c10::optional<Tensor>& seed, const Tensor& q, bool* seed64) {
+  TORCH_CHECK(dropout_p >= 0.0 && dropout_p < 1.0, "dropout_p must be in [0, 1), got ", dropout_p);
+  *seed64 = false;
+  if (dropout_p == 0.0) return nullptr;
+  TORCH_CHECK(seed.has_value(), "dropout_p > 0 needs a seed");
+  TORCH_CHECK(seed->numel() == 1 && (seed->scalar_type() == at::kInt || seed->scalar_type() == at::kLong),
+              "seed: expected a one-element int32 or int64 tensor");
+  TORCH_CHECK(seed->device() == q.device(), "seed: expected it on ", q.device(), ", got ", seed->device());
+  *seed64 = seed->scalar_type() == at::kLong;
+  return seed->data_ptr();
+}
 // returns (out [B,S,H,D] view — memory laid out [S,B,H,D] when sbhd_out —, lse [B,H,S] fp32)
 static std::vector<Tensor> flash_attn_fwd(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
                                           bool sbhd_out, const c10::optional<Tensor>& key_padding_mask, int64_t window,
-                                          int64_t q_offset) {
+                                          int64_t q_offset, double dropout_p, const c10::optional<Tensor>& seed,
+                                          int64_t head_offset) {
   check_qkv(q, "q"); check_qkv(k, "k"); check_qkv(v, "v");
   const int B = q.size(0), S = q.size(1), H = q.size(2), D = q.size(3), Skv = k.size(1), Hkv = k.size(2);
   TORCH_CHECK(k.size(0) == B && v.size(0) == B && v.size(1) == Skv && v.size(2) == Hkv && H % Hkv == 0);
   TORCH_CHECK(k.size(3) == D && v.size(3) == D, "q, k and v must have the same head_dim");
   long kpm_sb;
   const void* kpm = check_kpm(key_padding_mask, q, B, Skv, &kpm_sb);
+  bool seed64;
+  const void* seed_p = check_dropout(dropout_p, seed, q, &seed64);
   c10::cuda::CUDAGuard guard(q.device());
   Tensor out = sbhd_out ? at::empty({S, B, H, D}, q.options()).transpose(0, 1) : at::empty({B, S, H, D}, q.options());
   Tensor lse = at::empty({B, H, S}, q.options().dtype(at::kFloat));
   const long qs[3] = {q.stride(0), q.stride(1), q.stride(2)}, ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   const long vs[3] = {v.stride(0), v.stride(1), v.stride(2)}, os[3] = {out.stride(0), out.stride(1), out.stride(2)};
   nxd::flash_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, Skv, H, Hkv, D,
-                      qs, ks, vs, os, (float)scale, causal, kpm, kpm_sb, window, q_offset, stream());
+                      qs, ks, vs, os, (float)scale, causal, kpm, kpm_sb, window, q_offset, dropout_p, seed_p, seed64,
+                      head_offset, stream());
   return {out, lse};
 }
 
 static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& o,
                                           const Tensor& lse, bool causal, double scale, bool sbhd_out,
                                           const c10::optional<Tensor>& dlse, const c10::optional<Tensor>& key_padding_mask,
-                                          int64_t window, int64_t q_offset) {
+                                          int64_t window, int64_t q_offset, double dropout_p,
+                                          const c10::optional<Tensor>& seed, int64_t head_offset) {
   check_qkv(q, "q"); check_qkv(k, "k"); check_qkv(v, "v"); check_qkv(go, "grad_out"); check_qkv(o, "out");
   const int B = q.size(0), S = q.size(1), H = q.size(2), D = q.size(3), Skv = k.size(1), Hkv = k.size(2);
   TORCH_CHECK(k.size(3) == D && v.size(3) == D && go.size(3) == D && o.size(3) == D,
@@ -599,6 +617,8 @@ static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, con
   TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * H * S);
   long kpm_sb;
   const void* kpm = check_kpm(key_padding_mask, q, B, Skv, &kpm_sb);
+  bool seed64;
+  const void* seed_p = check_dropout(dropout_p, seed, q, &seed64);
   c10::cuda::CUDAGuard guard(q.device());
   auto mk = [&](int s, int h) {
     return sbhd_out ? at::empty({s, B, h, D}, q.options()).transpose(0, 1) : at::empty({B, s, h, D}, q.options());
@@ -615,7 +635,8 @@ static std::vector<Tensor> flash_attn_bwd(const Tensor& go, const Tensor& q, con
   }
   nxd::flash_attn_bwd(go.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), dlse_p,
                       dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr<float>(), B, S, Skv, H, Hkv, D, gs, qs, ks,
-                      vs, os, dqs, dks, dvs, (float)scale, causal, kpm, kpm_sb, window, q_offset, stream());
+                      vs, os, dqs, dks, dvs, (float)scale, causal, kpm, kpm_sb, window, q_offset, dropout_p, seed_p, seed64,
+                      head_offset, stream());
   return {dq, dk, dv};
 }
 
@@ -900,10 +921,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("grouped_gemm", &grouped_gemm);
   m.def("grouped_wgrad", &grouped_wgrad);
   m.def("flash_attn_fwd", &flash_attn_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("causal"), py::arg("scale"),
-        py::arg("sbhd_out"), py::arg("key_padding_mask") = py::none(), py::arg("window") = 0, py::arg("q_offset") = 0);
+        py::arg("sbhd_out"), py::arg("key_padding_mask") = py::none(), py::arg("window") = 0, py::arg("q_offset") = 0,
+        py::arg("dropout_p") = 0.0, py::arg("seed") = py::none(), py::arg("head_offset") = 0);
   m.def("flash_attn_bwd", &flash_attn_bwd, py::arg("go"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"), py::arg("lse"),
         py::arg("causal"), py::arg("scale"), py::arg("sbhd_out"), py::arg("dlse") = py::none(),
-        py::arg("key_padding_mask") = py::none(), py::arg("window") = 0, py::arg("q_offset") = 0);
+        py::arg("key_padding_mask") = py::none(), py::arg("window") = 0, py::arg("q_offset") = 0, py::arg("dropout_p") = 0.0,
+        py::arg("seed") = py::none(), py::arg("head_offset") = 0);
   m.def("ag_gemm_bf16", &ag_gemm_bf16);
   m.def("gemm_rs_bf16", &gemm_rs_bf16);
   m.def("zero1_reduce_scatter", &zero1_reduce_scatter);

@@ -154,16 +154,19 @@ void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int 
 // in elements.  kpm: optional key-padding mask, uint8 [B, S_kv] with row stride kpm_sb (key visible iff nonzero), or null.
 // window: sliding window W (causal only; query i sees keys i − W < j ≤ i), or 0 for none.  q_offset ≥ 0 (window only): global
 // position of query row 0 minus that of key row 0, so query i sees keys i + q_offset − W < j ≤ i + q_offset.
+// dropout_p ∈ [0, 1): attention dropout by the rule in attention_sm90.cu, with the seed read on the device (int64 when
+// seed64, else int32; needed when dropout_p > 0) and head h of this call counted as global head head_offset + h.
 void flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int S_q, int S_kv, int H,
                     int Hkv, int D, const long* qs, const long* ks, const long* vs, const long* os, float scale, bool causal,
-                    const void* kpm, long kpm_sb, long window, long q_offset, cudaStream_t st);
+                    const void* kpm, long kpm_sb, long window, long q_offset, double dropout_p, const void* seed,
+                    bool seed64, long head_offset, cudaStream_t st);
 
 // delta: fp32 scratch [B, H, S_q]; dlse may be null
 void flash_attn_bwd(const void* go, const void* q, const void* k, const void* v, const void* o, const float* lse,
                     const float* dlse, void* dq, void* dk, void* dv, float* delta, int B, int S_q, int S_kv, int H, int Hkv,
                     int D, const long* gs, const long* qs, const long* ks, const long* vs, const long* os, const long* dqs,
                     const long* dks, const long* dvs, float scale, bool causal, const void* kpm, long kpm_sb, long window,
-                    long q_offset, cudaStream_t st);
+                    long q_offset, double dropout_p, const void* seed, bool seed64, long head_offset, cudaStream_t st);
 
 // W ≤ 64 new tokens per sequence against a KV cache (speculation / Medusa verification): q [B,W,H,D] bf16, k/v caches
 // [B,L,Hkv,D] bf16 or e4m3 (kv_e4m3), D ∈ {64, 80, 96, 128}, H/Hkv ∈ {1,2,4,8}; mask uint8 [W,W] and depth int64 [W] (both

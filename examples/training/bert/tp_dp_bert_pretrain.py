@@ -34,6 +34,8 @@ def main():
     p.add_argument("--optimizer", default="AdamW", choices=["AdamW", "LAMB"],
                    help="LAMB is accepted and runs AdamW (layer-wise trust ratios are not implemented)")
     p.add_argument("--lr", type=float, default=1e-4)
+    p.add_argument("--dropout", type=float, default=0.0,
+                   help="hidden and attention-probability dropout (bert-large-uncased trains with 0.1)")
     add_checkpoint_args(p)
     a = p.parse_args()
     dev = init_distributed()
@@ -43,7 +45,8 @@ def main():
     shapes = {"large": dict(hidden_size=1024, num_hidden_layers=24, num_attention_heads=16, intermediate_size=4096),
               "base": dict(hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072),
               "tiny": dict(hidden_size=128, num_hidden_layers=2, num_attention_heads=4, intermediate_size=256, vocab_size=1024)}[a.model]
-    mcfg = BertConfig(dtype=dtype, device=dev, max_position_embeddings=max(512, a.seq_len), **shapes)
+    mcfg = BertConfig(dtype=dtype, device=dev, max_position_embeddings=max(512, a.seq_len), hidden_dropout_prob=a.dropout,
+                      attention_probs_dropout_prob=a.dropout, **shapes)
 
     def model_fn():
         torch.manual_seed(1234)

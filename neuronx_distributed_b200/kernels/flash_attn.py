@@ -15,7 +15,7 @@ from typing import Optional
 
 import torch
 
-from ..ops.attention import flash_attention
+from ..ops.attention import flash_attention, flash_kernels_apply
 from .kernel_utils import cast
 
 
@@ -32,15 +32,23 @@ def get_flash_attn_kernels(use_sharded: bool = False):
 
 class NKIAttnFunc(torch.autograd.Function):
     """Name kept for code that calls ``NKIAttnFunc.apply`` directly.  Delegates to the differentiable
-    ``flash_attention`` op (its own autograd node carries the backward kernel)."""
+    ``flash_attention`` op (its own autograd node carries the backward kernel).
+
+    ``dropout_p`` > 0 is the fused kernel's attention dropout, as in the reference: it needs inputs the flash kernels take
+    (CUDA bf16, head_dim 64, 80, 96 or 128) and raises ``AssertionError`` otherwise.  ``seed`` (a one-element integer
+    tensor) or, when None, one drawn from the default generator on the device (``kernel_utils.get_seed``).  Attention
+    dropout on any other input is ``ops.attention.flash_attention(dropout_p=…)``."""
 
     @staticmethod
     def apply(q, k, v, softmax_scale=None, causal: bool = True, mixed_precision: bool = True, seed=None, dropout_p: float = 0.0,  # noqa: D102
               use_sharded: bool = False, transpose_nki_inputs: bool = True, lnc: int = 1):
-        assert dropout_p == 0.0, "attention dropout is not supported by the fused kernel"
         if transpose_nki_inputs:                              # q, k arrive as [B, H, D, S]
             q, k = q.permute(0, 1, 3, 2), k.permute(0, 1, 3, 2)
-        out = flash_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), causal, softmax_scale)
+        q, k, v = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
+        if dropout_p > 0.0:
+            assert flash_kernels_apply(q, k, v, causal), \
+                "attention dropout runs in the fused kernel: CUDA bf16 q, k, v with head_dim 64, 80, 96 or 128"
+        out = flash_attention(q, k, v, causal, softmax_scale, dropout_p=dropout_p, dropout_seed=seed)
         return out.transpose(1, 2)
 
 

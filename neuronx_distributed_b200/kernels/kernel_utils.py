@@ -13,8 +13,10 @@ def check_xla_bf16_flags() -> bool:
 
 
 def get_seed(dropout_p: float, device) -> torch.Tensor | None:
-    """Dropout seed for the attention kernel: drawn from (and advancing) the device RNG stream that the TP-aware RNG
-    tracker manages, so dropout patterns differ across TP ranks exactly where they should."""
+    """Dropout seed for the attention kernels: a one-element int32 tensor drawn on ``device`` from (and advancing) its
+    default generator, without a host sync.  TP ranks draw the same seed (the default stream is seeded alike inside a TP
+    group) and differ through their global head indices; activation checkpointing restores the generator, so a recompute
+    draws the same seed."""
     if dropout_p <= 0.0:
         return None
     return torch.randint(0, 2 ** 31 - 1, (1,), device=device, dtype=torch.int32)

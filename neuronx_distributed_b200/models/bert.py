@@ -29,6 +29,7 @@ class BertConfig:
     type_vocab_size: int = 2
     layer_norm_eps: float = 1e-12
     hidden_dropout_prob: float = 0.0
+    attention_probs_dropout_prob: float = 0.0    # dropout on the attention probabilities (training only)
     initializer_range: float = 0.02
     dtype: torch.dtype = torch.bfloat16
     device: Optional[torch.device] = None
@@ -66,6 +67,8 @@ class BertSelfAttention(nn.Module):
         tp = ps.get_tensor_model_parallel_size()
         self.heads_local = cfg.num_attention_heads // tp
         self.head_dim = cfg.hidden_size // cfg.num_attention_heads
+        self.dropout_p = cfg.attention_probs_dropout_prob
+        self.head_offset = ps.get_tensor_model_parallel_rank() * self.heads_local     # global index of the first local head
         mk = dict(bias=True, gather_output=False, init_method=_init(cfg.initializer_range), dtype=cfg.dtype, device=cfg.device)
         self.query = ColumnParallelLinear(cfg.hidden_size, cfg.hidden_size, **mk)
         self.key = ColumnParallelLinear(cfg.hidden_size, cfg.hidden_size, **mk)
@@ -76,7 +79,8 @@ class BertSelfAttention(nn.Module):
     def forward(self, x, key_padding_mask):
         B, S, _ = x.shape
         q, k, v = (lin(x).view(B, S, self.heads_local, self.head_dim) for lin in (self.query, self.key, self.value))
-        o = ops.attention.flash_attention(q, k, v, causal=False, key_padding_mask=key_padding_mask)   # bidirectional
+        drop = dict(dropout_p=self.dropout_p, head_offset=self.head_offset) if self.training and self.dropout_p > 0 else {}
+        o = ops.attention.flash_attention(q, k, v, causal=False, key_padding_mask=key_padding_mask, **drop)   # bidirectional
         return self.dense(o.reshape(B, S, self.heads_local * self.head_dim))
 
 

@@ -30,6 +30,7 @@ class GPTNeoXConfig:
     max_position_embeddings: int = 2048
     layer_norm_eps: float = 1e-5
     use_parallel_residual: bool = True
+    attention_dropout: float = 0.0           # dropout on the attention probabilities (training only)
     initializer_range: float = 0.02
     sequence_parallel_enabled: bool = False
     activation_checkpointing: str = "none"
@@ -56,6 +57,7 @@ class GPTNeoXAttention(nn.Module):
         self.cfg = cfg
         self.heads_local = cfg.num_attention_heads // tp
         self.head_dim = cfg.head_dim
+        self.head_offset = ps.get_tensor_model_parallel_rank() * self.heads_local     # global index of the first local head
         self.rot = int(self.head_dim * cfg.rotary_pct)
         sp = cfg.sequence_parallel_enabled
         # HF layout: output rows ordered head-major [h0:(q,k,v), h1:(q,k,v), …] → plain dim-0 sharding keeps whole heads
@@ -74,7 +76,9 @@ class GPTNeoXAttention(nn.Module):
         if self.rot > 0:
             q = torch.cat([ops.rope.apply_rotary(q[..., : self.rot].contiguous(), cos, sin), q[..., self.rot:]], dim=-1)
             k = torch.cat([ops.rope.apply_rotary(k[..., : self.rot].contiguous(), cos, sin), k[..., self.rot:]], dim=-1)
-        o = ops.attention.flash_attention(q.contiguous(), k.contiguous(), v.contiguous(), causal=True)
+        p = self.cfg.attention_dropout
+        drop = dict(dropout_p=p, head_offset=self.head_offset) if self.training and p > 0 else {}
+        o = ops.attention.flash_attention(q.contiguous(), k.contiguous(), v.contiguous(), causal=True, **drop)
         return self.dense(o.transpose(0, 1).reshape(S, B, self.heads_local * self.head_dim))
 
 

@@ -4,13 +4,17 @@ otherwise the PyTorch SDPA library call, which is flagged as a *library* path in
 ``kernels/flash_attn.py:162-212`` (``nki_flash_attn_func``), ``modeling_llama_nxd.py:468-475``.
 
 Layout: q ``[B, S, Hq, D]``, k/v ``[B, S, Hkv, D]`` → out ``[B, S, Hq, D]``.
+
+Attention dropout follows one rule on every path, :func:`attention_dropout_keep`, so a seed drops the same (b, h, i, j) on
+the kernels and off them.
 """
 from __future__ import annotations
 
 import math
 import os
-from typing import Optional
+from typing import Optional, Union
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -32,6 +36,89 @@ def window_visibility(s_q: int, s_kv: int, window: Optional[int], device=None, q
     j = torch.arange(s_kv, device=device)[None, :]
     vis = j <= i
     return vis if window is None else vis & (j > i - window)
+
+
+_PHILOX_M = (np.uint64(0xD2511F53), np.uint64(0xCD9E8D57))
+_PHILOX_W = (np.uint64(0x9E3779B9), np.uint64(0xBB67AE85))
+_U32 = np.uint64(0xFFFFFFFF)
+
+
+def philox4x32_10(counter, key):
+    """Philox4x32-10 (Salmon et al., SC'11; the generator of torch's CUDA RNG) on numpy arrays: ``counter`` is four
+    broadcastable arrays of 32-bit words, ``key`` two 32-bit words → the four output words as uint64 arrays.  32×32-bit
+    products are exact in uint64."""
+    c0, c1, c2, c3 = (np.asarray(c, dtype=np.uint64) & _U32 for c in counter)
+    k0, k1 = np.uint64(key[0]) & _U32, np.uint64(key[1]) & _U32
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + _PHILOX_W[0]) & _U32, (k1 + _PHILOX_W[1]) & _U32
+        p0, p1 = c0 * _PHILOX_M[0], c2 * _PHILOX_M[1]
+        c0, c1, c2, c3 = (p1 >> np.uint64(32)) ^ c1 ^ k0, p1 & _U32, (p0 >> np.uint64(32)) ^ c3 ^ k1, p0 & _U32
+    return c0, c1, c2, c3
+
+
+def dropout_keep_threshold(p: float) -> int:
+    """round((1 − p)·2³²), at most 2³² − 1: a Philox word below it keeps its element (the kernels compute it alike)."""
+    return min(math.floor((1.0 - p) * 4294967296.0 + 0.5), 4294967295)
+
+
+def attention_dropout_keep(seed, B: int, H: int, S_q: int, S_kv: int, p: float, head_offset: int = 0) -> torch.Tensor:
+    """``[B, H, S_q, S_kv]`` bool (CPU): which attention probabilities dropout with probability ``p`` keeps.  The rule of
+    the flash kernels (``csrc/attention_sm90.cu``): element (b, h, i, j) — query row i, key row j, global head
+    g = ``head_offset`` + h — is kept iff word 2·((i >> 3) & 1) + ((j >> 3) & 1) of Philox4x32-10 with key (seed low word,
+    seed high word) and counter (j & ~8, i & ~8, g, b) is below :func:`dropout_keep_threshold`.  It depends on nothing
+    else, so tensor-parallel ranks, which hold heads ``head_offset`` … ``head_offset + H − 1``, together drop what one
+    unsharded run drops.  ``seed``: an int or a one-element integer tensor."""
+    if isinstance(seed, torch.Tensor):
+        seed = int(seed.reshape(-1)[0].item())
+    seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    i = np.arange(S_q, dtype=np.uint64)[None, None, :, None]
+    j = np.arange(S_kv, dtype=np.uint64)[None, None, None, :]
+    g = np.arange(head_offset, head_offset + H, dtype=np.uint64)[None, :, None, None]
+    b = np.arange(B, dtype=np.uint64)[:, None, None, None]
+    not8 = np.uint64(~8 & 0xFFFFFFFF)
+    words = philox4x32_10((j & not8, i & not8, g, b), (seed & 0xFFFFFFFF, seed >> 32))
+    sel = (((i >> np.uint64(3)) & np.uint64(1)) * np.uint64(2) + ((j >> np.uint64(3)) & np.uint64(1)))
+    w = np.where(sel == 0, words[0], np.where(sel == 1, words[1], np.where(sel == 2, words[2], words[3])))
+    return torch.from_numpy(np.broadcast_to(w < np.uint64(dropout_keep_threshold(p)), (B, H, S_q, S_kv)).copy())
+
+
+def _check_dropout(p: float) -> float:
+    if not 0.0 <= float(p) < 1.0:
+        raise ValueError(f"dropout_p must be in [0, 1), got {p}")
+    return float(p)
+
+
+def _dropout_seed(seed, p: float, device) -> torch.Tensor:
+    """The seed as the kernels read it (a one-element integer tensor on ``device``); ``None`` draws one from the default
+    generator of ``device`` without a host sync."""
+    if seed is None:
+        from ..kernels.kernel_utils import get_seed
+        return get_seed(p, device)
+    if isinstance(seed, torch.Tensor):
+        return seed.to(device)
+    return torch.tensor([int(seed)], dtype=torch.int64, device=device)
+
+
+def _dropout_attention(q, k, v, causal: bool, scale: float, key_padding_mask, window: Optional[int], p: float, seed,
+                       head_offset: int):
+    """Attention with dropout off the kernels: the explicit softmax in fp32, with the mask of
+    :func:`attention_dropout_keep`.  A query row that sees no key gets 0, as on the kernels."""
+    B, sq, H, _ = q.shape
+    sk, hkv = k.shape[1], k.shape[2]
+    qt, kt, vt = q.transpose(1, 2).float(), k.transpose(1, 2).float(), v.transpose(1, 2).float()
+    if H != hkv:
+        kt, vt = kt.repeat_interleave(H // hkv, dim=1), vt.repeat_interleave(H // hkv, dim=1)
+    visible = torch.ones(1, 1, 1, sk, dtype=torch.bool, device=q.device)
+    if key_padding_mask is not None:
+        visible = key_padding_mask.to(q.device).bool()[:, None, None, :]
+    if causal:
+        visible = visible & window_visibility(sq, sk, window, q.device)
+    s = (qt @ kt.transpose(-1, -2) * scale).masked_fill(~visible, torch.finfo(torch.float32).min)
+    probs = torch.softmax(s, dim=-1).masked_fill(~visible, 0.0)
+    keep = attention_dropout_keep(seed, B, H, sq, sk, p, head_offset).to(q.device)
+    probs = probs * (keep.float() * (1.0 / (1.0 - p)))
+    return (probs @ vt).transpose(1, 2).to(q.dtype)
 
 
 def _sdpa(q, k, v, causal: bool, scale: Optional[float], key_padding_mask: Optional[torch.Tensor] = None,
@@ -90,39 +177,44 @@ def _tma_view(t: torch.Tensor) -> torch.Tensor:
 
 
 def _flash_backward(go, q, k, v, o, lse, causal: bool, scale: float, mask=None, window: int = 0, q_offset: int = 0,
-                    sbhd_out: bool = False, dlse=None):
+                    sbhd_out: bool = False, dlse=None, dropout_p: float = 0.0, seed=None, head_offset: int = 0):
     """``(dq, dk, dv)`` of the flash kernels for the rows' output ``o`` and log-normaliser ``lse``: a δ pre-pass, a dK/dV
-    kernel and a dQ kernel.  ``dlse``: the gradient into ``lse``, or None."""
+    kernel and a dQ kernel.  ``dlse``: the gradient into ``lse``, or None.  ``dropout_p`` / ``seed`` / ``head_offset``:
+    those of the forward."""
     _ext.count_launch(3)
     tv = _tma_view
     return _ext.ext().flash_attn_bwd(tv(go.to(o.dtype)), tv(q), tv(k), tv(v), tv(o), lse.contiguous(), bool(causal),
-                                     float(scale), sbhd_out, dlse, mask, int(window), int(q_offset))
+                                     float(scale), sbhd_out, dlse, mask, int(window), int(q_offset), float(dropout_p), seed,
+                                     int(head_offset))
 
 
 class _FlashAttn(torch.autograd.Function):
     """Flash attention (``csrc/attention_sm90.cu``) → ``(o, lse)``; forward saves (q, k, v, o, lse, mask).  LSE is a
     differentiable output: ring attention merges per-block results through their LSEs, and a gradient into LSE only shifts
     δ in the backward kernel (``dS = P∘(dP − (δ − g_lse))``).  ``sbhd_out``: outputs and gradients are laid out ``[S,B,H,D]``
-    in memory (returned as ``[B,S,H,D]`` views), so a model's ``[S,B,H·D]`` reshape is free."""
+    in memory (returned as ``[B,S,H,D]`` views), so a model's ``[S,B,H·D]`` reshape is free.  ``dropout_p`` > 0: attention
+    dropout with the device ``seed`` (saved for the backward) and global head offset ``head_offset``."""
 
     @staticmethod
-    def forward(ctx, q, k, v, causal, scale, mask, window, q_offset, sbhd_out):
+    def forward(ctx, q, k, v, causal, scale, mask, window, q_offset, sbhd_out, dropout_p=0.0, seed=None, head_offset=0):
         ctx.set_materialize_grads(False)
         q, k, v = _tma_view(q), _tma_view(k), _tma_view(v)
         _ext.count_launch()
-        o, lse = _ext.ext().flash_attn_fwd(q, k, v, bool(causal), float(scale), sbhd_out, mask, int(window), int(q_offset))
-        ctx.save_for_backward(q, k, v, o, lse, mask)
-        ctx.args = (causal, scale, window, q_offset, sbhd_out)
+        o, lse = _ext.ext().flash_attn_fwd(q, k, v, bool(causal), float(scale), sbhd_out, mask, int(window), int(q_offset),
+                                           float(dropout_p), seed, int(head_offset))
+        ctx.save_for_backward(q, k, v, o, lse, mask, seed)
+        ctx.args = (causal, scale, window, q_offset, sbhd_out, dropout_p, head_offset)
         return o, lse
 
     @staticmethod
     def backward(ctx, go, g_lse):
-        q, k, v, o, lse, mask = ctx.saved_tensors
-        causal, scale, window, q_offset, sbhd_out = ctx.args
+        q, k, v, o, lse, mask, seed = ctx.saved_tensors
+        causal, scale, window, q_offset, sbhd_out, dropout_p, head_offset = ctx.args
         go = torch.zeros_like(o) if go is None else go
         dlse = None if g_lse is None else g_lse.float().contiguous()
-        dq, dk, dv = _flash_backward(go, q, k, v, o, lse, causal, scale, mask, window, q_offset, sbhd_out, dlse)
-        return dq, dk, dv, None, None, None, None, None, None
+        dq, dk, dv = _flash_backward(go, q, k, v, o, lse, causal, scale, mask, window, q_offset, sbhd_out, dlse, dropout_p,
+                                     seed, head_offset)
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None
 
 
 def _window_args(name: str, causal: bool, sliding_window: Optional[int], q_offset: int = 0) -> int:
@@ -150,7 +242,8 @@ def flash_attention_with_lse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, 
 
 def flash_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True,
                     scale: Optional[float] = None, key_padding_mask: Optional[torch.Tensor] = None,
-                    sliding_window: Optional[int] = None) -> torch.Tensor:
+                    sliding_window: Optional[int] = None, dropout_p: float = 0.0,
+                    dropout_seed: Optional[Union[int, torch.Tensor]] = None, head_offset: int = 0) -> torch.Tensor:
     """softmax(q·kᵀ·scale)·v for q ``[B, S_q, H, D]``, k/v ``[B, S_kv, Hkv, D]`` (H a multiple of Hkv) → ``[B, S_q, H, D]``.
 
     ``causal``: query i sees keys ≤ i (needs S_q == S_kv on the own kernels).  ``key_padding_mask``: ``[B, S_kv]`` bool
@@ -162,11 +255,23 @@ def flash_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: b
 
     On the own kernels a masked key contributes nothing and gets dK = dV = 0, and a query row that sees no key at all gets
     O = 0 and dQ = 0.  The SDPA fallback (CPU, other dtypes or head sizes) follows SDPA's rule for such a row, which is NaN
-    on some SDPA backends and versions."""
+    on some SDPA backends and versions.
+
+    ``dropout_p`` ∈ [0, 1): attention dropout on the probabilities, by the rule of :func:`attention_dropout_keep` for
+    ``dropout_seed`` (an int or a one-element int32 / int64 tensor) and global heads ``head_offset`` … ``head_offset + H − 1``
+    (a tensor-parallel rank passes rank · H).  Without a seed one is drawn from the default generator of q's device, on the
+    device, so activation checkpointing, which restores that generator, recomputes the same mask.  Off the kernels, p > 0
+    runs the explicit softmax with that mask (a host computation), so a seed drops the same elements on every path."""
     window = _window_args("flash_attention", causal, sliding_window)
+    dropout_p = _check_dropout(dropout_p)
     scale = scale if scale is not None else 1.0 / math.sqrt(q.shape[-1])
     if flash_kernels_apply(q, k, v, causal):
-        return _FlashAttn.apply(q, k, v, causal, scale, _kernel_mask(key_padding_mask), window, 0, True)[0]
+        seed = _dropout_seed(dropout_seed, dropout_p, q.device) if dropout_p > 0 else None
+        return _FlashAttn.apply(q, k, v, causal, scale, _kernel_mask(key_padding_mask), window, 0, True, dropout_p, seed,
+                                head_offset)[0]
+    if dropout_p > 0:
+        seed = _dropout_seed(dropout_seed, dropout_p, q.device)
+        return _dropout_attention(q, k, v, causal, scale, key_padding_mask, window or None, dropout_p, seed, head_offset)
     return _sdpa(q, k, v, causal, scale, key_padding_mask, window or None)
 
 

@@ -41,6 +41,7 @@ class _Rope(torch.autograd.Function):
         cos, sin = ctx.saved_tensors
         if ctx.cuda:
             _ext.count_launch()
+            g = g if g.stride(-1) == 1 else g.contiguous()        # autograd may hand a gradient with a strided head dim
             return _ext.ext().rope_apply(g, cos.contiguous().float(), sin.contiguous().float(), -1.0), None, None
         return rotate(g, cos, sin, -1.0), None, None
 

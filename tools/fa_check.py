@@ -1,6 +1,6 @@
 """Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
 usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]] [--kv-fp8] [--spec] [--rolling]
-                                [--decode-dims]
+                                [--decode-dims] [--dropout]
 
 --perf times forward and forward+backward of the own kernels and of SDPA in the same process, alternating, at the shapes
 the models run (BERT-large with right padding, ViT-B/16, GPT-NeoX-20B per rank at TP=8, Pythia-2.8B, Llama-2-7B).  FLOPs
@@ -44,7 +44,11 @@ attention (H 32, Hkv 8, D 64), Phi-3-mini (H = Hkv = 32, D 96) and Pythia-2.8B h
 kernel on a Mistral-7B head geometry (H 32, Hkv 8) as the control; B = 1, 8, 32, L = 4096 and 32768 (pairs that fit the
 card), bf16 and e4m3 caches holding the same values, one-token decode, a 5-token chain and a random 64-node tree.  GB/s is
 the K and V bytes of the visible cache rows (from the shapes) over the time of the call.  The D = 128 control's torch path
-is timed only at B = 1 (it is the one the kernels have replaced since they exist).  The partial at B = 8, L = 4096."""
+is timed only at B = 1 (it is the one the kernels have replaced since they exist).  The partial at B = 8, L = 4096.
+
+--dropout (with --perf) times attention dropout: the own kernels at p = 0.1 against the same kernels at p = 0 and against
+SDPA with dropout_p = 0.1, forward and (with --bwd) forward + backward, alternating in one process, at the BERT-large
+(right-padded, D = 64) and GPT-NeoX-20B per TP = 8 rank (D = 96) shapes of --perf."""
 import argparse
 import json
 import math
@@ -152,6 +156,58 @@ def perf(e, bwd: bool):
         rec["own_vs_sdpa_fwd"] = round(rec["sdpa_fwd_ms"] / rec["own_fwd_ms"], 2)
         if bwd:
             rec["own_vs_sdpa_fwd_bwd"] = round(rec["sdpa_fwd_bwd_ms"] / rec["own_fwd_bwd_ms"], 2)
+        print(json.dumps(rec), flush=True)
+
+
+DROPOUT_SHAPES = ("bert_large", "neox20b_tp8")
+
+
+def dropout_perf(e, bwd: bool, p: float = 0.1):
+    dev = torch.device("cuda")
+    print(json.dumps(gpu_info()), flush=True)
+    g = torch.Generator(device=dev).manual_seed(0)
+    seed = torch.tensor([1234], dtype=torch.int64, device=dev)
+    for (name, B, S, H, D, causal, pad) in PERF_SHAPES:
+        if name not in DROPOUT_SHAPES:
+            continue
+        q, k, v, go = (torch.randn(B, S, H, D, device=dev, generator=g).bfloat16() for _ in range(4))
+        scale = 1.0 / math.sqrt(D)
+        mask = bias = None
+        if pad > 0:
+            lens = (S * (1.0 - 2 * pad * torch.rand(B, device=dev, generator=g))).long().clamp(1, S)
+            mask = torch.arange(S, device=dev)[None, :] < lens[:, None]
+            bias = torch.zeros(B, 1, 1, S, device=dev, dtype=q.dtype).masked_fill(~mask[:, None, None, :], float("-inf"))
+        qt, kt, vt, gt = (t.transpose(1, 2) for t in (q, k, v, go))
+        qr, kr, vr = (t.detach().requires_grad_(True) for t in (qt, kt, vt))
+
+        def own(pp):
+            def f():
+                return e.flash_attn_fwd(q, k, v, causal, scale, True, mask, 0, 0, pp, seed)
+
+            def fb():
+                o, lse = f()
+                e.flash_attn_bwd(go, q, k, v, o, lse, causal, scale, True, None, mask, 0, 0, pp, seed)
+            return f, fb
+
+        def sdpa_f(qq=qt, kk=kt, vv=vt):
+            return torch.nn.functional.scaled_dot_product_attention(qq, kk, vv, attn_mask=bias, dropout_p=p,
+                                                                    is_causal=causal and bias is None)
+
+        def sdpa_fb():
+            torch.autograd.grad(sdpa_f(qr, kr, vr), (qr, kr, vr), gt)
+
+        fns = {"own_p0_fwd": own(0.0)[0], f"own_p{p}_fwd": own(p)[0], f"sdpa_p{p}_fwd": sdpa_f}
+        if bwd:
+            fns.update({"own_p0_fwd_bwd": own(0.0)[1], f"own_p{p}_fwd_bwd": own(p)[1], f"sdpa_p{p}_fwd_bwd": sdpa_fb})
+        t = {key: [] for key in fns}
+        for _ in range(3):                          # alternate, keep each one's best
+            for key, fn in fns.items():
+                t[key].append(time_fn(fn))
+        rec = {"bench": name + "_dropout", "B": B, "S": S, "H": H, "D": D, "causal": causal, "p": p}
+        rec.update({key + "_ms": round(min(vals), 4) for key, vals in t.items()})
+        for step in ("fwd", "fwd_bwd") if bwd else ("fwd",):
+            rec[f"dropout_overhead_{step}"] = round(rec[f"own_p{p}_{step}_ms"] / rec[f"own_p0_{step}_ms"], 3)
+            rec[f"own_vs_sdpa_dropout_{step}"] = round(rec[f"sdpa_p{p}_{step}_ms"] / rec[f"own_p{p}_{step}_ms"], 2)
         print(json.dumps(rec), flush=True)
 
 
@@ -606,6 +662,7 @@ def main():
     ap.add_argument("--rolling", action="store_true", help="with --perf: decode / verification on rolling vs linear KV caches")
     ap.add_argument("--decode-dims", action="store_true",
                     help="with --perf: decode / verification / flash-decoding partial at head_dim 64, 80, 96 vs the torch path")
+    ap.add_argument("--dropout", action="store_true", help="with --perf: attention dropout p = 0.1 vs p = 0 and SDPA")
     ap.add_argument("--head-dim", type=int, default=128, choices=attention.FLASH_HEAD_DIMS)
     a = ap.parse_args()
     if a.perf and a.window and a.cp > 1 and not torch.cuda.is_available():
@@ -674,6 +731,8 @@ def main():
             rolling_perf()
         elif a.decode_dims:
             decode_dims_perf()
+        elif a.dropout:
+            dropout_perf(e, a.bwd)
         elif a.window and a.cp > 1:
             cp_window_perf(a.bwd, a.cp)
         else:
