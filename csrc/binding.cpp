@@ -277,7 +277,11 @@ static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, 
   TORCH_CHECK(kc.dim() == 4 && kc.stride(3) == 1 && vc.sizes() == kc.sizes() && vc.strides() == kc.strides());
   TORCH_CHECK(positions.scalar_type() == at::kLong && positions.is_contiguous() && positions.numel() == q.size(0));
   CHECK_IN(cos_t); CHECK_IN(sin_t);
-  TORCH_CHECK(cos_t.scalar_type() == at::kFloat && cos_t.size(1) == q.size(3) / 2 && cos_t.size(0) >= kc.size(1));
+  // the tables' width is half the rotary width R: R = D rotates the whole head, R < D (GPT-NeoX rotary_pct) only its first R dims
+  TORCH_CHECK(cos_t.scalar_type() == at::kFloat && cos_t.size(0) >= kc.size(1) && sin_t.sizes() == cos_t.sizes(),
+              "decode_rope_kv: cos and sin must be fp32 tables of the same shape, at least as long as the cache");
+  TORCH_CHECK(cos_t.dim() == 2 && cos_t.size(1) >= 1 && 2 * cos_t.size(1) <= q.size(3),
+              "decode_rope_kv: the cos/sin tables must be [n_pos, R/2] with rotary width R even and 2 <= R <= head_dim");
   // rolling: positions run past the ring, up to the table length, which bounds the rotation instead of L (both tables are
   // read, so the shorter one bounds it).  The W slots of one call are distinct rows when W <= L, which the caller keeps
   // (LlamaForInference: W <= 64 < L).
@@ -296,7 +300,7 @@ static Tensor decode_rope_kv(const Tensor& q, const Tensor& k, const Tensor& v, 
   nxd::decode_rope_kv(q.data_ptr(), k.data_ptr(), v.data_ptr(), positions.data_ptr<long>(), dp, cos_t.data_ptr<float>(),
                       sin_t.data_ptr<float>(), q_out.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, W, H, Hkv, D, L, n_pos, qs, ks,
                       vs, kc.stride(0), kc.stride(1), kc.stride(2), stream(), e4m3, 1.0f / (float)k_scale, 1.0f / (float)v_scale,
-                      rolling);
+                      rolling, 2 * (int)cos_t.size(1));
   return q_out;
 }
 
@@ -505,7 +509,9 @@ static Tensor gemv_mx_grouped(const Tensor& x, const Tensor& w, const Tensor& sc
   nxd::gemv_mx_grouped(x.data_ptr(), w.data_ptr(), scale.data_ptr(), expert.data_ptr<long>(), y.data_ptr(), S, N, K, E, (int)fmt, stream());
   return y;
 }
-static Tensor gemv(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& residual) {
+// y = act(x · wᵀ + bias) + residual; act: 0 none, 1 exact GELU (erf), 2 tanh GELU
+static Tensor gemv(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& residual, const c10::optional<Tensor>& bias,
+                   int64_t act) {
   TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && x.dim() == 2 && w.dim() == 2);
   TORCH_CHECK(x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1) && x.size(0) >= 1 && x.size(0) <= 8 && x.size(1) % 8 == 0);
   TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(w.data_ptr()) % 16 == 0,
@@ -517,7 +523,14 @@ static Tensor gemv(const Tensor& x, const Tensor& w, const c10::optional<Tensor>
     TORCH_CHECK(residual->is_contiguous() && residual->sizes() == y.sizes() && residual->scalar_type() == at::kBFloat16);
     res = residual->data_ptr();
   }
-  nxd::gemv_bf16(x.data_ptr(), w.data_ptr(), res, y.data_ptr(), x.size(0), w.size(0), x.size(1), stream());
+  TORCH_CHECK(act >= 0 && act <= 2, "gemv: act must be 0 (none), 1 (exact GELU) or 2 (tanh GELU)");
+  const void* bp = nullptr;
+  if (bias.has_value()) {
+    TORCH_CHECK(bias->is_cuda() && bias->is_contiguous() && bias->dim() == 1 && bias->size(0) == w.size(0) &&
+                bias->scalar_type() == at::kBFloat16, "gemv: bias must be a contiguous bf16 CUDA tensor [N]");
+    bp = bias->data_ptr();
+  }
+  nxd::gemv_bf16(x.data_ptr(), w.data_ptr(), res, y.data_ptr(), x.size(0), w.size(0), x.size(1), stream(), bp, (int)act);
   return y;
 }
 
@@ -914,7 +927,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("row_argmax", &row_argmax);
   m.def("row_topk", &row_topk);
   m.def("row_topk_supported", &row_topk_supported);
-  m.def("gemv", &gemv, py::arg("x"), py::arg("w"), py::arg("residual") = py::none());
+  m.def("gemv", &gemv, py::arg("x"), py::arg("w"), py::arg("residual") = py::none(), py::kw_only(), py::arg("bias") = py::none(),
+        py::arg("act") = 0);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("gemm_fp8_block", &gemm_fp8_block);
   m.def("quantize_fp8_groups", &quantize_fp8_groups);

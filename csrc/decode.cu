@@ -233,11 +233,22 @@ __global__ void __launch_bounds__(HD) decode_combine_partial_kernel(const float*
   if (d == 0) { fin_ml[bh * 2] = mn * 0.6931471805599453f; fin_ml[bh * 2 + 1] = ls; }
 }
 
+__device__ __forceinline__ float gemv_act(float h, int act) {
+  switch (act) {
+    case 1: return 0.5f * h * (1.f + erff(h * 0.70710678118654752f));
+    case 2: return 0.5f * h * (1.f + tanhf(0.7978845608028654f * (h + 0.044715f * h * h * h)));
+    default: return h;
+  }
+}
+
 // y[m, n] = Σ_k x[m, k] · W[n, k]; one warp per output column n (8 columns per 256-thread CTA), M ≤ 8 rows of x kept hot in L1.
-template <int M>
+// EPI: the epilogue also adds bias[n] (when given) and applies act (gemv_act; 1: exact GELU, 2: tanh GELU, as in
+// csrc/moe_tkg.cu) before the residual, y = act(x·Wᵀ + bias) + residual with one bf16 rounding.  EPI = false is the plain
+// kernel; its two extra parameters are not read.
+template <int M, bool EPI>
 __global__ void __launch_bounds__(256) gemv_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w,
                                                    const __nv_bfloat16* __restrict__ residual, __nv_bfloat16* __restrict__ y,
-                                                   int N, int K) {
+                                                   int N, int K, const __nv_bfloat16* __restrict__ bias, int act) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n = blockIdx.x * 8 + warp;
   if (n >= N) return;
@@ -269,6 +280,10 @@ __global__ void __launch_bounds__(256) gemv_kernel(const __nv_bfloat16* __restri
     const float v = warp_sum(acc[m]);
     if (lane == 0) {
       float r = v;
+      if constexpr (EPI) {
+        if (bias) r += __bfloat162float(bias[n]);
+        r = gemv_act(r, act);
+      }
       if (residual) r += __bfloat162float(residual[(long)m * N + n]);
       y[(long)m * N + n] = __float2bfloat16_rn(r);
     }
@@ -294,7 +309,10 @@ __device__ __forceinline__ __nv_fp8_e4m3 quant_e4m3(__nv_bfloat16 x, float inv) 
 // a ring of L rows and the slot is (positions[b] + w) mod L.  One warp per head row; cos/sin rows gathered by position.
 // HF rotate-half convention (csrc/elementwise.cu rope_kernel).  An e4m3 cache gets the bf16 rows a bf16 cache would hold,
 // quantised by quant_e4m3 with k_inv = 1/k_scale and v_inv = 1/v_scale.
-template <typename T, bool ROLL>
+// PARTIAL (GPT-NeoX rotary_pct < 1): only dims [0, 2·rot_half) of q and k are rotated, rotate-half within them (pairs
+// (c, rot_half + c), tables of width rot_half); dims [2·rot_half, D) are copied (k quantised on an e4m3 cache).  The full-
+// rotary kernels (PARTIAL = false) do not read rot_half.
+template <typename T, bool ROLL, bool PARTIAL>
 __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                                             const __nv_bfloat16* __restrict__ v, const long* __restrict__ positions,
                                                             const long* __restrict__ depth, const float* __restrict__ cos_t,
@@ -302,7 +320,7 @@ __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16
                                                             T* __restrict__ kc, T* __restrict__ vc, int B, int W, int H, int Hkv,
                                                             int D, int L, int n_pos, long q_sb, long q_ss, long q_sh, long k_sb,
                                                             long k_ss, long k_sh, long v_sb, long v_ss, long v_sh, long c_sb,
-                                                            long c_ss, long c_sh, float k_inv, float v_inv) {
+                                                            long c_ss, long c_sh, float k_inv, float v_inv, int rot_half) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int rows = B * W * (H + 2 * Hkv);
   if (warp >= rows) return;
@@ -319,7 +337,7 @@ __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16
   q += b * q_sb + w * q_ss;
   k += b * k_sb + w * k_ss;
   v += b * v_sb + w * v_ss;
-  const int half = D / 2;
+  const int half = PARTIAL ? rot_half : D / 2;
   if (r < H + Hkv) {                                   // q or k head: rotate
     const bool is_q = r < H;
     const int h = is_q ? r : r - H;
@@ -349,6 +367,16 @@ __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16
         }
       }
     }
+    if constexpr (PARTIAL) {                           // pass-through dims
+      for (int c = 2 * half + lane; c < D; c += 32) {
+        if constexpr (sizeof(T) == 2) {
+          dst[c] = src[c];
+        } else {
+          if (is_q) dst[c] = src[c];
+          else reinterpret_cast<T*>(dst)[c] = quant_e4m3(src[c], k_inv);
+        }
+      }
+    }
   } else {                                             // v head: copy
     const int h = r - H - Hkv;
     const __nv_bfloat16* src = v + (long)h * v_sh;
@@ -366,21 +394,25 @@ __global__ void __launch_bounds__(128) decode_rope_kv_kernel(const __nv_bfloat16
 void decode_rope_kv(const void* q, const void* k, const void* v, const long* positions, const long* depth, const float* cos_t,
                     const float* sin_t, void* q_out, void* kc, void* vc, int B, int W, int H, int Hkv, int D, int L, int n_pos,
                     const long* qs, const long* ks, const long* vs, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3,
-                    float k_inv, float v_inv, bool rolling) {
+                    float k_inv, float v_inv, bool rolling, int rot) {
   const int rows = B * W * (H + 2 * Hkv);
   const int grid = (rows * 32 + 127) / 128;
-#define NXD_ROPE_KV(T, R)                                                                                                     \
-  decode_rope_kv_kernel<T, R><<<grid, 128, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, \
-      positions, depth, cos_t, sin_t, (__nv_bfloat16*)q_out, (T*)kc, (T*)vc, B, W, H, Hkv, D, L, n_pos, qs[0], qs[1], qs[2],   \
-      ks[0], ks[1], ks[2], vs[0], vs[1], vs[2], c_sb, c_ss, c_sh, k_inv, v_inv)
+#define NXD_ROPE_KV_P(T, R, P)                                                                                                   \
+  decode_rope_kv_kernel<T, R, P><<<grid, 128, 0, st>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, \
+      positions, depth, cos_t, sin_t, (__nv_bfloat16*)q_out, (T*)kc, (T*)vc, B, W, H, Hkv, D, L, n_pos, qs[0], qs[1], qs[2],      \
+      ks[0], ks[1], ks[2], vs[0], vs[1], vs[2], c_sb, c_ss, c_sh, k_inv, v_inv, rot / 2)
+#define NXD_ROPE_KV(T, R)                        \
+  if (rot < D) NXD_ROPE_KV_P(T, R, true);        \
+  else NXD_ROPE_KV_P(T, R, false)
   if (kv_e4m3) {
-    if (rolling) NXD_ROPE_KV(__nv_fp8_e4m3, true);
-    else NXD_ROPE_KV(__nv_fp8_e4m3, false);
+    if (rolling) { NXD_ROPE_KV(__nv_fp8_e4m3, true); }
+    else { NXD_ROPE_KV(__nv_fp8_e4m3, false); }
   } else {
-    if (rolling) NXD_ROPE_KV(__nv_bfloat16, true);
-    else NXD_ROPE_KV(__nv_bfloat16, false);
+    if (rolling) { NXD_ROPE_KV(__nv_bfloat16, true); }
+    else { NXD_ROPE_KV(__nv_bfloat16, false); }
   }
 #undef NXD_ROPE_KV
+#undef NXD_ROPE_KV_P
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 
@@ -427,11 +459,16 @@ void decode_combine(const float* part_o, const float* part_ml, void* out, int ro
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 
-void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, cudaStream_t st) {
+void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, cudaStream_t st,
+               const void* bias, int act) {
   const int grid = (N + 7) / 8;
-#define NXD_GEMV(Mv)                                                                                                \
-  gemv_kernel<Mv><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)w, (const __nv_bfloat16*)residual, \
-                                        (__nv_bfloat16*)y, N, K)
+  const bool epi = bias != nullptr || act != 0;
+#define NXD_GEMV_E(Mv, E)                                                                                              \
+  gemv_kernel<Mv, E><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)w, (const __nv_bfloat16*)residual, \
+                                           (__nv_bfloat16*)y, N, K, (const __nv_bfloat16*)bias, act)
+#define NXD_GEMV(Mv)           \
+  if (epi) NXD_GEMV_E(Mv, true); \
+  else NXD_GEMV_E(Mv, false)
   switch (M) {
     case 1: NXD_GEMV(1); break;
     case 2: NXD_GEMV(2); break;
@@ -444,6 +481,7 @@ void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int 
     default: nxd_throw("gemv_bf16: M must be 1..8", __FILE__, __LINE__);
   }
 #undef NXD_GEMV
+#undef NXD_GEMV_E
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 

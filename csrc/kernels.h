@@ -144,11 +144,14 @@ void decode_attention(const void* q, const void* k, const void* v, const long* p
 void decode_rope_kv(const void* q, const void* k, const void* v, const long* positions, const long* depth, const float* cos_t,
                     const float* sin_t, void* q_out, void* kc, void* vc, int B, int W, int H, int Hkv, int D, int L, int n_pos,
                     const long* qs, const long* ks, const long* vs, long c_sb, long c_ss, long c_sh, cudaStream_t st, bool kv_e4m3,
-                    float k_inv, float v_inv, bool rolling);   // kv_e4m3: the cache stores k·k_inv and v·v_inv as e4m3
+                    float k_inv, float v_inv, bool rolling, int rot);   // kv_e4m3: the cache stores k·k_inv and v·v_inv as e4m3;
+                                                                         // rot: rotary width R (even, 2 ≤ R ≤ D; R < D: dims ≥ R copied)
 // merge of per-split decode partials [rows·splits, D] + (max, sum) → bf16 row r at out + (r / H)·o_sb + (r % H)·o_sh
 void decode_combine(const float* part_o, const float* part_ml, void* out, int rows, int splits, int D, long o_sb, long o_sh,
                     int H, cudaStream_t st);
-void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, cudaStream_t st);
+// bias: optional bf16 [N]; act: 0 none, 1 exact GELU, 2 tanh GELU (csrc/moe_tkg.cu numbering) → y = act(x·Wᵀ + bias) + residual
+void gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, cudaStream_t st,
+               const void* bias = nullptr, int act = 0);
 
 // ---- attention (attention_sm90.cu): q [B,S_q,H,D], k/v [B,S_kv,Hkv,D] bf16 views, D ∈ {64, 80, 96, 128}; strides = (b, s, h)
 // in elements.  kpm: optional key-padding mask, uint8 [B, S_kv] with row stride kpm_sb (key visible iff nonzero), or null.

@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""Serve an HF Llama checkpoint and check it against ``transformers`` — counterpart of the reference's
+"""Serve an HF Llama / Mixtral / GPT-NeoX (Pythia) checkpoint and check it against ``transformers`` — counterpart of the reference's
 ``examples/inference/run_hf.py`` (HF config + weights + tokenizer → TP-sharded model → ``generate``).
 
   torchrun --nproc-per-node 8 examples/inference/run_hf.py --model_path /models/Llama-2-7b-hf --tp_degree 8 --check_accuracy
   python examples/inference/run_hf.py            # no --model_path: a random tiny HF Llama is created in memory (offline demo)
+  python examples/inference/run_hf.py --family gpt_neox     # the same with a tiny random HF GPT-NeoX
 
 Every rank memory-maps the safetensors files and keeps only its shard (``models.hf_compat.load_hf_checkpoint``); the decode
-loop is the CUDA-graph captured serving path of ``LlamaForInference``.  ``--check_accuracy`` also runs the HF model on rank 0
+loop is the CUDA-graph captured serving path of ``LlamaForInference`` (``GPTNeoXForInference`` for a ``gpt_neox`` config).  ``--check_accuracy`` also runs the HF model on rank 0
 (CPU, fp32) and reports how many greedy tokens agree — the reference runner's ``check_accuracy`` flow."""
 import argparse
 import os
@@ -20,6 +21,8 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "examples", "training"))
 
 from neuronx_distributed_b200.models import hf_compat  # noqa: E402
+from neuronx_distributed_b200.models.gpt_neox import GPTNeoXConfig  # noqa: E402
+from neuronx_distributed_b200.models.gpt_neox_inference import GPTNeoXForInference  # noqa: E402
 from neuronx_distributed_b200.models.llama_inference import LlamaForInference  # noqa: E402
 from neuronx_distributed_b200.parallel_layers import parallel_state as ps  # noqa: E402
 from training_utils import init_distributed  # noqa: E402
@@ -29,6 +32,7 @@ def main():
     p = argparse.ArgumentParser()
     p.add_argument("--model_path", default=None, help="HF model directory (config.json + *.safetensors [+ tokenizer])")
     p.add_argument("--tp_degree", type=int, default=None)
+    p.add_argument("--family", choices=("llama", "gpt_neox"), default="llama", help="model of the offline demo (no --model_path)")
     p.add_argument("--prompt", action="append", default=None)
     p.add_argument("--max_new_tokens", type=int, default=16)
     p.add_argument("--seq_len", type=int, default=128)
@@ -50,9 +54,15 @@ def main():
             tokenizer = transformers.AutoTokenizer.from_pretrained(a.model_path, padding_side="right")
     else:
         torch.manual_seed(0)
-        hc = transformers.LlamaConfig(vocab_size=512, hidden_size=128, intermediate_size=352, num_hidden_layers=2, num_attention_heads=8,
-                                      num_key_value_heads=4, max_position_embeddings=a.seq_len, attn_implementation="eager")
-        hf_model = transformers.LlamaForCausalLM(hc).eval()
+        if a.family == "gpt_neox":
+            hc = transformers.GPTNeoXConfig(vocab_size=512, hidden_size=128, intermediate_size=512, num_hidden_layers=2,
+                                            num_attention_heads=4, rotary_pct=0.25, hidden_act="gelu_fast",
+                                            max_position_embeddings=a.seq_len, attn_implementation="eager")
+            hf_model = transformers.GPTNeoXForCausalLM(hc).eval()
+        else:
+            hc = transformers.LlamaConfig(vocab_size=512, hidden_size=128, intermediate_size=352, num_hidden_layers=2, num_attention_heads=8,
+                                          num_key_value_heads=4, max_position_embeddings=a.seq_len, attn_implementation="eager")
+            hf_model = transformers.LlamaForCausalLM(hc).eval()
         hf_cfg, state = hc, hf_model.state_dict()
         a.check_accuracy = True
     cfg = hf_compat.config_from_hf(hf_cfg, dtype=dtype, device=dev, max_position_embeddings=a.seq_len)
@@ -65,7 +75,10 @@ def main():
     lm_cls = None
     if hasattr(cfg, "num_local_experts"):                        # Mixtral / DBRX checkpoints: same serving wrapper, MoE decoder
         from neuronx_distributed_b200.models.mixtral import MixtralForCausalLM as lm_cls
-    model = LlamaForInference(cfg, batch_size=1, max_seq_len=a.seq_len, lm_cls=lm_cls).eval()
+    if isinstance(cfg, GPTNeoXConfig):
+        model = GPTNeoXForInference(cfg, batch_size=1, max_seq_len=a.seq_len).eval()
+    else:
+        model = LlamaForInference(cfg, batch_size=1, max_seq_len=a.seq_len, lm_cls=lm_cls).eval()
     res = hf_compat.load_hf_checkpoint(model, state)
     assert not res.missing_keys, res.missing_keys
 

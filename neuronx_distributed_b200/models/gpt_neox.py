@@ -30,6 +30,7 @@ class GPTNeoXConfig:
     max_position_embeddings: int = 2048
     layer_norm_eps: float = 1e-5
     use_parallel_residual: bool = True
+    hidden_act: str = "gelu"                 # HF name: "gelu" (erf), or "gelu_fast" / "gelu_new" / "gelu_pytorch_tanh" (tanh)
     attention_dropout: float = 0.0           # dropout on the attention probabilities (training only)
     initializer_range: float = 0.02
     sequence_parallel_enabled: bool = False
@@ -82,10 +83,16 @@ class GPTNeoXAttention(nn.Module):
         return self.dense(o.transpose(0, 1).reshape(S, B, self.heads_local * self.head_dim))
 
 
+_GELU_APPROX = {"gelu": "none", "gelu_fast": "tanh", "gelu_new": "tanh", "gelu_pytorch_tanh": "tanh"}
+
+
 class GPTNeoXMLP(nn.Module):
     def __init__(self, cfg: GPTNeoXConfig):
         super().__init__()
         sp = cfg.sequence_parallel_enabled
+        if cfg.hidden_act not in _GELU_APPROX:
+            raise ValueError(f"hidden_act {cfg.hidden_act!r} is not supported (one of {sorted(_GELU_APPROX)})")
+        self.gelu_approximate = _GELU_APPROX[cfg.hidden_act]
         self.dense_h_to_4h = ColumnParallelLinear(cfg.hidden_size, cfg.intermediate_size, bias=True, gather_output=False,
                                                   init_method=_init(cfg.initializer_range), sequence_parallel_enabled=sp,
                                                   sequence_dimension=0, dtype=cfg.dtype, device=cfg.device)
@@ -94,7 +101,7 @@ class GPTNeoXMLP(nn.Module):
                                                sequence_dimension=0, dtype=cfg.dtype, device=cfg.device)
 
     def forward(self, x):
-        return self.dense_4h_to_h(torch.nn.functional.gelu(self.dense_h_to_4h(x)))
+        return self.dense_4h_to_h(torch.nn.functional.gelu(self.dense_h_to_4h(x), approximate=self.gelu_approximate))
 
 
 class GPTNeoXLayer(nn.Module):

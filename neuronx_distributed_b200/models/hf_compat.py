@@ -56,22 +56,37 @@ def _as_dict(hf_config: Any) -> Dict[str, Any]:
 
 def _family(d: Dict[str, Any]) -> str:
     mt = str(d.get("model_type", "")).lower()
-    if mt in ("mixtral", "dbrx"):
+    if mt in ("mixtral", "dbrx", "gpt_neox"):
         return mt
     if mt in ("llama", "mistral", "qwen2", ""):
         return "llama"
-    raise ValueError(f"unsupported HF model_type {mt!r} (llama / mistral / mixtral / dbrx)")
+    raise ValueError(f"unsupported HF model_type {mt!r} (llama / mistral / mixtral / dbrx / gpt_neox)")
 
 
 def config_from_hf(hf_config: Any, **overrides):
-    """``LlamaConfig`` / ``MixtralConfig`` / ``DbrxConfig`` from an HF config object, dict, ``config.json`` or model directory.
-    ``overrides`` (``dtype=…, device=…, sequence_parallel_enabled=…``) are applied last."""
+    """``LlamaConfig`` / ``MixtralConfig`` / ``DbrxConfig`` / ``GPTNeoXConfig`` from an HF config object, dict, ``config.json``
+    or model directory.  ``overrides`` (``dtype=…, device=…, sequence_parallel_enabled=…``) are applied last."""
+    from .gpt_neox import GPTNeoXConfig
     from .llama import LlamaConfig
     from .mixtral import DbrxConfig, MixtralConfig
 
     d = _as_dict(hf_config)
     fam = _family(d)
-    if fam == "dbrx":
+    if fam == "gpt_neox":
+        if d.get("tie_word_embeddings", False):
+            raise ValueError("gpt_neox: tied word embeddings are not supported (embed_out is a separate weight)")
+        # the rotary settings: rotary_pct / rotary_emb_base in Pythia / NeoX config.json files, rope_parameters
+        # {partial_rotary_factor, rope_theta} in transformers >= 5
+        rp = d.get("rope_parameters") or {}
+        pct = next((v for v in (d.get("rotary_pct"), rp.get("partial_rotary_factor"), d.get("partial_rotary_factor")) if v is not None), None)
+        base = next((v for v in (d.get("rotary_emb_base"), rp.get("rope_theta"), d.get("rope_theta")) if v is not None), None)
+        kw = dict(vocab_size=d["vocab_size"], hidden_size=d["hidden_size"], intermediate_size=d["intermediate_size"],
+                  num_hidden_layers=d["num_hidden_layers"], num_attention_heads=d["num_attention_heads"],
+                  max_position_embeddings=d.get("max_position_embeddings"), layer_norm_eps=d.get("layer_norm_eps"),
+                  use_parallel_residual=d.get("use_parallel_residual"), hidden_act=d.get("hidden_act"),
+                  rotary_pct=None if pct is None else float(pct), rotary_emb_base=None if base is None else float(base))
+        cls = GPTNeoXConfig
+    elif fam == "dbrx":
         attn, ffn = d.get("attn_config", {}), d.get("ffn_config", {})
         kw = dict(vocab_size=d["vocab_size"], hidden_size=d["d_model"], intermediate_size=ffn["ffn_hidden_size"],
                   num_hidden_layers=d["n_layers"], num_attention_heads=d["n_heads"], num_key_value_heads=attn.get("kv_n_heads", d["n_heads"]),
@@ -520,6 +535,7 @@ def load_hf_checkpoint(model, path_or_state, cfg=None, strict: bool = True):
         return _load_into_pipeline_stage(pp, model, hf_sd, cfg, strict)
     fam = _encoder_family(model)
     if fam is not None:                               # BERT / ViT: renames (+ QKV fusion); GPT-NeoX: HF names as they are
+        model = model.lm if isinstance(getattr(model, "lm", None), torch.nn.Module) else model   # serving wrapper
         full = {"bert": hf_to_nxd_bert_state_dict, "vit": hf_to_nxd_vit_state_dict, "gptneox": dict}[fam](hf_sd)
         full = {k: v for k, v in full.items() if not k.endswith(("rotary_emb.inv_freq", "attention.bias", "attention.masked_bias"))}
         want = model.state_dict()

@@ -37,13 +37,13 @@ class LlamaForInference(nn.Module):
         self.cfg = cfg
         self.lm = (lm_cls or LlamaForCausalLM)(cfg)
         self.batch_size, self.max_seq_len = batch_size, max_seq_len
-        attn0 = self._core.layers[0].self_attn
         # flash decoding (reference examples/inference ``flash_decoding_enabled``): TP ranks that hold replicas of the same KV
         # heads shard the cache along the SEQUENCE inside that replica group instead of storing it ``m`` times
         self.flash_decoding, self.kv_group, self.kv_rank, shards = bool(flash_decoding), None, 0, 1
         if flash_decoding:
             import torch.distributed as dist
 
+            attn0 = self._core.layers[0].self_attn
             self.kv_group = getattr(attn0.qkv_proj, "kv_group", None)
             assert self.kv_group is not None and dist.get_world_size(self.kv_group) > 1, \
                 "flash decoding needs replicated KV heads (tensor-parallel size > number of KV heads)"
@@ -55,18 +55,30 @@ class LlamaForInference(nn.Module):
         if kv_quant is not None and kv_quant.dequant_dtype != cfg.dtype:
             raise ValueError(f"kv_quant.dequant_dtype ({kv_quant.dequant_dtype}) must be the model dtype ({cfg.dtype}): "
                              "attention off the kernels reads the de-quantised cache next to the model's queries")
-        self.kv = KVCacheManager(cfg.num_hidden_layers, batch_size, max_seq_len, attn0.num_kv_heads_local, cfg.head_dim,
+        self.kv = KVCacheManager(cfg.num_hidden_layers, batch_size, max_seq_len, self._kv_heads_local(), cfg.head_dim,
                                  dtype=cfg.dtype, device=cfg.device, kv_quant=kv_quant, num_cores_per_group=shards,
                                  rolling_window=cfg.sliding_window if rolling_kv_cache else None)
         self.sampler = sampler or Sampler(top_k=1, vocab_parallel=True)
         self.on_device_sampling = on_device_sampling
-        cos, sin = ops.rope.rope_tables(max_seq_len, cfg.head_dim, cfg.rope_theta, cfg.device, 0, cfg.rope_scaling_factor)
+        cos, sin = self._rope_tables(max_seq_len)
         self.register_buffer("rope_cos", cos, persistent=False)
         self.register_buffer("rope_sin", sin, persistent=False)
 
+    # ------------------------------------------------------------------ what another decoder family overrides
     @property
     def _core(self):
         return getattr(self.lm, "model", self.lm)        # Llama nests the decoder under .model, Mixtral/DBRX do not
+
+    def _kv_heads_local(self) -> int:
+        return self._core.layers[0].self_attn.num_kv_heads_local
+
+    def _rope_tables(self, max_seq_len: int):
+        """``(cos, sin) [max_seq_len, R/2]``: the rotary width R is twice the tables' width (R = head_dim here)."""
+        c = self.cfg
+        return ops.rope.rope_tables(max_seq_len, c.head_dim, c.rope_theta, c.device, 0, c.rope_scaling_factor)
+
+    def _logits(self, h: torch.Tensor) -> torch.Tensor:
+        return self.lm.lm_head(h)
 
     def load_state_dict(self, sd, strict: bool = True):
         return self.lm.load_state_dict(sd, strict=strict)
@@ -78,8 +90,6 @@ class LlamaForInference(nn.Module):
     def _attn_block(self, layer_idx: int, layer, x: torch.Tensor, positions: Optional[torch.Tensor], prefill: bool,
                     kv_len: Optional[int], tree=None, prompt_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
         att = layer.self_attn
-        sw = self.cfg.sliding_window                       # Mistral / Mixtral window (None: full causal attention)
-        roll = {"rolling": True} if self.kv.rolling else {}   # ring cache: the kernels and torch paths map positions to rows
         h = layer.input_layernorm(x)
         q, k, v = att.qkv_proj(h)                          # [S, B, h*D]
         S, B = q.shape[0], q.shape[1]
@@ -87,13 +97,25 @@ class LlamaForInference(nn.Module):
         q = q.reshape(S, B, att.num_heads_local, D).transpose(0, 1)
         k = k.reshape(S, B, att.num_kv_heads_local, D).transpose(0, 1)
         v = v.reshape(S, B, att.num_kv_heads_local, D).transpose(0, 1).contiguous()
+        o = self._attention(layer_idx, q, k, v, positions, prefill, kv_len, tree, prompt_lens)
+        o = o.transpose(0, 1).reshape(S, B, att.num_heads_local * D)
+        return _row_linear_plus_residual(att.o_proj, o, x)
+
+    def _attention(self, layer_idx: int, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, positions: Optional[torch.Tensor],
+                   prefill: bool, kv_len: Optional[int], tree=None, prompt_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """RoPE, the cache write and attention of one layer: q ``[B, S, H, D]``, k / v ``[B, S, Hkv, D]`` (any b / s / h
+        strides) → o ``[B, S, H, D]``.  The rotary width R is twice the tables' width: R < D (GPT-NeoX ``rotary_pct``)
+        rotates dims [0, R) and passes the rest through, on the kernel and on the torch paths alike."""
+        S = q.shape[1]
+        sw = getattr(self.cfg, "sliding_window", None)     # Mistral / Mixtral window (None: full causal attention)
+        roll = {"rolling": True} if self.kv.rolling else {}   # ring cache: the kernels and torch paths map positions to rows
         # (k_scale, v_scale) when the decode kernels read the cache as stored; the defaults (1.0) are not passed on, so a bf16
         # cache makes the calls it makes without quantisation
         scales = self.kv.kernel_scales()
         scale_kw = {} if scales in (None, (1.0, 1.0)) else {"k_scale": scales[0], "v_scale": scales[1]}
         if prefill:
             cos, sin = self.rope_cos[:S], self.rope_sin[:S]
-            q, k = ops.rope.apply_rotary(q, cos, sin), ops.rope.apply_rotary(k, cos, sin)
+            q, k = _rotary(ops.rope.apply_rotary, q, cos, sin), _rotary(ops.rope.apply_rotary, k, cos, sin)
             if self.flash_decoding:
                 self.kv.write_prefill_sharded(layer_idx, k, v, self.kv_rank)
             else:
@@ -103,9 +125,9 @@ class LlamaForInference(nn.Module):
             assert S == 1 and tree is None, "flash decoding serves plain token generation (no speculation window)"
             from ..modules.attention.flash_decode import flash_decode_attention
 
-            cos = self.rope_cos[positions].unsqueeze(1)     # [B, 1, D/2]
+            cos = self.rope_cos[positions].unsqueeze(1)     # [B, 1, R/2]
             sin = self.rope_sin[positions].unsqueeze(1)
-            q, k = ops.rope.rotate(q, cos, sin), ops.rope.rotate(k, cos, sin)
+            q, k = _rotary(ops.rope.rotate, q, cos, sin), _rotary(ops.rope.rotate, k, cos, sin)
             self.kv.write_decode_sharded(layer_idx, k, v, positions, self.kv_rank)                  # owner-only write
             kc, vc = self.kv.stored(layer_idx) if scales is not None else self.kv.get(layer_idx)
             o = flash_decode_attention(q, kc, vc, positions, self.kv_group, sliding_window=sw, **scale_kw)
@@ -125,8 +147,8 @@ class LlamaForInference(nn.Module):
             else:
                 d = torch.arange(S, device=q.device) if depth is None else depth
                 idx = (positions.unsqueeze(1) + d.unsqueeze(0)).clamp(max=self.max_seq_len - 1)
-                cos, sin = self.rope_cos[idx], self.rope_sin[idx]                 # [B, W, D/2]
-                q, k = ops.rope.rotate(q, cos, sin), ops.rope.rotate(k, cos, sin)
+                cos, sin = self.rope_cos[idx], self.rope_sin[idx]                 # [B, W, R/2]
+                q, k = _rotary(ops.rope.rotate, q, cos, sin), _rotary(ops.rope.rotate, k, cos, sin)
                 self.kv.write_window(layer_idx, k, v, positions)
                 kc, vc = self.kv.get(layer_idx, kv_len)
                 scale_kw = {}                                                     # kv.get de-quantised the cache
@@ -136,8 +158,7 @@ class LlamaForInference(nn.Module):
                 o = ops.attention.speculation_attention(q, kc, vc, positions, tree_mask, depth, sw, **scale_kw, **roll)
             else:
                 o = ops.attention.speculation_attention_torch(q, kc, vc, positions, tree_mask, depth, sw, **roll)
-        o = o.transpose(0, 1).reshape(S, B, att.num_heads_local * D)
-        return _row_linear_plus_residual(att.o_proj, o, x)
+        return o
 
     def _tkg_block(self, layer_idx: int, layer):
         """Decode-time fused view of a MoE layer (shares its router / experts / norm; owns no parameters).  Kept outside the
@@ -188,14 +209,14 @@ class LlamaForInference(nn.Module):
             last = h[-1]
         else:
             last = h[last_token_index, torch.arange(B, device=h.device)]
-        logits = self.lm.lm_head(last.unsqueeze(0))[0].float()                   # [B, V/tp]
+        logits = self._logits(last.unsqueeze(0))[0].float()                   # [B, V/tp]
         return self.sampler.sample(logits) if self.on_device_sampling else logits
 
     @torch.no_grad()
     def token_generation(self, input_ids: torch.Tensor, positions: torch.Tensor, kv_len: Optional[int] = None) -> torch.Tensor:
         """``input_ids`` [B, 1], ``positions`` [B] → next token ids [B]."""
         h = self._body(input_ids, positions, False, kv_len)
-        logits = self.lm.lm_head(h)[0].float()
+        logits = self._logits(h)[0].float()
         return self.sampler.sample(logits) if self.on_device_sampling else logits
 
     @torch.no_grad()
@@ -209,7 +230,7 @@ class LlamaForInference(nn.Module):
         dev = input_ids.device
         tree = None if tree_mask is None else (tree_mask.to(dev, torch.bool).contiguous(), tree_depth.to(dev, torch.long).contiguous())
         h = self._body(input_ids, positions, False, kv_len, tree)                # [W, B, H]
-        logits = self.lm.lm_head(h).float()                                       # [W, B, V/tp]
+        logits = self._logits(h).float()                                          # [W, B, V/tp]
         W, B = logits.shape[:2]
         out = self.sampler.sample(logits.reshape(W * B, -1)).view(W, B).t() if self.on_device_sampling else logits.transpose(0, 1)
         return (out, h.transpose(0, 1)) if return_hidden else out
@@ -228,21 +249,31 @@ class LlamaForInference(nn.Module):
         return torch.stack(out, dim=1)
 
 
+def _rotary(rot, x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch.Tensor:
+    """``rot`` (``ops.rope.apply_rotary`` / ``ops.rope.rotate``) on the first R = 2·cos.shape[-1] dims of x; the rest pass."""
+    R = 2 * cos.shape[-1]
+    if R == x.shape[-1]:
+        return rot(x, cos, sin)
+    return torch.cat([rot(x[..., :R].contiguous(), cos, sin), x[..., R:]], dim=-1)
+
+
 def _row_linear_plus_residual(lin, inp: torch.Tensor, residual: torch.Tensor) -> torch.Tensor:
-    """``residual + RowParallelLinear(inp)``.  At decode (<= 8 rows, bf16, no bias) this is ONE kernel: the GEMV with the residual
-    in its epilogue (tp = 1) or the fused GEMV + in-switch all-reduce + residual (tp > 1, csrc/nvls_coll.cu)."""
+    """``residual + RowParallelLinear(inp)``.  At decode (<= 8 rows, bf16) this is ONE kernel: the GEMV with the bias and the
+    residual in its epilogue (tp = 1) or, without a bias, the fused GEMV + in-switch all-reduce + residual (tp > 1,
+    csrc/nvls_coll.cu)."""
     M = inp.numel() // inp.shape[-1]
     w = lin.weight
+    bias = getattr(lin, "bias", None)
     e = ops._ext.ext() if inp.is_cuda else None
-    if (e is not None and M <= 8 and inp.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and getattr(lin, "bias", None) is None
-            and not torch.is_grad_enabled() and getattr(lin, "reduce_output", True) and w.shape[1] % 8 == 0 and w.shape[0] % 8 == 0
+    if (e is not None and M <= 8 and inp.dtype == torch.bfloat16 and w.dtype == torch.bfloat16
+            and (bias is None or bias.dtype == torch.bfloat16) and not torch.is_grad_enabled() and getattr(lin, "reduce_output", True) and w.shape[1] % 8 == 0 and w.shape[0] % 8 == 0
             and not getattr(lin, "sequence_parallel_enabled", False)):
         x2 = inp.reshape(M, inp.shape[-1]).contiguous()
         r2 = residual.reshape(M, residual.shape[-1]).contiguous()
         tp = lin.tensor_model_parallel_size
         if tp == 1 and hasattr(e, "gemv") and x2.data_ptr() % 16 == 0 and w.data_ptr() % 16 == 0:   # 16-byte vector loads
             ops._ext.count_launch()
-            return e.gemv(x2, w, r2).view_as(residual)
-        if tp > 1 and ops.tp_fused.get_backend() == "fused" and ops.nvls.gemv_all_reduce_eligible(x2, w):
+            return (e.gemv(x2, w, r2) if bias is None else e.gemv(x2, w, r2, bias=bias)).view_as(residual)
+        if tp > 1 and bias is None and ops.tp_fused.get_backend() == "fused" and ops.nvls.gemv_all_reduce_eligible(x2, w):
             return ops.nvls.gemv_all_reduce(x2, w, lin.tensor_parallel_group, residual=r2).view_as(residual)
     return residual + lin(inp)

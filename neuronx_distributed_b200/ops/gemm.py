@@ -18,6 +18,17 @@ from . import _ext
 
 _MIN_DIM = 64
 
+#: activation codes of the decode GEMV epilogue (``csrc/decode.cu`` gemv_act): HF ``hidden_act`` name → code
+GEMV_ACT = {"gelu": 1, "gelu_fast": 2, "gelu_new": 2, "gelu_pytorch_tanh": 2}
+
+
+def _act_torch(y: torch.Tensor, act: int) -> torch.Tensor:
+    if act == 0:
+        return y
+    if act not in (1, 2):
+        raise ValueError(f"act must be 0 (none), 1 (exact GELU) or 2 (tanh GELU), got {act}")
+    return torch.nn.functional.gelu(y, approximate="none" if act == 1 else "tanh")
+
 
 def fused_wgrad_enabled() -> bool:
     return os.environ.get("NXD_DISABLE_FUSED_WGRAD", "0") != "1" and os.environ.get("NXD_DISABLE_TCGEN05_GEMM", "0") != "1"
@@ -47,12 +58,24 @@ def _gemv_eligible(a: torch.Tensor, b: torch.Tensor, M: int, K: int, trans_a: bo
 
 
 def matmul(a: torch.Tensor, b: torch.Tensor, trans_a: bool = False, trans_b: bool = False,
-           out: torch.Tensor | None = None, accumulate: bool = False, out_dtype=None) -> torch.Tensor:
-    """``op(a) @ op(b)`` for 2-D tensors. ``accumulate`` adds into ``out`` (fp32 or bf16)."""
+           out: torch.Tensor | None = None, accumulate: bool = False, out_dtype=None, bias: torch.Tensor | None = None,
+           act: int = 0) -> torch.Tensor:
+    """``op(a) @ op(b)`` for 2-D tensors. ``accumulate`` adds into ``out`` (fp32 or bf16).  ``bias [N]`` and ``act`` (a
+    :data:`GEMV_ACT` code; 0 none) give ``act(op(a) @ op(b) + bias)``: in the decode GEMV's epilogue when it runs, else as
+    separate ops on the result (not with ``out``)."""
     M = a.shape[1] if trans_a else a.shape[0]
     K = a.shape[0] if trans_a else a.shape[1]
     N = b.shape[0] if trans_b else b.shape[1]
     out_dtype = out_dtype or (out.dtype if out is not None else a.dtype)
+    if bias is not None or act:
+        if out is not None:
+            raise ValueError("matmul: bias / act do not combine with out=")
+        if (_gemv_eligible(a, b, M, K, trans_a, trans_b, out, out_dtype)
+                and (bias is None or (bias.dtype == torch.bfloat16 and bias.is_contiguous() and bias.shape == (N,)))):
+            _ext.count_launch()
+            return _ext.ext().gemv(a, b, None, bias=bias, act=act)
+        y = matmul(a, b, trans_a, trans_b, out_dtype=out_dtype)
+        return _act_torch(y if bias is None else y + bias, act)
     if _gemv_eligible(a, b, M, K, trans_a, trans_b, out, out_dtype):
         # decode-time GEMV: a bandwidth problem (every weight byte read once), not a tensor-core one — csrc/decode.cu
         _ext.count_launch()
@@ -80,10 +103,10 @@ def matmul(a: torch.Tensor, b: torch.Tensor, trans_a: bool = False, trans_b: boo
     return res.to(out_dtype)
 
 
-def linear_nt(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
-    """``x[..., K] @ w[N, K]^T``."""
+def linear_nt(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, act: int = 0) -> torch.Tensor:
+    """``act(x[..., K] @ w[N, K]^T + bias)`` (see :func:`matmul`)."""
     x2 = x.reshape(-1, x.shape[-1])
-    return matmul(x2, w, False, True).view(*x.shape[:-1], w.shape[0])
+    return matmul(x2, w, False, True, bias=bias, act=act).view(*x.shape[:-1], w.shape[0])
 
 
 # ---------------------------------------------------------------------------------------------------------------------
