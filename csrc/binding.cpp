@@ -179,6 +179,8 @@ static Tensor gemm_fp8_block(const Tensor& a, const Tensor& b, const Tensor& sca
   TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn && a.dim() == 2 && b.dim() == 2 &&
               a.size(1) == b.size(1), "gemm_fp8_block: a [M, K] and b [N, K] must be e4m3");
   const int M = a.size(0), K = a.size(1), N = b.size(0);
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(a.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(b.data_ptr()) % 16 == 0,
+              "gemm_fp8_block: a and b must start 16-byte aligned (TMA)");
   TORCH_CHECK(group > 0 && K % group == 0, "gemm_fp8_block: K must be a multiple of the group size");
   TORCH_CHECK(scale_a.is_cuda() && scale_a.scalar_type() == at::kFloat && scale_a.dim() == 2 && scale_a.size(0) == K / group &&
               scale_a.size(1) == M && scale_a.stride(1) == 1 && reinterpret_cast<uintptr_t>(scale_a.data_ptr()) % 16 == 0,
@@ -196,6 +198,7 @@ static Tensor gemm_fp8_block(const Tensor& a, const Tensor& b, const Tensor& sca
 static std::vector<Tensor> quantize_fp8_groups(const Tensor& x, int64_t group, bool mx, double clamp_bound) {
   CHECK_IN(x);
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.size(1) % group == 0, "quantize_fp8_groups: bf16 [M, K], K % group == 0");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "quantize_fp8_groups: x must start 16-byte aligned");
   const int M = x.size(0), K = x.size(1);
   const long ld = ((long)M + 3) / 4 * 4;
   c10::cuda::CUDAGuard guard(x.device());

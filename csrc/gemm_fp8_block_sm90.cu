@@ -173,6 +173,22 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_co
 // One warp quantises a 256-element segment of one row: lane l holds elements 8l..8l+7 (one 16-byte load), the G/8 lanes of a
 // group reduce their absmax with shuffles.  Warps are ordered row-fastest so that neighbouring warps write neighbouring
 // scales of the group-major scale buffer.
+//
+// Non-finite input: a group holding a NaN, or ±inf with no clamp, gets a NaN scale and NaN codes, so every output that reads
+// it is NaN.  fmaxf / fminf return the other operand when one is NaN, which would turn NaN into a finite code (and the MX
+// exponent of an infinite amax overflows the int shift into a finite scale), so the clamp, the amax and its shuffle
+// reduction use the NaN-propagating forms; their .ftz matches what fmaxf / fminf compile to under --use_fast_math.
+NXD_DEVICE float max_nan(float a, float b) {
+  float r;
+  asm("max.ftz.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+NXD_DEVICE float min_nan(float a, float b) {
+  float r;
+  asm("min.ftz.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
 template <int G, bool MX>
 __global__ void __launch_bounds__(256)
 quantize_fp8_groups_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q, float* __restrict__ s, int M, int K,
@@ -192,18 +208,21 @@ quantize_fp8_groups_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restr
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float2 f = __bfloat1622float2(h[i]);
-      v[2 * i] = fminf(fmaxf(f.x, -clamp_bound), clamp_bound);
-      v[2 * i + 1] = fminf(fmaxf(f.y, -clamp_bound), clamp_bound);
+      v[2 * i] = min_nan(max_nan(f.x, -clamp_bound), clamp_bound);
+      v[2 * i + 1] = min_nan(max_nan(f.y, -clamp_bound), clamp_bound);
     }
 #pragma unroll
-    for (int i = 0; i < 8; ++i) amax = fmaxf(amax, fabsf(v[i]));
+    for (int i = 0; i < 8; ++i) amax = max_nan(amax, fabsf(v[i]));
   }
 #pragma unroll
-  for (int off = 1; off < G / 8; off <<= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, off));
+  for (int off = 1; off < G / 8; off <<= 1) amax = max_nan(amax, __shfl_xor_sync(0xffffffffu, amax, off));
   if (!live) return;
   float scale;
-  if constexpr (MX) {
-    // OCP MX: 2^(floor(log2 amax) - 8), amax clamped to 2^-100; log2 rounded to fp32 first, as the torch quantiser does
+  if (!(amax <= 3.402823466e38f)) {
+    scale = __int_as_float(0x7fffffff);                        // NaN, or ±inf with no clamp: NaN scale, NaN codes
+  } else if constexpr (MX) {
+    // OCP MX: 2^(floor(log2 amax) - 8), amax clamped to 2^-100; log2 rounded to fp32 first, as the torch quantiser does.
+    // amax is finite here, so -100 <= e <= 127 and the biased exponent e - 8 + 127 is in [19, 246]: no overflow
     const float e = floorf((float)log2((double)fmaxf(amax, 0x1p-100f)));
     scale = __int_as_float(((int)e - 8 + 127) << 23);
   } else {
@@ -214,7 +233,7 @@ quantize_fp8_groups_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restr
   uint32_t lo = 0, hi = 0;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    const float c = fminf(fmaxf(__fdiv_rn(v[i], scale), -448.f), 448.f);
+    const float c = min_nan(max_nan(__fdiv_rn(v[i], scale), -448.f), 448.f);   // NaN → the e4m3 NaN code 0x7F
     const uint32_t b = (uint32_t)__nv_cvt_float_to_fp8(c, __NV_SATFINITE, __NV_E4M3);
     if (i < 4) lo |= b << (8 * i); else hi |= b << (8 * (i - 4));
   }

@@ -45,7 +45,8 @@ def scaled_linear(xq: torch.Tensor, xs: torch.Tensor, wq: torch.Tensor, ws: torc
 # ---- block-scaled ----------------------------------------------------------------------------------------------------
 def _quantize_groups_reference(x2: torch.Tensor, group_size: int, rule: str, clamp_bound: Optional[float]
                                ) -> Tuple[torch.Tensor, torch.Tensor]:
-    """Torch oracle of the group quantiser: ``[M, K]`` → (e4m3 ``[M, K]``, fp32 ``[M, K/G]``)."""
+    """Torch oracle of the group quantiser: ``[M, K]`` → (e4m3 ``[M, K]``, fp32 ``[M, K/G]``).  A group whose amax is not
+    finite (a NaN, or ±inf with no clamp) gets a NaN scale, so all its codes are NaN."""
     M, K = x2.shape
     xf = x2.float()
     if clamp_bound is not None:
@@ -56,6 +57,7 @@ def _quantize_groups_reference(x2: torch.Tensor, group_size: int, rule: str, cla
         scale = torch.pow(2.0, torch.floor(torch.log2(amax.clamp(min=2.0 ** -100))) - 8)
     else:
         scale = (amax / _E4M3_MAX).clamp(min=1e-12)
+    scale = torch.where(torch.isfinite(amax), scale, float("nan"))
     q = (xb / scale.unsqueeze(-1)).clamp(-_E4M3_MAX, _E4M3_MAX).to(torch.float8_e4m3fn).reshape(M, K)
     return q, scale
 
@@ -67,18 +69,20 @@ def quantize_groups(x: torch.Tensor, group_size: int, rule: str = "absmax", clam
 
     ``rule="absmax"``: ``scale = max(amax / 448, 1e-12)`` (per-row ``quantize_activation_dynamic`` when G = K);
     ``rule="mx"``: OCP MX ``scale = 2^(⌊log2 amax⌋ − 8)`` (``mx_torch.quantize_mx``).  Codes are ``clamp(x / scale, ±448)`` rounded
-    to nearest-even; ``clamp_bound`` clips ``x`` first.  On CUDA (bf16 input) the scales are a transposed view of the group-major
-    buffer :func:`blockscaled_linear` streams, and codes and scales are bit-identical to the torch oracle on the same CUDA tensor
-    (torch computes ``amax / 448`` as a product with the rounded reciprocal on CUDA and as a true division on CPU, so an absmax
-    scale can differ in the last bit between devices)."""
+    to nearest-even; ``clamp_bound`` clips ``x`` first.  A group holding a NaN, or ±inf when there is no clamp, gets a NaN
+    scale and NaN codes, so every output that reads it is NaN rather than a finite-looking number.  On CUDA (bf16 input,
+    16-byte aligned rows) the scales are a transposed view of the group-major buffer :func:`blockscaled_linear` streams.
+    Codes and scales equal the torch oracle on the same CUDA tensor bit for bit, except that the sign of a NaN code is not
+    defined.  torch computes ``amax / 448`` as a product with the rounded reciprocal on CUDA and as a true division on CPU,
+    so an absmax scale can differ in the last bit between devices."""
     assert rule in ("absmax", "mx"), rule
     K = x.shape[-1]
     assert K % group_size == 0, f"K={K} is not a multiple of the group size {group_size}"
     lead = x.shape[:-1]
     x2 = x.reshape(-1, K)
     if (group_size in GROUP_SIZES and x2.dtype == torch.bfloat16 and K % 8 == 0 and _ext.use_cuda(x2)
-            and hasattr(_ext.ext(), "quantize_fp8_groups")):
-        _ext.count_launch()
+            and hasattr(_ext.ext(), "quantize_fp8_groups") and x2.contiguous().data_ptr() % 16 == 0):
+        _ext.count_launch()                         # the kernel loads 16-byte vectors: an unaligned view takes the oracle
         q, sbuf = _ext.ext().quantize_fp8_groups(x2.contiguous(), group_size, rule == "mx",
                                                  float("inf") if clamp_bound is None else float(clamp_bound))
         xs = sbuf[:, : x2.shape[0]].t()
@@ -108,8 +112,8 @@ def blockscaled_linear(xq: torch.Tensor, xs: torch.Tensor, wq: torch.Tensor, ws:
     """``dequant(xq, xs) @ dequant(wq, ws)ᵀ`` for e4m3 codes with one scale per ``group_size`` input features.
 
     ``xq [..., K]`` / ``xs [..., K/G]`` as :func:`quantize_groups` returns them; ``wq [N, K]``; ``ws`` fp32 or E8M0 ``[N, K/G]`` or
-    ``[N/bn, K/G]``.  CUDA with e4m3 operands, G ∈ {32, 64, 128}, ``K % 128 == 0``, ``N % 8 == 0`` and bf16 output: the
-    block-scaled wgmma GEMM; otherwise the fp32 oracle."""
+    ``[N/bn, K/G]``.  CUDA with e4m3 operands starting 16-byte aligned, G ∈ {32, 64, 128}, ``K % 128 == 0``, ``N % 8 == 0``
+    and bf16 output: the block-scaled wgmma GEMM; otherwise the fp32 oracle."""
     K = xq.shape[-1]
     lead = xq.shape[:-1]
     x2 = xq.reshape(-1, K)
@@ -118,7 +122,8 @@ def blockscaled_linear(xq: torch.Tensor, xs: torch.Tensor, wq: torch.Tensor, ws:
     sb = weight_scales_kn(ws, N, K, group_size)
     if (group_size in GROUP_SIZES and K % 128 == 0 and N % 8 == 0 and out_dtype == torch.bfloat16
             and xq.dtype == torch.float8_e4m3fn and wq.dtype == torch.float8_e4m3fn and _ext.use_cuda(x2, wq, xs2, sb)
-            and hasattr(_ext.ext(), "gemm_fp8_block")):
+            and hasattr(_ext.ext(), "gemm_fp8_block")
+            and x2.contiguous().data_ptr() % 16 == 0 and wq.contiguous().data_ptr() % 16 == 0):   # TMA needs 16-byte starts
         sa = xs2.t()                                # [K/G, M]: a view of the quantiser's group-major buffer needs no copy
         if not (sa.dtype == torch.float32 and sa.stride(1) == 1 and sa.stride(0) >= M and sa.stride(0) % 4 == 0
                 and sa.data_ptr() % 16 == 0):

@@ -1,7 +1,8 @@
 """On-GPU numerics + timing smoke for every hand-written kernel (run under gpurun).
 
 usage: python tools/gpu_check.py [elementwise|gemm|gemm_perf|decode|fp8|fp8_block|grouped|all]
-(decode / fp8 / fp8_block / grouped given by name also run their timing entries)
+(decode / fp8 / grouped given by name also run their timing entries; fp8_block is timing only, its numerics are
+in tests/test_fp8_blockscaled_gpu.py)
 Each check prints one line `CHECK name PASS/FAIL max_err=…`; results are also appended to
 gpurun_out/gpu_check.jsonl.  Comparison target is always a plain PyTorch fp32 reference."""
 import json
@@ -232,63 +233,8 @@ def check_fp8(perf=False):
         report("gemm_fp8_perf_8192", True, ms=t, tflops=2.0 * M * N * K / t / 1e9)
 
 
-def _wide_scales(*shape):
-    """fp32 scales spread over 2^-12 … 2^12, varying per group and per row / column: a wrong scale index is not hidden."""
-    return torch.pow(2.0, torch.randint(-12, 13, shape, device=dev).float()) * (1 + torch.rand(shape, device=dev))
-
-
 def _fp8_codes(*shape):
     return (torch.randn(*shape, device=dev) * 64).clamp(-448, 448).to(torch.float8_e4m3fn)
-
-
-def _normerr(a, b):
-    a, b = a.double(), b.double()
-    return float((a - b).norm() / b.norm())
-
-
-def check_fp8_block(perf=False):
-    """Block-scaled fp8 GEMM (csrc/gemm_fp8_block_sm90.cu) and its group quantiser vs the torch oracles on the same CUDA
-    tensors: the quantiser bit for bit, the GEMM against the fp32 product of the de-quantised operands."""
-    from neuronx_distributed_b200.ops import gemm_fp8
-
-    torch.manual_seed(0)
-    for G in (32, 64, 128):
-        for rule in ("absmax", "mx"):
-            for M, cb in ((1, None), (7, None), (200, 3.0), (4096, None)):
-                K = 1024
-                x = (torch.randn(M, K, device=dev) * torch.pow(2.0, torch.randint(-30, 30, (M, K // G, 1), device=dev).float())
-                     .repeat_interleave(G, 1).reshape(M, K)).bfloat16()
-                n0 = ops._ext.launches()
-                q, s = gemm_fp8.quantize_groups(x, G, rule, cb)
-                ran = ops._ext.launches() > n0
-                qr, sr = gemm_fp8._quantize_groups_reference(x, G, rule, cb)
-                same = torch.equal(q.view(torch.uint8), qr.view(torch.uint8)) and torch.equal(s, sr)
-                report(f"quantize_fp8_groups_G{G}_{rule}_M{M}{'_clamp' if cb else ''}", ran and same, kernel=int(ran),
-                       code_mismatch=int((q.view(torch.uint8) != qr.view(torch.uint8)).sum()))
-    for (M, N, K) in [(128, 128, 128), (200, 264, 384), (8, 4096, 4096), (4096, 11008, 4096), (4096, 4096, 11008)]:
-        for G in (32, 64, 128):
-            for two_d, e8m0 in ((False, False), (True, False), (False, True), (True, True)):
-                if (M * N * K > 1e10) and (two_d or e8m0) and G != 128:
-                    continue                              # big shapes: every G with 1-D fp32 scales, every layout at G = 128
-                if two_d and N % 128:
-                    continue
-                xq, wq = _fp8_codes(M, K), _fp8_codes(N, K)
-                xs = _wide_scales(M, K // G)
-                rows = N // 128 if two_d else N
-                if e8m0:
-                    ws = torch.randint(127 - 12, 127 + 13, (rows, K // G), device=dev, dtype=torch.uint8)
-                else:
-                    ws = _wide_scales(rows, K // G)
-                n0 = ops._ext.launches()
-                y = gemm_fp8.blockscaled_linear(xq, xs, wq, ws, G)
-                ran = ops._ext.launches() > n0
-                ref = gemm_fp8._dequant_groups(xq, xs, G) @ gemm_fp8._dequant_groups(
-                    wq, gemm_fp8.weight_scales_kn(ws, N, K, G).t(), G).t()          # fp32 oracle (no TF32)
-                err = _normerr(y, ref)
-                report(f"gemm_fp8_block_{M}x{N}x{K}_G{G}{'_2d' if two_d else ''}{'_e8m0' if e8m0 else ''}",
-                       ran and err < 4e-3, err=err, kernel=int(ran))
-    if perf:
-        check_fp8_block_perf()
 
 
 def check_fp8_block_perf():
@@ -373,8 +319,8 @@ if __name__ == "__main__":
         check_decode(perf=what == "decode")
     if what in ("fp8", "all"):
         check_fp8(perf=what == "fp8")
-    if what in ("fp8_block", "all"):
-        check_fp8_block(perf=what == "fp8_block")
+    if what == "fp8_block":                       # numerics: tests/test_fp8_blockscaled_gpu.py
+        check_fp8_block_perf()
     if what in ("grouped", "all"):
         check_grouped(perf=what == "grouped")
     if what in ("gemm_perf", "all"):
