@@ -49,7 +49,9 @@ constexpr int kABytes = BLOCK_M * BLOCK_K * 2;   // 16 KB
 constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;   // 32 KB
 constexpr int kStageBytes = kABytes + kBBytes;   // 48 KB
 constexpr int kThreads = 384;                    // producer warpgroup + 2 consumer warpgroups
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int kEpiBoxBytes = 64 * 128;           // TMA epilogue box: 64 rows x 128 bytes (64 bf16 / 32 fp32 columns)
+constexpr int kEpiBytes = 2 * 2 * kEpiBoxBytes;  // two boxes per consumer warpgroup: 32 KB
+constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 constexpr int kMaxRowBlocks = 64;   // flag index = source_rank * kMaxRowBlocks + row_block (shape independent)
 
 struct CommDev {
@@ -215,19 +217,78 @@ NXD_DEVICE void store_tile(const float (&acc)[128], OutT* orow0, OutT* orow1, in
   }
 }
 
+// TMA epilogue of one consumer warpgroup's 64 x 256 slice (rows row_base.., columns n0..): it leaves in boxes of 64 rows x
+// 128 bytes, each written into one of the warpgroup's two 128B-swizzled staging buffers and sent by one thread as a bulk
+// tensor store, or, to accumulate into fp32, a bulk tensor reduce-add performed at L2.  The tensor map clips rows >= M and
+// columns >= N.  Per element the arithmetic is the register epilogue's: the fp32 accumulator (times the fp8 scales), rounded
+// once to bf16 for a bf16 out, or added once in fp32 to the old value (which, unlike the register path's flush-to-zero
+// FADD, keeps subnormal operands and sums: DESIGN.md §2).
+//
+// Ordering: every thread fences its shared-memory writes for the async proxy; before the warpgroup barrier the leader waits
+// until its previous box has been read out of shared memory, so after the barrier the other buffer is free to rewrite.
+template <typename OutT, bool FP8>
+NXD_DEVICE void store_tile_tma(const float (&acc)[128], const CUtensorMap* tma_out, uint32_t stage, int row_base, int n0,
+                               int M, int N, bool reduce_add, const CommDev& comm, uint32_t bar_id, bool leader) {
+  constexpr int kCols = 128 / sizeof(OutT);        // columns of a box
+  constexpr int kJ = kCols / 8;                    // accumulator column groups (8 columns each) of a box
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+  const int r = wq * 16 + (lane >> 2);             // box rows r and r + 8; both have r % 8 = lane / 4 → same swizzle
+  const int sw = lane >> 2;
+  float sa0 = 1.f, sa1 = 1.f;
+  if constexpr (FP8) {
+    const int row0 = row_base + r;
+    sa0 = comm.scale_a[row0 < M ? row0 : 0]; sa1 = comm.scale_a[row0 + 8 < M ? row0 + 8 : 0];
+  }
+#pragma unroll
+  for (int box = 0; box < BLOCK_N / kCols; ++box) {
+    const uint32_t buf = stage + (box & 1) * kEpiBoxBytes;
+#pragma unroll
+    for (int jj = 0; jj < kJ; ++jj) {
+      const int j = box * kJ + jj;
+      float v0 = acc[4 * j], v1 = acc[4 * j + 1], v2 = acc[4 * j + 2], v3 = acc[4 * j + 3];
+      if constexpr (FP8) {
+        const int col = n0 + 8 * j + 2 * (lane & 3);
+        const float sb0 = col < N ? comm.scale_b[col] : 0.f, sb1 = col < N ? comm.scale_b[col + 1] : 0.f;
+        v0 *= sa0 * sb0; v1 *= sa0 * sb1; v2 *= sa1 * sb0; v3 *= sa1 * sb1;
+      }
+      // 16-byte chunk c of row r sits at chunk c ^ (r % 8) (SWIZZLE_128B)
+      if constexpr (sizeof(OutT) == 2) {
+        const int off = ((jj ^ sw) << 4) + 4 * (lane & 3);
+        const __nv_bfloat162 h0 = __floats2bfloat162_rn(v0, v1), h1 = __floats2bfloat162_rn(v2, v3);
+        st_shared_b32(buf + r * 128 + off, *(const uint32_t*)&h0);
+        st_shared_b32(buf + (r + 8) * 128 + off, *(const uint32_t*)&h1);
+      } else {
+        const int off = (((2 * jj + ((lane & 3) >> 1)) ^ sw) << 4) + 8 * (lane & 1);
+        st_shared_v2f32(buf + r * 128 + off, v0, v1);
+        st_shared_v2f32(buf + (r + 8) * 128 + off, v2, v3);
+      }
+    }
+    fence_proxy_async_smem();
+    if (leader) bulk_wait_group_read<0>();
+    named_barrier_sync(bar_id, 128);
+    if (leader) {
+      if (reduce_add) tma_reduce_add_2d(tma_out, buf, n0 + box * kCols, row_base);
+      else tma_store_2d(tma_out, buf, n0 + box * kCols, row_base);
+      bulk_commit_group();
+    }
+  }
+}
+
 // Structure (one persistent CTA per SM, 384 threads):
 //   warpgroup 0     TMA producer : one thread fills a 4-stage ring of 128B-swizzled [128 x 64] A / [256 x 64] B tiles
 //   warpgroups 1-2  consumers    : consumer c owns rows 64c..64c+63 of the 128 x 256 tile, issues wgmma m64n256k16 from
 //                                  shared memory into a register accumulator (one wgmma group in flight, which releases
-//                                  the previous stage), then stores the tile straight from registers.
+//                                  the previous stage), then stores the tile: through shared memory by TMA when
+//                                  `tma_epi` is set (store_tile_tma, MODE 0 / 3), else straight from registers.
 template <bool A_KMAJOR, bool B_KMAJOR, int MODE, typename OutT, bool FP8 = false>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                 const __grid_constant__ CUtensorMap tma_a_local, OutT* __restrict__ out, int M, int N, int K, int accumulate,
-                 CommDev comm) {
+                 const __grid_constant__ CUtensorMap tma_a_local, const __grid_constant__ CUtensorMap tma_out,
+                 OutT* __restrict__ out, int M, int N, int K, int accumulate, int tma_epi, CommDev comm) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B needs 1 KB alignment
-  uint64_t* bars = (uint64_t*)(smem + kStages * kStageBytes);
+  uint8_t* epi_stage = smem + kStages * kStageBytes;                               // [2 warpgroups][2 boxes] of 8 KB
+  uint64_t* bars = (uint64_t*)(epi_stage + kEpiBytes);
   // [0,kStages) full, [kStages,2kStages) empty
   const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + kStages);
   const uint32_t smem_base = smem_u32(smem);
@@ -431,8 +492,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         fence_acc(acc);
         if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_empty + 8 * prev_stage);
 
-        const int row0 = m_blk * BLOCK_M + cw * 64 + wq * 16 + (lane >> 2);
         const int n0 = n_blk * BLOCK_N;
+        if constexpr (MODE == 0 || MODE == 3) {
+          if (tma_epi) {
+            // named barrier 2 + cw: 0 is __syncthreads, 1 the MODE 2 / 6 publish barrier
+            store_tile_tma<OutT, FP8>(acc, &tma_out, smem_u32(epi_stage) + cw * 2 * kEpiBoxBytes, m_blk * BLOCK_M + cw * 64,
+                                      n0, M, N, accumulate != 0, comm, 2 + cw, (threadIdx.x & 127) == 0);
+            continue;
+          }
+        }
+        const int row0 = m_blk * BLOCK_M + cw * 64 + wq * 16 + (lane >> 2);
         OutT *orow0, *orow1;
         if constexpr (MODE == 2) {
           // partial tile goes to the owner's staging slot [src = my rank][row in chunk][N]
@@ -474,6 +543,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
           }
         }
       }
+      // the last boxes' global writes are complete before the kernel ends (the next kernel may read `out` on another stream)
+      if ((MODE == 0 || MODE == 3) && tma_epi && (threadIdx.x & 127) == 0) bulk_wait_group<0>();
     }
   }
 
@@ -657,16 +728,31 @@ CUtensorMap make_tmap_2d(const void* ptr, CUtensorMapDataType dt, uint64_t rows,
 
 int device_sm_count() { return sm_count(); }
 
-template <bool AK, bool BK, int MODE, typename OutT>
+// The TMA epilogue (MODE 0 / 3) writes `out` [M, N] through a tensor map, which needs a 16-byte aligned base and row pitch.
+// A bf16 accumulate stays on the register epilogue: a bf16 reduce-add would round the product to bf16 before the add.
+// Returns false (register epilogue) when the map does not fit.
+template <typename OutT>
+static bool out_tmap(const void* out, int M, int N, bool accumulate, CUtensorMap* map) {
+  constexpr bool bf16 = sizeof(OutT) == 2;
+  if ((uintptr_t)out % 16 || ((size_t)N * sizeof(OutT)) % 16 || (accumulate && bf16)) return false;
+  *map = make_tmap_2d(out, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, M, N,
+                      (uint64_t)N * sizeof(OutT), kEpiBoxBytes / 64 / sizeof(OutT), 64, CU_TENSOR_MAP_SWIZZLE_128B);
+  return true;
+}
+
+template <bool AK, bool BK, int MODE, typename OutT, bool FP8 = false>
 static void launch(const CUtensorMap& ta, const CUtensorMap& tb, void* out, int M, int N, int K, bool accumulate,
                    const CommDev& c, int grid, cudaStream_t st, const CUtensorMap* ta_local = nullptr) {
-  auto kern = gemm_bf16_kernel<AK, BK, MODE, OutT>;
+  auto kern = gemm_bf16_kernel<AK, BK, MODE, OutT, FP8>;
   static bool configured = false;
   if (!configured) {
     NXD_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     configured = true;
   }
-  kern<<<grid, kThreads, kSmemBytes, st>>>(ta, tb, ta_local ? *ta_local : ta, (OutT*)out, M, N, K, accumulate ? 1 : 0, c);
+  CUtensorMap to = ta;
+  const bool tma_epi = (MODE == 0 || MODE == 3) && out_tmap<OutT>(out, M, N, accumulate, &to);
+  kern<<<grid, kThreads, kSmemBytes, st>>>(ta, tb, ta_local ? *ta_local : ta, to, (OutT*)out, M, N, K, accumulate ? 1 : 0,
+                                           tma_epi ? 1 : 0, c);
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 
@@ -756,14 +842,7 @@ void gemm_fp8(const void* a, const void* b, void* out, int M, int N, int K, cons
   c.scale_a = scale_a; c.scale_b = scale_b;
   const int tiles = ((M + BLOCK_M - 1) / BLOCK_M) * ((N + BLOCK_N - 1) / BLOCK_N);
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  auto kern = gemm_bf16_kernel<true, true, 0, __nv_bfloat16, true>;
-  static bool configured = false;
-  if (!configured) {
-    NXD_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    configured = true;
-  }
-  kern<<<grid, kThreads, kSmemBytes, st>>>(ta, tb, ta, (__nv_bfloat16*)out, M, N, K, 0, c);
-  NXD_CUDA_CHECK(cudaGetLastError());
+  launch<true, true, 0, __nv_bfloat16, true>(ta, tb, out, M, N, K, false, c, grid, st);
 }
 
 bool gemm_self_check_supported() { return true; }

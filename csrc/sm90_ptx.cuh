@@ -64,6 +64,32 @@ NXD_DEVICE void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
+// Bulk tensor store of a shared-memory box to global memory, and the same with an element-wise add performed at L2
+// (the element type is the tensor map's).  Both belong to the issuing thread's current bulk async-group.
+NXD_DEVICE void tma_store_2d(const CUtensorMap* map, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
+}
+NXD_DEVICE void tma_reduce_add_2d(const CUtensorMap* map, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
+}
+NXD_DEVICE void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// .read: the groups' shared-memory sources may be overwritten; without it: their global writes are also complete
+template <int N>
+NXD_DEVICE void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+NXD_DEVICE void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+NXD_DEVICE void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+NXD_DEVICE void st_shared_v2f32(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+NXD_DEVICE void named_barrier_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 // ------------------------------------------------------------------ wgmma
 // Shared-memory matrix descriptor of wgmma (cute::GMMA::GmmaDescriptor): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
 // base offset [49,52) (0: every operand tile is 1 KB aligned), layout type [62,64) (1 = SWIZZLE_128B).

@@ -1,7 +1,7 @@
 """On-GPU numerics + timing smoke for every hand-written kernel (run under gpurun).
 
 usage: python tools/gpu_check.py [elementwise|gemm|gemm_perf|decode|fp8|fp8_block|grouped|all]
-(decode / fp8 / grouped given by name also run their timing entries; fp8_block is timing only, its numerics are
+(gemm / decode / fp8 / grouped given by name also run their timing entries; fp8_block is timing only, its numerics are
 in tests/test_fp8_blockscaled_gpu.py)
 Each check prints one line `CHECK name PASS/FAIL max_err=…`; results are also appended to
 gpurun_out/gpu_check.jsonl.  Comparison target is always a plain PyTorch fp32 reference."""
@@ -163,17 +163,44 @@ def check_gemm(perf=False):
     report("gemm_f32_accumulate", relerr(out, ref) < 1e-3, err=relerr(out, ref))
 
 
+def _gpu_info(query="name,power.limit,clocks.sm,clocks.max.sm"):
+    import subprocess
+
+    r = subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader"], capture_output=True, text=True)
+    lines = r.stdout.strip().splitlines()
+    return lines[0] if lines else torch.cuda.get_device_name()
+
+
 def check_gemm_perf():
-    peaks = {}
-    for (M, N, K) in [(4096, 1536, 4096), (4096, 2752, 4096), (4096, 4096, 512), (4096, 4096, 1376), (4096, 4000, 4096),
-                      (4096, 12288, 4096), (4096, 22016, 4096), (4096, 4096, 11008), (8192, 8192, 8192)]:
-        a = torch.randn(M, K, device=dev, dtype=torch.bfloat16); b = torch.randn(N, K, device=dev, dtype=torch.bfloat16)
-        out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-        t_own = timeit(lambda: ops._ext.ext().gemm_bf16(a, b, out, False, True, False))
-        t_lib = timeit(lambda: torch.matmul(a, b.t()))
+    """The bf16 GEMM at the Llama-2-7B training step's shapes (4096 tokens) in its three layouts: `nt` forward
+    x[M, K]·W[N, K]ᵀ, `nn` the same product with W stored [K, N], and `tn` weight gradient gᵀ·x into an fp32 [N, K] out, once
+    storing and once accumulating (as into ZeRO-1's main_grad).  cuBLAS through torch where it has the same product."""
+    report("gpu_info", True, gpu=_gpu_info())
+    e = ops._ext.ext()
+    M = 4096
+    bf = dict(device=dev, dtype=torch.bfloat16)
+    for (N, K) in [(12288, 4096), (4096, 4096), (22016, 4096), (4096, 11008), (32000, 4096)]:
         fl = 2.0 * M * N * K
-        report(f"gemm_perf_{M}x{N}x{K}", True, own_ms=t_own, cublas_ms=t_lib, own_tflops=fl / t_own / 1e9,
-               cublas_tflops=fl / t_lib / 1e9)
+        x = torch.randn(M, K, **bf)
+        w = torch.randn(N, K, **bf)
+        y = torch.empty(M, N, **bf)
+        rows = {"nt": (timeit(lambda: e.gemm_bf16(x, w, y, False, True, False)), timeit(lambda: torch.matmul(x, w.t())))}
+        wkn = w.t().contiguous()
+        rows["nn"] = (timeit(lambda: e.gemm_bf16(x, wkn, y, False, False, False)), timeit(lambda: torch.matmul(x, wkn)))
+        del wkn, y
+        g = torch.randn(M, N, **bf)
+        dw = torch.zeros(N, K, device=dev, dtype=torch.float32)
+        try:
+            lib = timeit(lambda: torch.mm(g.t(), x, out_dtype=torch.float32))
+        except (RuntimeError, TypeError):
+            lib = None
+        rows["tn_store"] = (timeit(lambda: e.gemm_bf16(g, x, dw, True, False, False)), lib)
+        rows["tn_accumulate"] = (timeit(lambda: e.gemm_bf16(g, x, dw, True, False, True)), None)
+        clk = _gpu_info("clocks.sm")
+        for layout, (t_own, t_lib) in rows.items():
+            extra = {} if t_lib is None else {"cublas_ms": t_lib, "cublas_tflops": fl / t_lib / 1e9}
+            report(f"gemm_perf_{layout}_M{M}_N{N}_K{K}", True, own_ms=t_own, own_tflops=fl / t_own / 1e9, sm_clock=clk, **extra)
+        del g, dw, x, w
 
 
 def check_decode(perf=False):
@@ -323,7 +350,7 @@ if __name__ == "__main__":
         check_fp8_block_perf()
     if what in ("grouped", "all"):
         check_grouped(perf=what == "grouped")
-    if what in ("gemm_perf", "all"):
+    if what in ("gemm", "gemm_perf", "all"):
         check_gemm_perf()
     bad = [r["name"] for r in RESULTS if not r["ok"]]
     print("SUMMARY", len(RESULTS) - len(bad), "passed,", len(bad), "failed", bad, flush=True)
