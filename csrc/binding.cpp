@@ -194,6 +194,39 @@ static Tensor gemm_fp8_block(const Tensor& a, const Tensor& b, const Tensor& sca
   return out;
 }
 
+// grouped (MoE) mode: a e4m3 [M, K] in block_rows-row blocks, block i using expert block_expert[i]; b e4m3 [E, N, K]
+// (K-major experts); scale_a as gemm_fp8_block; scale_b fp32 [E, K/group, N] → bf16 [M, N]
+static Tensor grouped_gemm_fp8_block(const Tensor& a, const Tensor& b, const Tensor& scale_a, const Tensor& scale_b,
+                                     const Tensor& block_expert, int64_t block_rows, int64_t group) {
+  CHECK_IN(a); CHECK_IN(b); CHECK_IN(scale_b); CHECK_IN(block_expert);
+  TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn && a.dim() == 2 && b.dim() == 3 &&
+              a.size(1) == b.size(2), "grouped_gemm_fp8_block: a [M, K] and b [E, N, K] must be e4m3");
+  const int M = a.size(0), K = a.size(1), E = b.size(0), N = b.size(1);
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(a.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(b.data_ptr()) % 16 == 0 &&
+              reinterpret_cast<uintptr_t>(scale_b.data_ptr()) % 16 == 0,
+              "grouped_gemm_fp8_block: a, b and scale_b must start 16-byte aligned (TMA)");
+  TORCH_CHECK(group == 32 || group == 64 || group == 128, "grouped_gemm_fp8_block: group size must be 32, 64 or 128");
+  TORCH_CHECK(K % 128 == 0 && N % 8 == 0, "grouped_gemm_fp8_block: needs K % 128 == 0 and N % 8 == 0");
+  TORCH_CHECK(block_rows > 0 && block_rows % 128 == 0, "grouped_gemm_fp8_block: block_rows must be a positive multiple of 128");
+  TORCH_CHECK(block_expert.scalar_type() == at::kInt && block_expert.dim() == 1 && block_expert.numel() * block_rows == M,
+              "grouped_gemm_fp8_block: block_expert must be int32 [M / block_rows]");
+  TORCH_CHECK(scale_a.is_cuda() && scale_a.scalar_type() == at::kFloat && scale_a.dim() == 2 && scale_a.size(0) == K / group &&
+              scale_a.size(1) == M && scale_a.stride(1) == 1 && scale_a.stride(0) >= M && scale_a.stride(0) % 4 == 0 &&
+              reinterpret_cast<uintptr_t>(scale_a.data_ptr()) % 16 == 0,
+              "grouped_gemm_fp8_block: scale_a must be fp32 [K/group, M] with unit column stride, a row stride >= M that is a "
+              "multiple of 4 and a 16-byte aligned start");
+  TORCH_CHECK(scale_b.scalar_type() == at::kFloat && scale_b.dim() == 3 && scale_b.size(0) == E && scale_b.size(1) == K / group &&
+              scale_b.size(2) == N, "grouped_gemm_fp8_block: scale_b must be fp32 [E, K/group, N]");
+  TORCH_CHECK(b.device() == a.device() && scale_a.device() == a.device() && scale_b.device() == a.device() &&
+              block_expert.device() == a.device(), "grouped_gemm_fp8_block: all operands must be on one device");
+  c10::cuda::CUDAGuard guard(a.device());
+  Tensor out = at::empty({M, N}, a.options().dtype(at::kBFloat16));
+  nxd::grouped_gemm_fp8_block(a.data_ptr(), b.data_ptr(), out.data_ptr(), scale_a.data_ptr<float>(), scale_a.stride(0),
+                              scale_b.data_ptr<float>(), M, N, K, E, block_expert.data_ptr<int>(), (int)block_rows, (int)group,
+                              stream());
+  return out;
+}
+
 // x bf16 [M, K] → (e4m3 [M, K], fp32 scales [K/group, round_up(M, 4)]: group-major, the layout gemm_fp8_block reads)
 static std::vector<Tensor> quantize_fp8_groups(const Tensor& x, int64_t group, bool mx, double clamp_bound) {
   CHECK_IN(x);
@@ -934,6 +967,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("act") = 0);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("gemm_fp8_block", &gemm_fp8_block);
+  m.def("grouped_gemm_fp8_block", &grouped_gemm_fp8_block);
   m.def("quantize_fp8_groups", &quantize_fp8_groups);
   m.def("grouped_gemm", &grouped_gemm);
   m.def("grouped_wgrad", &grouped_wgrad);

@@ -15,6 +15,15 @@
 //   warpgroups 1-2  consumers    : consumer c owns rows 64c..64c+63 of the tile; per group it issues G/32 wgmma m64n128k32
 //                                  (the first with scale_d = 0), waits, and promotes; the stage is released after its last
 //                                  group.  The two consumers are independent, so one's promotion overlaps the other's MMAs.
+//
+// Grouped mode (GROUPED = true, MoE experts): the rows of A come in `block_rows`-row blocks and block i is multiplied by expert
+// block_expert[i].  B is every expert's K-major [N, K] weight stacked into one [E·N, K] tensor map and the weight scales are
+// stacked into one [E·K/G, N] map, so the tile's expert only shifts two TMA row coordinates: e·N for the B tile and e·K/G for
+// the scale rows.  block_rows % 128 == 0, so a 128-row tile lies inside one block and its expert is block_expert[m0 / block_rows].
+// Ragged N (N % 128 != 0): the last column tile of expert e reads B rows e·N + n0 + j with n0 + j >= N, which are the first rows
+// of expert e + 1 (only the last expert's over-read is past the map and zero-filled).  Column j of a tile depends only on B row
+// n0 + j and scale column n0 + j (whose over-read is always past the scale map's N columns, so zero), and columns >= N are never
+// stored: the neighbour's rows, NaN included, cannot reach a stored element.
 #include <cuda.h>
 #include <cuda_fp8.h>
 
@@ -51,11 +60,12 @@ NXD_DEVICE void tile_coords(int tile, int tiles_m, int tiles_n, int& m_blk, int&
   n_blk = in / gsz;
 }
 
-template <int G>
+template <int G, bool GROUPED>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                       const __grid_constant__ CUtensorMap tma_sa, const __grid_constant__ CUtensorMap tma_sb,
-                      __nv_bfloat16* __restrict__ out, int M, int N, int K) {
+                      __nv_bfloat16* __restrict__ out, int M, int N, int K, const int* __restrict__ block_expert,
+                      int block_rows) {
   using C = Cfg<G>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B needs 1 KB alignment
@@ -85,6 +95,12 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_co
         int m_blk, n_blk;
         tile_coords(tile, tiles_m, tiles_n, m_blk, n_blk);
         const int m0 = m_blk * BM, n0 = n_blk * BN;
+        int b_row = n0, sb_row = 0;                     // grouped: the tile's expert shifts the B and weight-scale rows
+        if constexpr (GROUPED) {
+          const int e = block_expert[m0 / block_rows];
+          b_row += e * N;
+          sb_row = e * (K / G);
+        }
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait_bounded(bar_empty + 8 * stage, phase ^ 1);
           const uint32_t full = bar_full + 8 * stage;
@@ -92,9 +108,9 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_co
           const uint32_t sa = smem_base + stage * C::kStageBytes, sb = sa + kTileBytes;
           const uint32_t ssa = sb + kTileBytes, ssb = ssa + C::kScaleBytes;
           tma_load_2d(sa, &tma_a, full, kb * BK, m0);                       // box {128 k, 128 m}
-          tma_load_2d(sb, &tma_b, full, kb * BK, n0);                       // box {128 k, 128 n}
+          tma_load_2d(sb, &tma_b, full, kb * BK, b_row);                    // box {128 k, 128 n}
           tma_load_2d(ssa, &tma_sa, full, m0, kb * C::kGroups);             // box {128 m, groups}
-          tma_load_2d(ssb, &tma_sb, full, n0, kb * C::kGroups);             // box {128 n, groups}
+          tma_load_2d(ssb, &tma_sb, full, n0, sb_row + kb * C::kGroups);    // box {128 n, groups}
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -241,18 +257,20 @@ quantize_fp8_groups_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restr
   if ((lane & (G / 8 - 1)) == 0) s[(long)(col / G) * s_ld + row] = scale;
 }
 
-template <int G>
+// E = 1 and block_expert = nullptr: the dense GEMM.  Otherwise b is [E·N, K] and sb [E·K/G, N] (grouped mode).
+template <int G, bool GROUPED>
 void launch_gemm(const void* a, const void* b, void* out, const float* sa, long sa_ld, const float* sb, int M, int N, int K,
-                 cudaStream_t st) {
+                 int E, const int* block_expert, int block_rows, cudaStream_t st) {
   using C = Cfg<G>;
   const int groups = K / G;
   const CUtensorMap ta = make_tmap_2d(a, CU_TENSOR_MAP_DATA_TYPE_UINT8, M, K, K, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);
-  const CUtensorMap tb = make_tmap_2d(b, CU_TENSOR_MAP_DATA_TYPE_UINT8, N, K, K, BK, BN, CU_TENSOR_MAP_SWIZZLE_128B);
+  const CUtensorMap tb = make_tmap_2d(b, CU_TENSOR_MAP_DATA_TYPE_UINT8, (uint64_t)E * N, K, K, BK, BN,
+                                      CU_TENSOR_MAP_SWIZZLE_128B);
   const CUtensorMap tsa = make_tmap_2d(sa, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, groups, M, sa_ld * 4, BM, C::kGroups,
                                        CU_TENSOR_MAP_SWIZZLE_NONE);
-  const CUtensorMap tsb = make_tmap_2d(sb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, groups, N, (uint64_t)N * 4, BN, C::kGroups,
-                                       CU_TENSOR_MAP_SWIZZLE_NONE);
-  auto kern = gemm_fp8_block_kernel<G>;
+  const CUtensorMap tsb = make_tmap_2d(sb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (uint64_t)E * groups, N, (uint64_t)N * 4, BN,
+                                       C::kGroups, CU_TENSOR_MAP_SWIZZLE_NONE);
+  auto kern = gemm_fp8_block_kernel<G, GROUPED>;
   static bool configured = false;
   if (!configured) {
     NXD_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
@@ -260,7 +278,8 @@ void launch_gemm(const void* a, const void* b, void* out, const float* sa, long 
   }
   const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
   const int sms = device_sm_count();
-  kern<<<tiles < sms ? tiles : sms, kThreads, C::kSmemBytes, st>>>(ta, tb, tsa, tsb, (__nv_bfloat16*)out, M, N, K);
+  kern<<<tiles < sms ? tiles : sms, kThreads, C::kSmemBytes, st>>>(ta, tb, tsa, tsb, (__nv_bfloat16*)out, M, N, K,
+                                                                   block_expert, block_rows);
   NXD_CUDA_CHECK(cudaGetLastError());
 }
 
@@ -282,10 +301,28 @@ void gemm_fp8_block(const void* a, const void* b, void* out, const float* scale_
                                                   __FILE__, __LINE__);
   if (M == 0) return;
   switch (group) {
-    case 32: fp8b::launch_gemm<32>(a, b, out, scale_a, scale_a_ld, scale_b, M, N, K, st); break;
-    case 64: fp8b::launch_gemm<64>(a, b, out, scale_a, scale_a_ld, scale_b, M, N, K, st); break;
-    case 128: fp8b::launch_gemm<128>(a, b, out, scale_a, scale_a_ld, scale_b, M, N, K, st); break;
+    case 32: fp8b::launch_gemm<32, false>(a, b, out, scale_a, scale_a_ld, scale_b, M, N, K, 1, nullptr, 0, st); break;
+    case 64: fp8b::launch_gemm<64, false>(a, b, out, scale_a, scale_a_ld, scale_b, M, N, K, 1, nullptr, 0, st); break;
+    case 128: fp8b::launch_gemm<128, false>(a, b, out, scale_a, scale_a_ld, scale_b, M, N, K, 1, nullptr, 0, st); break;
     default: nxd_throw("block-scaled fp8 GEMM: group size must be 32, 64 or 128", __FILE__, __LINE__);
+  }
+}
+
+void grouped_gemm_fp8_block(const void* a, const void* b, void* out, const float* scale_a, long scale_a_ld,
+                            const float* scale_b, int M, int N, int K, int E, const int* block_expert, int block_rows,
+                            int group, cudaStream_t st) {
+  if (K % fp8b::BK || N % 8) nxd_throw("grouped block-scaled fp8 GEMM needs K % 128 == 0 and N % 8 == 0", __FILE__, __LINE__);
+  if (block_rows <= 0 || block_rows % fp8b::BM || M % block_rows)
+    nxd_throw("grouped block-scaled fp8 GEMM: block_rows must be a positive multiple of 128 dividing M", __FILE__, __LINE__);
+  if (scale_a_ld % 4 || scale_a_ld < M)
+    nxd_throw("grouped block-scaled fp8 GEMM: A-scale row stride must be >= M and a multiple of 4", __FILE__, __LINE__);
+  if (E <= 0) nxd_throw("grouped block-scaled fp8 GEMM: needs at least one expert", __FILE__, __LINE__);
+  if (M == 0) return;
+  switch (group) {
+    case 32: fp8b::launch_gemm<32, true>(a, b, out, scale_a, scale_a_ld, scale_b, M, N, K, E, block_expert, block_rows, st); break;
+    case 64: fp8b::launch_gemm<64, true>(a, b, out, scale_a, scale_a_ld, scale_b, M, N, K, E, block_expert, block_rows, st); break;
+    case 128: fp8b::launch_gemm<128, true>(a, b, out, scale_a, scale_a_ld, scale_b, M, N, K, E, block_expert, block_rows, st); break;
+    default: nxd_throw("grouped block-scaled fp8 GEMM: group size must be 32, 64 or 128", __FILE__, __LINE__);
   }
 }
 

@@ -92,6 +92,11 @@ void gemm_fp8(const void* a, const void* b, void* out, int M, int N, int K, cons
 // out[M,N] (bf16) = Σ_g (a[:, g] · b[:, g]ᵀ) ∘ scale_a[g, :M] ⊗ scale_b[g, :N];  scale_a [K/group, scale_a_ld], scale_b [K/group, N]
 void gemm_fp8_block(const void* a, const void* b, void* out, const float* scale_a, long scale_a_ld, const float* scale_b,
                     int M, int N, int K, int group, cudaStream_t st);
+// grouped (MoE) mode: rows [i·block_rows, (i+1)·block_rows) of a use expert e = block_expert[i]: b [E·N, K] (rows e·N ..),
+// scale_b [E·K/group, N] (rows e·K/group ..); block_rows % 128 == 0 and M % block_rows == 0
+void grouped_gemm_fp8_block(const void* a, const void* b, void* out, const float* scale_a, long scale_a_ld,
+                            const float* scale_b, int M, int N, int K, int E, const int* block_expert, int block_rows,
+                            int group, cudaStream_t st);
 // x bf16 [M, K] → q e4m3 [M, K] and fp32 scale [K/group, scale_ld] (group-major); mx: OCP MX power-of-two scales, else absmax / 448
 void quantize_fp8_groups(const void* x, void* q, float* scale, int M, int K, long scale_ld, int group, bool mx, float clamp_bound,
                          cudaStream_t st);

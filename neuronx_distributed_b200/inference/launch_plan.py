@@ -53,7 +53,7 @@ _EXT_PURE = frozenset({"rmsnorm_fwd", "rmsnorm_bwd", "add_rmsnorm_fwd", "add_rms
                        "ce_stats", "ce_backward", "decode_attention", "decode_attention_partial", "gemv", "gemv_mx",
                        "moe_block_tkg", "moe_block_metadata", "row_argmax", "row_topk", "flash_attn_fwd",
                        "flash_attn_bwd", "moe_block_tkg_supported", "row_topk_supported", "grouped_gemm",
-                       "gemm_fp8_block", "quantize_fp8_groups"})
+                       "gemm_fp8_block", "quantize_fp8_groups", "grouped_gemm_fp8_block"})
 # … and the ones that write exactly these positional arguments (everything else they take is read-only)
 _EXT_WRITES = {"gemm_bf16": (2,), "gemm_fp8": (2,), "grouped_wgrad": (2,), "decode_rope_kv": (6, 7),
                "multi_tensor_sq_norm": (1,)}

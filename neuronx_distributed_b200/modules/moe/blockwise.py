@@ -11,6 +11,9 @@ of ``block_size`` and each block is multiplied by exactly one expert's weights:
 On CUDA the two projections are grouped wgmma GEMMs (``ops.gemm.grouped_matmul`` → MODE 3/4 of
 ``csrc/gemm_sm90.cu``): the block's expert only shifts the TMA coordinate of the weight tile, the backward runs the
 grouped dgrad and a per-expert segmented wgrad, and nothing syncs with the host.  On CPU it is a gathered einsum.
+Quantised expert layers run their own ``grouped_linear``: W8A8 block-wise e4m3 experts quantise each projection's input
+per token and run the grouped block-scaled FP8 GEMM (``ops.gemm_fp8.grouped_blockscaled_linear``); weight-only experts
+are de-quantised to the activation dtype once per call and run the bf16 grouped GEMM (inference only).
 """
 from __future__ import annotations
 
@@ -65,17 +68,33 @@ def build_block_metadata(expert_index: torch.Tensor, num_experts: int, block_siz
     return block_to_expert, tp2id, counts
 
 
+def _weight_of(proj) -> torch.Tensor:
+    return proj if isinstance(proj, torch.Tensor) else proj.weight
+
+
+def _grouped(x: torch.Tensor, proj, b2e: torch.Tensor, seg_first: torch.Tensor, block_size: int) -> torch.Tensor:
+    if isinstance(proj, torch.Tensor):
+        from ... import ops
+
+        return ops.gemm.grouped_matmul(x, proj, b2e, seg_first, block_size)
+    return proj.grouped_linear(x, b2e, seg_first, block_size)
+
+
+def _projection(layer):
+    """What the grouped path multiplies by: a float expert layer's weight, or a quantised layer itself."""
+    return layer if hasattr(layer, "grouped_linear") else layer.weight
+
+
 def blockwise_mlp_from_metadata(hidden: torch.Tensor, expert_affinities_masked: torch.Tensor, gate_up_proj_weight: torch.Tensor,
                                 down_proj_weight: torch.Tensor, token_position_to_id: torch.Tensor, block_to_expert: torch.Tensor,
                                 block_size: int, activation, gate_up_proj_bias: Optional[torch.Tensor] = None,
                                 down_proj_bias: Optional[torch.Tensor] = None, pre_scale: bool = False) -> torch.Tensor:
     """The dropless computation for a GIVEN block layout: ``out[t] += aff[t, e(b)] · MLP_{e(b)}(hidden[t])`` for every slot of
     every block ``b`` holding token ``t`` (``-1`` slots are padding).  ``expert_affinities_masked`` is ``[T, E]``.
-    ``pre_scale`` multiplies the expert input by the affinity instead of the output (early affinity modulation)."""
-    from ... import ops
-
+    ``pre_scale`` multiplies the expert input by the affinity instead of the output (early affinity modulation).  A projection
+    is a ``[E, K, N]`` weight or a quantised expert-fused layer, which runs its own ``grouped_linear``."""
     T, H = hidden.shape
-    E = gate_up_proj_weight.shape[0]
+    E = _weight_of(gate_up_proj_weight).shape[0]
     nb = block_to_expert.numel()
     tp2id = token_position_to_id[: nb * block_size].long()
     b2e = block_to_expert.long()
@@ -88,11 +107,11 @@ def blockwise_mlp_from_metadata(hidden: torch.Tensor, expert_affinities_masked: 
     x = hidden[gather_ids] * valid.unsqueeze(-1).to(hidden.dtype)                   # [nb·B, H]
     if pre_scale:
         x = x * aff.unsqueeze(-1).to(x.dtype)
-    h = ops.gemm.grouped_matmul(x, gate_up_proj_weight, b2e, seg_first, block_size)
+    h = _grouped(x, gate_up_proj_weight, b2e, seg_first, block_size)
     if gate_up_proj_bias is not None:
         h = h + gate_up_proj_bias[slot_e].to(h.dtype)
     h = activation(h)
-    y = ops.gemm.grouped_matmul(h.contiguous(), down_proj_weight, b2e, seg_first, block_size)
+    y = _grouped(h.contiguous(), down_proj_weight, b2e, seg_first, block_size)
     if down_proj_bias is not None:
         y = y + down_proj_bias[slot_e].to(y.dtype)
     scale = (aff > 0).to(y.dtype) if pre_scale else aff.to(y.dtype)
@@ -110,8 +129,8 @@ def blockwise_expert_mlp(hidden: torch.Tensor, expert_affinities: torch.Tensor, 
         denom = expert_affinities.gather(1, expert_index).sum(-1, keepdim=True).clamp(min=1e-9)
         expert_affinities = expert_affinities / denom
     proj = experts.gate_up_proj if experts.glu_mlp else experts.up_proj
-    return blockwise_mlp_from_metadata(hidden, expert_affinities, proj.weight, experts.down_proj.weight, tp2id, b2e, block_size,
-                                       experts.activation, proj.bias,
+    return blockwise_mlp_from_metadata(hidden, expert_affinities, _projection(proj), _projection(experts.down_proj), tp2id, b2e,
+                                       block_size, experts.activation, proj.bias,
                                        None if experts.down_proj.bias is None else experts.down_proj.bias / experts.down_proj.tp)
 
 

@@ -8,6 +8,9 @@
   one ``wgmma m64n128k32.e4m3`` chain per group into a temporary accumulator that is promoted into the fp32 main accumulator
   with the group's scales, in registers.  Weight scales may be per (row, group) ``[N, K/G]`` or per 2-D block ``[N/bn, K/G]``,
   fp32 or E8M0.
+* :func:`grouped_blockscaled_linear` — the same product for MoE experts on the dropless block layout: rows come in
+  ``block_size``-row blocks and block i uses the weights of expert ``block_to_expert[i]``.  CUDA: the grouped mode of the same
+  kernel, where the block's expert only shifts the TMA rows of the weight tile and of its scales.
 * :func:`quantize_groups` — the matching per-token activation quantiser (``absmax`` or OCP ``mx`` scale rule); CUDA: one
   bandwidth-bound kernel that writes the codes and the scales in the layout the GEMM reads.
 
@@ -135,3 +138,51 @@ def blockscaled_linear(xq: torch.Tensor, xs: torch.Tensor, wq: torch.Tensor, ws:
         return y.view(*lead, N)
     y = _dequant_groups(x2, xs2, group_size) @ _dequant_groups(wq.reshape(N, K), sb.t(), group_size).t()
     return y.to(out_dtype).view(*lead, N)
+
+
+def expert_weight_scales_kn(ws: torch.Tensor, n: int, k: int, group_size: int) -> torch.Tensor:
+    """Expert weight scales ``[E, K/G, N]`` (block axis 1) or ``[E, K/G, N/bn]`` (2-D blocks), fp32 or E8M0 ``uint8`` → the fp32
+    ``[E, K/G, N]`` layout of :func:`grouped_blockscaled_linear`'s kernel, as :func:`weight_scales_kn` does per expert.  A
+    contiguous fp32 ``[E, K/G, N]`` is returned as it is."""
+    s = torch.pow(2.0, ws.float() - 127.0) if ws.dtype == torch.uint8 else ws.float()
+    assert s.dim() == 3 and s.shape[1] == k // group_size, f"expert scales {tuple(ws.shape)} do not have K/G = {k // group_size} rows"
+    if s.shape[2] != n:
+        assert n % s.shape[2] == 0, f"{s.shape[2]} scale columns do not tile {n} weight columns"
+        s = s.repeat_interleave(n // s.shape[2], dim=2)
+    return s.contiguous()
+
+
+def grouped_blockscaled_linear(xq: torch.Tensor, xs: torch.Tensor, wq: torch.Tensor, ws: torch.Tensor,
+                               block_to_expert: torch.Tensor, block_size: int, group_size: int,
+                               out_dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """``y[i·B:(i+1)·B] = dequant(xq, xs)[i·B:(i+1)·B] @ dequant(wq[e], ws[e])`` with ``e = block_to_expert[i]``.  Inference only.
+
+    ``xq [nb·B, K]`` / ``xs [nb·B, K/G]`` as :func:`quantize_groups` returns them; ``wq`` e4m3 ``[E, K, N]`` (in, out);
+    ``ws`` fp32 or E8M0 ``[E, K/G, N]`` or ``[E, K/G, N/bn]``.  CUDA with ``wq`` stored K-major (strides ``(N·K, 1, K)``, as
+    ``wq.transpose(1, 2).contiguous().transpose(1, 2)`` leaves it), 16-byte aligned operands, G ∈ {32, 64, 128},
+    ``K % 128 == 0``, ``N % 8 == 0``, ``B % 128 == 0`` and bf16 output: one launch of the grouped block-scaled kernel;
+    otherwise the fp32 oracle of the same quantised operands."""
+    K, M = xq.shape[-1], xq.shape[0]
+    E, N = wq.shape[0], wq.shape[2]
+    nb = block_to_expert.numel()
+    assert xq.dim() == 2 and wq.dim() == 3 and wq.shape[1] == K and M == nb * block_size, \
+        f"xq {tuple(xq.shape)}, wq {tuple(wq.shape)}, {nb} blocks of {block_size}"
+    xs2 = xs.reshape(M, K // group_size)
+    sb = expert_weight_scales_kn(ws, N, K, group_size)
+    wt = wq.transpose(1, 2)                                   # [E, N, K]: a view of K-major storage, no copy
+    if (group_size in GROUP_SIZES and K % 128 == 0 and N % 8 == 0 and block_size % 128 == 0 and out_dtype == torch.bfloat16
+            and xq.dtype == torch.float8_e4m3fn and wq.dtype == torch.float8_e4m3fn and wt.is_contiguous()
+            and _ext.use_cuda(xq, wq, xs2, sb, block_to_expert) and hasattr(_ext.ext(), "grouped_gemm_fp8_block")
+            and xq.contiguous().data_ptr() % 16 == 0 and wt.data_ptr() % 16 == 0 and sb.data_ptr() % 16 == 0):
+        sa = xs2.t()                                          # [K/G, M]: a view of the quantiser's group-major buffer
+        if not (sa.dtype == torch.float32 and sa.stride(1) == 1 and sa.stride(0) >= M and sa.stride(0) % 4 == 0
+                and sa.data_ptr() % 16 == 0):
+            buf = torch.zeros(K // group_size, (M + 3) // 4 * 4, dtype=torch.float32, device=xq.device)
+            buf[:, :M] = xs2.t()
+            sa = buf[:, :M]
+        b2e = block_to_expert if block_to_expert.dtype == torch.int32 else block_to_expert.int()
+        _ext.count_launch()
+        return _ext.ext().grouped_gemm_fp8_block(xq.contiguous(), wt, sa, sb, b2e, block_size, group_size)
+    xd = _dequant_groups(xq, xs2, group_size).view(nb, block_size, K)
+    wd = (wq.float().reshape(E, K // group_size, group_size, N) * sb.unsqueeze(2)).reshape(E, K, N)
+    return torch.bmm(xd, wd[block_to_expert.long()]).reshape(M, N).to(out_dtype)

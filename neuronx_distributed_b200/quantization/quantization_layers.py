@@ -346,14 +346,16 @@ class BaseQuantizeParallelLinear(ProcessGroupSafeDeepcopy, nn.Module, metaclass=
 
     def _blockscaled_group(self) -> int:
         """Size G of the K-blocks when the layer runs W8A8 on the block-scaled FP8 GEMM (block-wise e4m3 weight, dynamic
-        activations, G ∈ {32, 64, 128} dividing this rank's K so row-parallel shards keep whole blocks), else 0."""
+        activations, G ∈ {32, 64, 128} dividing this rank's K so row-parallel shards keep whole blocks), else 0.  K is
+        axis 1 of both a dense ``[N, K]`` and an expert-fused ``[E, K, N]`` weight; expert scales must be per expert."""
         if (self.quantization_type != QuantizationType.BLOCKWISE_SYMMETRIC
                 or self.activation_quantization_type != ActivationQuantizationType.DYNAMIC
-                or self.weight.dtype != torch.float8_e4m3fn or self.weight.dim() != 2 or self.mx_swizzle
+                or self.weight.dtype != torch.float8_e4m3fn or self.weight.dim() not in (2, 3) or self.mx_swizzle
                 or 1 not in self.block_axis):
             return 0
         G, K = self.block_size[self.block_axis.index(1)], self.weight.shape[1]
-        if G not in (32, 64, 128) or K % G or self.scale.dim() != 2 or self.scale.shape[1] != K // G:
+        if (G not in (32, 64, 128) or K % G or self.scale.dim() != self.weight.dim() or self.scale.shape[1] != K // G
+                or (self.weight.dim() == 3 and self.scale.shape[0] != self.weight.shape[0])):
             return 0
         return G
 
@@ -401,10 +403,19 @@ class BaseQuantizeParallelLinear(ProcessGroupSafeDeepcopy, nn.Module, metaclass=
         return torch.nn.functional.linear(x.to(out_dtype), self._dequantized_weight(self.weight, self.scale, out_dtype))
 
     def _linear_experts(self, x: torch.Tensor, expert_indices: Optional[torch.Tensor]) -> torch.Tensor:
-        """``x [E, …, K] · weight[E, K, N]`` → ``[E, …, N]`` (expert-fused layers; weight-only quantisation)."""
+        """``x [E, …, K] · weight[E, K, N]`` → ``[E, …, N]`` (expert-fused layers).  W8A8 expert layers quantise ``x`` per
+        token and K-block as the grouped path does and run the fp32 oracle of the quantised operands."""
         weight, scale = _index_experts(self.weight, expert_indices), _index_experts(self.scale, expert_indices) \
             if self.scale.shape[0] > 1 else self.scale
         dt = x.dtype
+        G = self._blockscaled_group()
+        if G:
+            from ..ops import gemm_fp8
+
+            K = x.shape[-1]
+            xq, xs = gemm_fp8.quantize_groups(x, G, "absmax", None if self.clamp_bound == float("inf") else self.clamp_bound)
+            xd = gemm_fp8._dequant_groups(xq.reshape(-1, K), xs.reshape(-1, K // G), G).reshape(x.shape)
+            return torch.einsum("e...h,ehi->e...i", xd, blockwise_scale_dequantize(weight, scale, torch.float32)).to(dt)
         if self._scale_is_output_only(2):
             y = torch.einsum("e...h,ehi->e...i", x, direct_cast_dequantize(weight, dt))
             s = self._scale_f32(scale)
@@ -635,6 +646,18 @@ class QuantizedRowParallel(BaseQuantizeParallelLinear):
 # =====================================================================================================================
 # Expert-fused (MoE)
 # =====================================================================================================================
+def _check_expert_activation_quantization(t) -> None:
+    if ActivationQuantizationType(t) == ActivationQuantizationType.STATIC:
+        raise ValueError("expert-fused layers take no static input scale: activation quantisation must be none or dynamic")
+
+
+def _expert_activation_quantization(q_config: BASE_QCONFIG_DICT_TYPE) -> ActivationQuantizationType:
+    """The q_config's activation quantisation for expert-fused layers.  A static input scale belongs to one dense layer
+    and the fused experts have none, so a static config leaves the experts weight-only."""
+    t = ActivationQuantizationType(q_config.get("activation_quantization_type"))
+    return ActivationQuantizationType.NONE if t == ActivationQuantizationType.STATIC else t
+
+
 class _QuantizedExpertMixin(ExpertFusedLinear):
     autograd_func_class = ExpertFusedLinearWithAsyncCommunication
     _default_channel_axis = 2
@@ -651,6 +674,49 @@ class _QuantizedExpertMixin(ExpertFusedLinear):
             ps.get_expert_model_parallel_rank()
         self.local_expert_ids = ps.get_experts_for_expert_parallel_rank(r, num_experts, self.ep)
         self.is_prefill, self.is_fused_gate_up = is_prefill, is_fused_gate_up
+
+    def _k_major_weight(self) -> torch.Tensor:
+        """The weight with its storage K-major (strides ``(N·K, 1, K)``), the layout Hopper's e4m3 wgmma reads, keeping its
+        logical ``[E, K, N]`` shape and values: every einsum path and ``state_dict()`` see the same tensor.  The expert
+        constructors relayout a W8A8 weight once; loading a checkpoint or moving the layer to another device copies into
+        that layout.  Only a weight whose storage was replaced since is relaid out here, once, and never under CUDA-graph
+        capture."""
+        w = self.weight
+        if not w.transpose(1, 2).is_contiguous():
+            if w.is_cuda and torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("W8A8 expert weight is not K-major: run one forward before CUDA-graph capture")
+            w.data = w.data.transpose(1, 2).contiguous().transpose(1, 2)
+        return w
+
+    def _expert_scales_kn(self, G: int) -> torch.Tensor:
+        """fp32 ``[E, K/G, N]`` weight scales of the grouped block-scaled GEMM.  2-D blocks and E8M0 scales are expanded once
+        per scale tensor (and again only after it is written); fp32 ``[E, K/G, N]`` scales are used as they are."""
+        from ..ops import gemm_fp8
+
+        s = self.scale
+        key = (s.data_ptr(), s._version, s.device, s.dtype, tuple(s.shape))
+        cached = self.__dict__.get("_scales_kn")
+        if cached is None or cached[0] != key:
+            cached = (key, gemm_fp8.expert_weight_scales_kn(s, self.weight.shape[2], self.weight.shape[1], G))
+            self.__dict__["_scales_kn"] = cached
+        return cached[1]
+
+    def grouped_linear(self, x: torch.Tensor, block_to_expert: torch.Tensor, seg_first_block: torch.Tensor,
+                       block_size: int) -> torch.Tensor:
+        """Dropless block layout: ``x [nb·B, K]``, block i through local expert ``block_to_expert[i]`` → ``[nb·B, N]``.
+        W8A8 layers quantise ``x`` per token and K-block and run the grouped block-scaled FP8 GEMM (two launches, no
+        de-quantised weight); weight-only layers de-quantise their experts to ``x``'s dtype once and run the grouped GEMM."""
+        from ..ops import gemm
+
+        G = self._blockscaled_group()
+        if G:
+            from ..ops import gemm_fp8
+
+            xq, xs = gemm_fp8.quantize_groups(x, G, "absmax", None if self.clamp_bound == float("inf") else self.clamp_bound)
+            return gemm_fp8.grouped_blockscaled_linear(xq, xs, self._k_major_weight(), self._expert_scales_kn(G),
+                                                       block_to_expert, block_size, G, out_dtype=x.dtype)
+        w = self._dequantized_weight(self.weight, self.scale, x.dtype)
+        return gemm.grouped_matmul(x, w, block_to_expert, seg_first_block, block_size)
 
     def _expert_bias(self, y: torch.Tensor, expert_indices: Optional[torch.Tensor], scale: float = 1.0) -> torch.Tensor:
         if self.bias is None:
@@ -670,7 +736,10 @@ class QuantizedExpertFusedColumnParallel(QuantizedColumnParallel, _QuantizedExpe
                  quantization_per_channel_axis: Optional[int] = None, tensor_model_parallel_group=None,
                  block_axis: Optional[List[int]] = None, block_size: Optional[List[int]] = None,
                  scale_dtype: Union[torch.dtype, ScaleDtype] = torch.float32, expert_model_parallel_group=None,
-                 is_prefill: bool = True, rank_ordering: Optional[Sequence[int]] = None, is_fused_gate_up: bool = False):
+                 is_prefill: bool = True, rank_ordering: Optional[Sequence[int]] = None, is_fused_gate_up: bool = False,
+                 activation_quantization_type: Optional[Union[ActivationQuantizationType, str]] = None,
+                 clamp_bound: float = float("inf")):
+        _check_expert_activation_quantization(activation_quantization_type)
         nn.Module.__init__(self)                    # attributes needed by the config hooks before the parent ctor runs
         self._expert_setup(num_experts, expert_model_parallel_group, is_prefill, is_fused_gate_up)
         qt = QuantizationType(quantization_type)
@@ -683,11 +752,14 @@ class QuantizedExpertFusedColumnParallel(QuantizedColumnParallel, _QuantizedExpe
                          sequence_parallel_enabled=False, keep_master_weight=keep_master_weight,
                          quantization_per_channel_axis=quantization_per_channel_axis,
                          tensor_model_parallel_group=tensor_model_parallel_group, block_axis=block_axis,
-                         block_size=block_size, scale_dtype=scale_dtype, rank_ordering=rank_ordering)
+                         block_size=block_size, scale_dtype=scale_dtype, rank_ordering=rank_ordering,
+                         activation_quantization_type=activation_quantization_type, clamp_bound=clamp_bound)
         for k in ("num_experts", "ep", "expert_model_parallel_group", "_n_local_experts", "num_local_experts",
                   "is_prefill", "is_fused_gate_up", "local_expert_ids"):
             self.__dict__[k] = saved[k]
         self._mark_expert_parallel_weights(expert_parallel_group_size=self.ep, is_prefill=is_prefill)
+        if self._blockscaled_group():
+            self._k_major_weight()
 
     def _setup_for_weight_and_bias_config(self, bias: bool) -> None:
         self.weight_shape = (self._n_local_experts, self.input_size, self.output_size_per_partition)
@@ -712,7 +784,9 @@ class QuantizedExpertFusedColumnParallel(QuantizedColumnParallel, _QuantizedExpe
             quantization_per_channel_axis=q_config.get("quantization_per_channel_axis"),
             tensor_model_parallel_group=mod.tensor_parallel_group, expert_model_parallel_group=mod.expert_model_parallel_group,
             is_prefill=mod.is_prefill, block_axis=q_config.get("block_axis"), block_size=q_config.get("block_size"),
-            scale_dtype=q_config.get("scale_dtype", torch.float32), is_fused_gate_up=mod.is_fused_gate_up)
+            scale_dtype=q_config.get("scale_dtype", torch.float32), is_fused_gate_up=mod.is_fused_gate_up,
+            activation_quantization_type=_expert_activation_quantization(q_config),
+            clamp_bound=q_config.get("clamp_bound", float("inf")))
         new_mod._maybe_quantize_from(mod)
         return cls._apply_post_quantization_hook(mod, new_mod)
 
@@ -727,7 +801,10 @@ class QuantizedExpertFusedRowParallel(QuantizedRowParallel, _QuantizedExpertMixi
                  quantization_per_channel_axis: Optional[int] = None, tensor_model_parallel_group=None,
                  block_axis: Optional[List[int]] = None, block_size: Optional[List[int]] = None,
                  scale_dtype: Union[torch.dtype, ScaleDtype] = torch.float32, expert_model_parallel_group=None,
-                 is_prefill: bool = True, rank_ordering: Optional[Sequence[int]] = None, is_fused_gate_up: bool = False):
+                 is_prefill: bool = True, rank_ordering: Optional[Sequence[int]] = None, is_fused_gate_up: bool = False,
+                 activation_quantization_type: Optional[Union[ActivationQuantizationType, str]] = None,
+                 clamp_bound: float = float("inf")):
+        _check_expert_activation_quantization(activation_quantization_type)
         nn.Module.__init__(self)
         self._expert_setup(num_experts, expert_model_parallel_group, is_prefill, is_fused_gate_up)
         qt = QuantizationType(quantization_type)
@@ -740,11 +817,14 @@ class QuantizedExpertFusedRowParallel(QuantizedRowParallel, _QuantizedExpertMixi
                          sequence_parallel_enabled=False, keep_master_weight=keep_master_weight,
                          quantization_per_channel_axis=quantization_per_channel_axis, reduce_output=reduce_output,
                          tensor_model_parallel_group=tensor_model_parallel_group, block_axis=block_axis,
-                         block_size=block_size, scale_dtype=scale_dtype, rank_ordering=rank_ordering)
+                         block_size=block_size, scale_dtype=scale_dtype, rank_ordering=rank_ordering,
+                         activation_quantization_type=activation_quantization_type, clamp_bound=clamp_bound)
         for k in ("num_experts", "ep", "expert_model_parallel_group", "_n_local_experts", "num_local_experts",
                   "is_prefill", "is_fused_gate_up", "local_expert_ids"):
             self.__dict__[k] = saved[k]
         self._mark_expert_parallel_weights(expert_parallel_group_size=self.ep, is_prefill=is_prefill)
+        if self._blockscaled_group():
+            self._k_major_weight()
 
     def _setup_for_weight_and_bias_config(self, bias: bool) -> None:
         self.weight_shape = (self._n_local_experts, self.input_size_per_partition, self.output_size)
@@ -768,6 +848,8 @@ class QuantizedExpertFusedRowParallel(QuantizedRowParallel, _QuantizedExpertMixi
             quantization_per_channel_axis=q_config.get("quantization_per_channel_axis"),
             tensor_model_parallel_group=mod.tensor_parallel_group, expert_model_parallel_group=mod.expert_model_parallel_group,
             is_prefill=mod.is_prefill, block_axis=q_config.get("block_axis"), block_size=q_config.get("block_size"),
-            scale_dtype=q_config.get("scale_dtype", torch.float32), is_fused_gate_up=mod.is_fused_gate_up)
+            scale_dtype=q_config.get("scale_dtype", torch.float32), is_fused_gate_up=mod.is_fused_gate_up,
+            activation_quantization_type=_expert_activation_quantization(q_config),
+            clamp_bound=q_config.get("clamp_bound", float("inf")))
         new_mod._maybe_quantize_from(mod)
         return cls._apply_post_quantization_hook(mod, new_mod)
