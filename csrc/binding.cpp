@@ -748,6 +748,14 @@ static void zero1_reduce_scatter(const Tensor& peer_bufs, int64_t grad_off_bytes
                                  int64_t epoch, int64_t rank, int64_t world, int64_t shard_numel, double scale, Tensor out,
                                  Tensor done_ctr, bool grads_fp32, int64_t sub_begin, int64_t sub_len, int64_t max_ctas) {
   TORCH_CHECK(sub_begin >= 0 && sub_len >= 0 && sub_begin + sub_len <= shard_numel && sub_begin % 8 == 0 && sub_len % 8 == 0);
+  // 16-byte loads of every peer's shard and float4 stores into `out`: misaligned offsets or a short `out` would read or
+  // write outside the buffers instead of failing
+  TORCH_CHECK(shard_numel >= 0 && shard_numel % 8 == 0, "zero1_reduce_scatter: shard_numel must be a multiple of 8");
+  TORCH_CHECK(grad_off_bytes >= 0 && grad_off_bytes % 16 == 0, "zero1_reduce_scatter: grad_off_bytes must be a multiple of 16");
+  TORCH_CHECK(out.is_cuda() && out.is_contiguous() && out.scalar_type() == at::kFloat && out.numel() >= shard_numel,
+              "zero1_reduce_scatter: out must be a contiguous fp32 CUDA tensor of at least shard_numel elements");
+  TORCH_CHECK(world >= 1 && world <= 8 && rank >= 0 && rank < world && peer_bufs.numel() >= world && peer_flags.numel() >= world,
+              "zero1_reduce_scatter: 1 <= world <= 8, 0 <= rank < world, one peer pointer per rank");
   c10::cuda::CUDAGuard g(out.device());
   nxd::zero1_reduce_scatter(peer_bufs.data_ptr<int64_t>(), grad_off_bytes, peer_flags.data_ptr<int64_t>(), (int)flag_off,
                             (uint32_t)epoch, (int)rank, (int)world, shard_numel, sub_begin, sub_len, (float)scale,
@@ -757,6 +765,14 @@ static void zero1_reduce_scatter(const Tensor& peer_bufs, int64_t grad_off_bytes
 static void zero1_all_gather(const Tensor& master, const Tensor& peer_bufs, int64_t param_off_bytes, const Tensor& peer_flags,
                              int64_t flag_off, int64_t epoch, int64_t rank, int64_t world, int64_t shard_numel,
                              Tensor done_ctr, bool params_bf16) {
+  // the kernel moves 8 master elements per thread with 16-byte stores: a shard_numel that is not a multiple of 8 would drop
+  // its tail, a short master would be read past its end
+  TORCH_CHECK(shard_numel >= 0 && shard_numel % 8 == 0, "zero1_all_gather: shard_numel must be a multiple of 8");
+  TORCH_CHECK(master.is_cuda() && master.is_contiguous() && master.scalar_type() == at::kFloat && master.numel() >= shard_numel,
+              "zero1_all_gather: master must be a contiguous fp32 CUDA tensor of at least shard_numel elements");
+  TORCH_CHECK(param_off_bytes >= 0 && param_off_bytes % 16 == 0, "zero1_all_gather: param_off_bytes must be a multiple of 16");
+  TORCH_CHECK(world >= 1 && world <= 8 && rank >= 0 && rank < world && peer_bufs.numel() >= world && peer_flags.numel() >= world,
+              "zero1_all_gather: 1 <= world <= 8, 0 <= rank < world, one peer pointer per rank");
   c10::cuda::CUDAGuard g(master.device());
   nxd::zero1_all_gather(master.data_ptr<float>(), peer_bufs.data_ptr<int64_t>(), param_off_bytes,
                         peer_flags.data_ptr<int64_t>(), (int)flag_off, (uint32_t)epoch, (int)rank, (int)world, shard_numel,

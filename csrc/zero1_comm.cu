@@ -140,6 +140,7 @@ void zero1_reduce_scatter(const int64_t* peer_bufs, long grad_off_bytes, const i
 void zero1_all_gather(const float* master, const int64_t* peer_bufs, long param_off_bytes, const int64_t* peer_flags,
                       int flag_off, uint32_t epoch, int rank, int world, long shard_numel, uint32_t* done_ctr, int param_dt,
                       cudaStream_t st) {
+  if (world > 8) nxd_throw("zero1 kernels support up to 8 ranks per group", __FILE__, __LINE__);
   const int grid = sms();
   if (param_dt == kBF16)
     zero1_ag_kernel<__nv_bfloat16><<<grid, 512, 0, st>>>(master, peer_bufs, param_off_bytes, peer_flags, flag_off, epoch, rank,
