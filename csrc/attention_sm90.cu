@@ -542,8 +542,10 @@ __global__ void __launch_bounds__(kThreads) spec_attn_kernel(const SpecParams p)
     sBits[w] = bits;
   }
   __syncthreads();
-  // tokens [w_lo, w_hi) of this row tile (G divides 64): their smallest depth and the window columns any of them sees
-  const int w_lo = r0 / G, w_hi = min((r0 + BT) / G, W);
+  // tokens [w_lo, w_hi) with a row in this tile: their smallest depth and the window columns any of them sees.  When G does
+  // not divide 64, a token's G rows can straddle two tiles, and the one holding its first rows must count it too (round up).
+  constexpr int kRoundUp = BT % G == 0 ? 0 : G - 1;
+  const int w_lo = r0 / G, w_hi = min((r0 + BT + kRoundUp) / G, W);
   int dmin = INT32_MAX;
   uint64_t seen = 0;
   for (int w = w_lo; w < w_hi; ++w) { dmin = min(dmin, sDepth[w]); seen |= sBits[w]; }
@@ -1120,13 +1122,7 @@ void speculation_attention(const void* q, const void* k, const void* v, const lo
     else with_roll(hd, g, std::false_type{});
   };
   dispatch_head_dim(D, "speculation_attention", [&](auto hd) {
-    switch (G) {
-      case 1: with_cache(hd, std::integral_constant<int, 1>{}); break;
-      case 2: with_cache(hd, std::integral_constant<int, 2>{}); break;
-      case 4: with_cache(hd, std::integral_constant<int, 4>{}); break;
-      case 8: with_cache(hd, std::integral_constant<int, 8>{}); break;
-      default: nxd_throw("speculation_attention: unsupported GQA group size", __FILE__, __LINE__);
-    }
+    dispatch_gqa_group(G, "speculation_attention", [&](auto g) { with_cache(hd, g); });
   });
   NXD_CUDA_CHECK(cudaGetLastError());
   // row (b·W + w)·H + h of the partials → out [B, W, H, D]

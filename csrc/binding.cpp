@@ -420,7 +420,6 @@ static Tensor speculation_attention(const Tensor& q, const Tensor& k, const Tens
   const char* fn = "speculation_attention";
   const bool e4m3 = check_decode_args(fn, q, k, v, positions, k_scale, v_scale, 64);
   const int B = q.size(0), W = q.size(1), H = q.size(2), D = q.size(3), L = k.size(1), Hkv = k.size(2), G = H / Hkv;
-  TORCH_CHECK(G == 1 || G == 2 || G == 4 || G == 8, fn, ": the GQA group size must be 1, 2, 4 or 8");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0 && q.stride(0) % 8 == 0 && q.stride(1) % 8 == 0,
               fn, ": q rows must be 16-byte aligned");
   TORCH_CHECK(e4m3 || ((reinterpret_cast<uintptr_t>(k.data_ptr()) | reinterpret_cast<uintptr_t>(v.data_ptr())) % 16 == 0 &&

@@ -41,6 +41,24 @@ inline void dispatch_head_dim(int D, const char* fn, F&& f) {
   }
 }
 
+// f(std::integral_constant<int, G>{}) for a runtime GQA group size G = H / Hkv: the groups the token-generation kernels
+// (decode, flash-decoding, verification) are instantiated for (ops.attention.DECODE_GQA_GROUPS).  They keep G query rows
+// in registers, so G > 8 would spill.
+template <class F>
+inline void dispatch_gqa_group(int G, const char* fn, F&& f) {
+  switch (G) {
+    case 1: f(std::integral_constant<int, 1>{}); break;
+    case 2: f(std::integral_constant<int, 2>{}); break;
+    case 3: f(std::integral_constant<int, 3>{}); break;
+    case 4: f(std::integral_constant<int, 4>{}); break;
+    case 5: f(std::integral_constant<int, 5>{}); break;
+    case 6: f(std::integral_constant<int, 6>{}); break;
+    case 7: f(std::integral_constant<int, 7>{}); break;
+    case 8: f(std::integral_constant<int, 8>{}); break;
+    default: nxd_throw(std::string(fn) + ": the GQA group size must be 1 to 8", __FILE__, __LINE__);
+  }
+}
+
 // ---------------------------------------------------------------- type helpers
 template <typename T> struct Vec8;  // 8 elements of a 16-bit type = 16 bytes
 template <> struct Vec8<__nv_bfloat16> { uint4 raw; };

@@ -431,17 +431,11 @@ void decode_attention(const void* q, const void* k, const void* v, const long* p
 #define NXD_DEC_R(T, Gv)             \
   if (rolling) NXD_DEC(T, Gv, true); \
   else NXD_DEC(T, Gv, false)
-#define NXD_DEC_G(T)                                                                      \
-  switch (G) {                                                                            \
-    case 1: NXD_DEC_R(T, 1); break;                                                       \
-    case 2: NXD_DEC_R(T, 2); break;                                                       \
-    case 4: NXD_DEC_R(T, 4); break;                                                       \
-    case 8: NXD_DEC_R(T, 8); break;                                                       \
-    default: nxd_throw("decode_attention: unsupported GQA group size", __FILE__, __LINE__); \
-  }
-    if (kv_e4m3) NXD_DEC_G(__nv_fp8_e4m3)
-    else NXD_DEC_G(__nv_bfloat16)
-#undef NXD_DEC_G
+    dispatch_gqa_group(G, "decode_attention", [&](auto g) {
+      constexpr int Gv = decltype(g)::value;
+      if (kv_e4m3) NXD_DEC_R(__nv_fp8_e4m3, Gv);
+      else NXD_DEC_R(__nv_bfloat16, Gv);
+    });
 #undef NXD_DEC_R
 #undef NXD_DEC
     if (fin_o != nullptr) decode_combine_partial_kernel<HD><<<B * H, HD, 0, st>>>(part_o, part_ml, fin_o, fin_ml, splits);

@@ -12,8 +12,11 @@ reference's ``examples/inference/run_llama.py`` / ``runner.py`` (trace → load 
   # Mistral-7B geometry (sliding window 4096): a rolling KV cache keeps 4096 + 64 rows per sequence instead of 8192
   torchrun --nproc-per-node 1 examples/inference/run_llama.py --model mistral-7b --batch_size 16 --max_prompt_length 2048 \
       --sequence_length 8192 --benchmark --num_runs 1 --rolling_kv_cache
-  # Llama-3.2-1B geometry (head_dim 64, 4 query heads per KV head) with random weights
+  # Llama-3.2-1B geometry (head_dim 64, 4 query heads per KV head, Llama-3 RoPE scaling) with random weights
   torchrun --nproc-per-node 1 examples/inference/run_llama.py --model llama3.2-1b --batch_size 16 --max_prompt_length 2048 \
+      --sequence_length 4096 --benchmark
+  # Llama-3.2-3B (3 query heads per KV head) and Qwen2.5-7B (7 per KV head, q / k / v bias) geometries
+  torchrun --nproc-per-node 1 examples/inference/run_llama.py --model qwen2.5-7b --batch_size 8 --max_prompt_length 2048 \
       --sequence_length 4096 --benchmark
 """
 import argparse
@@ -44,17 +47,32 @@ def mistral_7b_config(**kw) -> LlamaConfig:
                        num_key_value_heads=8, sliding_window=4096, **kw)
 
 
+# the rope_scaling of the Llama-3.2 config.json files
+LLAMA3_2_ROPE_SCALING = {"factor": 32.0, "low_freq_factor": 1.0, "high_freq_factor": 4.0, "original_max_position_embeddings": 8192}
+
+
 def llama3_2_1b_config(**kw) -> LlamaConfig:
-    """Llama-3.2-1B geometry: head_dim 2048 / 32 = 64, 8 KV heads (GQA group 4), rope_theta 500000.  Llama-3's rope
-    frequency scaling is not applied, so real Llama-3.2 weights would not reproduce the reference logits."""
+    """Llama-3.2-1B geometry: head_dim 2048 / 32 = 64, 8 KV heads (GQA group 4), rope_theta 500000, Llama-3 RoPE scaling."""
     return LlamaConfig(vocab_size=128256, hidden_size=2048, intermediate_size=8192, num_hidden_layers=16, num_attention_heads=32,
-                       num_key_value_heads=8, rope_theta=500000.0, **kw)
+                       num_key_value_heads=8, rope_theta=500000.0, rope_scaling=dict(LLAMA3_2_ROPE_SCALING), **kw)
+
+
+def llama3_2_3b_config(**kw) -> LlamaConfig:
+    """Llama-3.2-3B geometry: head_dim 128, 24 / 8 heads (GQA group 3), rope_theta 500000, Llama-3 RoPE scaling."""
+    return LlamaConfig(vocab_size=128256, hidden_size=3072, intermediate_size=8192, num_hidden_layers=28, num_attention_heads=24,
+                       num_key_value_heads=8, rope_theta=500000.0, rope_scaling=dict(LLAMA3_2_ROPE_SCALING), **kw)
+
+
+def qwen2_5_7b_config(**kw) -> LlamaConfig:
+    """Qwen2.5-7B geometry: head_dim 128, 28 / 4 heads (GQA group 7), q / k / v bias, rope_theta 10⁶."""
+    return LlamaConfig(vocab_size=152064, hidden_size=3584, intermediate_size=18944, num_hidden_layers=28, num_attention_heads=28,
+                       num_key_value_heads=4, rope_theta=1e6, rms_norm_eps=1e-6, qkv_bias=True, **kw)
 
 
 def main():
     p = argparse.ArgumentParser()
-    p.add_argument("--model", default="tiny", choices=["tiny", "7b", "13b", "mistral-7b", "llama3.2-1b"],
-                   help="model geometry, random weights; llama3.2-1b runs without Llama-3 rope scaling")
+    p.add_argument("--model", default="tiny", choices=["tiny", "7b", "13b", "mistral-7b", "llama3.2-1b", "llama3.2-3b", "qwen2.5-7b"],
+                   help="model geometry, random weights; the Llama-3.2 geometries carry Llama-3 RoPE scaling, qwen2.5-7b q / k / v bias")
     p.add_argument("--tp_degree", type=int, default=1)
     p.add_argument("--batch_size", type=int, default=1)
     p.add_argument("--max_prompt_length", type=int, default=128)
@@ -79,7 +97,7 @@ def main():
     dtype = torch.bfloat16 if dev.type == "cuda" else torch.float32
     kw = dict(dtype=dtype, device=dev, max_position_embeddings=a.sequence_length)
     cfg = {"7b": llama2_7b_config, "13b": llama2_13b_config, "mistral-7b": mistral_7b_config,
-           "llama3.2-1b": llama3_2_1b_config}.get(a.model, lambda **k: LlamaConfig(
+           "llama3.2-1b": llama3_2_1b_config, "llama3.2-3b": llama3_2_3b_config, "qwen2.5-7b": qwen2_5_7b_config}.get(a.model, lambda **k: LlamaConfig(
         vocab_size=4096, hidden_size=512, intermediate_size=1408, num_hidden_layers=4, num_attention_heads=8, **k))(**kw)
     if a.num_layers > 0:
         cfg.num_hidden_layers = a.num_layers

@@ -101,8 +101,14 @@ def config_from_hf(hf_config: Any, **overrides):
                   tie_word_embeddings=bool(d.get("tie_word_embeddings", False)), pad_token_id=d.get("pad_token_id"))
         scaling = d.get("rope_parameters") or d.get("rope_scaling") or {}       # transformers>=5 keeps theta + scaling together
         kw["rope_theta"] = float(d.get("rope_theta") or scaling.get("rope_theta") or 10000.0)
-        if scaling.get("type", scaling.get("rope_type")) == "linear":
+        rope_type = scaling.get("type", scaling.get("rope_type"))
+        if rope_type == "linear":
             kw["rope_scaling_factor"] = float(scaling["factor"])
+        elif rope_type == "llama3":                  # Llama-3.1 / 3.2 frequency rescaling
+            kw["rope_scaling"] = {k: scaling[k] for k in ("factor", "low_freq_factor", "high_freq_factor",
+                                                          "original_max_position_embeddings")}
+        # Qwen2 biases q / k / v (not o_proj)
+        kw["qkv_bias"] = str(d.get("model_type", "")).lower() == "qwen2"
         cls = LlamaConfig
         if str(d.get("model_type", "")).lower() in ("mistral", "mixtral"):
             # Mistral / Mixtral attend within a sliding window (None: full attention).  Qwen2 carries the field too but

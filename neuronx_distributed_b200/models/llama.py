@@ -40,6 +40,11 @@ class LlamaConfig:
     rms_norm_eps: float = 1e-5
     rope_theta: float = 10000.0
     rope_scaling_factor: float = 1.0
+    # Llama-3.1 / 3.2 frequency rescaling: the "llama3" keys of a Hugging Face rope_scaling (factor, low_freq_factor,
+    # high_freq_factor, original_max_position_embeddings); None = plain RoPE
+    rope_scaling: Optional[dict] = None
+    # bias on the q / k / v projections (Qwen2); o_proj has none
+    qkv_bias: bool = False
     initializer_range: float = 0.02
     tie_word_embeddings: bool = False
     sequence_parallel_enabled: bool = False
@@ -122,7 +127,7 @@ class LlamaAttention(nn.Module):
         self.qkv_proj = GQAQKVColumnParallelLinear(
             cfg.hidden_size,
             [cfg.num_attention_heads * self.head_dim, cfg.num_key_value_heads * self.head_dim],
-            bias=False, gather_output=False, init_method=init, sequence_parallel_enabled=sp,
+            bias=cfg.qkv_bias, gather_output=False, init_method=init, sequence_parallel_enabled=sp,
             kv_size_multiplier=kv_mult, fuse_qkv=cfg.fuse_qkv, dtype=cfg.dtype, sequence_dimension=0,
             head_dim=self.head_dim, device=cfg.device,
         )
@@ -236,7 +241,7 @@ class LlamaModel(nn.Module):
         c = self._rope_cache
         if c is None or c[0] != seq_len or c[1] != offset or c[2] != device:
             cos, sin = ops.rope.rope_tables(seq_len, self.cfg.head_dim, self.cfg.rope_theta, device, offset,
-                                            self.cfg.rope_scaling_factor)
+                                            self.cfg.rope_scaling_factor, self.cfg.rope_scaling)
             self._rope_cache = (seq_len, offset, device, cos, sin)
             c = self._rope_cache
         return c[3], c[4]
@@ -255,7 +260,8 @@ class LlamaModel(nn.Module):
             zz = self.__dict__.get("_rope_cache_zz")
             if zz is None or zz[0] != (S, r, cp, input_ids.device):
                 tabs = [ops.rope.rope_tables(c, self.cfg.head_dim, self.cfg.rope_theta, input_ids.device, off,
-                                             self.cfg.rope_scaling_factor) for off in (r * c, (2 * cp - 1 - r) * c)]
+                                             self.cfg.rope_scaling_factor, self.cfg.rope_scaling)
+                        for off in (r * c, (2 * cp - 1 - r) * c)]
                 zz = ((S, r, cp, input_ids.device), torch.cat([tabs[0][0], tabs[1][0]]), torch.cat([tabs[0][1], tabs[1][1]]))
                 self.__dict__["_rope_cache_zz"] = zz
             cos, sin = zz[1], zz[2]

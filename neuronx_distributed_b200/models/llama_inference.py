@@ -75,7 +75,7 @@ class LlamaForInference(nn.Module):
     def _rope_tables(self, max_seq_len: int):
         """``(cos, sin) [max_seq_len, R/2]``: the rotary width R is twice the tables' width (R = head_dim here)."""
         c = self.cfg
-        return ops.rope.rope_tables(max_seq_len, c.head_dim, c.rope_theta, c.device, 0, c.rope_scaling_factor)
+        return ops.rope.rope_tables(max_seq_len, c.head_dim, c.rope_theta, c.device, 0, c.rope_scaling_factor, c.rope_scaling)
 
     def _logits(self, h: torch.Tensor) -> torch.Tensor:
         return self.lm.lm_head(h)

@@ -53,17 +53,17 @@ def _local_partial(q_all: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Te
 
     An fp8 cache holds k / ``k_scale`` and v / ``v_scale`` (one scale per tensor).
 
-    CUDA / bf16 q / bf16 or e4m3 cache / head_dim in ``FLASH_HEAD_DIMS``: the split-KV decode kernel (``csrc/decode.cu`` ``decode_attn_kernel`` +
-    the partial combine): K/V are read once per KV head for the whole GQA group.  Otherwise fp32 torch math."""
+    CUDA / bf16 q / bf16 or e4m3 cache / head_dim in ``FLASH_HEAD_DIMS`` / H / Hkv in ``DECODE_GQA_GROUPS``: the split-KV
+    decode kernel (``csrc/decode.cu`` ``decode_attn_kernel`` + the partial combine): K/V are read once per KV head for the whole GQA group.  Otherwise fp32 torch math."""
     from ...ops import _ext
-    from ...ops.attention import FLASH_HEAD_DIMS, check_kv_scales, check_window, speculation_visibility
+    from ...ops.attention import DECODE_GQA_GROUPS, FLASH_HEAD_DIMS, check_kv_scales, check_window, speculation_visibility
 
     window = check_window(sliding_window)
     kw = check_kv_scales(k_cache, v_cache, k_scale, v_scale)
     B, _, H, D = q_all.shape
     l_local, Hkv = k_cache.shape[1], k_cache.shape[2]
     if (_ext.use_cuda(q_all, k_cache, v_cache) and q_all.dtype == torch.bfloat16 and k_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn)
-            and D in FLASH_HEAD_DIMS and H % Hkv == 0 and (H // Hkv) in (1, 2, 4, 8) and hasattr(_ext.ext(), "decode_attention_partial")):
+            and D in FLASH_HEAD_DIMS and H % Hkv == 0 and (H // Hkv) in DECODE_GQA_GROUPS and hasattr(_ext.ext(), "decode_attention_partial")):
         _ext.count_launch(2)
         o, ml = _ext.ext().decode_attention_partial(q_all.contiguous(), k_cache, v_cache, local_pos.to(torch.long).contiguous(),
                                                     float(scale), window, **kw)

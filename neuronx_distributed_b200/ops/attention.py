@@ -24,6 +24,10 @@ from . import _ext
 #: head sizes the flash kernels are compiled for
 FLASH_HEAD_DIMS = (64, 80, 96, 128)
 
+#: GQA group sizes H / Hkv the token-generation kernels (decode, flash-decoding, verification) are compiled for; they keep
+#: the group's query rows in registers, so larger groups take :func:`speculation_attention_torch`
+DECODE_GQA_GROUPS = (1, 2, 3, 4, 5, 6, 7, 8)
+
 #: fp8 KV-cache dtypes: stored as k / k_scale and v / v_scale, de-quantised off the kernels (the decode kernels read e4m3)
 FP8_KV_DTYPES = (torch.float8_e4m3fn, torch.float8_e5m2)
 
@@ -335,7 +339,7 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     e = _ext.ext() if q.is_cuda else None
     if (e is not None and hasattr(e, "decode_attention") and D in FLASH_HEAD_DIMS and q.dtype == torch.bfloat16
-            and k_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn) and H // Hkv in (1, 2, 4, 8) and k_cache.stride(3) == 1
+            and k_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn) and H // Hkv in DECODE_GQA_GROUPS and k_cache.stride(3) == 1
             and v_cache.stride(3) == 1):
         _ext.count_launch(2)
         return e.decode_attention(q.contiguous(), k_cache, v_cache, positions.to(torch.long).contiguous(), float(scale), window,
@@ -427,7 +431,7 @@ def speculation_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch
     rows holding slot c in row c mod L (``KVCacheManager`` in rolling mode); needs SW > 0 and SW + W − 1 ≤ L, and the rule
     above then applies to logical slots without the bound at L.
 
-    CUDA bf16 q with a head_dim in :data:`FLASH_HEAD_DIMS`, W ≤ 64, H / Hkv ∈ {1, 2, 4, 8} and a bf16 or fp8 e4m3 cache whose
+    CUDA bf16 q with a head_dim in :data:`FLASH_HEAD_DIMS`, W ≤ 64, H / Hkv in :data:`DECODE_GQA_GROUPS` and a bf16 or fp8 e4m3 cache whose
     rows are aligned as :func:`decode_attention` needs: the kernel in ``csrc/attention_sm90.cu``, which reads each K / V
     row once for all W tokens and the GQA group, reads e4m3 as stored, and with a window only the slots some token can see.
     ``tree_mask`` and ``tree_depth`` are never read on the host there, so the call can be captured in a CUDA graph.  Otherwise
@@ -441,7 +445,7 @@ def speculation_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch
     align = 16 if k_cache.dtype == torch.bfloat16 else 8
     if (e is not None and hasattr(e, "speculation_attention") and D in FLASH_HEAD_DIMS and q.dtype == torch.bfloat16
             and k_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn) and W <= SPEC_MAX_TOKENS
-            and H // k_cache.shape[2] in (1, 2, 4, 8)
+            and H // k_cache.shape[2] in DECODE_GQA_GROUPS
             and all(t.stride(3) == 1 and t.data_ptr() % align == 0 and all(s % 8 == 0 for s in t.stride()[:3])
                     for t in (k_cache, v_cache))):
         if tree_mask is not None:

@@ -7,6 +7,8 @@ fp32 (position ``s`` of the *global* sequence; callers slice for CP/SP offsets).
 """
 from __future__ import annotations
 
+from typing import Optional
+
 import torch
 
 from . import _ext
@@ -51,8 +53,16 @@ def apply_rotary(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch
 
 
 def rope_tables(seq_len: int, dim: int, base: float = 10000.0, device=None, offset: int = 0,
-                scaling: float = 1.0):
+                scaling: float = 1.0, rope_scaling: Optional[dict] = None):
+    """cos / sin ``[seq_len, dim/2]`` fp32 for positions ``offset ..``.  ``scaling``: linear position scaling.
+    ``rope_scaling``: Llama-3 frequency rescaling (the ``"llama3"`` keys of a Hugging Face ``rope_scaling``: ``factor``,
+    ``low_freq_factor``, ``high_freq_factor``, ``original_max_position_embeddings``), applied to the inverse frequencies
+    by :func:`~neuronx_distributed_b200.modules.attention.utils.apply_scaling`."""
     inv = 1.0 / (base ** (torch.arange(0, dim, 2, dtype=torch.float32, device=device) / dim))
+    if rope_scaling is not None:
+        from ..modules.attention.utils import apply_scaling      # not at module level: ``modules`` imports ``ops``
+
+        inv = apply_scaling(inv, **rope_scaling)
     t = (torch.arange(offset, offset + seq_len, dtype=torch.float32, device=device)) / scaling
     fr = torch.outer(t, inv)
     return fr.cos(), fr.sin()

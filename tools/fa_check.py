@@ -1,6 +1,6 @@
 """Numerics + timing of the flash-attention kernels against a plain fp32 PyTorch reference and SDPA (cuDNN).
 usage: python tools/fa_check.py [--head-dim 64|80|96|128] [--perf] [--bwd] [--window [--cp N]] [--kv-fp8] [--spec] [--rolling]
-                                [--decode-dims] [--dropout]
+                                [--decode-dims] [--decode-groups] [--dropout]
 
 --perf times forward and forward+backward of the own kernels and of SDPA in the same process, alternating, at the shapes
 the models run (BERT-large with right padding, ViT-B/16, GPT-NeoX-20B per rank at TP=8, Pythia-2.8B, Llama-2-7B).  FLOPs
@@ -45,6 +45,10 @@ kernel on a Mistral-7B head geometry (H 32, Hkv 8) as the control; B = 1, 8, 32,
 card), bf16 and e4m3 caches holding the same values, one-token decode, a 5-token chain and a random 64-node tree.  GB/s is
 the K and V bytes of the visible cache rows (from the shapes) over the time of the call.  The D = 128 control's torch path
 is timed only at B = 1 (it is the one the kernels have replaced since they exist).  The partial at B = 8, L = 4096.
+
+--decode-groups (with --perf) times the same table at the GQA groups 3, 5, 6 and 7 the kernels took from the torch path:
+Llama-3.2-3B (H 24, Hkv 8), Qwen2.5-14B (H 40, Hkv 8), Qwen2.5-1.5B (H 12, Hkv 2), Qwen2.5-7B (H 28, Hkv 4) and its TP = 4
+shard (H 7, Hkv 1) at D = 128, and Qwen2.5-0.5B (H 14, Hkv 2, D 64); the torch path is timed at every shape.
 
 --dropout (with --perf) times attention dropout: the own kernels at p = 0.1 against the same kernels at p = 0 and against
 SDPA with dropout_p = 0.1, forward and (with --bwd) forward + backward, alternating in one process, at the BERT-large
@@ -425,16 +429,28 @@ DECODE_DIM_SHAPES = [
 ]
 
 
-def decode_dims_perf():
+# name, H, Hkv, D: the GQA groups 3, 5, 6 and 7 of --decode-groups
+DECODE_GROUP_SHAPES = [
+    ("llama3.2_3b", 24, 8, 128),
+    ("qwen2.5_14b", 40, 8, 128),
+    ("qwen2.5_1.5b", 12, 2, 128),
+    ("qwen2.5_7b", 28, 4, 128),
+    ("qwen2.5_7b_tp4", 7, 1, 128),
+    ("qwen2.5_0.5b", 14, 2, 64),
+]
+
+
+def decode_dims_perf(shapes=DECODE_DIM_SHAPES, time_old=lambda D, B: D != 128 or B == 1):
     """Decode, verification and flash decoding's partial at head_dim 64 / 80 / 96 (and the D = 128 control) on the kernels
-    against the torch paths those head sizes took before, alternating in one process, on a full cache (p = L − W)."""
+    against the torch paths those head sizes took before, alternating in one process, on a full cache (p = L − W).
+    ``shapes`` / ``time_old(D, B)``: the geometries, and where the torch path is timed (--decode-groups: all of them)."""
     from neuronx_distributed_b200.modules.attention.flash_decode import _local_partial
 
     dev = torch.device("cuda")
     print(json.dumps(gpu_info()), flush=True)
     ks, vs = 0.05, 0.05
     windows = [(n, m, d, W) for n, m, d, W in spec_windows(dev) if n != "tree10"]
-    for name, H, Hkv, D in DECODE_DIM_SHAPES:
+    for name, H, Hkv, D in shapes:
         for L in (4096, 32768):
             for B in (1, 8, 32):
                 if 2 * B * L * Hkv * D * 2 > 24 * 2 ** 30:                 # bf16 + e4m3 + de-quantised copies must fit
@@ -462,18 +478,18 @@ def decode_dims_perf():
                         n0 = _ext.launches()
                         o_new = new()
                         assert _ext.launches() == n0 + 2, "the kernel did not run"
-                        time_old = D != 128 or B == 1
+                        timed_old = time_old(D, B)
                         t = {"new": [], "old": []}
                         iters = 20 if B * L <= 32768 else 5
                         rec = {"bench": f"{name}_{wname}", "cache": cache, "B": B, "L": L, "H": H, "Hkv": Hkv, "D": D, "W": W}
-                        if time_old:
+                        if timed_old:
                             o_old = old()
                             rec["rel_err_vs_old"] = round(((o_new.float() - o_old.float()).abs().max()
                                                            / o_old.float().abs().max()).item(), 5)
                             del o_old
                         for _ in range(3):                         # alternate, keep each one's best
                             t["new"].append(time_fn(new, iters))
-                            if time_old:
+                            if timed_old:
                                 t["old"].append(time_fn(old, iters))
                         elt = 2 if cache == "bf16" else 1
                         rec["kv_bytes"] = nbytes = 2 * B * L * Hkv * D * elt        # K and V rows, each read once
@@ -662,6 +678,8 @@ def main():
     ap.add_argument("--rolling", action="store_true", help="with --perf: decode / verification on rolling vs linear KV caches")
     ap.add_argument("--decode-dims", action="store_true",
                     help="with --perf: decode / verification / flash-decoding partial at head_dim 64, 80, 96 vs the torch path")
+    ap.add_argument("--decode-groups", action="store_true",
+                    help="with --perf: decode / verification / flash-decoding partial at GQA groups 3, 5, 6, 7 vs the torch path")
     ap.add_argument("--dropout", action="store_true", help="with --perf: attention dropout p = 0.1 vs p = 0 and SDPA")
     ap.add_argument("--head-dim", type=int, default=128, choices=attention.FLASH_HEAD_DIMS)
     a = ap.parse_args()
@@ -731,6 +749,8 @@ def main():
             rolling_perf()
         elif a.decode_dims:
             decode_dims_perf()
+        elif a.decode_groups:
+            decode_dims_perf(DECODE_GROUP_SHAPES, lambda D, B: True)
         elif a.dropout:
             dropout_perf(e, a.bwd)
         elif a.window and a.cp > 1:
