@@ -775,6 +775,11 @@ void gemm_bf16(const void* a, const void* b, void* out, int M, int N, int K, boo
   if (comm.mode != 0) {
     if (c.rows_per_rank % BLOCK_M || M % comm.world) nxd_throw("fused TP GEMM needs rows/rank % 128 == 0", __FILE__, __LINE__);
     if (comm.mode == 2 && (N % 8)) nxd_throw("GEMM→RS needs N % 8 == 0", __FILE__, __LINE__);
+    if (comm.mode == 1) {
+      if (N % 8 || K % 8) nxd_throw("AG→GEMM needs N and K multiples of 8", __FILE__, __LINE__);
+      // no pusher: the GEMM CTAs wait for the shards forever; no GEMM CTA: nothing is computed
+      if (comm.comm_sms < 1 || comm.comm_sms >= sms) nxd_throw("AG→GEMM: comm_sms must leave GEMM CTAs", __FILE__, __LINE__);
+    }
   }
 #define NXD_LAUNCH(AKv, BKv)                                                                                          \
   do {                                                                                                                \

@@ -34,6 +34,16 @@ _FLAGS_AG = 0
 _FLAGS_RS = 2048
 _NFLAGS = 4096
 _COMM_SMS = int(os.environ.get("NXD_AG_COMM_SMS", "16"))     # CTAs (of one per SM) that only push the all-gather
+
+
+def checked_comm_sms(comm_sms: int, sm_count: int) -> int:
+    """``comm_sms`` if the cudaIpc all-gather→GEMM (one CTA per SM) can run with that many pushing CTAs, else ``ValueError``:
+    with none, nobody pushes and the GEMM CTAs wait for the shards forever; with ``sm_count`` or more, no CTA computes."""
+    if not 1 <= int(comm_sms) < int(sm_count):
+        raise ValueError(f"NXD_AG_COMM_SMS={comm_sms}: the fused all-gather→GEMM needs 1 <= comm CTAs < {sm_count} (the SM count)")
+    return int(comm_sms)
+
+
 # NVLS variants (MODE 5 / 6 of csrc/gemm_sm90.cu): "1" = use them when the TP group's symmetric region got a multicast mapping (default),
 # "0" = never, "force" = also without multicast (unicast fallback inside the same kernels; loopback tests of the protocol).
 _NVLS_MODE = os.environ.get("NXD_TP_NVLS", "1")
@@ -215,28 +225,16 @@ class TPWorkspace:
             return self.ag_gemm_nvls(a_shard, b, trans_b)
         if ms // BLOCK_M > MAX_ROW_BLOCKS:
             raise RuntimeError(f"fused AG→GEMM without NVLS supports at most {MAX_ROW_BLOCKS * BLOCK_M} rows per rank (got {ms})")
+        comm_sms = checked_comm_sms(_COMM_SMS, torch.cuda.get_device_properties(a_shard.device).multi_processor_count)
         self._ensure(M * K * 2, 0)
         self.ag_epoch += 1
         off = (self.ag_epoch & 1) * self.ag_bytes
         out = torch.empty(M, N, dtype=out_dtype, device=a_shard.device)
         _ext.count_launch()
         _ext.ext().ag_gemm_bf16(a_shard, b, out, trans_b, self.ws.local_ptr, self.ws.ptrs, self.ws.flag_ptrs, off, _FLAGS_AG,
-                                self.ag_epoch, self.rank, self.world, _COMM_SMS)
+                                self.ag_epoch, self.rank, self.world, comm_sms)
         gathered = self.ws.local_tensor(off, (M, K), torch.bfloat16)
         return out, gathered
-
-    def _poison(self, off: int, nbytes: int) -> None:
-        """NXD_SYMM_POISON=1: NaN-fill the payload half that is NOT live, so any read of stale-epoch data shows up as NaN.
-        Safe with respect to peers: a rank only reaches call n+1 (which writes that half on its peers) after every peer has
-        finished call n-1, and the fill is stream-ordered before this rank's own call n+1."""
-        from ..utils.profiling import poison_enabled
-
-        if poison_enabled() and self.world > 1:
-            torch.cuda.synchronize()
-            dist.barrier(group=self.group)       # debug mode: make the fill race-free by construction
-            self.ws.local_tensor(off, (nbytes // 2,), torch.bfloat16).fill_(float("nan"))
-            torch.cuda.synchronize()
-            dist.barrier(group=self.group)
 
     # ------------------------------------------------------------------ GEMM → reduce-scatter
     def gemm_rs(self, a: torch.Tensor, b: torch.Tensor, trans_b: bool, gemm_join: bool = True) -> torch.Tensor:
@@ -445,6 +443,12 @@ def select(x: torch.Tensor, weight: torch.Tensor, in_mode: str, out_mode: str, s
     def no(reason: str):
         _log_once(f"{kind}:{reason}", f"fused {kind} TP linear not used ({reason}): falling back to NCCL collective + plain GEMM")
         return None
+
+    # Before anything that synchronises or allocates (workspace, nvls_enabled), which a capture forbids.  The kernels take
+    # their epochs, counter targets and claim base from the host at launch: a replayed graph would repeat them, find the
+    # flags already past them, and read stale partials without waiting (MODE 6 would claim no reduction item at all).
+    if torch.cuda.is_current_stream_capturing():
+        return no("CUDA graph capture: the fused kernels take host-side epochs that a replay would repeat")
 
     if x.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16:
         return no(f"dtype {x.dtype}/{weight.dtype}, kernels are bf16")

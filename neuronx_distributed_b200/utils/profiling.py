@@ -4,9 +4,6 @@
   are bracketed so Nsight timelines show the schedule.  The reference's only timeline is a host-clock Chrome trace that is
   force-disabled (``pipeline/model.py:336-339``).
 * ``device_timer()`` — CUDA-event stopwatch (device time, not host time) for step / phase timing.
-* ``poison_enabled()`` — ``NXD_SYMM_POISON=1`` debug mode of the peer-memory kernels: after every fused call the payload half that
-  the *next-but-one* call will reuse is filled with NaN, so a consumer that reads data from a stale epoch (a protocol bug)
-  produces NaNs immediately instead of plausible numbers.
 """
 from __future__ import annotations
 
@@ -56,7 +53,3 @@ class device_timer:
             import time
             self.ms = (time.perf_counter() - self._t0) * 1e3
         return False
-
-
-def poison_enabled() -> bool:
-    return os.environ.get("NXD_SYMM_POISON", "0") == "1"

@@ -11,6 +11,7 @@ import torch
 import torch.multiprocessing as mp
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+FLT_MIN = 2.0 ** -126                           # smallest normal fp32 (and bf16)
 
 
 def _free_port() -> int:
@@ -77,3 +78,74 @@ def run_distributed(fn, world: int, *args, use_cuda: bool = False, timeout: floa
     assert not alive, "distributed test timed out"
     for p in procs:
         assert p.exitcode == 0, f"worker exit code {p.exitcode}"
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Bit-exact checks of the peer-memory kernels run by loopback workers: inputs from seeds, fp32 emulation in a given order,
+# bit comparison, failures collected until every rank has made its whole call sequence
+# ---------------------------------------------------------------------------------------------------------------------
+def _randn(n, seed, dtype, spread=12):
+    """``n`` normal numbers of ``dtype``: Gaussian times 2^k, k uniform in [-spread, spread], so that fp32 sums of a few of
+    them round and the summation order shows in the last bit."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    x = torch.randn(n, device="cuda", generator=g)
+    if spread:
+        x = x * torch.exp2(torch.randint(-spread, spread + 1, (n,), device="cuda", generator=g).float())
+    x = x.to(dtype)
+    return torch.where(x.float().abs() < FLT_MIN, torch.ones_like(x), x)
+
+
+def _emulate(parts, order):
+    """fp32 sum of ``parts[p]`` for p in ``order``, starting from +0, inputs flushed to zero below FLT_MIN as the kernels'
+    FTZ adds do."""
+    acc = torch.zeros(parts[0].shape, dtype=torch.float32, device=parts[0].device)
+    for p in order:
+        x = parts[p].float()
+        acc = acc + torch.where(x.abs() < FLT_MIN, torch.zeros_like(x), x)
+    return acc
+
+
+def _bits(t):
+    return t.contiguous().view({1: torch.uint8, 2: torch.int16, 4: torch.int32}[t.element_size()])
+
+
+def _same(a, b):
+    """Bit for bit, except that any NaN equals any NaN (the payload is not compared)."""
+    if a.shape != b.shape or a.dtype != b.dtype:
+        return False
+    an, bn = torch.isnan(a), torch.isnan(b)
+    return torch.equal(an, bn) and torch.equal(_bits(a)[~an], _bits(b)[~bn])
+
+
+def _first_diff(a, b):
+    a, b = a.reshape(-1), b.reshape(-1)
+    d = (_bits(a) != _bits(b)).nonzero().reshape(-1)
+    if d.numel() == 0:
+        return "NaN positions differ"
+    i = int(d[0])
+    return f"{d.numel()} elements differ, first at {i}: {a[i].item()!r} vs {b[i].item()!r}"
+
+
+class _Checks:
+    """Collects failures instead of raising, so that no rank leaves the call sequence early (its peers would wait on its
+    flags); ``settle`` compares the failures of all ranks over gloo and raises on every rank if there is one."""
+
+    def __init__(self):
+        self.errs = []
+
+    def same(self, got, want, what):
+        if not _same(got, want):
+            self.errs.append(f"{what}: {_first_diff(got, want) if got.shape == want.shape else 'shape/dtype'}")
+
+    def true(self, ok, what):
+        if not ok:
+            self.errs.append(what)
+
+    def settle(self):
+        import torch.distributed as dist
+
+        torch.cuda.synchronize()
+        every = [None] * dist.get_world_size()
+        dist.all_gather_object(every, self.errs)
+        bad = [f"rank {r}: {e}" for r, es in enumerate(every) for e in es]
+        assert not bad, "\n".join(bad[:40])

@@ -1,8 +1,8 @@
-"""Single-GPU loopback: TWO processes on cuda:0 run the cross-rank kernels against each other (the driver's 1-GPU `pytest -m gpu`
-then exercises the flag / epoch protocols of the fused TP kernels, the NVLS-layout collectives and the symmetric-memory
-exchange instead of skipping them).  No multicast mapping exists between two contexts of one device, so the NVLS kernels run
-their unicast fallback (same protocol, peer pointers instead of the multicast address); the references are plain fp32 matmuls
-computed locally — every rank can rebuild all ranks' inputs from the seeds, no library collective is involved."""
+"""Single-GPU loopback: TWO processes on cuda:0 run the cross-rank kernels against each other (a one-GPU `pytest -m gpu`
+then exercises the flag / epoch protocols of the NVLS-layout collectives and the symmetric-memory exchange instead of
+skipping them; the fused TP GEMMs have their own file, test_tp_gemm_collectives_gpu.py).  No multicast mapping exists
+between two contexts of one device, so the NVLS kernels run their unicast fallback (same protocol, peer pointers instead of
+the multicast address); the references are plain fp32 matmuls computed locally — every rank can rebuild all ranks' inputs from the seeds, no library collective is involved."""
 import pytest
 import torch
 
@@ -49,45 +49,3 @@ def _symm_and_collectives(rank, world):
 
 def test_loopback_symmetric_memory_and_collectives():
     run_distributed(_symm_and_collectives, 2, use_cuda="loopback", timeout=240)
-
-
-def _fused_tp(rank, world):
-    import os
-
-    os.environ["NXD_TP_NVLS"] = "force"
-    os.environ["NXD_SYMM_MIN_MB"] = "1"                    # small floor: the shapes below force re-layouts of the region
-    import torch.distributed as dist
-
-    from neuronx_distributed_b200.ops import _fused_impl
-
-    _fused_impl._NVLS_MODE = "force"
-    ws = _fused_impl.workspace(dist.group.WORLD)
-    assert ws.nvls_enabled() and not ws.nv.has_multicast
-    for wire in ("bf16", "fp32"):
-        os.environ["NXD_TP_WIRE"] = wire
-        # (rows per rank, N, K, trans_b): trans_b=False is the [K, N] MN-major weight operand of the backward (dgrad)
-        cases = [(256, 512, 256, True), (512, 1000, 512, True), (256, 512, 256, True), (128, 384, 256, True),
-                 (128, 256, 384, False), (256, 512, 256, False)]
-        for it, (ms, N, K, tb) in enumerate(cases):
-            xs = [_inputs(r, (ms, K), 40 + it) for r in range(world)]
-            w = _inputs(0, (N, K) if tb else (K, N), 50 + it, 0.05)
-            wt = w.float().t() if tb else w.float()
-            out, gathered = ws.ag_gemm(xs[rank], w, tb)
-            full = torch.cat(xs)
-            assert torch.equal(gathered, full)
-            assert _relerr(out, full.float() @ wt) < 2e-2, (wire, it)
-            # GEMM → reduce-scatter: every rank has its own [world*ms, K] operand
-            a = [_inputs(r, (world * ms, K), 60 + it) for r in range(world)]
-            o = ws.gemm_rs(a[rank], w, tb)
-            ref = sum(x.float() @ wt for x in a)[rank * ms:(rank + 1) * ms]
-            assert _relerr(o, ref) < 2e-2, (wire, it)
-    os.environ["NXD_TP_WIRE"] = "bf16"
-    # a larger shape mid-stream re-lays the region out (barrier, epochs keep counting) and must keep working, first call included
-    xs = [_inputs(r, (2048, 1024), 70) for r in range(world)]
-    w = _inputs(0, (512, 1024), 71, 0.05)
-    out, _ = ws.ag_gemm(xs[rank], w, True)
-    assert _relerr(out, torch.cat(xs).float() @ w.float().t()) < 2e-2
-
-
-def test_loopback_fused_tp_kernels_vs_fp32_reference():
-    run_distributed(_fused_tp, 2, use_cuda="loopback", timeout=300)

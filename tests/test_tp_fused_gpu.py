@@ -7,10 +7,7 @@ from dist_utils import run_distributed
 pytestmark = [pytest.mark.gpu, pytest.mark.multigpu]
 
 
-def _fused_vs_nccl(rank, world, push="tma"):
-    import os
-
-    os.environ["NXD_TP_PUSH"] = push            # read per kernel call: tma (default) | ldst | stream
+def _fused_vs_nccl(rank, world):
     from neuronx_distributed_b200 import ops
     from neuronx_distributed_b200.parallel_layers import ColumnParallelLinear, RowParallelLinear
     from neuronx_distributed_b200.parallel_layers import parallel_state as ps
@@ -39,12 +36,6 @@ def _fused_vs_nccl(rank, world, push="tma"):
         err = float((a - b).abs().max() / (b.abs().max() + 1e-6))
         assert err < 3e-2, (name, err)
     assert ops._ext.launches() > 0
-
-
-@pytest.mark.parametrize("push", ["ldst", "stream"])
-def test_fused_tp_other_pusher_modes_match_nccl(push):
-    """The register-staged and the streaming (no drain between items) pushers implement the same protocol as the default."""
-    run_distributed(_fused_vs_nccl, 2, push, use_cuda=True, timeout=240)
 
 
 def test_fused_tp_matches_nccl():

@@ -75,25 +75,25 @@ def main():
     # optional sweep: comm-CTA split × micro-batch rows (fused kernels only)
     if "--sweep" in sys.argv:
         sweep = []
+        comm_sms0, nvls_config0 = _fused_impl._COMM_SMS, dict(_fused_impl.NVLS_CONFIG)
         for M in (4096, 16384):
             if (M // world) % 256 or M // world // 128 > 64:
                 continue
-            for push, ag, rs in (("tma", 12, 16), ("tma", 24, 24), ("tma", 32, 32), ("stream", 12, 16), ("stream", 24, 24),
-                                 ("stream", 32, 32), ("ldst", 12, 16)):
-                os.environ["NXD_TP_PUSH"] = push
-                _fused_impl.CONFIG["comm_ctas_ag"], _fused_impl.CONFIG["comm_ctas_rs"] = ag, rs
+            for ag, rs in ((12, 16), (24, 24), (32, 32)):
+                # cudaIpc kernels take the all-gather split from _COMM_SMS, the NVLS kernels both splits from NVLS_CONFIG
+                _fused_impl._COMM_SMS = _fused_impl.NVLS_CONFIG["comm_ctas_ag"] = ag
+                _fused_impl.NVLS_CONFIG["comm_ctas_rs"] = rs
                 x = torch.randn(M // world, H, device="cuda", dtype=torch.bfloat16)
                 w = torch.randn(2 * I // world, H, device="cuda", dtype=torch.bfloat16)
                 t_ag = timeit(lambda: ws.ag_gemm(x, w, True), iters=10, warmup=3)
                 x2 = torch.randn(M, I // world, device="cuda", dtype=torch.bfloat16)
                 w2 = torch.randn(H, I // world, device="cuda", dtype=torch.bfloat16)
                 t_rs = timeit(lambda: ws.gemm_rs(x2, w2, True), iters=10, warmup=3)
-                rec = {"sweep": True, "M": M, "push": push, "comm_ctas_ag": ag, "comm_ctas_rs": rs, "ag_gemm_gate_up_us": t_ag, "gemm_rs_down_us": t_rs}
+                rec = {"sweep": True, "M": M, "comm_ctas_ag": ag, "comm_ctas_rs": rs, "ag_gemm_gate_up_us": t_ag, "gemm_rs_down_us": t_rs}
                 sweep.append(rec)
                 if rank == 0:
                     print(json.dumps(rec), flush=True)
-        _fused_impl.CONFIG["comm_ctas_ag"], _fused_impl.CONFIG["comm_ctas_rs"] = 0, 0
-        os.environ["NXD_TP_PUSH"] = "tma"
+        _fused_impl._COMM_SMS, _fused_impl.NVLS_CONFIG = comm_sms0, nvls_config0
         res.append({"sweep": sweep})
     # raw collectives for reference
     x = torch.randn(S // world, H, device="cuda", dtype=torch.bfloat16)
