@@ -160,16 +160,51 @@ static void fused_adamw(const std::vector<Tensor>& p, const std::vector<Tensor>&
                    grad_scale.data_ptr<float>(), hf_form ? 1 : 0, stream());
 }
 
-static void gemm_fp8(const Tensor& a, const Tensor& b, Tensor out, const Tensor& scale_a, const Tensor& scale_b) {
+// out bf16 [M, N], or fp32 [M, N] that `accumulate` adds into (the fp8 weight gradient into an fp32 main_grad)
+static void gemm_fp8(const Tensor& a, const Tensor& b, Tensor out, const Tensor& scale_a, const Tensor& scale_b, bool accumulate) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kFloat8_e4m3fn && b.scalar_type() == at::kFloat8_e4m3fn);
-  TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && out.is_contiguous() && out.scalar_type() == at::kBFloat16);
+  TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && out.is_contiguous() &&
+              (out.scalar_type() == at::kBFloat16 || out.scalar_type() == at::kFloat));
+  TORCH_CHECK(!accumulate || out.scalar_type() == at::kFloat, "gemm_fp8: accumulate needs an fp32 out");
+  // the register epilogue (out without a 16-byte aligned tensor map) stores element pairs
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(out.data_ptr()) % (2 * out.element_size()) == 0,
+              "gemm_fp8: out must start aligned to two elements");
   const int M = a.size(0), K = a.size(1), N = b.size(0);
   TORCH_CHECK(b.size(1) == K && out.size(0) == M && out.size(1) == N && K % 16 == 0 && N % 8 == 0);
   TORCH_CHECK(scale_a.scalar_type() == at::kFloat && scale_a.numel() == M && scale_b.scalar_type() == at::kFloat &&
               scale_b.numel() == N && scale_a.is_contiguous() && scale_b.is_contiguous());
   c10::cuda::CUDAGuard guard(a.device());
   nxd::gemm_fp8(a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, scale_a.data_ptr<float>(), scale_b.data_ptr<float>(),
-                stream());
+                dt_code(out), accumulate, stream());
+}
+
+// x bf16 [M, K] → (e4m3 [M, K], fp32 [M]): one absmax scale per row
+static std::vector<Tensor> quantize_fp8_rows(const Tensor& x) {
+  CHECK_IN(x);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.size(1) % 8 == 0, "quantize_fp8_rows: bf16 [M, K], K % 8 == 0");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "quantize_fp8_rows: x must start 16-byte aligned");
+  const int M = x.size(0), K = x.size(1);
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor q = at::empty({M, K}, x.options().dtype(at::kFloat8_e4m3fn));
+  Tensor s = at::empty({M}, x.options().dtype(at::kFloat));
+  nxd::quantize_fp8_rows(x.data_ptr(), q.data_ptr(), s.data_ptr<float>(), M, K, stream());
+  return {q, s};
+}
+
+// x bf16 [R, C] → (e4m3 [C, R], fp32 [C]): the rows of xᵀ, one absmax scale per column of x
+static std::vector<Tensor> quantize_fp8_cols_t(const Tensor& x) {
+  CHECK_IN(x);
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.size(0) % 16 == 0 && x.size(1) % 8 == 0,
+              "quantize_fp8_cols_t: bf16 [R, C], R % 16 == 0 (the e4m3 rows are a TMA operand) and C % 8 == 0");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "quantize_fp8_cols_t: x must start 16-byte aligned");
+  const int R = x.size(0), C = x.size(1);
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor q = at::empty({C, R}, x.options().dtype(at::kFloat8_e4m3fn));
+  Tensor s = at::empty({C}, x.options().dtype(at::kFloat));
+  Tensor amax = at::zeros({C}, x.options().dtype(at::kInt));
+  nxd::quantize_fp8_cols_t(x.data_ptr(), q.data_ptr(), s.data_ptr<float>(), reinterpret_cast<uint32_t*>(amax.data_ptr<int>()),
+                           R, C, stream());
+  return {q, s};
 }
 
 // a e4m3 [M, K], b e4m3 [N, K]; scale_a fp32 [K/group, M] with unit column stride (row stride >= M, a multiple of 4);
@@ -980,10 +1015,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("row_topk_supported", &row_topk_supported);
   m.def("gemv", &gemv, py::arg("x"), py::arg("w"), py::arg("residual") = py::none(), py::kw_only(), py::arg("bias") = py::none(),
         py::arg("act") = 0);
-  m.def("gemm_fp8", &gemm_fp8);
+  m.def("gemm_fp8", &gemm_fp8, py::arg("a"), py::arg("b"), py::arg("out"), py::arg("scale_a"), py::arg("scale_b"),
+        py::arg("accumulate") = false);
   m.def("gemm_fp8_block", &gemm_fp8_block);
   m.def("grouped_gemm_fp8_block", &grouped_gemm_fp8_block);
   m.def("quantize_fp8_groups", &quantize_fp8_groups);
+  m.def("quantize_fp8_rows", &quantize_fp8_rows);
+  m.def("quantize_fp8_cols_t", &quantize_fp8_cols_t);
   m.def("grouped_gemm", &grouped_gemm);
   m.def("grouped_wgrad", &grouped_wgrad);
   m.def("flash_attn_fwd", &flash_attn_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("causal"), py::arg("scale"),

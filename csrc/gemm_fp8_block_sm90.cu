@@ -28,6 +28,7 @@
 #include <cuda_fp8.h>
 
 #include "common.cuh"
+#include "fp8_rule.cuh"
 #include "kernels.h"
 #include "sm90_ptx.cuh"
 
@@ -191,20 +192,9 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_co
 // scales of the group-major scale buffer.
 //
 // Non-finite input: a group holding a NaN, or ±inf with no clamp, gets a NaN scale and NaN codes, so every output that reads
-// it is NaN.  fmaxf / fminf return the other operand when one is NaN, which would turn NaN into a finite code (and the MX
-// exponent of an infinite amax overflows the int shift into a finite scale), so the clamp, the amax and its shuffle
-// reduction use the NaN-propagating forms; their .ftz matches what fmaxf / fminf compile to under --use_fast_math.
-NXD_DEVICE float max_nan(float a, float b) {
-  float r;
-  asm("max.ftz.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-  return r;
-}
-NXD_DEVICE float min_nan(float a, float b) {
-  float r;
-  asm("min.ftz.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-  return r;
-}
-
+// it is NaN (the clamp, the amax and its shuffle reduction propagate NaN: fp8_rule.cuh; the MX exponent of an infinite amax
+// would overflow the int shift into a finite scale, so it is tested first).  The absmax scale and the codes are the shared
+// rule of fp8_rule.cuh.
 template <int G, bool MX>
 __global__ void __launch_bounds__(256)
 quantize_fp8_groups_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q, float* __restrict__ s, int M, int K,
@@ -234,23 +224,22 @@ quantize_fp8_groups_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restr
   for (int off = 1; off < G / 8; off <<= 1) amax = max_nan(amax, __shfl_xor_sync(0xffffffffu, amax, off));
   if (!live) return;
   float scale;
-  if (!(amax <= 3.402823466e38f)) {
-    scale = __int_as_float(0x7fffffff);                        // NaN, or ±inf with no clamp: NaN scale, NaN codes
-  } else if constexpr (MX) {
-    // OCP MX: 2^(floor(log2 amax) - 8), amax clamped to 2^-100; log2 rounded to fp32 first, as the torch quantiser does.
-    // amax is finite here, so -100 <= e <= 127 and the biased exponent e - 8 + 127 is in [19, 246]: no overflow
-    const float e = floorf((float)log2((double)fmaxf(amax, 0x1p-100f)));
-    scale = __int_as_float(((int)e - 8 + 127) << 23);
+  if constexpr (MX) {
+    if (!e4m3_amax_finite(amax)) {
+      scale = __int_as_float(0x7fffffff);                      // NaN, or ±inf with no clamp: NaN scale, NaN codes
+    } else {
+      // OCP MX: 2^(floor(log2 amax) - 8), amax clamped to 2^-100; log2 rounded to fp32 first, as the torch quantiser does.
+      // amax is finite here, so -100 <= e <= 127 and the biased exponent e - 8 + 127 is in [19, 246]: no overflow
+      const float e = floorf((float)log2((double)fmaxf(amax, 0x1p-100f)));
+      scale = __int_as_float(((int)e - 8 + 127) << 23);
+    }
   } else {
-    // torch evaluates `amax / 448` on a CUDA tensor as a product with the rounded reciprocal: the same here, bit for bit
-    scale = fmaxf(amax * (1.f / 448.f), 1e-12f);
+    scale = e4m3_absmax_scale(amax);
   }
-  // true division (not a reciprocal multiply) so the codes are bit-identical to the torch quantisers
   uint32_t lo = 0, hi = 0;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    const float c = min_nan(max_nan(__fdiv_rn(v[i], scale), -448.f), 448.f);   // NaN → the e4m3 NaN code 0x7F
-    const uint32_t b = (uint32_t)__nv_cvt_float_to_fp8(c, __NV_SATFINITE, __NV_E4M3);
+    const uint32_t b = e4m3_code(v[i], scale);
     if (i < 4) lo |= b << (8 * i); else hi |= b << (8 * (i - 4));
   }
   *(uint2*)(q + (size_t)row * K + col) = make_uint2(lo, hi);

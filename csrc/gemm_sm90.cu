@@ -837,17 +837,21 @@ void grouped_wgrad_bf16(const void* a, const void* b, void* out, int rows_total,
   else launch<false, false, 4, float>(ta, tb, out, Mo, No, rows_total, accumulate, c, grid, st);
 }
 
-// out[M,N] (bf16) = (a_e4m3[M,K] · b_e4m3[N,K]ᵀ) ∘ scale_a[M] ⊗ scale_b[N]   (quantised inference linear)
+// out[M,N] = (a_e4m3[M,K] · b_e4m3[N,K]ᵀ) ∘ scale_a[M] ⊗ scale_b[N]: bf16 (quantised linears), or fp32 (the fp8 weight
+// gradient), which `accumulate` adds into (TMA reduce-add at L2 when out's tensor map fits, else the register epilogue)
 void gemm_fp8(const void* a, const void* b, void* out, int M, int N, int K, const float* scale_a, const float* scale_b,
-              cudaStream_t st) {
+              int out_dt, bool accumulate, cudaStream_t st) {
   if (K % 16) nxd_throw("fp8 GEMM needs K % 16 == 0", __FILE__, __LINE__);
+  if (out_dt != kBF16 && out_dt != kF32) nxd_throw("fp8 GEMM writes bf16 or fp32", __FILE__, __LINE__);
+  if (accumulate && out_dt != kF32) nxd_throw("fp8 GEMM accumulates into fp32 only", __FILE__, __LINE__);
   const CUtensorMap ta = make_tmap_u8(a, M, K, BLOCK_M);
   const CUtensorMap tb = make_tmap_u8(b, N, K, BLOCK_N);
   CommDev c{};
   c.scale_a = scale_a; c.scale_b = scale_b;
   const int tiles = ((M + BLOCK_M - 1) / BLOCK_M) * ((N + BLOCK_N - 1) / BLOCK_N);
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  launch<true, true, 0, __nv_bfloat16, true>(ta, tb, out, M, N, K, false, c, grid, st);
+  if (out_dt == kBF16) launch<true, true, 0, __nv_bfloat16, true>(ta, tb, out, M, N, K, false, c, grid, st);
+  else launch<true, true, 0, float, true>(ta, tb, out, M, N, K, accumulate, c, grid, st);
 }
 
 bool gemm_self_check_supported() { return true; }

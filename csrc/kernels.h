@@ -86,8 +86,14 @@ void zero1_all_gather(const float* master, const int64_t* peer_bufs, long param_
                       int flag_off, uint32_t epoch, int rank, int world, long shard_numel, uint32_t* done_ctr, int param_dt,
                       cudaStream_t st);
 
+// out[M,N] (+)= (a_e4m3[M,K] · b_e4m3[N,K]ᵀ) ∘ scale_a[M] ⊗ scale_b[N]; out_dt kBF16, or kF32 (accumulate: add into out)
 void gemm_fp8(const void* a, const void* b, void* out, int M, int N, int K, const float* scale_a, const float* scale_b,
-              cudaStream_t st);
+              int out_dt, bool accumulate, cudaStream_t st);
+// ---- row-wise e4m3 quantisers of fp8 training (fp8_quant.cu), rule of fp8_rule.cuh
+// x bf16 [M, K] → q e4m3 [M, K], scale fp32 [M]; K % 8 == 0
+void quantize_fp8_rows(const void* x, void* q, float* scale, int M, int K, cudaStream_t st);
+// x bf16 [R, C] → q e4m3 [C, R] (= rows of xᵀ), scale fp32 [C]; amax_bits: zeroed u32 scratch [C]; R % 16 == 0, C % 8 == 0
+void quantize_fp8_cols_t(const void* x, void* q, float* scale, uint32_t* amax_bits, int R, int C, cudaStream_t st);
 // ---- block-scaled fp8 GEMM and its activation quantiser (gemm_fp8_block_sm90.cu); group = 32, 64 or 128 elements of K
 // out[M,N] (bf16) = Σ_g (a[:, g] · b[:, g]ᵀ) ∘ scale_a[g, :M] ⊗ scale_b[g, :N];  scale_a [K/group, scale_a_ld], scale_b [K/group, N]
 void gemm_fp8_block(const void* a, const void* b, void* out, const float* scale_a, long scale_a_ld, const float* scale_b,

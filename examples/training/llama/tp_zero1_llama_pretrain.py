@@ -33,6 +33,8 @@ def get_args(argv=None):
     p.add_argument("--num_layers", "--num_layer", dest="num_layers", type=int, default=-1)
     p.add_argument("--hidden_size", type=int, default=-1, help="override the hidden size of the chosen model (shape experiments)")
     p.add_argument("--fuse_qkv", type=int, default=1, help="one fused QKV weight per layer (1) or separate q / k / v weights (0)")
+    p.add_argument("--fp8_training", type=int, default=0,
+                   help="row-wise scaled FP8 (e4m3) GEMMs in the decoder's qkv / o / gate_up / down projections (1) or bf16 (0)")
     p.add_argument("--tensor_parallel_size", type=int, default=8)
     p.add_argument("--context_parallel_size", type=int, default=1)
     p.add_argument("--cp_layout", default="contiguous", choices=["contiguous", "zigzag"],
@@ -162,6 +164,7 @@ def main(argv=None):
     if a.hidden_size > 0:
         mcfg.hidden_size = a.hidden_size
     mcfg.fuse_qkv = bool(a.fuse_qkv)
+    mcfg.fp8_training = bool(a.fp8_training)
 
     def model_fn():
         torch.manual_seed(a.seed)

@@ -59,6 +59,9 @@ class LlamaConfig:
     device: Optional[torch.device] = None       # construct parameters directly here (e.g. cuda)
     # sliding-window attention (Mistral / Mixtral): query i sees keys i − W < j ≤ i; None = full causal attention
     sliding_window: Optional[int] = None
+    # row-wise scaled FP8 (e4m3) GEMMs in the decoder's qkv, o, gate_up and down projections (tp_linear(fp8=True));
+    # lm_head, the embedding and MoE experts stay bf16, and parameters and checkpoints are those of a bf16 model
+    fp8_training: bool = False
 
     def __post_init__(self):
         if self.num_key_value_heads is None:
@@ -105,6 +108,7 @@ class LlamaMLP(nn.Module):
             cfg.intermediate_size, cfg.hidden_size, bias=False, input_is_parallel=True, init_method=init,
             sequence_parallel_enabled=sp, sequence_dimension=0, dtype=cfg.dtype, device=cfg.device,
         )
+        self.gate_up_proj.fp8_training = self.down_proj.fp8_training = cfg.fp8_training
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         return self.down_proj(ops.act.swiglu(self.gate_up_proj(x)))
@@ -135,6 +139,7 @@ class LlamaAttention(nn.Module):
             cfg.num_attention_heads * self.head_dim, cfg.hidden_size, bias=False, input_is_parallel=True,
             init_method=init, sequence_parallel_enabled=sp, sequence_dimension=0, dtype=cfg.dtype, device=cfg.device,
         )
+        self.qkv_proj.fp8_training = self.o_proj.fp8_training = cfg.fp8_training
 
     def forward(self, x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch.Tensor:
         # x: [S(/tp), B, H]  →  q/k/v: [S, B, h_local*D]

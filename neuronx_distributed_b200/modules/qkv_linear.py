@@ -64,6 +64,9 @@ def replicate_kv(weight: torch.Tensor, multiplier: int, head_dim_rows: Optional[
 
 
 class GQAQKVColumnParallelLinear(BaseParallelLayer):
+    #: run the fused q/k/v GEMMs as row-wise scaled e4m3 products (``tp_linear(fp8=True)``), as on ``BaseParallelLinear``
+    fp8_training: bool = False
+
     def __init__(
         self,
         input_size: int,
@@ -197,7 +200,7 @@ class GQAQKVColumnParallelLinear(BaseParallelLayer):
         qp, kvp = self.q_output_size_per_partition, self.kv_output_size_per_partition
         m = self.kv_size_multiplier
         out = tp_linear(input, w, None, in_mode, "none", self.sequence_dimension, self.tensor_parallel_group,
-                        self.reduce_dtype, dgrad_col_scale=(qp, 1.0 / m) if m > 1 else None)
+                        self.reduce_dtype, dgrad_col_scale=(qp, 1.0 / m) if m > 1 else None, fp8=self.fp8_training)
         if b is not None:
             out = out + b
         q, k, v = torch.split(out, [qp, kvp, kvp], dim=-1)
@@ -252,14 +255,15 @@ def gqa_qkv_linear_with_async_allreduce(input: torch.Tensor, weight_q, weight_k,
                                         async_grad_allreduce: bool, sequence_parallel_enabled: bool, kv_size_multiplier: int = 1,
                                         weight_qkv=None, bias_qkv=None, fuse_qkv: bool = False, output_size_q: Optional[int] = None,
                                         output_size_kv: Optional[int] = None, reduce_dtype: torch.dtype = torch.float32,
-                                        sequence_dimension: int = 0, process_group=None, kv_group=None):
+                                        sequence_dimension: int = 0, process_group=None, kv_group=None, fp8: bool = False):
     """``(q, k, v) = split(x · [Wq; Wk; Wv]ᵀ)`` as ONE GEMM on the local shards.
 
     * ``sequence_parallel_enabled`` — the input is all-gathered along the sequence dim inside the GEMM kernel (fused
       AG→GEMM over NVLink peer memory) and its gradient is reduce-scattered; otherwise ``async_grad_allreduce`` all-reduces
       the input gradient over the TP group, overlapped with the weight-gradient GEMM;
     * ``kv_size_multiplier > 1`` — K/V heads are replicated across groups of TP ranks: the K and V gradients are summed over
-      the KV-shared group (``parallel_state.get_kv_shared_group``) so the replicas stay identical."""
+      the KV-shared group (``parallel_state.get_kv_shared_group``) so the replicas stay identical;
+    * ``fp8`` — the GEMMs are row-wise scaled e4m3 products (``tp_linear(fp8=True)``)."""
     group = process_group if process_group is not None else ps.get_tensor_model_parallel_group()
     tp = dist.get_world_size(group)
     if fuse_qkv:
@@ -273,7 +277,7 @@ def gqa_qkv_linear_with_async_allreduce(input: torch.Tensor, weight_q, weight_k,
         qp, kvp = weight_q.shape[0], weight_k.shape[0]
     in_mode = "gather" if sequence_parallel_enabled else ("copy" if (async_grad_allreduce and tp > 1) else "none")
     out = tp_linear(input, w, None, in_mode, "none", sequence_dimension, group, reduce_dtype,
-                    dgrad_col_scale=(qp, 1.0 / kv_size_multiplier) if kv_size_multiplier > 1 else None)
+                    dgrad_col_scale=(qp, 1.0 / kv_size_multiplier) if kv_size_multiplier > 1 else None, fp8=fp8)
     if b is not None:
         out = out + b
     q, k, v = torch.split(out, [qp, kvp, kvp], dim=-1)

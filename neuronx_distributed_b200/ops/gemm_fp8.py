@@ -13,11 +13,14 @@
   kernel, where the block's expert only shifts the TMA rows of the weight tile and of its scales.
 * :func:`quantize_groups` — the matching per-token activation quantiser (``absmax`` or OCP ``mx`` scale rule); CUDA: one
   bandwidth-bound kernel that writes the codes and the scales in the layout the GEMM reads.
+* :func:`fp8_forward`, :func:`fp8_dgrad`, :func:`fp8_wgrad` — the three products of a row-wise scaled FP8 training linear on
+  :func:`scaled_linear`'s kernel, fed by :func:`quantize_rows` / :func:`quantize_cols_t` (``csrc/fp8_quant.cu``).
 
 CPU, and shapes or dtypes the kernels do not take: the fp32 oracle of the same quantised operands.  Reference:
 quantization/quantization_layers.py (scaled matmul of the quantised parallel layers)."""
 from __future__ import annotations
 
+import os
 from typing import Optional, Tuple
 
 import torch
@@ -29,20 +32,110 @@ GROUP_SIZES = (32, 64, 128)
 
 
 def scaled_linear(xq: torch.Tensor, xs: torch.Tensor, wq: torch.Tensor, ws: torch.Tensor,
-                  out_dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+                  out_dtype: torch.dtype = torch.bfloat16, out: Optional[torch.Tensor] = None,
+                  accumulate: bool = False) -> torch.Tensor:
+    """``(xq @ wqᵀ) · xs[:, None] · ws[None, :]`` for e4m3 ``xq [..., K]`` and ``wq [N, K]``.  ``out``: an fp32 ``[M, N]``
+    tensor to write, or with ``accumulate`` to add into (per element ``old + product`` in fp32, one rounding)."""
     shape = xq.shape
     x2 = xq.reshape(-1, shape[-1])
     s2 = xs.reshape(-1, 1).float()
+    if out is not None:
+        assert out.dtype == torch.float32 and out.shape == (x2.shape[0], wq.shape[0]), "out must be fp32 [M, N]"
+        out_dtype = torch.float32
+    assert not accumulate or out is not None, "accumulate needs out"
     e = _ext.ext() if x2.is_cuda else None
     if (e is not None and hasattr(e, "gemm_fp8") and x2.shape[1] % 16 == 0 and wq.shape[0] % 8 == 0
-            and xq.dtype == torch.float8_e4m3fn and wq.dtype == torch.float8_e4m3fn and out_dtype == torch.bfloat16):
-        out = torch.empty(x2.shape[0], wq.shape[0], dtype=out_dtype, device=x2.device)
+            and xq.dtype == torch.float8_e4m3fn and wq.dtype == torch.float8_e4m3fn
+            and (out_dtype == torch.bfloat16 or (out is not None and out.is_contiguous() and out.data_ptr() % 8 == 0))):
+        if out is None:
+            out = torch.empty(x2.shape[0], wq.shape[0], dtype=out_dtype, device=x2.device)
         _ext.count_launch()
         e.gemm_fp8(x2.contiguous(), wq.contiguous(), out, s2.expand(x2.shape[0], 1).contiguous().view(-1),
-                   ws.float().reshape(-1).expand(wq.shape[0]).contiguous())
+                   ws.float().reshape(-1).expand(wq.shape[0]).contiguous(), accumulate)
         return out.view(*shape[:-1], wq.shape[0])
     y = (x2.float() @ wq.float().t()) * s2 * ws.float().reshape(1, -1)
+    if out is not None:
+        return out.add_(y) if accumulate else out.copy_(y)
     return y.to(out_dtype).view(*shape[:-1], wq.shape[0])
+
+
+# ---- row-wise scaled FP8 training ------------------------------------------------------------------------------------
+# A linear y = x·Wᵀ (x [M, K], W [N, K], g = dL/dy [M, N]) runs three e4m3 GEMMs on operands quantised by one rule,
+# rows(t) = one absmax scale per row of t (the group rule with G = the row length) and cols_t(t) = rows(tᵀ):
+#
+#   forward         rows(x)  [M, K] · rows(W)   [N, K]ᵀ → bf16 y  [M, N]
+#   input gradient  rows(g)  [M, N] · cols_t(W) [K, N]ᵀ → bf16 dx [M, K]
+#   weight gradient cols_t(g)[N, M] · cols_t(x) [K, M]ᵀ → fp32 dW [N, K]   (or added into an fp32 main_grad)
+#
+# e4m3 wgmma reads K-major operands only, hence the transposed copies of W, g and x.  CUDA (bf16 operands, M, N, K multiples
+# of 16, 16-byte aligned starts): csrc/fp8_quant.cu and the fp8 GEMM of csrc/gemm_sm90.cu.  Otherwise, and with
+# NXD_DISABLE_TCGEN05_GEMM=1, the torch oracle quantiser and the fp32 matmul of the dequantised operands.
+def _rows_reference(t: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    q, s = _quantize_groups_reference(t, t.shape[1], "absmax", None)
+    return q, s.reshape(-1)
+
+
+def quantize_rows(t: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``t [R, C]`` → (e4m3 ``[R, C]``, fp32 ``[R]``): ``s_r = max(amax_r / 448, 1e-12)``, codes ``RNE(clamp(t / s, ±448))``; a
+    row holding a NaN or ±inf gets a NaN scale and NaN codes.  CUDA kernel for bf16 with ``C % 8 == 0`` and a 16-byte aligned
+    start, bit for bit the oracle on the same device (NaN sign excepted); otherwise the oracle."""
+    t = t.contiguous()
+    if (t.dtype == torch.bfloat16 and t.shape[1] % 8 == 0 and t.numel() > 0 and _ext.use_cuda(t)
+            and hasattr(_ext.ext(), "quantize_fp8_rows") and t.data_ptr() % 16 == 0):
+        _ext.count_launch()
+        q, s = _ext.ext().quantize_fp8_rows(t)
+        return q, s
+    return _rows_reference(t)
+
+
+def quantize_cols_t(t: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``t [R, C]`` → (e4m3 ``[C, R]``, fp32 ``[C]``) = :func:`quantize_rows` of ``tᵀ``: one scale per column of ``t``, the codes
+    transposed so that a GEMM contracting over R reads them K-major.  CUDA kernels for bf16 with ``R % 16 == 0`` (the rows are
+    a TMA operand), ``C % 8 == 0`` and a 16-byte aligned start; otherwise the oracle."""
+    t = t.contiguous()
+    if (t.dtype == torch.bfloat16 and t.shape[0] % 16 == 0 and t.shape[1] % 8 == 0 and t.numel() > 0 and _ext.use_cuda(t)
+            and hasattr(_ext.ext(), "quantize_fp8_cols_t") and t.data_ptr() % 16 == 0):
+        _ext.count_launch(2)                        # column absmax, then quantise-and-transpose
+        q, s = _ext.ext().quantize_fp8_cols_t(t)
+        return q, s
+    return _rows_reference(t.t())
+
+
+def _fp8_product(a: torch.Tensor, a_cols_t: bool, b: torch.Tensor, b_cols_t: bool, M: int, N: int, K: int,
+                 out: Optional[torch.Tensor] = None, accumulate: bool = False) -> torch.Tensor:
+    """``Q(a) · Q(b)ᵀ`` with Q = cols_t or rows per operand, for a linear of ``M`` tokens, ``N`` outputs and ``K`` inputs."""
+    a, b = a.contiguous(), b.contiguous()
+    if (os.environ.get("NXD_DISABLE_TCGEN05_GEMM", "0") != "1" and M > 0 and M % 16 == 0 and N % 16 == 0 and K % 16 == 0
+            and a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and a.data_ptr() % 16 == 0 and b.data_ptr() % 16 == 0
+            and _ext.use_cuda(a, b) and hasattr(_ext.ext(), "quantize_fp8_cols_t")):
+        aq, sa = quantize_cols_t(a) if a_cols_t else quantize_rows(a)
+        bq, sb = quantize_cols_t(b) if b_cols_t else quantize_rows(b)
+        return scaled_linear(aq, sa, bq, sb, out=out, accumulate=accumulate)
+    aq, sa = _rows_reference(a.t() if a_cols_t else a)
+    bq, sb = _rows_reference(b.t() if b_cols_t else b)
+    y = (aq.float() * sa.reshape(-1, 1)) @ (bq.float() * sb.reshape(-1, 1)).t()
+    if out is not None:
+        return out.add_(y) if accumulate else out.copy_(y)
+    return y.bfloat16()
+
+
+def fp8_forward(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
+    """bf16 ``y [M, N] = rows(x) · rows(W)ᵀ`` for ``x [M, K]``, ``W [N, K]``."""
+    return _fp8_product(x, False, w, False, x.shape[0], w.shape[0], w.shape[1])
+
+
+def fp8_dgrad(g: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
+    """bf16 ``dx [M, K] = rows(g) · cols_t(W)ᵀ`` for ``g [M, N]``, ``W [N, K]``."""
+    return _fp8_product(g, False, w, True, g.shape[0], w.shape[0], w.shape[1])
+
+
+def fp8_wgrad(g: torch.Tensor, x: torch.Tensor, out: Optional[torch.Tensor] = None, accumulate: bool = False) -> torch.Tensor:
+    """fp32 ``dW [N, K] = cols_t(g) · cols_t(x)ᵀ`` for ``g [M, N]``, ``x [M, K]``, written into ``out`` or, with
+    ``accumulate``, added to it (fp32 ``old + product``, one rounding: the TMA reduce-add on CUDA)."""
+    if out is None:
+        out = torch.empty(g.shape[1], x.shape[1], dtype=torch.float32, device=g.device)
+        accumulate = False
+    return _fp8_product(g, True, x, True, g.shape[0], g.shape[1], x.shape[1], out, accumulate)
 
 
 # ---- block-scaled ----------------------------------------------------------------------------------------------------

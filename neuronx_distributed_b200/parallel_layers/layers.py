@@ -139,6 +139,8 @@ class BaseParallelLinear(BaseParallelLayer):
 
     arg_init_method: Optional[Callable[..., Any]] = None
     pad: bool = False
+    #: run the layer's GEMMs as row-wise scaled e4m3 products (``tp_linear(fp8=True)``); parameters and checkpoints are unchanged
+    fp8_training: bool = False
 
     def _init_weight(self, w: torch.Tensor) -> None:
         if self.arg_init_method is None:
@@ -404,21 +406,38 @@ def _flat2d(x: torch.Tensor) -> torch.Tensor:
     return x.reshape(-1, x.shape[-1])
 
 
-def wgrad(go2d: torch.Tensor, x2d: torch.Tensor, weight: torch.Tensor):
+def _add_to_main_grad(weight: torch.Tensor, product: Callable[[torch.Tensor, bool], Any]) -> bool:
+    """The ZeRO-1 ``main_grad`` protocol of a weight gradient.  If the optimizer gave the weight an fp32 ``main_grad``,
+    ``product(main_grad, accumulate)`` writes the gradient into it (overwriting while ``main_grad_fresh`` is set, the first
+    contribution since ``zero_grad``), and ``_nxd_grad_ready`` tells the overlapped reduce-scatter that it is final.  Returns
+    False, with nothing done, when there is no such buffer."""
+    mg = getattr(weight, "main_grad", None)
+    if not (mg is not None and mg.dtype == torch.float32 and mg.is_contiguous() and mg.shape == weight.shape):
+        return False
+    product(mg, not getattr(weight, "main_grad_fresh", False))
+    weight.main_grad_fresh = False
+    cb = getattr(weight, "_nxd_grad_ready", None)      # ZeRO-1 overlapped reduce-scatter: this gradient is final
+    if cb is not None:
+        cb(weight)
+    return True
+
+
+def wgrad(go2d: torch.Tensor, x2d: torch.Tensor, weight: torch.Tensor, fp8: bool = False):
     """``dW = goᵀ @ x``.  If the optimizer gave the weight an fp32 ``main_grad`` buffer (ZeRO-1 with fp32 gradient
     accumulation) the GEMM epilogue accumulates straight into it — no bf16 gradient tensor, no cast, no separate
-    add kernel — and ``None`` is returned to autograd (Megatron-style gradient-accumulation fusion)."""
-    from .. import ops
+    add kernel — and ``None`` is returned to autograd (Megatron-style gradient-accumulation fusion).
 
-    mg = getattr(weight, "main_grad", None)
-    if (mg is not None and go2d.is_cuda and go2d.dtype == torch.bfloat16 and mg.dtype == torch.float32
-            and mg.is_contiguous() and mg.shape == weight.shape and ops.gemm.fused_wgrad_enabled()):
-        fresh = getattr(weight, "main_grad_fresh", False)
-        ops.gemm.matmul(go2d, x2d, True, False, out=mg, accumulate=not fresh)
-        weight.main_grad_fresh = False
-        cb = getattr(weight, "_nxd_grad_ready", None)      # ZeRO-1 overlapped reduce-scatter: this gradient is final
-        if cb is not None:
-            cb(weight)
+    ``fp8``: the row-wise scaled e4m3 product ``cols_t(go) · cols_t(x)ᵀ`` (``ops.gemm_fp8.fp8_wgrad``), reduce-added into the
+    ``main_grad`` in fp32, or without one a fresh fp32 result cast to the weight's dtype."""
+    from .. import ops
+    from ..ops import gemm_fp8
+
+    if fp8:
+        if _add_to_main_grad(weight, lambda mg, acc: gemm_fp8.fp8_wgrad(go2d, x2d, out=mg, accumulate=acc)):
+            return None
+        return gemm_fp8.fp8_wgrad(go2d, x2d).to(weight.dtype)
+    if (go2d.is_cuda and go2d.dtype == torch.bfloat16 and ops.gemm.fused_wgrad_enabled()
+            and _add_to_main_grad(weight, lambda mg, acc: ops.gemm.matmul(go2d, x2d, True, False, out=mg, accumulate=acc))):
         return None
     return ops.gemm.matmul(go2d, x2d, True, False)
 
@@ -434,19 +453,25 @@ class _TPLinear(torch.autograd.Function):
       * ``"none"``   → ``"reduce"`` : Row, no SP. fwd GEMM→AR ; bwd GEMM
     Semantics follow reference layers.py:434-532 and layers_utils.py:16-140 (input is saved
     *sharded* and re-gathered in backward; dgrad collective overlaps wgrad).
+
+    ``fp8``: the three GEMMs are the row-wise scaled e4m3 products of ``ops.gemm_fp8`` (``fp8_forward`` / ``fp8_dgrad`` /
+    ``fp8_wgrad``) around the library collectives; the fused TP kernels are bf16, so they are not dispatched.
     """
 
     @staticmethod
-    def forward(ctx, x, weight, bias, in_mode, out_mode, seq_dim, group, reduce_dtype, save_for_backward, dgrad_col_scale=None):
+    def forward(ctx, x, weight, bias, in_mode, out_mode, seq_dim, group, reduce_dtype, save_for_backward, dgrad_col_scale=None,
+                fp8=False):
         from .. import ops
+        from ..ops import gemm_fp8
 
         ctx.in_mode, ctx.out_mode, ctx.seq_dim, ctx.group = in_mode, out_mode, seq_dim, group
         ctx.dgrad_col_scale = dgrad_col_scale
         ctx.reduce_dtype = reduce_dtype
         ctx.has_bias = bias is not None
         ctx.x_requires_grad = x.requires_grad
+        ctx.fp8 = fp8
         n = dist.get_world_size(group)
-        fused = ops.tp_fused.dispatch(x, weight, in_mode, out_mode, seq_dim, group)
+        fused = None if fp8 else ops.tp_fused.dispatch(x, weight, in_mode, out_mode, seq_dim, group)
         if fused is not None:
             ctx.fused = True
             y = fused.forward(x, weight)
@@ -462,7 +487,7 @@ class _TPLinear(torch.autograd.Function):
             if save_for_backward:
                 ctx.save_for_backward(x, weight)
             total = comm.all_gather(x, dim=seq_dim, group=group) if (in_mode == "gather" and n > 1) else x
-            if (n > 1 and out_mode == "reduce" and not torch.is_grad_enabled() and total.is_cuda
+            if (n > 1 and out_mode == "reduce" and not fp8 and not torch.is_grad_enabled() and total.is_cuda
                     and total.numel() // total.shape[-1] <= 8 and ops.tp_fused.get_backend() == "fused"
                     and ops.nvls.gemv_all_reduce_eligible(total.reshape(-1, total.shape[-1]), weight)):
                 # decode-time Row-parallel linear: GEMV and the all-reduce of its fp32 partials in ONE kernel
@@ -471,7 +496,10 @@ class _TPLinear(torch.autograd.Function):
                 if bias is not None:
                     y = y + bias
                 return y
-            y = ops.gemm.linear_nt(total, weight)          # wgmma kernel on CUDA bf16, torch.matmul otherwise
+            if fp8:
+                y = gemm_fp8.fp8_forward(_flat2d(total), weight).view(*total.shape[:-1], weight.shape[0])
+            else:
+                y = ops.gemm.linear_nt(total, weight)      # wgmma kernel on CUDA bf16, torch.matmul otherwise
             if n > 1 and out_mode in ("scatter", "reduce"):
                 od = y.dtype
                 yr = y.to(reduce_dtype) if reduce_dtype is not None else y
@@ -487,6 +515,7 @@ class _TPLinear(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gy):
         from .. import ops
+        from ..ops import gemm_fp8
 
         group, seq_dim = ctx.group, ctx.seq_dim
         n = dist.get_world_size(group)
@@ -509,7 +538,7 @@ class _TPLinear(torch.autograd.Function):
             fused = ops.tp_fused.dispatch(x, weight, in_mode, out_mode, seq_dim, group)
             gx, gw, gbias = fused.backward(x, weight, gy, ctx.has_bias, ctx.x_requires_grad, weight.requires_grad,
                                            gathered, gy_dgrad=(gy_d if gy_d is not gy else None))
-            return gx, gw, gbias, None, None, None, None, None, None, None
+            return gx, gw, gbias, None, None, None, None, None, None, None, None
         x, weight = ctx.saved_tensors
 
         # ---- grad wrt the GEMM output (undo the output collective) -----------------
@@ -525,7 +554,11 @@ class _TPLinear(torch.autograd.Function):
         work = None
         if ctx.x_requires_grad:
             g_d = g_out if gy_d is gy else gy_d          # dgrad_col_scale is only used with out_mode "none" (g_out is gy)
-            gx = ops.gemm.matmul(_flat2d(g_d), weight, False, False).view(*g_out.shape[:-1], weight.shape[1])
+            if ctx.fp8:
+                gx = gemm_fp8.fp8_dgrad(_flat2d(g_d), weight)
+            else:
+                gx = ops.gemm.matmul(_flat2d(g_d), weight, False, False)
+            gx = gx.view(*g_out.shape[:-1], weight.shape[1])
             if n > 1 and in_mode == "copy":
                 work = comm.all_reduce(gx, group=group, async_op=True)  # overlaps wgrad
             elif n > 1 and in_mode == "gather":
@@ -536,10 +569,10 @@ class _TPLinear(torch.autograd.Function):
         gw = None
         if weight.requires_grad:
             total = comm.all_gather(x, dim=seq_dim, group=group) if (in_mode == "gather" and n > 1) else x
-            gw = wgrad(_flat2d(g_out), _flat2d(total), weight)
+            gw = wgrad(_flat2d(g_out), _flat2d(total), weight, fp8=ctx.fp8)
         if work is not None:
             work.wait()
-        return gx, gw, gbias, None, None, None, None, None, None, None
+        return gx, gw, gbias, None, None, None, None, None, None, None, None
 
 
 def tp_linear(
@@ -554,9 +587,14 @@ def tp_linear(
     save_for_backward: bool = True,
     autocast: bool = False,
     dgrad_col_scale=None,
+    fp8: bool = False,
 ) -> torch.Tensor:
     """``dgrad_col_scale=(first_col, scale)``: output-gradient columns ``>= first_col`` are multiplied by ``scale`` for the
-    input-gradient GEMM only (weight gradient sees them unscaled) — the GQA KV-replication correction."""
+    input-gradient GEMM only (weight gradient sees them unscaled) — the GQA KV-replication correction.
+
+    ``fp8``: forward, input-gradient and weight-gradient GEMMs in e4m3 with one absmax scale per row of each operand
+    (``ops.gemm_fp8``: rows(x)·rows(W)ᵀ, rows(g)·cols_t(W)ᵀ, cols_t(g)·cols_t(x)ᵀ); the bias, the collectives and the tensors
+    saved for backward stay bf16."""
     assert dgrad_col_scale is None or out_mode == "none"
     group = group if group is not None else ps.get_tensor_model_parallel_group()
     if autocast or torch.is_autocast_enabled():
@@ -566,8 +604,9 @@ def tp_linear(
         bias = bias.to(dt) if bias is not None else None
         with torch.autocast(device_type="cuda" if x.is_cuda else "cpu", enabled=False):
             return _TPLinear.apply(x, weight, bias, in_mode, out_mode, seq_dim, group, reduce_dtype, save_for_backward,
-                                   dgrad_col_scale)
-    return _TPLinear.apply(x, weight, bias, in_mode, out_mode, seq_dim, group, reduce_dtype, save_for_backward, dgrad_col_scale)
+                                   dgrad_col_scale, fp8)
+    return _TPLinear.apply(x, weight, bias, in_mode, out_mode, seq_dim, group, reduce_dtype, save_for_backward, dgrad_col_scale,
+                           fp8)
 
 
 class LinearWithAsyncCommunication:
@@ -736,7 +775,8 @@ class ColumnParallelLinear(BaseParallelLinear):
         else:
             in_mode = "copy" if tp > 1 else "none"
         out = tp_linear(
-            input, weight, None, in_mode, "none", self.sequence_dimension, self.tensor_parallel_group, self.reduce_dtype
+            input, weight, None, in_mode, "none", self.sequence_dimension, self.tensor_parallel_group, self.reduce_dtype,
+            fp8=self.fp8_training,
         )
         if self.gather_output:
             out = mappings.gather_from_tensor_model_parallel_region(out, self.tensor_parallel_group)
@@ -869,7 +909,7 @@ class RowParallelLinear(BaseParallelLinear):
         weight = self.weight if slice_indices is None else self.weight.index_select(1, slice_indices)
         out = tp_linear(
             x, weight, None, "none", out_mode, self.sequence_dimension, self.tensor_parallel_group,
-            self.reduce_dtype,
+            self.reduce_dtype, fp8=self.fp8_training,
         )
         if self.skip_bias_add:
             return out, self.bias
